@@ -1,7 +1,8 @@
 #!/usr/bin/env python
-"""Headline benchmark: RepVGG-A0 224x224 bf16 TRAINING throughput (images/s) on N B200s of one node.
+"""Headline benchmark: RepVGG-A0 224x224 bf16 TRAINING throughput (images/s) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 20 --warmup 5                       # this repo's CUDA path (default arm)
+    python bench.py --gpus 1 --steps 20 --warmup 5 --dump-outputs DIR    # + what the last timed step computed, as .npy
     python -m torch.distributed.run --nproc-per-node N ... bench.py --gpus N --steps K --warmup W
     python bench.py --impl reference --steps 2 --warmup 1                # reference algorithm on the host CPU cores
 
@@ -32,18 +33,19 @@ IMAGENET_STD = (0.229, 0.224, 0.225)
 
 
 def measured_peaks():
-    """Roofline denominators: MEASURED_PEAKS.json (driver-written) or the profiling guide's fallback."""
+    """Roofline denominators: MEASURED_PEAKS.json (measured on the machine, when present) or the H100 SXM data sheet
+    (3.35 TB/s HBM3, 989 dense BF16 TFLOP/s at 700 W)."""
     path = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         with open(path) as f:
             d = json.load(f)
         return {"hbm_gbs": d["hbm_gbs"], "bf16_tflops": d.get("bf16_tflops_sustained", d["bf16_tflops"]), "src": "measured"}
-    return {"hbm_gbs": 6650.0, "bf16_tflops": 1400.0, "src": "fallback"}
+    return {"hbm_gbs": 3350.0, "bf16_tflops": 989.0, "src": "datasheet"}
 
 
 class ClockSampler:
     """Samples SM clocks / throttle reasons while the timed region runs: NVML from a background thread (4 Hz; a
-    100 ms `nvidia-smi -lms` poller was measured to slow kernel launches of the process under test by 2x), falling
+    fast `nvidia-smi -lms` poller slows the kernel launches of the process under test), falling
     back to a 500 ms `nvidia-smi` loop when the NVML binding is unavailable."""
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,"
          "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap")
@@ -281,9 +283,9 @@ def run_reference(args, rank):
 
 
 def cpu_threads() -> int:
-    """Threads for the CPU legs. Measured on the 128-thread GPU host (tools/cpu_thread_probe.py, fwd+bwd of an 8-image
-    batch): 8 threads 0.26 s, 16 threads 0.21 s, 32 threads 0.30 s, 64 threads 0.70 s - torch's CPU convolutions stop
-    scaling at ~16 threads for this workload, so the CPU legs use min(16, cpu_count). Override: HB_CPU_THREADS."""
+    """Threads for the CPU legs: torch's CPU convolutions stop scaling at about 16 threads for an 8-image batch of this
+    workload (tools/cpu_thread_probe.py measures it on a given host), so the CPU legs use min(16, cpu_count).
+    Override: HB_CPU_THREADS."""
     env = os.environ.get("HB_CPU_THREADS")
     if env:
         return max(1, int(env))
@@ -321,7 +323,7 @@ def cpu_baseline(budget_s: float = 20.0):
 
 
 def gpu_eager_baseline(batch: int, dev, steps: int = 5):
-    """The reference's own execution model on the SAME B200 (SURVEY §8d, BASELINE.md §3.4): stock torch eager modules
+    """The reference's own execution model on the SAME GPU (SURVEY §8d, BASELINE.md §3.4): stock torch eager modules
     (cuDNN / ATen kernels), bf16 autocast, channels_last, per-tensor AdaBelief update written as the reference writes it
     (~9 ATen launches per parameter tensor). Uses the oracle's module tree (reference algorithm, stock torch layers); it
     is a reported baseline measured beside the product, never part of it."""
@@ -415,16 +417,6 @@ def roofline_leg(K, run_step, opt_step, n_params: int, step_ms: float, images: i
     roof["traffic"] = None
     roof["algorithmic_bytes"] = d["bytes"] / d["launches"]
     roof["algorithmic_flops"] = d["flops"] / d["launches"]
-    try:
-        with open(os.path.join(ROOT, "profiles", "r02_traffic.json")) as f:
-            tk = json.load(f)["kernels"]
-        names = dom.split("+")      # ncu prints template arguments: conv_fprop_kernel<0>, bn_act_fwd_kernel<3, 1>, ...
-        famk = [v for k, v in tk.items() if any(k == n or k.startswith(n + "<") for n in names)]
-        if famk:
-            roof["traffic"] = sum(k["dram_read_bytes"] + k["dram_write_bytes"] for k in famk) / max(sum(k["launches"] for k in famk), 1)
-            roof["traffic_source"] = "ncu dram__bytes_read.sum + dram__bytes_write.sum (profiles/r02_traffic.json), per launch"
-    except (OSError, KeyError, ValueError):
-        pass
     roof["kernel"] = dom
     roof["peak_source"] = peaks["src"]
     roof["peaks"] = {"bf16_tflops_sustained": peaks["bf16_tflops"], "hbm_gbs": peaks["hbm_gbs"]}
@@ -438,6 +430,26 @@ def roofline_leg(K, run_step, opt_step, n_params: int, step_ms: float, images: i
 
 TRAIN_MACS = {"repvgg_a0": 2.821e9, "repvgg_a1": 4.329e9, "rexnet1_0x": 0.398e9, "yolov4": 45.52e9, "unet3p": 195.49e9,
               "resnet50": 4.09e9, "resnet18": 1.81e9, "mobileone_s0": 1.07e9}
+
+
+# ------------------------------------------------------------------------------------------------ output dump
+DUMP_PARAM_SAMPLE = 1 << 22     # parameters beyond this many elements are dumped as a fixed, seeded sample (16 MB)
+
+
+def dump_outputs(out_dir: str, loss, model) -> None:
+    """What the timed train step hands back after its last timed iteration: the loss it returned and the parameters it
+    updated (all parameters flattened in ``model.parameters()`` order, fp32; when the model is larger than 2^22 elements,
+    the sorted elements of ``torch.randperm(n, generator=manual_seed(1234))[:2^22]``), as DIR/loss.npy and DIR/params.npy.
+    Inputs are seeded, so two builds run with the same arguments can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    flat = torch.cat([p.detach().reshape(-1).float() for p in model.parameters()])
+    np.save(os.path.join(out_dir, "loss.npy"), loss.detach().float().reshape(1).cpu().numpy())
+    if flat.numel() > DUMP_PARAM_SAMPLE:
+        g = torch.Generator(device="cpu").manual_seed(1234)
+        idx = torch.randperm(flat.numel(), generator=g)[:DUMP_PARAM_SAMPLE].sort().values
+        flat = flat[idx.to(flat.device)]
+    np.save(os.path.join(out_dir, "params.npy"), flat.cpu().numpy())
 
 
 # ------------------------------------------------------------------------------------------------ main arm
@@ -523,6 +535,8 @@ def measure(args, wl: Workload, rank: int, local_rank: int, world: int, full: bo
     launches = lib().hb_launch_count() + (graphed.launches_per_replay * args.steps if graphed is not None else 0)
     ms = e0.elapsed_time(e1) / args.steps
     clocks = sampler.stop() if rank == 0 else None
+    if rank == 0 and getattr(args, "dump_outputs", None):
+        dump_outputs(args.dump_outputs, loss, model)
 
     # ---- timed region 2: end to end through the public API with host buffers -----------------------
     copy_stream = torch.cuda.Stream()
@@ -570,7 +584,7 @@ def measure(args, wl: Workload, rank: int, local_rank: int, world: int, full: bo
         "config": {"workload": wl.desc, "batch_per_gpu": batch, "global_batch": images, "parallelism": f"dp{world}",
                    "allreduce": ("none" if world == 1 else ("overlapped chunks on a side stream" if reducer is not None
                                                             else "single all-reduce after backward")),
-                   "l2": "per-step working set (GBs of activations) exceeds the 126 MB L2; no explicit flush",
+                   "l2": "per-step working set (GBs of activations) exceeds the 50 MB L2; no explicit flush",
                    "launch": "cuda_graph" if graphed is not None else "eager"},
         "e2e": {"value": images / ms_e2e * 1e3, "unit": "images/s", "ms_per_step": ms_e2e,
                 "h2d_bytes_per_step": int(sum(t.numel() * t.element_size() for t in host)), "d2h_bytes_per_step": 4,
@@ -613,7 +627,13 @@ def main():
     ap.add_argument("--no-direct-grads", action="store_true", help="let autograd accumulate parameter gradients (A/B switch)")
     ap.add_argument("--no-overlap", action="store_true", help="N > 1: one all-reduce after backward instead of overlapped chunks")
     ap.add_argument("--no-secondary", action="store_true", help="skip the ReXNet-1.0x leg (BASELINE configs[1]) at N=1")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's loss and updated parameters as DIR/*.npy (float32)")
     args = ap.parse_args()
+    if args.dump_outputs and (args.impl == "reference" or args.micro):
+        ap.error("--dump-outputs writes what the timed train step of the CUDA path computed: it needs --impl b200 and no --micro")
+    if args.impl != "reference" and args.steps < 1:
+        ap.error("--steps must be at least 1 (the timed region averages over the steps)")
     if args.config:
         args.model = {1: "rexnet1_0x", 2: "repvgg_a1", 3: "yolov4", 4: "unet3p"}[args.config]
 
@@ -648,7 +668,7 @@ def main():
             gc.collect()
             torch.cuda.empty_cache()
             sargs = argparse.Namespace(**vars(args))
-            sargs.steps, sargs.warmup, sargs.batch = 10, 3, 0
+            sargs.steps, sargs.warmup, sargs.batch, sargs.dump_outputs = 10, 3, 0, None
             sec = measure(sargs, Workload("rexnet1_0x"), 0, local_rank, 1, full=False)
             result["secondary"] = {"workload": sec["config"]["workload"] + ", batch 256, CUDA-graph replay, inputs resident in HBM",
                                    "images_per_s": sec["value"], "ms_per_step": sec["ms_per_step"], "steps": sec["steps"],

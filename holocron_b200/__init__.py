@@ -1,4 +1,4 @@
-"""holocron_b200: B200-native (sm_100a) implementation of the data-parallel training hot path of frgfm/Holocron.
+"""holocron_b200: H100-native (sm_90a) implementation of the data-parallel training hot path of frgfm/Holocron.
 
 Public surface mirrors ``holocron.nn`` / ``holocron.nn.functional`` / ``holocron.ops`` / ``holocron.optim`` /
 ``holocron.models`` for the hot-path components (see DESIGN.md). All compute goes through the C-ABI CUDA library

@@ -9,7 +9,7 @@ namespace hb {
 enum Act { ACT_NONE = 0, ACT_RELU = 1, ACT_RELU6 = 2, ACT_SILU = 3, ACT_LEAKY = 4, ACT_MISH = 5, ACT_HARDMISH = 6, ACT_FRELU = 7 };
 
 // Fast-math forms (the BatchNorm / gate passes are HBM streams: with IEEE division, log1pf and tanhf the SiLU / Mish
-// variants were ALU-bound at ~1.3 TB/s, profiles/r02_launches_rexnet1_0x_b256.md). Relative error ~1e-6, far below bf16.
+// variants are ALU-bound instead). Relative error ~1e-6, far below bf16.
 //   sigmoid(z) = 1 / (1 + e^-z)
 //   mish(z)    = z * tanh(log(1 + e^z)) = z * n / (n + 2),  n = e^z (e^z + 2)        (tanh(log u) = (u^2-1)/(u^2+1))
 __device__ __forceinline__ float fast_sigmoid(float z) { return __fdividef(1.f, 1.f + __expf(-z)); }

@@ -131,7 +131,7 @@ struct FinalizeParams {
 // block = 8 channels (threadIdx.x: one 64-byte run of the [slot][C][2] partials) x 32 slot lanes (threadIdx.y). A lane adds
 // slots L, L + 32, ... with four independent loads in flight, the 32 lane sums are then combined 8-by-8 in lane order: a
 // fixed summation order (run-to-run identical) whose dependent-load chain is slots / 128 long. (32 channels x 8 lanes: slots /
-// 8 dependent L2 round trips and C / 32 blocks - two blocks for a 48-channel layer - made each of these ~10-20 us.)
+// 8 dependent L2 round trips and C / 32 blocks - two blocks for a 48-channel layer - is latency bound.)
 constexpr int kFinCh = 8, kFinLanes = 32;
 
 __global__ void __launch_bounds__(kFinCh * kFinLanes) bn_finalize_kernel(FinalizeParams p) {
@@ -242,11 +242,11 @@ __device__ __forceinline__ void lds8(const float* p, float* f);
 // Every thread streams ITS OWN 16-byte vectors (one per input tensor and row) global -> shared with cp.async, kDepth rows
 // ahead of the row it is computing on; nothing else reads those slots, so the ring needs no barrier at all. This puts
 // kDepth * (#inputs) * 16 B per thread in flight without holding them in registers: the register-staged version of these
-// kernels had ~36 KB per SM in flight and sat at 2.2 - 3.4 TB/s with long-scoreboard stalls (profiles/r01_bn_ncu.md);
-// HBM needs ~60 KB per SM (44 GB/s per SM x ~1.3 us loaded latency).
+// kernels had far fewer bytes per SM in flight than the HBM bandwidth x loaded latency product and stalled on long
+// scoreboard waits.
 // rows in flight per thread as a function of the number of streamed tensors NT: what matters is BYTES in flight per SM
 // (depth * NT * 16 B * 256 threads * resident blocks). With depth 3 the single-branch units (ReXNet / Darknet / UNet3+ /
-// YOLOv4: one input tensor) had only ~49 KB per SM in flight and ran at 1.6 TB/s; deeper rings for fewer tensors.
+// YOLOv4: one input tensor) keep too few bytes in flight with depth 3; deeper rings for fewer tensors.
 // depth + 1 slots: keep the slot count a power of two (the slot index is k % slots on a 64-bit row counter)
 __host__ __device__ constexpr int ring_depth(int nt) { return nt <= 2 ? 7 : 3; }
 
@@ -741,8 +741,7 @@ inline cudaError_t allow_smem(K kernel, size_t bytes) {
 
 // Resident blocks per SM of one kernel instantiation with SMEM dynamic bytes, asked from the runtime once. The grids are
 // persistent (every block walks M / gridDim.x rows), so a grid of 4 blocks per SM of a kernel that only fits 3 runs as one
-// full wave plus a one-third-occupied second wave: bn_act_fwd_kernel<2, 1> streamed at 3.3 TB/s with 592 blocks where the
-// 444-block <3, 1> reached 4.8 TB/s (profiles/r02_launches_repvgg_a0_b256.csv).
+// full wave plus a one-third-occupied second wave, which streams markedly slower than a grid of exactly the resident blocks.
 template <typename K>
 inline int resident_blocks(K kernel, size_t smem) {
   int n = 0;

@@ -70,8 +70,7 @@ __device__ __forceinline__ float pair_value(int mode, const Box& a, const Box& b
 
 // Tile = kRows rows of boxes1 x (blockDim.x * 4) columns of boxes2. A thread keeps its 4 boxes2 in registers, walks the
 // rows (boxes1 row = one broadcast 16-byte load) and writes 4 consecutive outputs per row - one 128-bit store when the
-// output row is 16-byte aligned. The first version did a 64-bit division and 8 scalar loads per PAIR (0.07-0.10 of the HBM
-// rate on 4096 x 4096). kMode is a template parameter so the per-pair switch is gone as well.
+// output row is 16-byte aligned. A 64-bit division and 8 scalar loads per PAIR would make this ALU bound. kMode is a template parameter so the per-pair switch is gone as well.
 constexpr int kRows = 16;
 
 template <int kMode>

@@ -1,10 +1,10 @@
-"""Builds libholocron_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_100a.
+"""Builds libholocron_b200.so (the C-ABI CUDA library) in-tree with nvcc for sm_90a.
 
 Usage: ``python -m holocron_b200.csrc.build [--force]``. Each ``.cu`` file is its own translation unit
 (compiled in parallel), then linked with ``nvcc -shared``. The cudart runtime is linked statically so
 that the library only depends on libcuda/libdl at load time; the TMA descriptor encoder
 (``cuTensorMapEncode*``) is resolved at run time through ``cudaGetDriverEntryPoint`` so there is no
-link-time dependency on libcuda either (this container has no driver).
+link-time dependency on libcuda either (the library builds on machines without a driver).
 """
 import os
 import subprocess
@@ -16,7 +16,7 @@ HERE = Path(__file__).resolve().parent
 OBJ = HERE / "build"
 LIB = HERE / "libholocron_b200.so"
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 CFLAGS = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "--expt-relaxed-constexpr",
           "-Xptxas", "-v", "-I", str(HERE), "-I", str(HERE.parent.parent / "include")]
 

@@ -1,4 +1,4 @@
-// Shared device helpers for the holocron_b200 sm_100a kernels.
+// Shared device helpers for the holocron_b200 sm_90a kernels.
 // Everything here is header-only; each .cu translation unit includes it.
 #pragma once
 #include <cuda_runtime.h>
@@ -10,7 +10,8 @@
 #define HB_DTYPE_BF16 1
 #define HB_DTYPE_F16 2
 
-#define HB_NUM_SMS 148
+
+#define HB_NUM_SMS (hb::num_sms())
 
 #include <atomic>
 extern std::atomic<long long> g_hb_launches;  // defined in runtime.cu
@@ -24,6 +25,20 @@ extern std::atomic<long long> g_hb_launches;  // defined in runtime.cu
   } while (0)
 
 namespace hb {
+
+// SM count of the current device (H100 SXM: 132, H100 PCIe: 114): sizes the persistent grids and the partial-sum slot
+// counts. Read from the runtime once per device.
+inline int num_sms() {
+  static int cache[64] = {0};
+  int dev = 0;
+  if (cudaGetDevice(&dev) != cudaSuccess || dev < 0 || dev >= 64) return 132;
+  if (cache[dev] == 0) {
+    int v = 0;
+    if (cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || v <= 0) v = 132;
+    cache[dev] = v;
+  }
+  return cache[dev];
+}
 
 // ---- scalar conversions -------------------------------------------------------------------
 template <typename T> __device__ __forceinline__ float to_f(T v);

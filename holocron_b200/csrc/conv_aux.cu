@@ -41,7 +41,7 @@ __global__ void pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* 
 }
 
 // Multi-tensor variant: one launch packs every filter of a network (table row = one filter, chunk = 4096 output
-// elements of one filter), instead of one ~5 us launch per layer and step.
+// elements of one filter), instead of one launch per layer and step.
 struct PackMeta {
   const float* w;
   __nv_bfloat16* wf;
@@ -60,7 +60,7 @@ __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackMeta*
   const size_t end = min(base + (size_t)kPackChunk, nf + nd);
   if (nf + nd < 0x7fffffffu) {
     // every filter of a real network: 32-bit index arithmetic (the four runtime div/mod pairs per element dominated this kernel
-    // when done on size_t: 277 us for RepVGG-A0's 18 M packed elements, 0.2 GB of DRAM traffic - ALU bound, not memory bound)
+    // when done on size_t: ALU bound, not memory bound, for RepVGG-A0's 18 M packed elements)
     const unsigned nf32 = (unsigned)nf, end32 = (unsigned)end;
     const unsigned R = m.R, S = m.S, CinP = m.CinP, CoutP = m.CoutP, Cin = m.Cin, Cout = m.Cout;
     for (unsigned i = (unsigned)base + threadIdx.x; i < end32; i += 256) {
@@ -178,8 +178,8 @@ __global__ void nchw_to_nhwc_pad_kernel(const T* __restrict__ x, __nv_bfloat16* 
 }
 
 // Explicit im2col for convolutions with a handful of input channels (network stems, Cin <= 4): the implicit-GEMM
-// kernels would pad such a Cin to a 64-channel K block (>= 87% of the tensor-core and TMA work wasted, measured 1.3 ms for
-// RepVGG's 3->48 stem at batch 256). Here the R*S*C patch of every output pixel is written once as one dense row of
+// kernels would pad such a Cin to a 64-channel K block (>= 87% of the tensor-core and TMA work wasted on
+// RepVGG's 3->48 stem). Here the R*S*C patch of every output pixel is written once as one dense row of
 // Kp = 32 (or 64) bf16 values, k = (r*S + s)*C + c, and the convolution becomes a plain [M, Kp] x [Kp, Cout] GEMM on the
 // tensor-core kernel (forward) / its wgrad twin (backward). x: NCHW of any float dtype.
 template <typename T>

@@ -1,25 +1,22 @@
 // Implicit-GEMM 2-D convolution (forward; also the data-gradient pass with transformed weights) on
-// the sm_100a tensor cores: NHWC bf16 activations, KRSC bf16 filters, fp32 accumulation in TMEM.
+// the sm_90a tensor cores: NHWC bf16 activations, KRSC bf16 filters, fp32 accumulation in registers (wgmma).
 //
 // GEMM view:  Y[m, co] = sum_{r,s,ci} X[pix(m) + (r,s), ci] * Wt[co, r, s, ci]
-//   M = N*Ho*Wo output pixels (tile 128 = the 128 TMEM lanes), N = Cout (tile BN <= 256 TMEM columns),
+//   M = N*Ho*Wo output pixels (tile 128 = two 64-row warpgroup MMAs), N = Cout (tile BN <= 128),
 //   K = R*S*Cin walked tap by tap in 64-channel blocks.
 // Replaces the cuDNN calls behind nn.Conv2d in holocron.models.utils.conv_sequence
 // (reference holocron/models/utils.py:28-86) and RepBlock (models/classification/repvgg.py:55-73).
 //
-// Pipeline (one persistent CTA per SM, 320 threads):
-//   warp 0      TMA producer: im2col-mode loads of the activation tile (hardware handles padding, stride,
-//               row/image wrap; out-of-range channels are zero-filled) + tiled loads of the filter slab,
-//               both landing 128B-swizzled in a multi-stage smem ring (mbarrier complete_tx).
-//   warp 1      MMA issuer: one elected thread issues tcgen05.mma (M=128, N=BN, K=16) x4 per stage,
-//               tcgen05.commit releases the smem stage / publishes the accumulator.
-//   warps 2-9   two epilogue warpgroups taking alternate tiles (one per TMEM accumulator): tcgen05.ld the accumulator
-//               (double-buffered in TMEM, so the epilogue of tile i
-//               overlaps the MMAs of tile i+1), fuse bias / activation, stage the bf16 tile in shared memory
-//               (bank-conflict-free padded rows) and write it out with fully coalesced 128-bit stores
-//               (+ residual add in that pass). The first version stored one 96-byte row per thread straight
-//               from registers: 32 L1TEX wavefronts per store instruction made L1TEX the busiest unit
-//               (profiles/r01_conv_fprop_ncu_full.md).
+// Pipeline (one persistent CTA per SM, 384 threads):
+//   warpgroup 0   TMA producer (one thread): im2col-mode loads of the activation tile (hardware handles padding,
+//                 stride, row/image wrap; out-of-range channels are zero-filled) + tiled loads of the filter slab,
+//                 both landing 128B-swizzled in a multi-stage smem ring (mbarrier complete_tx).
+//   warpgroups 1-2  consumers: each issues wgmma m64nBNk16 for its 64 rows of the 128-row tile (4 per 64-channel
+//                 block), keeps one block in flight while it releases the previous stage, then runs the epilogue
+//                 of the tile: bias / activation / patch normalisation from the accumulator registers into a bf16
+//                 staging tile in shared memory (padded rows, conflict-free), written out with fully coalesced
+//                 128-bit stores (+ residual add in that pass). The producer meanwhile fills the ring for the
+//                 next tile.
 #include <stdlib.h>
 #include "common.cuh"
 #include "tc_common.cuh"
@@ -32,9 +29,10 @@ using namespace tc;
 
 constexpr int kBM = 128;          // output pixels per tile
 constexpr int kBK = 64;           // channels per K block (one 128-byte swizzle row)
-constexpr int kUmmaK = 16;        // K per tcgen05.mma for 16-bit inputs
-constexpr int kThreads = 320;     // producer warp, MMA warp, 2 x 4 epilogue warps (alternate tiles)
-constexpr int kTmemCols = 512;    // two accumulators of up to 256 columns
+constexpr int kMmaK = 16;         // K per wgmma for 16-bit inputs
+constexpr int kThreads = 384;     // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumers = 256;
+constexpr int kMaxCols = 128;     // accumulator columns per thread set (both outputs in dual mode)
 constexpr int kABytes = kBM * kBK * 2;  // 16 KiB
 
 struct FpropParams {
@@ -46,7 +44,7 @@ struct FpropParams {
   int BN;           // Cout tile
   int num_m_tiles, num_n_tiles;
   int cblocks;      // ceil(Cin / 64)
-  int ksteps_last;  // 16-channel UMMA steps of the last channel block (Cin = 48 -> 3 instead of 4 zero-padded ones)
+  int ksteps_last;  // 16-channel MMA steps of the last channel block (Cin = 48 -> 3 instead of 4 zero-padded ones)
   // extra K blocks issued after the R*S*cblocks main ones:
   //   e_mode 1: a second source xe [M, Ce] (rows = the output rows) with filter we [Cout,1,1,Ce] accumulated into the
   //             SAME accumulator (K extension: dX = dgrad3x3(dY3) + dgrad1x1(dY1) in one kernel);
@@ -56,14 +54,14 @@ struct FpropParams {
   int nout;         // 1, or 2 in dual mode
   int stages;
   int b_stage_bytes;  // BN*128 rounded up to 1024
-  int out_pitch;      // bytes per row of the smem output staging tile (BN*2 + 16)
+  int out_pitch;      // bytes per row of the smem output staging tile (min(BN, 64)*2 + 16)
   int a_mode;         // 0: plain 2-D [M, C] matrix (1x1 s1 p0), 1: im2col
   int act;            // 0 none, 1 relu
   __nv_bfloat16* y;
   __nv_bfloat16* y2;              // dual mode: second output (same addressing as y)
   // optional per-channel statistics of the bf16 OUTPUT (what the BatchNorm that follows normalises): float
-  // [slots][Cout][2] = (sum, sum of squares) partials, slot = (blockIdx.x / num_n_tiles) * 2 + epilogue group; every
-  // (slot, channel) is written exactly once and the consumer adds the slots in a fixed order (deterministic)
+  // [slots][Cout][2] = (sum, sum of squares) partials, slot = (blockIdx.x / num_n_tiles) * 2 + consumer warpgroup;
+  // every (slot, channel) is written exactly once and the consumer adds the slots in a fixed order (deterministic)
   float* stats;
   float* stats2;
   const float* bias;              // [Cout] or null
@@ -78,24 +76,22 @@ struct FpropParams {
   int scatter, OH, OW, o_step, o_a, o_b;
 };
 
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
 // kStats: the epilogue also accumulates the output-column statistics (separate instantiation: the plain kernel carries
-// neither the 16 accumulator registers nor the extra shared-memory pass in its instruction stream)
+// neither the extra registers nor the extra shared-memory pass in its instruction stream)
 template <bool kStats>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2, const FpropParams p) {
   extern __shared__ __align__(1024) uint8_t smem_raw[];
-  // carve: [stages][A | B] then barriers
+  // carve: [stages][A | B], staging tile + row offset table, then barriers
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int stage_bytes = kABytes + p.b_stage_bytes;
-  // per epilogue group: [128][out_pitch] output staging tile + [128] row offset table
-  uint8_t* sout0 = smem + (size_t)p.stages * stage_bytes;
+  uint8_t* sout = smem + (size_t)p.stages * stage_bytes;
   const size_t sout_bytes = (((size_t)kBM * p.out_pitch + 15) & ~(size_t)15) + kBM * sizeof(long long);
-  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sout0 + 2 * sout_bytes);
+  uint64_t* full_bar = reinterpret_cast<uint64_t*>(sout + sout_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* tmem_full = empty_bar + p.stages;   // [2]
-  uint64_t* tmem_empty = tmem_full + 2;         // [2]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(tmem_empty + 2);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -104,15 +100,10 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     prefetch_tmap(&tmA);
     prefetch_tmap(&tmB);
     if (p.e_mode) { prefetch_tmap(&tmB2); if (p.e_mode == 1) prefetch_tmap(&tmA2); }
-    for (int i = 0; i < p.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    for (int i = 0; i < 2; ++i) { mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 4); }
+    for (int i = 0; i < p.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 32); }
     fence_barrier_init();
   }
-  if (warp == 1) { tmem_alloc(tmem_ptr, kTmemCols); }
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   // Tile walk: CTA b always works on Cout tile  b % num_n_tiles  (gridDim.x is a multiple of num_n_tiles) and takes the
   // pixel tiles  b / num_n_tiles + k * (gridDim.x / num_n_tiles): CTAs that run side by side share their A tile in L2, and
@@ -122,9 +113,9 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int kblocks = p.R * p.S * p.cblocks;
   const uint32_t tx_bytes = kABytes + p.BN * 128;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================= TMA producer =================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
         const int m0 = m_tile * kBM;
@@ -163,254 +154,232 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(kBM, p.BN, 0, 0);
-      const uint32_t dhi = desc_hi(1024, kLayoutSW128);
-      const uint32_t a_lo0 = desc_lo(smem_u32(smem), 16);
-      const uint32_t stage_lo = (uint32_t)stage_bytes >> 4;
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step, ++it) {
-        const int acc = it & 1;
-        const uint32_t acc_phase = (it >> 1) & 1;
-        mbar_wait(&tmem_empty[acc], acc_phase ^ 1);
-        tc_fence_after();
-        const uint32_t d_tmem = tmem_base + acc * 256;
-        int cb = 0;
-        for (int kb = 0; kb < kblocks; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = a_lo0 + (uint32_t)stage * stage_lo;
-          const uint32_t b_lo = a_lo + (kABytes >> 4);
-          const bool last_cb = ++cb == p.cblocks;
-          const int ks = last_cb ? p.ksteps_last : kBK / kUmmaK;
-          if (last_cb) cb = 0;
-          // fully unrolled with a predicate per step: the single issuing thread must not pay loop overhead per MMA (a
-          // runtime-trip-count loop here cost ~20 % on every layer: the kernel is issue-rate sensitive)
+    return;
+  }
+
+  // ================= consumers: MMA + epilogue =================
+  const int et = threadIdx.x - 128;        // 0..255
+  const int wg = et >> 7;                  // rows [64*wg, 64*wg + 64) of every tile
+  const int wet = et & 127;
+  const int frow = 64 * wg + frag_row(wet);   // this thread's first accumulator row (second: +8)
+  const int fcol = frag_col(wet);
+  const uint32_t dhi = desc_hi(1024);
+  const uint32_t a_lo0 = desc_lo(smem_u32(smem), 16) + (uint32_t)wg * ((64 * 128) >> 4);
+  const uint32_t stage_lo = (uint32_t)stage_bytes >> 4;
+  long long* row_off = reinterpret_cast<long long*>(sout + (((size_t)kBM * p.out_pitch + 15) & ~(size_t)15));
+  // column groups of <= 64 columns go through the fixed-size staging tile: gpo groups per output, nout outputs
+  const int gpo = (p.BN + 63) >> 6;
+  const int ngroups = p.nout * gpo;
+  // column statistics: this thread's running (sum0, sum1, sumsq0, sumsq1) of one column PAIR of each group over a fixed
+  // subset of its warpgroup's 64 tile rows, kept in registers across all tiles of the CTA
+  float st[4][4];
 #pragma unroll
-          for (int k = 0; k < kBK / kUmmaK; ++k)
-            if (k < ks) umma_f16_lh(d_tmem, a_lo + 2 * k, dhi, b_lo + 2 * k, dhi, idesc, (uint32_t)(kb | k));
-          umma_commit(&empty_bar[stage]);  // frees this smem stage once the MMAs have read it
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
+  for (int gi = 0; gi < 4; ++gi) { st[gi][0] = st[gi][1] = st[gi][2] = st[gi][3] = 0.f; }
+  const int col_base = n_tile * p.BN;
+  const int ncols_valid = min(p.BN, p.Cout - col_base);          // multiple of 16
+  float acc[kMaxCols / 2];
+  int stage = 0; uint32_t phase = 0;
+
+  for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
+    // ---- main loop: one K block in flight while the previous stage is handed back to the producer ----
+    int prev = -1, cb = 0;
+    const int nkb = kblocks + p.e_cblocks;
+    for (int kb = 0; kb < nkb; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      const uint32_t a_lo = a_lo0 + (uint32_t)stage * stage_lo;
+      const uint32_t b_lo = desc_lo(smem_u32(smem), 16) + (uint32_t)stage * stage_lo + (kABytes >> 4);
+      wgmma_fence();
+      if (kb < kblocks) {
+        const bool last_cb = ++cb == p.cblocks;
+        const int ks = last_cb ? p.ksteps_last : kBK / kMmaK;
+        if (last_cb) cb = 0;
+#pragma unroll
+        for (int k = 0; k < kBK / kMmaK; ++k)
+          if (k < ks)
+            wgmma_bf16<0, 0>(p.BN, acc, make_desc(a_lo + 2 * k, dhi), make_desc(b_lo + 2 * k, dhi), (uint32_t)(kb | k));
+      } else {
         // extra K blocks: same accumulator (e_mode 1) or the second accumulator, BN columns further (e_mode 2)
-        const uint32_t d_extra = d_tmem + (p.e_mode == 2 ? (uint32_t)p.BN : 0u);
-        for (int ecb = 0; ecb < p.e_cblocks; ++ecb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          const uint32_t a_lo = a_lo0 + (uint32_t)stage * stage_lo;
-          const uint32_t b_lo = a_lo + (kABytes >> 4);
-          const int ks = (ecb == p.e_cblocks - 1) ? p.e_ksteps_last : kBK / kUmmaK;
-          const uint32_t acc_first = p.e_mode == 2 ? (uint32_t)ecb : 1u;
+        const int ecb = kb - kblocks;
+        const int ks = (ecb == p.e_cblocks - 1) ? p.e_ksteps_last : kBK / kMmaK;
 #pragma unroll
-          for (int k = 0; k < kBK / kUmmaK; ++k)
-            if (k < ks) umma_f16_lh(d_extra, a_lo + 2 * k, dhi, b_lo + 2 * k, dhi, idesc, acc_first | (uint32_t)k);
-          umma_commit(&empty_bar[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+        for (int k = 0; k < kBK / kMmaK; ++k) {
+          if (k < ks) {
+            const uint64_t ad = make_desc(a_lo + 2 * k, dhi), bd = make_desc(b_lo + 2 * k, dhi);
+            if (p.e_mode == 2) {
+              const uint32_t sc = (uint32_t)(ecb | k);
+              // the second accumulator starts at column BN: a constant offset inside every case
+              switch (p.BN) {
+                case 16: wgmma_n16<0, 0>(acc + 8, ad, bd, sc); break;
+                case 32: wgmma_n32<0, 0>(acc + 16, ad, bd, sc); break;
+                case 48: wgmma_n48<0, 0>(acc + 24, ad, bd, sc); break;
+                case 64: wgmma_n64<0, 0>(acc + 32, ad, bd, sc); break;
+                default: break;
+              }
+            } else {
+              wgmma_bf16<0, 0>(p.BN, acc, ad, bd, 1u);
+            }
+          }
         }
-        umma_commit(&tmem_full[acc]);      // accumulator(s) complete
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);   // the MMAs that read stage `prev` are done
+      prev = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    // ---- epilogue ----
+    const int rows_valid = min(kBM, p.m_total - m_tile * kBM);
+    float nm[2] = {0.f, 0.f}, nr[2] = {1.f, 1.f};
+    if (p.norm_mean) {
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        const int m_row = m_tile * kBM + frow + 8 * h;
+        if (m_row < p.m_total) { nm[h] = __ldg(p.norm_mean + m_row); nr[h] = __ldg(p.norm_rstd + m_row); }
       }
     }
-  } else {
-    // ================= epilogue (warps 2..5 take the even tiles of this CTA, warps 6..9 the odd ones) =================
-    // One tile's epilogue is a chain of latencies (tcgen05.ld -> convert -> st.shared -> barrier -> ld.shared ->
-    // st.global); two groups on the two TMEM accumulators overlap two of those chains.
-    const int quarter = warp & 3;  // TMEM lane quarter this warp may access
-    const int group = (warp - 2) >> 2;
-    const int et = (threadIdx.x - 64) & 127;   // 0..127 inside the group
-    uint8_t* sout = sout0 + (size_t)group * sout_bytes;
-    long long* row_off = reinterpret_cast<long long*>(sout + (((size_t)kBM * p.out_pitch + 15) & ~(size_t)15));
-    // column groups of <= 64 accumulator columns go through a small fixed-size staging tile (keeps the smem for pipeline
-    // stages whatever BN is): gpo groups per output, nout outputs, at most 4 groups in total (host-checked)
-    const int gpo = (p.BN + 63) >> 6;
-    const int ngroups = p.nout * gpo;
-    // column statistics: this thread's running (sum0, sum1, sumsq0, sumsq1) of one column PAIR of each group over a fixed
-    // subset of the tile rows (rows rg, rg + rgs, ...), kept in registers across all tiles of the CTA
-    float st[4][4];
-#pragma unroll
-    for (int gi = 0; gi < 4; ++gi) { st[gi][0] = st[gi][1] = st[gi][2] = st[gi][3] = 0.f; }
-    const int col_base = n_tile * p.BN;
-    const int ncols_valid = min(p.BN, p.Cout - col_base);          // multiple of 16
-    for (int m_tile = m_first + group * m_step, it = group; m_tile < p.num_m_tiles; m_tile += 2 * m_step, it += 2) {
-      const int acc = it & 1;
-      const uint32_t acc_phase = (it >> 1) & 1;
-      mbar_wait(&tmem_full[acc], acc_phase);
-      tc_fence_after();
-      const int row_in_tile = quarter * 32 + lane;
-      const uint32_t taddr0 = tmem_base + acc * 256 + ((uint32_t)(quarter * 32) << 16);
-      const int rows_valid = min(kBM, p.m_total - m_tile * kBM);
-      uint8_t* srow = sout + (size_t)row_in_tile * p.out_pitch;
-      float nm = 0.f, nr = 1.f;
-      if (p.norm_mean) {
-        const int m_row = m_tile * kBM + row_in_tile;
-        if (m_row < p.m_total) { nm = __ldg(p.norm_mean + m_row); nr = __ldg(p.norm_rstd + m_row); }
+#pragma unroll 1
+    for (int gi = 0; gi < ngroups; ++gi) {
+      const int o = gi >= gpo ? 1 : 0;                 // output index (dual mode: 0 = RxS conv, 1 = 1x1 conv)
+      const int g0 = (gi - o * gpo) * 64;
+      const int gw = min(64, p.BN - g0);
+      __nv_bfloat16* yo = o ? p.y2 : p.y;
+      const bool first = o == 0;
+      const int cs0 = o * p.BN + g0;                   // first accumulator column of this group
+      consumer_sync();   // staging tile free
+      if (gi == 0 && et < kBM) {
+        // element offset of each output row of the tile (read by every thread in the copy-out below)
+        const long long m = (long long)m_tile * kBM + et;
+        if (!p.scatter) {
+          row_off[et] = m * p.Cout;
+        } else {
+          const int j = (int)(m % p.Wo), i = (int)((m / p.Wo) % p.Ho), n = (int)(m / ((long long)p.Wo * p.Ho));
+          row_off[et] = (((long long)n * p.OH + (long long)i * p.o_step + p.o_a) * p.OW + (long long)j * p.o_step + p.o_b) * p.Cout;
+        }
       }
 #pragma unroll
-      for (int gi = 0; gi < 4; ++gi) {
-        if (gi >= ngroups) break;
-        const int o = gi >= gpo ? 1 : 0;                 // output index (dual mode: 0 = RxS conv, 1 = 1x1 conv)
-        const int g0 = (gi - o * gpo) * 64;
-        const int gw = min(64, p.BN - g0);
-        const uint32_t taddr = taddr0 + (uint32_t)(o * p.BN);
-        __nv_bfloat16* yo = o ? p.y2 : p.y;
-        const bool first = o == 0;
-        if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");   // staging tile free
-        else asm volatile("bar.sync 2, 128;" ::: "memory");
-        if (gi == 0) {
-          // element offset of this thread's output row (read by every thread in the copy-out below)
-          const long long m = (long long)m_tile * kBM + et;
-          if (!p.scatter) {
-            row_off[et] = m * p.Cout;
-          } else {
-            const int j = (int)(m % p.Wo), i = (int)((m / p.Wo) % p.Ho), n = (int)(m / ((long long)p.Wo * p.Ho));
-            row_off[et] = (((long long)n * p.OH + (long long)i * p.o_step + p.o_a) * p.OW + (long long)j * p.o_step + p.o_b) * p.Cout;
-          }
-        }
-        for (int c = 0; c < gw; c += 32) {
-          uint32_t v[32];
-          const bool two = (c + 16) < gw;
-          tmem_ld_x16(taddr + g0 + c, v);
-          if (two) tmem_ld_x16(taddr + g0 + c + 16, v + 16);
-          tmem_ld_wait();
+      for (int j = 0; j < kMaxCols / 8; ++j) {
+        const int cs = 8 * j + fcol;                   // accumulator column of registers 4j .. 4j+3
+        if (cs >= cs0 && cs < cs0 + gw) {
+          const int cl = cs - cs0;                     // column inside the staged group
+          const int col = col_base + g0 + cl;
+          const bool ok = col < p.Cout;
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (h == 0 || two) {
-              float f[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[h * 16 + j]);
-              const int col = col_base + g0 + c + h * 16;
-              if (first && p.norm_mean && col < p.Cout) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = nr * (f[j] - nm * __ldg(p.norm_wsum + col + j));
-              }
-              if (first && p.bias && col < p.Cout) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] += __ldg(p.bias + col + j);
-              }
-              if (first && p.act == 1 && !p.residual) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = hb::relu_nan(f[j]);
-              }
-              uint4 ov[2];
-              __nv_bfloat162* ob = reinterpret_cast<__nv_bfloat162*>(ov);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) ob[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-              uint4* sp = reinterpret_cast<uint4*>(srow + (c + h * 16) * 2);
-              sp[0] = ov[0];
-              sp[1] = ov[1];
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+            if (first && p.norm_mean && ok) {
+              f0 = nr[h] * (f0 - nm[h] * __ldg(p.norm_wsum + col));
+              f1 = nr[h] * (f1 - nm[h] * __ldg(p.norm_wsum + col + 1));
             }
+            if (first && p.bias && ok) { f0 += __ldg(p.bias + col); f1 += __ldg(p.bias + col + 1); }
+            if (first && p.act == 1 && !p.residual) { f0 = hb::relu_nan(f0); f1 = hb::relu_nan(f1); }
+            *reinterpret_cast<__nv_bfloat162*>(sout + (size_t)(frow + 8 * h) * p.out_pitch + cl * 2) =
+                __floats2bfloat162_rn(f0, f1);
           }
         }
-        if (gi == ngroups - 1) {   // last TMEM read of this accumulator set: hand it back to the MMA warp
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[acc]);
+      }
+      consumer_sync();   // staged group visible to both warpgroups
+      const int chunks_per_row = gw / 8;
+      const int total_chunks = rows_valid * chunks_per_row;
+      int r = et / chunks_per_row, c8 = et - r * chunks_per_row;
+      const int dr = kConsumers / chunks_per_row, dc = kConsumers - dr * chunks_per_row;
+      const __nv_bfloat16* resid = first ? p.residual : nullptr;
+      if (!resid) {
+        for (int ch = et; ch < total_chunks; ch += kConsumers) {
+          if (g0 + c8 * 8 < ncols_valid) {
+            const uint4 val = *reinterpret_cast<const uint4*>(sout + (size_t)r * p.out_pitch + c8 * 16);
+            *reinterpret_cast<uint4*>(yo + (size_t)row_off[r] + col_base + g0 + c8 * 8) = val;
+          }
+          r += dr; c8 += dc;
+          if (c8 >= chunks_per_row) { c8 -= chunks_per_row; ++r; }
         }
-        if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");   // staged group visible to the whole group
-        else asm volatile("bar.sync 2, 128;" ::: "memory");
-        const int chunks_per_row = gw / 8;
-        const int total_chunks = rows_valid * chunks_per_row;
-        int r = et / chunks_per_row, c8 = et - r * chunks_per_row;
-        const int dr = 128 / chunks_per_row, dc = 128 - dr * chunks_per_row;
-        const __nv_bfloat16* resid = first ? p.residual : nullptr;
-        if (!resid) {
-          for (int ch = et; ch < total_chunks; ch += 128) {
-            if (g0 + c8 * 8 < ncols_valid) {
-              const uint4 val = *reinterpret_cast<const uint4*>(sout + (size_t)r * p.out_pitch + c8 * 16);
-              *reinterpret_cast<uint4*>(yo + (size_t)row_off[r] + col_base + g0 + c8 * 8) = val;
-            }
+      } else {
+        // residual add: the global loads of 4 trips are issued before the first one is consumed (one dependent
+        // global load per trip made this pass latency-bound)
+        for (int ch = et; ch < total_chunks; ch += 4 * kConsumers) {
+          size_t off[4];
+          int sidx[4];
+          uint4 rv[4];
+          bool ok[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u) {
+            ok[u] = (ch + u * kConsumers < total_chunks) && (g0 + c8 * 8 < ncols_valid);
+            sidx[u] = r * p.out_pitch + c8 * 16;
+            off[u] = ok[u] ? (size_t)row_off[r] + col_base + g0 + c8 * 8 : 0;
+            if (ok[u]) rv[u] = *reinterpret_cast<const uint4*>(resid + off[u]);
             r += dr; c8 += dc;
             if (c8 >= chunks_per_row) { c8 -= chunks_per_row; ++r; }
           }
-        } else {
-          // residual add: the global loads of 4 trips are issued before the first one is consumed (one dependent
-          // global load per trip made this pass latency-bound: +100 % on the 1x1 data-gradient launches)
-          for (int ch = et; ch < total_chunks; ch += 4 * 128) {
-            size_t off[4];
-            int sidx[4];
-            uint4 rv[4];
-            bool ok[4];
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              ok[u] = (ch + u * 128 < total_chunks) && (g0 + c8 * 8 < ncols_valid);
-              sidx[u] = r * p.out_pitch + c8 * 16;
-              off[u] = ok[u] ? (size_t)row_off[r] + col_base + g0 + c8 * 8 : 0;
-              if (ok[u]) rv[u] = *reinterpret_cast<const uint4*>(resid + off[u]);
-              r += dr; c8 += dc;
-              if (c8 >= chunks_per_row) { c8 -= chunks_per_row; ++r; }
-            }
+          for (int u = 0; u < 4; ++u) {
+            if (!ok[u]) continue;
+            uint4 val = *reinterpret_cast<const uint4*>(sout + sidx[u]);
+            __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(&val);
+            const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&rv[u]);
 #pragma unroll
-            for (int u = 0; u < 4; ++u) {
-              if (!ok[u]) continue;
-              uint4 val = *reinterpret_cast<const uint4*>(sout + sidx[u]);
-              __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(&val);
-              const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&rv[u]);
-#pragma unroll
-              for (int j = 0; j < 4; ++j) {
-                float2 fa = __bfloat1622float2(a[j]), fb = __bfloat1622float2(b[j]);
-                fa.x += fb.x; fa.y += fb.y;
-                if (p.act == 1) { fa.x = hb::relu_nan(fa.x); fa.y = hb::relu_nan(fa.y); }
-                a[j] = __floats2bfloat162_rn(fa.x, fa.y);
-              }
-              *reinterpret_cast<uint4*>(yo + off[u]) = val;
+            for (int jj = 0; jj < 4; ++jj) {
+              float2 fa = __bfloat1622float2(a[jj]), fb = __bfloat1622float2(b[jj]);
+              fa.x += fb.x; fa.y += fb.y;
+              if (p.act == 1) { fa.x = hb::relu_nan(fa.x); fa.y = hb::relu_nan(fa.y); }
+              a[jj] = __floats2bfloat162_rn(fa.x, fa.y);
             }
-          }
-        }
-        if (kStats && (o ? (p.stats2 != nullptr) : (p.stats != nullptr))) {
-          // per-channel sum / sum of squares of the staged (bf16-rounded) tile: thread = (column pair, row subset)
-          const int npairs = gw >> 1, rgs = 128 / npairs;
-          const int rg = et / npairs, pr = et - rg * npairs;
-          if (rg < rgs && g0 + pr * 2 < ncols_valid) {
-            const uint8_t* sp = sout + pr * 4;
-            float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-            for (int rr = rg; rr < rows_valid; rr += rgs) {
-              const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(sp + (size_t)rr * p.out_pitch));
-              s0 += f.x; s1 += f.y; q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-            }
-            st[gi][0] += s0; st[gi][1] += s1; st[gi][2] += q0; st[gi][3] += q1;
+            *reinterpret_cast<uint4*>(yo + off[u]) = val;
           }
         }
       }
-    }
-    // ---- statistics: fold the row subsets in a fixed order and write this (CTA, group)'s partial (every slot is written,
-    // zeros included, so the consumer can add all slots without a memset)
-    if (kStats && (p.stats || p.stats2)) {
-      const int slot = (blockIdx.x / p.num_n_tiles) * 2 + group;
-#pragma unroll
-      for (int gi = 0; gi < 4; ++gi) {
-        if (gi >= ngroups) break;
-        const int o = gi >= gpo ? 1 : 0;
-        float* so = o ? p.stats2 : p.stats;
-        if (!so) continue;
-        const int g0 = (gi - o * gpo) * 64;
-        const int gw = min(64, p.BN - g0);
+      if (kStats && (o ? (p.stats2 != nullptr) : (p.stats != nullptr))) {
+        // per-channel sum / sum of squares of the staged (bf16-rounded) tile: thread = (column pair, row subset of its
+        // warpgroup's 64 rows)
         const int npairs = gw >> 1, rgs = 128 / npairs;
-        if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-        else asm volatile("bar.sync 2, 128;" ::: "memory");
-        float4* scratch = reinterpret_cast<float4*>(sout);           // [128] float4, 2 KB <= staging tile
-        scratch[et] = make_float4(st[gi][0], st[gi][1], st[gi][2], st[gi][3]);
-        if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-        else asm volatile("bar.sync 2, 128;" ::: "memory");
-        if (et < gw && g0 + et < ncols_valid) {
-          const int pr = et >> 1, hi = et & 1;
-          float sv = 0.f, qv = 0.f;
-          for (int rg = 0; rg < rgs; ++rg) {
-            const float4 v = scratch[rg * npairs + pr];
-            sv += hi ? v.y : v.x;
-            qv += hi ? v.w : v.z;
+        const int rg = wet / npairs, pr = wet - rg * npairs;
+        const int row_end = min(64 * wg + 64, rows_valid);
+        if (rg < rgs && g0 + pr * 2 < ncols_valid) {
+          const uint8_t* sp = sout + pr * 4;
+          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
+          for (int rr = 64 * wg + rg; rr < row_end; rr += rgs) {
+            const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(sp + (size_t)rr * p.out_pitch));
+            s0 += f.x; s1 += f.y; q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
           }
-          float2* dst = reinterpret_cast<float2*>(so + ((size_t)slot * p.Cout + col_base + g0 + et) * 2);
-          *dst = make_float2(sv, qv);
+#pragma unroll
+          for (int g = 0; g < 4; ++g)
+            if (g == gi) { st[g][0] += s0; st[g][1] += s1; st[g][2] += q0; st[g][3] += q1; }
         }
       }
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, kTmemCols); }
+  // ---- statistics: fold the row subsets in a fixed order and write this (CTA, warpgroup)'s partial (every slot is
+  // written, zeros included, so the consumer can add all slots without a memset)
+  if (kStats && (p.stats || p.stats2)) {
+    const int slot = (blockIdx.x / p.num_n_tiles) * 2 + wg;
+#pragma unroll
+    for (int gi = 0; gi < 4; ++gi) {
+      if (gi >= ngroups) break;
+      const int o = gi >= gpo ? 1 : 0;
+      float* so = o ? p.stats2 : p.stats;
+      if (!so) continue;
+      const int g0 = (gi - o * gpo) * 64;
+      const int gw = min(64, p.BN - g0);
+      const int npairs = gw >> 1, rgs = 128 / npairs;
+      consumer_sync();
+      float4* scratch = reinterpret_cast<float4*>(sout) + wg * 128;   // [2][128] float4, 4 KB <= staging tile
+      scratch[wet] = make_float4(st[gi][0], st[gi][1], st[gi][2], st[gi][3]);
+      consumer_sync();
+      if (wet < gw && g0 + wet < ncols_valid) {
+        const int pr = wet >> 1, hi = wet & 1;
+        float sv = 0.f, qv = 0.f;
+        for (int rg = 0; rg < rgs; ++rg) {
+          const float4 v = scratch[rg * npairs + pr];
+          sv += hi ? v.y : v.x;
+          qv += hi ? v.w : v.z;
+        }
+        float2* dst = reinterpret_cast<float2*>(so + ((size_t)slot * p.Cout + col_base + g0 + wet) * 2);
+        *dst = make_float2(sv, qv);
+      }
+    }
+  }
 }
 
 }  // namespace
@@ -454,9 +423,9 @@ int fprop_launch(const FpropArgs& a) {
   p.stride = a.stride; p.pad_h = a.pad_h; p.pad_w = a.pad_w; p.dil = a.dil;
   p.R = R; p.S = S; p.Cin = Cin; p.Cout = Cout;
   p.scatter = a.scatter; p.OH = a.OH; p.OW = a.OW; p.o_step = a.o_step; p.o_a = a.o_a; p.o_b = a.o_b;
-  // Cout tile: whole Cout when it fits the accumulator columns (256, or 128 per output in dual mode), else the largest
-  // multiple of 16 below that limit that divides Cout (falls back to the limit with a masked tail).
-  const int bn_max = dual ? 128 : 256;
+  // Cout tile: whole Cout when it fits the accumulator registers (128 columns, or 64 per output in dual mode), else the
+  // largest multiple of 16 below that limit that divides Cout (falls back to the limit with a masked tail).
+  const int bn_max = dual ? 64 : 128;
   int BN = Cout;
   if (Cout > bn_max) {
     BN = bn_max;
@@ -467,14 +436,14 @@ int fprop_launch(const FpropArgs& a) {
   p.num_m_tiles = (p.m_total + kBM - 1) / kBM;
   p.num_n_tiles = (Cout + BN - 1) / BN;
   p.cblocks = (Cin + kBK - 1) / kBK;
-  p.ksteps_last = ((Cin - (p.cblocks - 1) * kBK) + kUmmaK - 1) / kUmmaK;
+  p.ksteps_last = ((Cin - (p.cblocks - 1) * kBK) + kMmaK - 1) / kMmaK;
   p.e_mode = kext ? 1 : (dual ? 2 : 0);
   const int ce = kext ? a.Ce : (dual ? Cin : 0);
   p.e_cblocks = (ce + kBK - 1) / kBK;
-  p.e_ksteps_last = p.e_cblocks ? ((ce - (p.e_cblocks - 1) * kBK) + kUmmaK - 1) / kUmmaK : 0;
+  p.e_ksteps_last = p.e_cblocks ? ((ce - (p.e_cblocks - 1) * kBK) + kMmaK - 1) / kMmaK : 0;
   p.b_stage_bytes = ((BN * 128) + 1023) & ~1023;
   p.out_pitch = (BN < 64 ? BN : 64) * 2 + 16;
-  const int out_bytes = (2 * (((kBM * p.out_pitch + 15) & ~15) + kBM * 8) + 1023) & ~1023;   // per group: staging + offsets
+  const int out_bytes = ((((kBM * p.out_pitch + 15) & ~15) + kBM * 8) + 1023) & ~1023;   // staging tile + row offsets
   const int stage_bytes = kABytes + p.b_stage_bytes;
   int stages = (204 * 1024 - out_bytes) / stage_bytes;
   if (stages > 8) stages = 8;
@@ -525,7 +494,7 @@ int fprop_launch(const FpropArgs& a) {
       return rc;
   }
 
-  const size_t smem_bytes = (size_t)stages * stage_bytes + out_bytes + (2 * stages + 4) * sizeof(uint64_t) + 16 + 1024;
+  const size_t smem_bytes = (size_t)stages * stage_bytes + out_bytes + 2 * stages * sizeof(uint64_t) + 1024;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(conv_fprop_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

@@ -1,24 +1,21 @@
 // "Row-window" 3x3 convolution (stride 1, pad 1) for the HBM/L2-bound layers (Cin <= 128, all filter taps resident
 // in shared memory): the input rows needed by a band of output rows are brought in ONCE per tile by a single tiled TMA
 // load (with a one-pixel zero halo supplied by TMA's out-of-bounds fill) and all nine filter taps are issued as
-// *shifted windows of that one buffer* - a tcgen05 shared-memory descriptor may start at any 128-byte row of a
-// 128B-swizzled TMA buffer because the swizzle is a function of the absolute shared-memory address
-// (probe: profiles/r01_umma_shifted_descriptor_probe.log).
+// *shifted windows of that one buffer* - a wgmma shared-memory descriptor may start at any 128-byte row of a
+// 128B-swizzled TMA buffer because the swizzle is a function of the absolute shared-memory address.
 //
-// Why: the first implicit-GEMM kernel (conv_fprop.cu) issues one im2col TMA load per tap, i.e. it reads every input
-// element 9x from L2; ncu showed the 48-channel 112^2 layer moving 8 TB/s out of L2 while DRAM sat at 11%
-// (profiles/r01_conv_fprop_ncu_full.md). Here a tile of TRO output rows loads TRO+2 input rows: 1.3-2x instead of 9x.
+// Why: the generic implicit-GEMM kernel (conv_fprop.cu) issues one im2col TMA load per tap, i.e. it reads every input
+// element 9x from L2. Here a tile of TRO output rows loads TRO+2 input rows: 1.3-2x instead of 9x.
 //
 // Geometry. Shared-memory row pitch Wp = W + 2 pixels (128 B each = one 64-channel block). A "sub-tile" is one
-// M = 128 MMA covering SR = floor(128 / Wp) output rows laid out with the SAME pitch Wp (so 2 junk columns per row);
-// for tap (r, s) its A operand is the buffer window starting at pixel row (sub*SR + r) * Wp + s. Junk accumulator rows
-// (q >= W, rows past the image) are skipped by the epilogue. The filter (all 9 taps x channel blocks) is loaded once
-// per CTA and stays resident.
+// M = 128 tile (two 64-row warpgroup MMAs) covering SR = floor(128 / Wp) output rows laid out with the SAME pitch Wp
+// (so 2 junk columns per row); for tap (r, s) its A operand is the buffer window starting at pixel row
+// (sub*SR + r) * Wp + s. Junk accumulator rows (q >= W, rows past the image) are skipped by the epilogue. The filter
+// (all 9 taps x channel blocks) is loaded once per CTA and stays resident.
 //
-// Same warp roles / double-buffered TMEM accumulators / smem-staged coalesced epilogue as conv_fprop.cu, with TWO
-// epilogue warpgroups (warps 2-5 and 6-9) that take alternate sub-tiles: one sub-tile's epilogue is a chain of
-// latencies (tcgen05.ld -> convert -> st.shared -> barrier -> ld.shared -> st.global, ~1.5 us) that four warps cannot
-// overlap with themselves, and on the 48..96-channel layers it - not the MMAs (0.7 us) - set the kernel time.
+// Warp roles: one TMA producer warpgroup and two consumer warpgroups (rows 0-63 and 64-127 of every sub-tile) that
+// issue the wgmma chain of a sub-tile and then run its epilogue (accumulator registers -> bf16 staging tile in shared
+// memory -> coalesced 128-bit stores); the producer meanwhile loads the next tile's rows into the other ring slot.
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "tmap.cuh"
@@ -27,21 +24,23 @@ namespace {
 
 using namespace tc;
 
-constexpr int kThreads = 320;      // TMA warp, MMA warp, 2 x 4 epilogue warps
-constexpr int kTmemCols = 512;
+constexpr int kThreads = 384;      // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumers = 256;
 
 struct RowsParams {
   int N, H, W, Cin, Cout;
   int Wp;        // smem row pitch in pixels (W + 2)
-  int SR;        // output rows per sub-tile (one M=128 MMA)
+  int SR;        // output rows per sub-tile (one M=128 tile)
   int NSUB;      // sub-tiles per tile
   int TRO;       // output rows per tile = SR * NSUB
   int CB;        // 64-channel blocks
-  int ksteps_last;  // UMMA k-steps (of 16 channels) in the last channel block
-  int BN;        // = Cout (multiple of 16, <= 256 / NSUB)
+  int ksteps_last;  // k-steps (of 16 channels) in the last channel block
+  int BN;        // = Cout (multiple of 16, <= 128)
   int tiles_per_img, num_tiles;
-  int stage_bytes;   // CB * (TRO+2) * Wp * 128, rounded to 1024
-  int cb_bytes;      // (TRO+2) * Wp * 128 rounded to 1024
+  int nstages;       // ring slots: 2, or 1 when two tiles' rows do not fit in shared memory
+  int stage_bytes;   // CB * (cb_bytes + nextra * ecb_bytes): the main rows and every extra source of one tile
+  int cb_bytes;      // bytes of one 64-channel block buffer of the main rows, rounded to 1024
+  int ecb_bytes;     // same for an extra source (no halo rows)
   int w_tap_bytes;   // BN * 128 rounded to 1024
   int out_pitch;
   int act;
@@ -52,6 +51,8 @@ struct RowsParams {
   float* stats;      // optional [2 * gridDim.x][Cout][2] (sum, sum of squares) partials of the bf16 output, see conv_fprop.cu
 };
 
+__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
+
 __global__ void __launch_bounds__(kThreads, 1)
 conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                  const __grid_constant__ CUtensorMap tmXe0, const __grid_constant__ CUtensorMap tmWe0,
@@ -59,37 +60,27 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint8_t* wsm = smem;                                          // [9 + nextra][CB][BN x 128 B]
-  uint8_t* stage0 = wsm + (size_t)(9 + p.nextra) * p.CB * p.w_tap_bytes;     // ring of 2 block buffers
-  uint8_t* sout0 = stage0 + (size_t)2 * p.stage_bytes;          // [2 groups][128][out_pitch]
+  uint8_t* stage0 = wsm + (size_t)(9 + p.nextra) * p.CB * p.w_tap_bytes;     // ring of nstages tile buffers
+  uint8_t* sout = stage0 + (size_t)p.nstages * p.stage_bytes;   // [128][out_pitch]
   const size_t sout_bytes = ((size_t)128 * p.out_pitch + 15) & ~size_t(15);
-  uint64_t* bars = reinterpret_cast<uint64_t*>(sout0 + 2 * sout_bytes);
+  uint64_t* bars = reinterpret_cast<uint64_t*>(sout + sout_bytes);
   uint64_t* full_bar = bars;        // [2]
   uint64_t* empty_bar = bars + 2;   // [2]
-  uint64_t* tmem_full = bars + 4;   // [2]
-  uint64_t* tmem_empty = bars + 6;  // [2]
-  uint64_t* w_bar = bars + 8;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 9);
+  uint64_t* w_bar = bars + 4;
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmX);
     prefetch_tmap(&tmW);
-    for (int i = 0; i < 2; ++i) {
-      mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1);
-      mbar_init(&tmem_full[i], 1); mbar_init(&tmem_empty[i], 8);
-    }
+    for (int i = 0; i < 2; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 32); }
     mbar_init(w_bar, 1);
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
-  if (warp == 0) {
+  if (warp < 4) {
     // ================= TMA producer =================
-    if (lane == 0) {
+    if (warp == 0 && lane == 0) {
       prefetch_tmap(&tmXe0); prefetch_tmap(&tmWe0); prefetch_tmap(&tmXe1); prefetch_tmap(&tmWe1);
       // resident filters: 9 taps x CB channel blocks (+ one 1x1 filter per extra source)
       mbar_arrive_expect_tx(w_bar, (uint32_t)((9 + p.nextra) * p.CB * p.BN * 128));
@@ -99,227 +90,180 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
       for (int e = 0; e < p.nextra; ++e)
         for (int cb = 0; cb < p.CB; ++cb)
           tma_load_3d(e == 0 ? &tmWe0 : &tmWe1, w_bar, wsm + (size_t)((9 + e) * p.CB + cb) * p.w_tap_bytes, cb * 64, 0, 0);
-      const uint32_t tx_main = (uint32_t)(p.CB * (p.TRO + 2) * p.Wp * 128);
-      const uint32_t tx_extra = (uint32_t)(p.CB * p.TRO * p.Wp * 128);
-      int blk = 0;   // running block counter: ring slot = blk & 1, phase = (blk >> 1) & 1
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x) {
+      const uint32_t tx = (uint32_t)(p.CB * ((p.TRO + 2) + p.nextra * p.TRO) * p.Wp * 128);
+      int it = 0;   // ring slot = it % nstages, phase = (it / nstages) & 1
+      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
         const int n = tile / p.tiles_per_img, p0 = (tile % p.tiles_per_img) * p.TRO;
-        for (int b = 0; b <= p.nextra; ++b, ++blk) {
-          const int st = blk & 1;
-          const uint32_t ph = (blk >> 1) & 1;
-          mbar_wait(&empty_bar[st], ph ^ 1);
-          mbar_arrive_expect_tx(&full_bar[st], b == 0 ? tx_main : tx_extra);
+        const int st = it % p.nstages;
+        mbar_wait(&empty_bar[st], ((it / p.nstages) & 1) ^ 1);
+        mbar_arrive_expect_tx(&full_bar[st], tx);
+        for (int b = 0; b <= p.nextra; ++b) {
           const CUtensorMap* tm = b == 0 ? &tmX : (b == 1 ? &tmXe0 : &tmXe1);
           const int h0 = b == 0 ? p0 - 1 : p0;   // the extra sources need no row halo (centre tap only)
           for (int cb = 0; cb < p.CB; ++cb) {
             // box (64 ch, Wp, rows, 1 image) at (c, w = -1, h0, n): halo and image borders = OOB zero fill
             asm volatile(
                 "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                ::"r"(smem_u32(stage0 + (size_t)st * p.stage_bytes + (size_t)cb * p.cb_bytes)),
+                ::"r"(smem_u32(stage0 + (size_t)st * p.stage_bytes + (size_t)p.CB * (b ? p.cb_bytes + (b - 1) * p.ecb_bytes : 0) +
+                               (size_t)cb * (b ? p.ecb_bytes : p.cb_bytes))),
                   "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(&full_bar[st])), "r"(cb * 64), "r"(-1), "r"(h0), "r"(n)
                 : "memory");
           }
         }
       }
     }
-  } else if (warp == 1) {
-    // ================= MMA issuer =================
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(128, p.BN, 0, 0);
-      const uint32_t dhi = desc_hi(1024, kLayoutSW128);
-      const uint32_t w_lo0 = desc_lo(smem_u32(wsm), 16);
-      const uint32_t w_tap_lo = (uint32_t)p.w_tap_bytes >> 4;
-      const uint32_t cb_lo = (uint32_t)p.cb_bytes >> 4;
-      mbar_wait(w_bar, 0);
-      int it = 0, blk = 0;
-      for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-        const int acc = it & 1;
-        mbar_wait(&tmem_empty[acc], ((it >> 1) & 1) ^ 1);   // accumulator set drained by the epilogue
-        for (int b = 0; b <= p.nextra; ++b, ++blk) {
-          const int st = blk & 1;
-          mbar_wait(&full_bar[st], (blk >> 1) & 1);         // block landed
-          tc_fence_after();
-          const uint32_t s_lo = desc_lo(smem_u32(stage0 + (size_t)st * p.stage_bytes), 16);
-          for (int sub = 0; sub < p.NSUB; ++sub) {
-            const uint32_t d_tmem = tmem_base + acc * 256 + sub * p.BN;
-            if (b == 0) {
-              uint32_t accum = 0;
+    return;
+  }
+
+  // ================= consumers =================
+  const int et = threadIdx.x - 128;          // 0..255
+  const int wg = et >> 7;                    // rows [64*wg, 64*wg + 64) of every sub-tile
+  const int frow = 64 * wg + frag_row(et & 127);
+  const int fcol = frag_col(et & 127);
+  const uint32_t dhi = desc_hi(1024);
+  const uint32_t w_lo0 = desc_lo(smem_u32(wsm), 16);
+  const uint32_t w_tap_lo = (uint32_t)p.w_tap_bytes >> 4;
+  const uint32_t cb_lo = (uint32_t)p.cb_bytes >> 4;
+  const uint32_t ecb_lo = (uint32_t)p.ecb_bytes >> 4;
+  const int chunks_per_row = p.BN / 8;
+  // column statistics: thread = (column pair pr, pixel subset rg) over the valid pixels of every sub-tile
+  const int npairs = p.BN >> 1, rgs = kConsumers / npairs;
+  const int st_rg = et / npairs, st_pr = et - st_rg * npairs;
+  const bool st_on = p.stats != nullptr && st_rg < rgs;
+  float st0 = 0.f, st1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+  float acc[64];
+  mbar_wait(w_bar, 0);
+  int it = 0;
+  for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
+    const int st = it % p.nstages;
+    const int n = tile / p.tiles_per_img, p0 = (tile % p.tiles_per_img) * p.TRO;
+    mbar_wait(&full_bar[st], (it / p.nstages) & 1);
+    // window start of this warpgroup's 64 rows: 64 pixel rows x 128 B further
+    const uint32_t s_lo = desc_lo(smem_u32(stage0 + (size_t)st * p.stage_bytes), 16) + (uint32_t)wg * ((64 * 128) >> 4);
+    for (int sub = 0; sub < p.NSUB; ++sub) {
+      wgmma_fence();
+      uint32_t accum = 0;
+#pragma unroll 1
+      for (int tap = 0; tap < 9; ++tap) {
+        const int r = tap / 3, s = tap % 3;
+        // 128-byte pixel rows: (row index) * 128 B >> 4 = row index * 8
+        uint32_t a_lo = s_lo + (uint32_t)(((sub * p.SR + r) * p.Wp + s) * 8);
+        uint32_t b_lo = w_lo0 + (uint32_t)(tap * p.CB) * w_tap_lo;
+        for (int cb = 0; cb < p.CB; ++cb) {
+          const int ks = (cb == p.CB - 1) ? p.ksteps_last : 4;
 #pragma unroll
-              for (int tap = 0; tap < 9; ++tap) {
-                const int r = tap / 3, s = tap % 3;
-                // 128-byte pixel rows: (row index) * 128 B >> 4 = row index * 8
-                uint32_t a_lo = s_lo + (uint32_t)(((sub * p.SR + r) * p.Wp + s) * 8);
-                uint32_t b_lo = w_lo0 + (uint32_t)(tap * p.CB) * w_tap_lo;
-                for (int cb = 0; cb < p.CB; ++cb) {
-                  const int ks = (cb == p.CB - 1) ? p.ksteps_last : 4;
-                  for (int k = 0; k < ks; ++k) {
-                    umma_f16_lh(d_tmem, a_lo + 2 * k, dhi, b_lo + 2 * k, dhi, idesc, accum);
-                    accum = 1;
-                  }
-                  a_lo += cb_lo;
-                  b_lo += w_tap_lo;
-                }
-              }
-            } else {
-              // centre-tap source: buffer row 0 is output row p0, columns start at w = -1 -> window offset 1 pixel
-              uint32_t a_lo = s_lo + (uint32_t)((sub * p.SR * p.Wp + 1) * 8);
-              uint32_t b_lo = w_lo0 + (uint32_t)((9 + b - 1) * p.CB) * w_tap_lo;
-              for (int cb = 0; cb < p.CB; ++cb) {
-                const int ks = (cb == p.CB - 1) ? p.ksteps_last : 4;
-                for (int k = 0; k < ks; ++k) umma_f16_lh(d_tmem, a_lo + 2 * k, dhi, b_lo + 2 * k, dhi, idesc, 1u);
-                a_lo += cb_lo;
-                b_lo += w_tap_lo;
-              }
+          for (int k = 0; k < 4; ++k) {
+            if (k < ks) {
+              wgmma_bf16<0, 0>(p.BN, acc, make_desc(a_lo + 2 * k, dhi), make_desc(b_lo + 2 * k, dhi), accum);
+              accum = 1;
             }
           }
-          umma_commit(&empty_bar[st]);   // ring slot may be refilled
+          a_lo += cb_lo;
+          b_lo += w_tap_lo;
         }
-        umma_commit(&tmem_full[acc]);    // accumulators of this tile complete
       }
-    }
-  } else {
-    // ================= epilogue (warps 2..5 = group 0, warps 6..9 = group 1) =================
-    const int quarter = warp & 3;             // TMEM lane quarter this warp may access
-    const int group = (warp - 2) >> 2;
-    const int et = (threadIdx.x - 64) & 127;  // thread index inside the group
-    uint8_t* sout = sout0 + (size_t)group * sout_bytes;
-    const int chunks_per_row = p.BN / 8;
-    // column statistics: thread = (column pair pr, pixel subset rg) over the valid pixels of every sub-tile it stages
-    const int npairs = p.BN >> 1, rgs = 128 / npairs;
-    const int st_rg = et / npairs, st_pr = et - st_rg * npairs;
-    const bool st_on = p.stats != nullptr && st_rg < rgs;
-    float st0 = 0.f, st1 = 0.f, sq0 = 0.f, sq1 = 0.f;
-    int it = 0;
-    long long subctr = 0;   // running sub-tile counter: sub-tile j belongs to group j & 1
-    for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-      const int st = it & 1;
-      const uint32_t ph = (it >> 1) & 1;
-      const int n = tile / p.tiles_per_img, p0 = (tile % p.tiles_per_img) * p.TRO;
-      mbar_wait(&tmem_full[st], ph);
-      tc_fence_after();
-      // last sub-tile of this tile that is mine (-1: none) -> after it this warp releases the accumulator set
-      int last_mine = -1;
-      for (int sub = 0; sub < p.NSUB; ++sub) if (((subctr + sub) & 1) == group) last_mine = sub;
-      if (last_mine < 0) {
-        tc_fence_before();
-        __syncwarp();
-        if (lane == 0) mbar_arrive(&tmem_empty[st]);
+      for (int e = 0; e < p.nextra; ++e) {
+        // centre-tap source: buffer row 0 is output row p0, columns start at w = -1 -> window offset 1 pixel
+        uint32_t a_lo = s_lo + (uint32_t)p.CB * (cb_lo + e * ecb_lo) + (uint32_t)((sub * p.SR * p.Wp + 1) * 8);
+        uint32_t b_lo = w_lo0 + (uint32_t)((9 + e) * p.CB) * w_tap_lo;
+        for (int cb = 0; cb < p.CB; ++cb) {
+          const int ks = (cb == p.CB - 1) ? p.ksteps_last : 4;
+#pragma unroll
+          for (int k = 0; k < 4; ++k)
+            if (k < ks) wgmma_bf16<0, 0>(p.BN, acc, make_desc(a_lo + 2 * k, dhi), make_desc(b_lo + 2 * k, dhi), 1u);
+          a_lo += ecb_lo;
+          b_lo += w_tap_lo;
+        }
       }
-      for (int sub = 0; sub < p.NSUB; ++sub) {
-        if (((subctr + sub) & 1) != group) continue;
-        const uint32_t taddr = tmem_base + st * 256 + sub * p.BN + ((uint32_t)(quarter * 32) << 16);
-        if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");   // staging tile free
-        else asm volatile("bar.sync 2, 128;" ::: "memory");
-        uint8_t* srow = sout + (size_t)(quarter * 32 + lane) * p.out_pitch;
-        for (int c = 0; c < p.BN; c += 32) {
-          uint32_t v[32];
-          const bool two = (c + 16) < p.BN;
-          tmem_ld_x16(taddr + c, v);
-          if (two) tmem_ld_x16(taddr + c + 16, v + 16);
-          tmem_ld_wait();
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(acc);
+      if (sub == p.NSUB - 1 && lane == 0) mbar_arrive(&empty_bar[st]);   // ring slot may be refilled
+
+      // ---- epilogue of this sub-tile ----
+      consumer_sync();   // staging tile free
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        const int col = 8 * j + fcol;
+        if (col < p.BN) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
-            if (h == 0 || two) {
-              float f[16];
-#pragma unroll
-              for (int j = 0; j < 16; ++j) f[j] = __uint_as_float(v[h * 16 + j]);
-              const int col = c + h * 16;
-              if (p.bias) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] += __ldg(p.bias + col + j);
-              }
-              if (p.act == 1 && !p.residual) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j) f[j] = hb::relu_nan(f[j]);
-              }
-              uint4 o[2];
-              __nv_bfloat162* ob = reinterpret_cast<__nv_bfloat162*>(o);
-#pragma unroll
-              for (int j = 0; j < 8; ++j) ob[j] = __floats2bfloat162_rn(f[2 * j], f[2 * j + 1]);
-              uint4* sp = reinterpret_cast<uint4*>(srow + col * 2);
-              sp[0] = o[0];
-              sp[1] = o[1];
-            }
-          }
-        }
-        if (sub == last_mine) {   // this warp's last TMEM read of the accumulator set
-          tc_fence_before();
-          __syncwarp();
-          if (lane == 0) mbar_arrive(&tmem_empty[st]);
-        }
-        if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");   // staged tile visible
-        else asm volatile("bar.sync 2, 128;" ::: "memory");
-        // copy-out: iterate over the VALID output pixels of this sub-tile (row-major), 16-byte chunks
-        const int row0 = p0 + sub * p.SR;
-        const int rows_valid = max(0, min(p.SR, min(p.H, p0 + p.TRO) - row0));
-        const int total = rows_valid * p.W * chunks_per_row;
-        // division-free walk: thread `et` starts at chunk et of the valid pixels and advances by 128 chunks per trip
-        int pix0 = et / chunks_per_row;
-        int c8 = et - pix0 * chunks_per_row;
-        int i = pix0 / p.W, q = pix0 - i * p.W;
-        const int dpix = 128 / chunks_per_row, dc = 128 - dpix * chunks_per_row;
-        const int di = dpix / p.W, dq = dpix - di * p.W;
-        for (int ch = et; ch < total; ch += 128) {
-          uint4 val = *reinterpret_cast<const uint4*>(sout + (size_t)(i * p.Wp + q) * p.out_pitch + c8 * 16);
-          const size_t off = ((size_t)(n * p.H + row0 + i) * p.W + q) * p.Cout + c8 * 8;
-          if (p.residual) {
-            const uint4 rv = *reinterpret_cast<const uint4*>(p.residual + off);
-            __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(&val);
-            const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-            for (int j = 0; j < 4; ++j) {
-              float2 fa = __bfloat1622float2(a[j]), fb = __bfloat1622float2(b[j]);
-              fa.x += fb.x; fa.y += fb.y;
-              if (p.act == 1) { fa.x = hb::relu_nan(fa.x); fa.y = hb::relu_nan(fa.y); }
-              a[j] = __floats2bfloat162_rn(fa.x, fa.y);
-            }
-          }
-          *reinterpret_cast<uint4*>(p.y + off) = val;
-          c8 += dc; q += dq; i += di;
-          if (c8 >= chunks_per_row) { c8 -= chunks_per_row; ++q; }
-          if (q >= p.W) { q -= p.W; ++i; }
-        }
-        if (st_on && !p.residual) {
-          // statistics of the staged bf16 tile over its valid pixels (junk columns q >= W and rows past the image skipped)
-          const int npix = rows_valid * p.W;
-          int si = st_rg / p.W, sq = st_rg - si * p.W;
-          const int sdi = rgs / p.W, sdq = rgs - sdi * p.W;
-          const uint8_t* sp = sout + st_pr * 4;
-          for (int v = st_rg; v < npix; v += rgs) {
-            const float2 f = __bfloat1622float2(
-                *reinterpret_cast<const __nv_bfloat162*>(sp + (size_t)(si * p.Wp + sq) * p.out_pitch));
-            st0 += f.x; st1 += f.y; sq0 = fmaf(f.x, f.x, sq0); sq1 = fmaf(f.y, f.y, sq1);
-            sq += sdq; si += sdi;
-            if (sq >= p.W) { sq -= p.W; ++si; }
+            float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
+            if (p.bias) { f0 += __ldg(p.bias + col); f1 += __ldg(p.bias + col + 1); }
+            if (p.act == 1 && !p.residual) { f0 = hb::relu_nan(f0); f1 = hb::relu_nan(f1); }
+            *reinterpret_cast<__nv_bfloat162*>(sout + (size_t)(frow + 8 * h) * p.out_pitch + col * 2) =
+                __floats2bfloat162_rn(f0, f1);
           }
         }
       }
-      subctr += p.NSUB;
+      consumer_sync();   // staged tile visible
+      // copy-out: iterate over the VALID output pixels of this sub-tile (row-major), 16-byte chunks
+      const int row0 = p0 + sub * p.SR;
+      const int rows_valid = max(0, min(p.SR, min(p.H, p0 + p.TRO) - row0));
+      const int total = rows_valid * p.W * chunks_per_row;
+      // division-free walk: thread `et` starts at chunk et of the valid pixels and advances by 256 chunks per trip
+      int pix0 = et / chunks_per_row;
+      int c8 = et - pix0 * chunks_per_row;
+      int i = pix0 / p.W, q = pix0 - i * p.W;
+      const int dpix = kConsumers / chunks_per_row, dc = kConsumers - dpix * chunks_per_row;
+      const int di = dpix / p.W, dq = dpix - di * p.W;
+      for (int ch = et; ch < total; ch += kConsumers) {
+        uint4 val = *reinterpret_cast<const uint4*>(sout + (size_t)(i * p.Wp + q) * p.out_pitch + c8 * 16);
+        const size_t off = ((size_t)(n * p.H + row0 + i) * p.W + q) * p.Cout + c8 * 8;
+        if (p.residual) {
+          const uint4 rv = *reinterpret_cast<const uint4*>(p.residual + off);
+          __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(&val);
+          const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&rv);
+#pragma unroll
+          for (int jj = 0; jj < 4; ++jj) {
+            float2 fa = __bfloat1622float2(a[jj]), fb = __bfloat1622float2(b[jj]);
+            fa.x += fb.x; fa.y += fb.y;
+            if (p.act == 1) { fa.x = hb::relu_nan(fa.x); fa.y = hb::relu_nan(fa.y); }
+            a[jj] = __floats2bfloat162_rn(fa.x, fa.y);
+          }
+        }
+        *reinterpret_cast<uint4*>(p.y + off) = val;
+        c8 += dc; q += dq; i += di;
+        if (c8 >= chunks_per_row) { c8 -= chunks_per_row; ++q; }
+        if (q >= p.W) { q -= p.W; ++i; }
+      }
+      if (st_on && !p.residual) {
+        // statistics of the staged bf16 tile over its valid pixels (junk columns q >= W and rows past the image skipped)
+        const int npix = rows_valid * p.W;
+        int si = st_rg / p.W, sq = st_rg - si * p.W;
+        const int sdi = rgs / p.W, sdq = rgs - sdi * p.W;
+        const uint8_t* sp = sout + st_pr * 4;
+        for (int v = st_rg; v < npix; v += rgs) {
+          const float2 f = __bfloat1622float2(
+              *reinterpret_cast<const __nv_bfloat162*>(sp + (size_t)(si * p.Wp + sq) * p.out_pitch));
+          st0 += f.x; st1 += f.y; sq0 = fmaf(f.x, f.x, sq0); sq1 = fmaf(f.y, f.y, sq1);
+          sq += sdq; si += sdi;
+          if (sq >= p.W) { sq -= p.W; ++si; }
+        }
+      }
     }
-    if (p.stats) {
-      // fold the pixel subsets in a fixed order; every (slot, channel) is written (zeros included)
-      if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-      else asm volatile("bar.sync 2, 128;" ::: "memory");
-      float4* scratch = reinterpret_cast<float4*>(sout);
-      scratch[et] = make_float4(st0, st1, sq0, sq1);
-      if (group == 0) asm volatile("bar.sync 1, 128;" ::: "memory");
-      else asm volatile("bar.sync 2, 128;" ::: "memory");
-      if (et < p.BN) {
-        const int pr = et >> 1, hi = et & 1;
-        float sv = 0.f, qv = 0.f;
+  }
+  if (p.stats) {
+    // fold the pixel subsets in a fixed order into slot 2*blockIdx.x; slot 2*blockIdx.x + 1 is written as zeros (every
+    // (slot, channel) is written)
+    consumer_sync();
+    float4* scratch = reinterpret_cast<float4*>(sout);   // [256] float4, 4 KB <= staging tile
+    scratch[et] = make_float4(st0, st1, sq0, sq1);
+    consumer_sync();
+    if (et < 2 * p.BN) {
+      const int c = et % p.BN, half = et / p.BN;
+      float sv = 0.f, qv = 0.f;
+      if (half == 0) {
+        const int pr = c >> 1, hi = c & 1;
         for (int rg = 0; rg < rgs; ++rg) {
           const float4 v = scratch[rg * npairs + pr];
           sv += hi ? v.y : v.x;
           qv += hi ? v.w : v.z;
         }
-        *reinterpret_cast<float2*>(p.stats + ((size_t)(blockIdx.x * 2 + group) * p.Cout + et) * 2) = make_float2(sv, qv);
       }
+      *reinterpret_cast<float2*>(p.stats + ((size_t)(blockIdx.x * 2 + half) * p.Cout + c) * 2) = make_float2(sv, qv);
     }
   }
-
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, kTmemCols); }
 }
 
 }  // namespace
@@ -345,24 +289,31 @@ int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, c
   p.w_tap_bytes = ((Cout * 128) + 1023) & ~1023;
   p.out_pitch = Cout * 2 + 16;
   const int w_bytes = (9 + nextra) * p.CB * p.w_tap_bytes;
-  const int out_bytes = ((2 * ((128 * p.out_pitch + 15) & ~15)) + 1023) & ~1023;   // one staging tile per epilogue group
+  const int out_bytes = (((128 * p.out_pitch + 15) & ~15) + 1023) & ~1023;   // one staging tile
   const int budget = 222 * 1024 - w_bytes - out_bytes - 256;
-  // largest NSUB whose two ring buffers fit in shared memory and whose accumulators fit half of TMEM
-  int nsub = 256 / Cout;
-  if (nsub > 8) nsub = 8;
+  // largest NSUB whose ring buffers (main rows + every extra source) fit in shared memory: two ring slots if
+  // possible, else one (the next tile's rows then load while the epilogue of the last sub-tile runs)
   const int max_rows_needed = (H + p.SR - 1) / p.SR;
-  if (nsub > max_rows_needed) nsub = max_rows_needed;
-  for (; nsub >= 1; --nsub) {
-    const int cb_bytes = (((nsub * p.SR + 2) * Wp * 128) + 1023) & ~1023;
-    // the last sub-tile's windows read up to 127 + 2*Wp + 2 pixel rows past its first row: keep them inside the buffer
-    const int reach = (((nsub - 1) * p.SR + 2) * Wp + 2 + 128) * 128;
-    const int need = cb_bytes > reach ? cb_bytes : ((reach + 1023) & ~1023);
-    if (2 * p.CB * need <= budget) { p.cb_bytes = need; break; }
+  int nsub = 0;
+  for (int nst = 2; nst >= 1 && nsub < 1; --nst) {
+    for (nsub = max_rows_needed < 8 ? max_rows_needed : 8; nsub >= 1; --nsub) {
+      const int tro = nsub * p.SR;
+      // the last sub-tile's windows read up to 127 + 2*Wp + 2 pixel rows past its first row: keep them inside the buffer
+      const int reach = (((nsub - 1) * p.SR + 2) * Wp + 2 + 128) * 128;
+      const int rows = (tro + 2) * Wp * 128;
+      const int need = ((rows > reach ? rows : reach) + 1023) & ~1023;
+      const int ereach = ((nsub - 1) * p.SR * Wp + 1 + 128) * 128, erows = tro * Wp * 128;
+      const int eneed = ((erows > ereach ? erows : ereach) + 1023) & ~1023;
+      if (nst * p.CB * (need + nextra * eneed) <= budget) {
+        p.nstages = nst; p.cb_bytes = need; p.ecb_bytes = eneed;
+        break;
+      }
+    }
   }
   if (nsub < 1) return -1;
   p.NSUB = nsub;
   p.TRO = nsub * p.SR;
-  p.stage_bytes = p.CB * p.cb_bytes;
+  p.stage_bytes = p.CB * (p.cb_bytes + nextra * p.ecb_bytes);
   p.tiles_per_img = (H + p.TRO - 1) / p.TRO;
   p.num_tiles = N * p.tiles_per_img;
   p.act = act;
@@ -391,7 +342,7 @@ int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, c
       if (tmap::encode_tiled_bf16(&tmWe[e], ws, 3, ewdims, ewstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
     }
   }
-  const size_t smem_bytes = (size_t)w_bytes + 2 * (size_t)p.stage_bytes + out_bytes + 256 + 1024;
+  const size_t smem_bytes = (size_t)w_bytes + (size_t)p.nstages * p.stage_bytes + out_bytes + 64 + 1024;
   static bool attr_set = false;
   if (!attr_set) {
     if (cudaFuncSetAttribute(conv_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)

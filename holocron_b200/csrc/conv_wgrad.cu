@@ -1,16 +1,16 @@
-// Weight-gradient of a 2-D convolution on the sm_100a tensor cores.
+// Weight-gradient of a 2-D convolution on the sm_90a tensor cores (wgmma).
 //
 //   dW[co, r, s, ci] = sum_m dY[m, co] * X[pix(m) + (r, s), ci]        (m over all N*Ho*Wo output pixels)
 //
 // GEMM view per filter tap: D[M = co][N = ci] += A[co, m] * B[ci, m] with the reduction (K) dimension being the
-// output pixels. Both operands are "MN-major" in shared memory (the pixel index is the slow one), which
-// tcgen05.mma supports directly for 16-bit types, so dY ([M_total, Cout] row-major) and the im2col view of X
+// output pixels. Both operands are "MN-major" in shared memory (the pixel index is the slow one), which wgmma
+// supports directly for 16-bit types (transposed operands), so dY ([M_total, Cout] row-major) and the im2col view of X
 // are loaded by TMA exactly as they sit in HBM - no transposes:
-//   A stage = 64 pixels x 128 co   (two 64-wide TMA boxes, 128B-swizzled rows = pixels)
-//   B stage = per tap: 64 pixels x Cin-tile (im2col TMA: padding / stride / row wrap handled in hardware)
-// One CTA owns (co tile, ci tile, tap group, pixel range); all taps of the group accumulate in separate TMEM
-// column ranges so the dY tile is loaded once per tap group. Results are reduced across pixel ranges with
-// fp32 red.global.add (or stored directly when there is a single range).
+//   A stage = 64 pixels x 128 co   (two 64-wide TMA boxes, 128B-swizzled rows = pixels; one per consumer warpgroup)
+//   B stage = 64 pixels x Cin-tile (im2col TMA: padding / stride / row wrap handled in hardware)
+// One CTA owns (co tile, ci tile, tap, pixel range) units; the accumulators (64 co x <= 128 ci per warpgroup) live in
+// registers. Results are reduced across pixel ranges with fp32 red.global.add, written as per-range partials for a
+// fixed-order reduction, or stored directly when there is a single range.
 // This replaces cuDNN's wgrad behind autograd for nn.Conv2d in the reference
 // (holocron/models/utils.py:71, models/classification/repvgg.py:55-62).
 #include <cstdlib>
@@ -23,17 +23,17 @@ namespace {
 using namespace tc;
 
 constexpr int kBKpix = 64;     // pixels (reduction) per stage
-constexpr int kThreads = 192;  // producer, MMA, 4 epilogue warps
-constexpr int kTmemCols = 512;
+constexpr int kThreads = 384;  // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumers = 256;
 constexpr int kChunkBytes = kBKpix * 128;  // one 64px x 64ch box = 8 KiB
 constexpr int kABytes = 2 * kChunkBytes;   // 128 co
 
 struct WgradParams {
   int m_total, Ho, Wo, stride, pad, dil, R, S, Cin, Cout;
-  int ci_tile;         // Cin tile (<= 256), multiple of 16 after rounding
+  int ci_tile;         // Cin tile (<= 128)
   int ci_chunks;       // ceil(ci_tile / 64)
-  int ci_cols;         // TMEM columns per tap (ci_tile rounded up to 32)
-  int taps_per_group;  // taps accumulated concurrently in TMEM
+  int n_last;          // MMA width of the last 64-channel chunk (ci_tile tail rounded up to 16)
+  int taps_per_group;  // taps per unit (1: the accumulators of one tap fill the register budget)
   int num_tap_groups, num_co_tiles, num_ci_tiles, k_splits;
   int kblocks_total;   // ceil(m_total / 64)
   int stages, stage_bytes;
@@ -49,24 +49,15 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
   uint64_t* empty_bar = full_bar + p.stages;
-  uint64_t* acc_full = empty_bar + p.stages;  // [1]
-  uint64_t* acc_empty = acc_full + 1;         // [1]
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(acc_empty + 1);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmDY);
     prefetch_tmap(&tmX);
-    for (int i = 0; i < p.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(acc_full, 1);
-    mbar_init(acc_empty, 4);
+    for (int i = 0; i < p.stages; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 32); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
 
   const int RS = p.R * p.S;
   const int num_units = p.num_co_tiles * p.num_ci_tiles * p.num_tap_groups * p.k_splits;
@@ -84,8 +75,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     kb1 = min(kb0 + per, p.kblocks_total);
   };
 
-  if (warp == 0) {
-    if (lane == 0) {
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         int co_t, ci_t, tg, ks, kb0, kb1;
@@ -114,108 +105,88 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
         }
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const int n_mma = (p.ci_tile + 15) & ~15;
-      const uint32_t idesc = make_idesc_bf16(128, n_mma, 1, 1);
-      const uint32_t dhi = desc_hi(1024, kLayoutSW128);
-      int stage = 0; uint32_t phase = 0;
-      int it = 0;
-      for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x, ++it) {
-        int co_t, ci_t, tg, ks, kb0, kb1;
-        decode(unit, co_t, ci_t, tg, ks);
-        kb_range(ks, kb0, kb1);
-        const int tap0 = tg * p.taps_per_group;
-        const int ntaps = min(p.taps_per_group, RS - tap0);
-        mbar_wait(acc_empty, (it & 1) ^ 1);
-        tc_fence_after();
-        for (int kb = kb0; kb < kb1; ++kb) {
-          mbar_wait(&full_bar[stage], phase);
-          tc_fence_after();
-          // 16 pixels = two 8-row swizzle atoms (SBO 1024 B); 64-channel chunks are LBO = 8 KiB apart
-          const uint32_t a_lo = desc_lo(smem_u32(smem + (size_t)stage * p.stage_bytes), kChunkBytes);
-          uint32_t b_lo = a_lo + (kABytes >> 4);
-          const uint32_t acc0 = kb > kb0 ? 1u : 0u;
-          for (int t = 0; t < ntaps; ++t) {
-#pragma unroll
-            for (int k = 0; k < kBKpix / 16; ++k)
-              umma_f16_lh(tmem_base + t * p.ci_cols, a_lo + k * (2048 >> 4), dhi, b_lo + k * (2048 >> 4), dhi, idesc,
-                          acc0 | (uint32_t)k);
-            b_lo += (uint32_t)b_tap_bytes >> 4;
-          }
-          umma_commit(&empty_bar[stage]);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
-        }
-        umma_commit(acc_full);
-      }
-    }
-  } else {
-    const int quarter = warp & 3;
-    int it = 0;
-    for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x, ++it) {
-      int co_t, ci_t, tg, ks, kb0, kb1;
-      decode(unit, co_t, ci_t, tg, ks);
-      kb_range(ks, kb0, kb1);
-      const int tap0 = tg * p.taps_per_group;
-      const int ntaps = min(p.taps_per_group, RS - tap0);
-      mbar_wait(acc_full, it & 1);
-      tc_fence_after();
-      const int co = co_t * 128 + quarter * 32 + lane;
-      const bool co_ok = co < p.Cout;
-      const uint32_t tbase = tmem_base + ((uint32_t)(quarter * 32) << 16);
-      if (kb1 <= kb0 && p.use_atomics == 2 && co_ok) {
-        // empty pixel range: this unit's slice of the partial buffer must still read as zero
-        for (int t = 0; t < ntaps; ++t)
-          for (int c = 0; c < p.ci_tile && ci_t * p.ci_tile + c < p.Cin; ++c)
-            p.ws[(size_t)ks * p.dw_elems + ((size_t)co * RS + tap0 + t) * p.Cin + ci_t * p.ci_tile + c] = 0.f;
-      }
-      if (kb1 > kb0) {
-        for (int t = 0; t < ntaps; ++t) {
-          const int tap = tap0 + t;
-          for (int c = 0; c < p.ci_tile; c += 16) {
-            uint32_t v[16];
-            tmem_ld_x16(tbase + t * p.ci_cols + c, v);
-            tmem_ld_wait();
-            const int ci = ci_t * p.ci_tile + c;
-            if (co_ok && ci < p.Cin) {
-              float* base = p.use_atomics == 2 ? p.ws + (size_t)ks * p.dw_elems : p.dw;
-              float* dst = base + ((size_t)co * RS + tap) * p.Cin + ci;
-              const int nvalid = min(16, p.Cin - ci);
-              if (p.use_atomics == 1) {
-#pragma unroll
-                for (int j = 0; j < 16; ++j)
-                  if (j < nvalid) atomicAdd(dst + j, __uint_as_float(v[j]));
-              } else {
-                if (nvalid == 16) {
-                  float4* d4 = reinterpret_cast<float4*>(dst);
-#pragma unroll
-                  for (int j = 0; j < 4; ++j)
-                    d4[j] = make_float4(__uint_as_float(v[4 * j]), __uint_as_float(v[4 * j + 1]),
-                                        __uint_as_float(v[4 * j + 2]), __uint_as_float(v[4 * j + 3]));
-                } else {
-#pragma unroll
-                  for (int j = 0; j < 16; ++j)
-                    if (j < nvalid) dst[j] = __uint_as_float(v[j]);
-                }
-              }
-            }
-          }
-        }
-      }
-      tc_fence_before();
-      __syncwarp();
-      if (lane == 0) mbar_arrive(acc_empty);
-    }
+    return;
   }
 
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, kTmemCols); }
+  // ================= consumers: warpgroup wg owns output channels [64*wg, 64*wg + 64) of the co tile =================
+  const int et = threadIdx.x - 128;
+  const int wg = et >> 7;
+  const int frow = frag_row(et & 127), fcol = frag_col(et & 127);
+  const uint32_t dhi = desc_hi(1024);
+  float acc[64];   // [chunk 0: 32 | chunk 1: 32]
+  int stage = 0; uint32_t phase = 0;
+  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+    int co_t, ci_t, tg, ks, kb0, kb1;
+    decode(unit, co_t, ci_t, tg, ks);
+    kb_range(ks, kb0, kb1);
+    const int tap = tg * p.taps_per_group;
+    int prev = -1;
+    for (int kb = kb0; kb < kb1; ++kb) {
+      mbar_wait(&full_bar[stage], phase);
+      // 16 pixels = two 8-row swizzle atoms (SBO 1024 B), i.e. 2048 B per k-step
+      const uint32_t s_lo = desc_lo(smem_u32(smem + (size_t)stage * p.stage_bytes), 16);
+      const uint32_t a_lo = s_lo + (uint32_t)wg * (kChunkBytes >> 4);
+      const uint32_t b_lo = s_lo + (kABytes >> 4);
+      const uint32_t acc0 = kb > kb0 ? 1u : 0u;
+      wgmma_fence();
+#pragma unroll
+      for (int k = 0; k < kBKpix / 16; ++k) {
+        const uint64_t ad = make_desc(a_lo + k * (2048 >> 4), dhi);
+        const uint32_t sc = acc0 | (uint32_t)k;
+        if (p.ci_chunks == 1) {
+          wgmma_bf16<1, 1>(p.n_last, acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
+        } else {
+          wgmma_n64<1, 1>(acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
+          const uint64_t bd = make_desc(b_lo + (kChunkBytes >> 4) + k * (2048 >> 4), dhi);
+          switch (p.n_last) {   // second chunk: accumulators 32.. (a constant offset inside every case)
+            case 16: wgmma_n16<1, 1>(acc + 32, ad, bd, sc); break;
+            case 32: wgmma_n32<1, 1>(acc + 32, ad, bd, sc); break;
+            case 48: wgmma_n48<1, 1>(acc + 32, ad, bd, sc); break;
+            case 64: wgmma_n64<1, 1>(acc + 32, ad, bd, sc); break;
+            default: break;
+          }
+        }
+      }
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+      prev = stage;
+      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+
+    const bool have = kb1 > kb0;   // empty pixel range: this unit's slice of the partial buffer must still read as zero
+    if (!have && p.use_atomics != 2) continue;
+    float* base = p.use_atomics == 2 ? p.ws + (size_t)ks * p.dw_elems : p.dw;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int co = co_t * 128 + 64 * wg + frow + 8 * h;
+      if (co >= p.Cout) continue;
+      float* drow = base + ((size_t)co * RS + tap) * p.Cin;
+#pragma unroll
+      for (int j = 0; j < 16; ++j) {
+        // register block j: chunk j / 8, columns 8 * (j % 8) + fcol of that chunk
+        const int c = (j >> 3) * 64 + 8 * (j & 7) + fcol;
+        const int ci = ci_t * p.ci_tile + c;
+        const int width = (j >> 3) + 1 < p.ci_chunks ? 64 : p.n_last;
+        if ((j >> 3) >= p.ci_chunks || 8 * (j & 7) >= width || c >= p.ci_tile || ci >= p.Cin) continue;
+        const float v0 = have ? acc[4 * j + 2 * h] : 0.f, v1 = have ? acc[4 * j + 2 * h + 1] : 0.f;
+        if (p.use_atomics == 1) {
+          atomicAdd(drow + ci, v0);
+          atomicAdd(drow + ci + 1, v1);
+        } else {
+          *reinterpret_cast<float2*>(drow + ci) = make_float2(v0, v1);   // Cin % 8 == 0 and ci even: 8-byte aligned
+        }
+      }
+    }
+  }
 }
 
 // dw[i] = sum_k ws[k][i] in a fixed order (deterministic). blockDim = (32, 8): threadIdx.x walks float4 columns,
 // threadIdx.y takes the slices k = y, y+8, ...; the 8 partial sums are combined through shared memory in y order.
-// (A single thread per column walking up to 148 slices serially took 23 us per launch: latency, not bandwidth.)
+// (A single thread per column walking a hundred or more slices serially is latency-bound, not bandwidth-bound.)
 // Elements [0, n_first) go to dw, [n_first, n) to dw2 (two gradient tensors filled by one launch; n_first % 4 == 0);
 // accumulate != 0: dw += sum instead of dw = sum (gradient accumulation straight into the parameter's .grad storage, what
 // autograd's AccumulateGrad would do with one more element-wise kernel per parameter and step).
@@ -285,21 +256,17 @@ int plan_wgrad(WgradPlan& plan, int N, int H, int W, int Cin, int Cout, int R, i
   p.R = R; p.S = S; p.Cin = Cin; p.Cout = Cout;
   const int RS = R * S;
   int ci_tile = Cin;
-  if (Cin > 256) {
-    ci_tile = 256;
-    for (int c = 256; c >= 64; c -= 64) if (Cin % c == 0) { ci_tile = c; break; }
+  if (Cin > 128) {
+    ci_tile = 128;
+    if (Cin % 128 != 0 && Cin % 64 == 0) ci_tile = 64;
   }
   p.ci_tile = ci_tile;
   p.ci_chunks = (ci_tile + 63) / 64;
-  p.ci_cols = (ci_tile + 15) & ~15;
-  p.taps_per_group = kTmemCols / p.ci_cols;
-  if (p.taps_per_group > RS) p.taps_per_group = RS;
-  auto stage_bytes_for = [&](int taps) { return kABytes + taps * p.ci_chunks * kChunkBytes; };
-  while (p.taps_per_group > 1 && 2 * stage_bytes_for(p.taps_per_group) > 200 * 1024) --p.taps_per_group;
-  p.stage_bytes = stage_bytes_for(p.taps_per_group);
+  p.n_last = ((ci_tile - (p.ci_chunks - 1) * 64) + 15) & ~15;
+  p.taps_per_group = 1;
+  p.stage_bytes = kABytes + p.ci_chunks * kChunkBytes;
   p.stages = (200 * 1024) / p.stage_bytes;
   if (p.stages > 6) p.stages = 6;
-  if (p.stages < 2) return (int)cudaErrorInvalidValue;
   p.num_tap_groups = (RS + p.taps_per_group - 1) / p.taps_per_group;
   p.num_co_tiles = (Cout + 127) / 128;
   p.num_ci_tiles = (Cin + ci_tile - 1) / ci_tile;
@@ -391,7 +358,7 @@ static int wgrad_impl(const void* x, const void* dy, float* dw, float* workspace
                                   CU_TENSOR_MAP_SWIZZLE_128B);
     if (rc) return rc;
   }
-  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + (2 * p.stages + 2) * sizeof(uint64_t) + 16 + 1024;
+  const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 2 * p.stages * sizeof(uint64_t) + 1024;
   static bool attr_set = false;
   if (!attr_set) {
     cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);

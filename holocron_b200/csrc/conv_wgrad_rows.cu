@@ -7,16 +7,14 @@
 // halo by out-of-bounds fill) and one brings the TRO rows of dY with the SAME pitch (its 2 extra columns per row are
 // out-of-bounds zeros), so for tap (r, s) the reduction over pixels is a plain dot product between the dY buffer and the
 // X buffer shifted by (r*Wp + s) pixel rows. Both operands are MN-major (pixel index = K): the X window is the A operand
-// (M = input channels), dY the B operand (N = output channels). Two taps share one M=128 MMA: the second 64-channel chunk
-// of A is addressed through the descriptor's leading-byte-offset = distance between the two taps' windows.
-// Accumulators (5 tap slots x Cout columns) live in TMEM for ALL tiles of a CTA; there is a single epilogue per CTA that
-// writes a partial dW, reduced afterwards in a fixed order (deterministic).
-// More channels than one CTA's TMEM can accumulate (Cin > 64 or Cout > 96) are split into (64-input-channel,
-// <=96-output-channel) groups; the CTAs of a group share the tiles between them, each group owns a disjoint part of dW.
-// RepVGG blocks: the 1x1 branch's weight gradient dW1[co, ci] = sum dY1[n,p,q,co] * X[n,p,q,ci] reads the same X rows
-// through the centre-tap window, so it rides along as a sixth accumulator slot fed by a second dY buffer (has_b1).
-// The generic kernel (conv_wgrad.cu) re-reads X nine times from L2 (one im2col load per tap): 0.94 ms for the 48-channel
-// 112^2 layer of RepVGG-A0 at batch 256 against an HBM time of 0.1 ms.
+// (M = 64 input channels), dY the B operand (N = output channels of the group).
+// Tap slots: the nine taps, plus, for RepVGG blocks (has_b1), the 1x1 branch's weight gradient
+// dW1[co, ci] = sum dY1[n,p,q,co] * X[n,p,q,ci], which reads the same X rows through the centre-tap window against a
+// second dY buffer. Each consumer warpgroup keeps TPW slots (TPW * NC / 2 <= 64 fp32 registers per thread) for ALL tiles
+// of the CTA; there is a single epilogue per CTA that writes a partial dW, reduced afterwards in a fixed order
+// (deterministic). Channels and slots beyond one CTA's registers are split into (64-input-channel, <= 64-output-channel,
+// slot range) groups; the CTAs of a group share the tiles between them, each group owns a disjoint part of dW.
+// The generic kernel (conv_wgrad.cu) re-reads X nine times from L2 (one im2col load per tap).
 #include "common.cuh"
 #include "tc_common.cuh"
 #include "tmap.cuh"
@@ -25,34 +23,34 @@ namespace {
 
 using namespace tc;
 
-constexpr int kThreads = 192;
-constexpr int kTmemCols = 512;
+constexpr int kThreads = 384;   // producer warpgroup + 2 consumer warpgroups
+constexpr int kConsumers = 256;
 
 struct WRowsParams {
   int N, H, W, Cin, Cout;
   int Wp, TRO, KS;       // smem row pitch, output rows per tile, 16-pixel k-steps per tile
-  int n_cig, n_cog, ngroups;   // groups of 64 input channels x groups of co_group output channels
-  int co_group;          // output channels per group (multiple of 16, <= 96)
-  int co_chunks;         // 64-channel chunks of dY per group (1 or 2)
-  int ncols;             // TMEM columns per tap slot (= co_group)
+  int n_cig, n_cog, n_sg, ngroups;   // groups of 64 input channels x groups of co_group output channels x slot ranges
+  int co_group;          // output channels per group (NC: 16, 32, 48 or 64)
+  int tpw;               // tap slots per consumer warpgroup
+  int nslots;            // 9, or 10 with the 1x1 branch
   int tiles_per_img, num_tiles;
-  int xbuf_bytes, ybuf_chunk_bytes, stage_bytes;
-  int has_b1;            // 1: also accumulate the 1x1 branch (slot 5, second dY source)
+  int xbuf_bytes, ybuf_bytes, stage_bytes;
+  int has_b1;            // 1: also accumulate the 1x1 branch (slot 9, second dY source)
   float* ws;             // [members][dw_elems (+ Cout*Cin)] partial sums
   long long dw_elems;    // Cout*9*Cin
   long long slice_elems; // dw_elems + (has_b1 ? Cout*Cin : 0)
 };
 
+template <int NC>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmDY,
                        const __grid_constant__ CUtensorMap tmDY1, const WRowsParams p) {
+  constexpr int TPW = 128 / NC > 8 ? 8 : 128 / NC;
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* bars = reinterpret_cast<uint64_t*>(smem + (size_t)2 * p.stage_bytes);
   uint64_t* full_bar = bars;       // [2]
   uint64_t* empty_bar = bars + 2;  // [2]
-  uint64_t* done_bar = bars + 4;
-  uint32_t* tmem_ptr = reinterpret_cast<uint32_t*>(bars + 5);
 
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   // zero both stages once: rows the TMA boxes never write (tails read by the shifted windows / the rounded-up K range)
@@ -62,22 +60,18 @@ conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
   if (warp == 0 && lane == 0) {
     prefetch_tmap(&tmX);
     prefetch_tmap(&tmDY);
-    for (int i = 0; i < 2; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], 1); }
-    mbar_init(done_bar, 1);
+    for (int i = 0; i < 2; ++i) { mbar_init(&full_bar[i], 1); mbar_init(&empty_bar[i], kConsumers / 32); }
     fence_barrier_init();
   }
-  if (warp == 1) tmem_alloc(tmem_ptr, kTmemCols);
   fence_proxy_async();   // generic-proxy zero fill ordered before the async-proxy (TMA / MMA) accesses
-  tc_fence_before();
   __syncthreads();
-  tc_fence_after();
-  const uint32_t tmem_base = *tmem_ptr;
   const int group = blockIdx.x % p.ngroups, member = blockIdx.x / p.ngroups, members = gridDim.x / p.ngroups;
-  const int ci0 = (group % p.n_cig) * 64, co0 = (group / p.n_cig) * p.co_group;
+  const int ci0 = (group % p.n_cig) * 64, co0 = ((group / p.n_cig) % p.n_cog) * p.co_group;
+  const int sg = group / (p.n_cig * p.n_cog);
 
-  if (warp == 0) {
-    if (lane == 0) {
-      const uint32_t tx = (uint32_t)((p.TRO + 2) * p.Wp * 128 + (1 + p.has_b1) * p.co_chunks * p.TRO * p.Wp * 128);
+  if (warp < 4) {
+    if (warp == 0 && lane == 0) {
+      const uint32_t tx = (uint32_t)((p.TRO + 2) * p.Wp * 128 + (1 + p.has_b1) * p.TRO * p.Wp * 128);
       if (p.has_b1) prefetch_tmap(&tmDY1);
       int it = 0;
       for (int tile = member; tile < p.num_tiles; tile += members, ++it) {
@@ -90,100 +84,85 @@ conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
             "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
             ::"r"(smem_u32(sx)), "l"(reinterpret_cast<uint64_t>(&tmX)), "r"(smem_u32(&full_bar[st])), "r"(ci0), "r"(-1),
               "r"(p0 - 1), "r"(n) : "memory");
-        for (int c = 0; c < p.co_chunks; ++c)
+        asm volatile(
+            "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
+            ::"r"(smem_u32(sx + p.xbuf_bytes)), "l"(reinterpret_cast<uint64_t>(&tmDY)),
+              "r"(smem_u32(&full_bar[st])), "r"(co0), "r"(0), "r"(p0), "r"(n) : "memory");
+        if (p.has_b1)
           asm volatile(
               "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-              ::"r"(smem_u32(sx + p.xbuf_bytes + c * p.ybuf_chunk_bytes)), "l"(reinterpret_cast<uint64_t>(&tmDY)),
-                "r"(smem_u32(&full_bar[st])), "r"(co0 + c * 64), "r"(0), "r"(p0), "r"(n) : "memory");
-        if (p.has_b1)
-          for (int c = 0; c < p.co_chunks; ++c)
-            asm volatile(
-                "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                ::"r"(smem_u32(sx + p.xbuf_bytes + (p.co_chunks + c) * p.ybuf_chunk_bytes)),
-                  "l"(reinterpret_cast<uint64_t>(&tmDY1)), "r"(smem_u32(&full_bar[st])), "r"(co0 + c * 64), "r"(0), "r"(p0), "r"(n)
-                : "memory");
+              ::"r"(smem_u32(sx + p.xbuf_bytes + p.ybuf_bytes)), "l"(reinterpret_cast<uint64_t>(&tmDY1)),
+                "r"(smem_u32(&full_bar[st])), "r"(co0), "r"(0), "r"(p0), "r"(n) : "memory");
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      const uint32_t idesc = make_idesc_bf16(128, p.ncols, 1, 1);   // both operands MN-major
-      const uint32_t dhi = desc_hi(1024, kLayoutSW128);
-      const uint32_t lbo_b = (uint32_t)p.ybuf_chunk_bytes;
-      bool any = false;
-      int it = 0;
-      for (int tile = member; tile < p.num_tiles; tile += members, ++it) {
-        const int st = it & 1;
-        mbar_wait(&full_bar[st], (it >> 1) & 1);
-        tc_fence_after();
-        const uint32_t sx = smem_u32(smem + (size_t)st * p.stage_bytes);
-        const uint32_t sy = sx + p.xbuf_bytes;
-        const uint32_t b_lo0 = desc_lo(sy, lbo_b);
-        for (int slot = 0; slot < 5; ++slot) {
-          const int ta = 2 * slot, tb = slot < 4 ? 2 * slot + 1 : 2 * slot;
-          const int off_a = (ta / 3) * p.Wp + (ta % 3), off_b = (tb / 3) * p.Wp + (tb % 3);
-          // A: M chunk 0 = tap a window, M chunk 1 = tap b window (LBO = distance between the windows)
-          const uint32_t a_lo0 = desc_lo(sx + off_a * 128, (uint32_t)((off_b - off_a) * 128));
-          const uint32_t d_tmem = tmem_base + slot * p.ncols;
-          for (int k = 0; k < p.KS; ++k)
-            umma_f16_lh(d_tmem, a_lo0 + k * (2048 >> 4), dhi, b_lo0 + k * (2048 >> 4), dhi, idesc, (any || k > 0) ? 1u : 0u);
-        }
-        if (p.has_b1) {
-          // 1x1 branch: centre-tap window of X (second M chunk = don't care) against the dY1 buffer
-          const uint32_t a_lo0 = desc_lo(sx + (p.Wp + 1) * 128, 0);
-          const uint32_t b1_lo0 = desc_lo(sy + p.co_chunks * p.ybuf_chunk_bytes, lbo_b);
-          const uint32_t d_tmem = tmem_base + 5 * p.ncols;
-          for (int k = 0; k < p.KS; ++k)
-            umma_f16_lh(d_tmem, a_lo0 + k * (2048 >> 4), dhi, b1_lo0 + k * (2048 >> 4), dhi, idesc, (any || k > 0) ? 1u : 0u);
-        }
-        any = true;
-        umma_commit(&empty_bar[st]);
-      }
-      umma_commit(done_bar);
-    }
-  } else {
-    // ================= single epilogue per CTA =================
-    const int quarter = warp & 3;
-    mbar_wait(done_bar, 0);
-    tc_fence_after();
-    const bool has_work = member < p.num_tiles;
-    float* out = p.ws + (size_t)member * p.slice_elems;
-    const int ci = ci0 + (quarter & 1) * 32 + lane;     // lanes 0-63: first tap of the slot, 64-127: second tap
-    const int which = quarter >> 1;
-    for (int slot = 0; slot < 5; ++slot) {
-      const int tap = 2 * slot + which;
-      const bool tap_ok = tap < 9 && (slot < 4 || which == 0);
-      for (int c = 0; c < p.ncols; c += 16) {
-        uint32_t v[16];
-        tmem_ld_x16(tmem_base + slot * p.ncols + c + ((uint32_t)(quarter * 32) << 16), v);
-        tmem_ld_wait();
-        if (tap_ok && ci < p.Cin) {
+    return;
+  }
+
+  // ================= consumers: warpgroup wg owns slots sg*2*TPW + wg*TPW + [0, TPW) =================
+  const int et = threadIdx.x - 128;
+  const int wg = et >> 7;
+  const int slot0 = sg * 2 * TPW + wg * TPW;
+  const uint32_t dhi = desc_hi(1024);
+  float acc[TPW][NC / 2];
+  bool any = false;
+  int it = 0;
+  for (int tile = member; tile < p.num_tiles; tile += members, ++it) {
+    const int st = it & 1;
+    mbar_wait(&full_bar[st], (it >> 1) & 1);
+    const uint32_t sx = smem_u32(smem + (size_t)st * p.stage_bytes);
+    const uint32_t sy = sx + p.xbuf_bytes;
+    wgmma_fence();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int co = co0 + c + j;
-            if (c + j < p.co_group && co < p.Cout) out[((size_t)co * 9 + tap) * p.Cin + ci] = has_work ? __uint_as_float(v[j]) : 0.f;
-          }
-        }
+    for (int t = 0; t < TPW; ++t) {
+      const int slot = slot0 + t;
+      if (slot >= p.nslots) break;
+      // slot < 9: tap window (r, s) against dY; slot 9: centre window against dY1
+      const int off = slot < 9 ? (slot / 3) * p.Wp + (slot % 3) : p.Wp + 1;
+      const uint32_t a_lo0 = desc_lo(sx + off * 128, 16);
+      const uint32_t b_lo0 = desc_lo(slot < 9 ? sy : sy + p.ybuf_bytes, 16);
+      for (int k = 0; k < p.KS; ++k) {
+        const uint64_t ad = make_desc(a_lo0 + k * (2048 >> 4), dhi), bd = make_desc(b_lo0 + k * (2048 >> 4), dhi);
+        const uint32_t sc = (any || k > 0) ? 1u : 0u;
+        if constexpr (NC == 16) wgmma_n16<1, 1>(acc[t], ad, bd, sc);
+        else if constexpr (NC == 32) wgmma_n32<1, 1>(acc[t], ad, bd, sc);
+        else if constexpr (NC == 48) wgmma_n48<1, 1>(acc[t], ad, bd, sc);
+        else wgmma_n64<1, 1>(acc[t], ad, bd, sc);
       }
     }
-    if (p.has_b1) {
-      float* out1 = out + p.dw_elems;   // [Cout][Cin]
-      for (int c = 0; c < p.ncols; c += 16) {
-        uint32_t v[16];
-        tmem_ld_x16(tmem_base + 5 * p.ncols + c + ((uint32_t)(quarter * 32) << 16), v);
-        tmem_ld_wait();
-        if (which == 0 && ci < p.Cin) {
+    wgmma_commit();
+    wgmma_wait<0>();
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            const int co = co0 + c + j;
-            if (c + j < p.co_group && co < p.Cout) out1[(size_t)co * p.Cin + ci] = has_work ? __uint_as_float(v[j]) : 0.f;
-          }
+    for (int t = 0; t < TPW; ++t) fence_regs(acc[t]);
+    any = true;
+    if (lane == 0) mbar_arrive(&empty_bar[st]);
+  }
+
+  // ================= single epilogue per CTA =================
+  const bool has_work = member < p.num_tiles;
+  float* out = p.ws + (size_t)member * p.slice_elems;
+  const int frow = frag_row(et & 127), fcol = frag_col(et & 127);
+#pragma unroll
+  for (int t = 0; t < TPW; ++t) {
+    const int slot = slot0 + t;
+    if (slot >= p.nslots) break;
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int ci = ci0 + frow + 8 * h;
+      if (ci >= p.Cin) continue;
+#pragma unroll
+      for (int j = 0; j < NC / 8; ++j) {
+#pragma unroll
+        for (int e = 0; e < 2; ++e) {
+          const int c = 8 * j + fcol + e;
+          const int co = co0 + c;
+          if (c >= p.co_group || co >= p.Cout) continue;
+          const float v = has_work ? acc[t][4 * j + 2 * h + e] : 0.f;
+          if (slot < 9) out[((size_t)co * 9 + slot) * p.Cin + ci] = v;
+          else out[p.dw_elems + (size_t)co * p.Cin + ci] = v;   // dW1 [Cout][Cin]
         }
       }
     }
   }
-  tc_fence_before();
-  __syncthreads();
-  if (warp == 1) { tc_fence_after(); tmem_dealloc(tmem_base, kTmemCols); }
 }
 
 struct WRowsPlan { WRowsParams p; int grid, members; size_t smem; };
@@ -195,14 +174,13 @@ bool plan_wrows(WRowsPlan& pl, int N, int H, int W, int Cin, int Cout, int num_c
   p.Wp = W + 2;
   p.n_cig = (Cin + 63) / 64;
   p.has_b1 = has_b1;
-  const int slots = 5 + has_b1;
-  const int max_group = ((kTmemCols / slots) / 16) * 16;   // 96 (5 slots) or 80 (6 slots)
-  p.n_cog = (Cout + max_group - 1) / max_group;
+  p.nslots = 9 + has_b1;
+  p.n_cog = (Cout + 63) / 64;
   p.co_group = (((Cout + p.n_cog - 1) / p.n_cog) + 15) & ~15;
-  p.ngroups = p.n_cig * p.n_cog;
-  p.co_chunks = (p.co_group + 63) / 64;
-  p.ncols = p.co_group;
-  if (slots * p.ncols > kTmemCols || p.ngroups > 16) return false;
+  p.tpw = 128 / p.co_group > 8 ? 8 : 128 / p.co_group;
+  p.n_sg = (p.nslots + 2 * p.tpw - 1) / (2 * p.tpw);
+  p.ngroups = p.n_cig * p.n_cog * p.n_sg;
+  if (p.ngroups > 32) return false;   // more groups re-read X too often: the generic kernel is the better choice
   int tro = H < 16 ? H : 16;
   for (; tro >= 1; --tro) {
     const int ks = (tro * p.Wp + 15) / 16;
@@ -210,9 +188,9 @@ bool plan_wrows(WRowsPlan& pl, int N, int H, int W, int Cin, int Cout, int num_c
     const int xrows = 2 * p.Wp + 2 + ks * 16;
     const int xbytes = ((xrows > (tro + 2) * p.Wp ? xrows : (tro + 2) * p.Wp) * 128 + 1023) & ~1023;
     const int ybytes = ((ks * 16) * 128 + 1023) & ~1023;
-    if (2 * (xbytes + (1 + has_b1) * p.co_chunks * ybytes) <= 220 * 1024) {
-      p.TRO = tro; p.KS = ks; p.xbuf_bytes = xbytes; p.ybuf_chunk_bytes = ybytes;
-      p.stage_bytes = xbytes + (1 + has_b1) * p.co_chunks * ybytes;
+    if (2 * (xbytes + (1 + has_b1) * ybytes) <= 220 * 1024) {
+      p.TRO = tro; p.KS = ks; p.xbuf_bytes = xbytes; p.ybuf_bytes = ybytes;
+      p.stage_bytes = xbytes + (1 + has_b1) * ybytes;
       break;
     }
   }
@@ -266,12 +244,20 @@ int hb_wgrad_rows_try(const void* x, const void* dy, const void* dy1, float* ws,
   }
   static bool attr_set = false;
   if (!attr_set) {
-    if (cudaFuncSetAttribute(conv_wgrad_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+    if (cudaFuncSetAttribute(conv_wgrad_rows_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
+        cudaFuncSetAttribute(conv_wgrad_rows_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
+        cudaFuncSetAttribute(conv_wgrad_rows_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
+        cudaFuncSetAttribute(conv_wgrad_rows_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
       return -1;
     attr_set = true;
   }
   if (pl.smem > 227 * 1024) return -1;
-  conv_wgrad_rows_kernel<<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p);
+  switch (p.co_group) {
+    case 16: conv_wgrad_rows_kernel<16><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
+    case 32: conv_wgrad_rows_kernel<32><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
+    case 48: conv_wgrad_rows_kernel<48><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
+    default: conv_wgrad_rows_kernel<64><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
+  }
   g_hb_launches.fetch_add(1, std::memory_order_relaxed);
   *slices_out = pl.members;
   return cudaGetLastError() == cudaSuccess ? 0 : -2;

@@ -56,7 +56,7 @@ __global__ void dropblock_apply_kernel(const T* x, T* out, const float* __restri
 }
 
 // channels_last fast path: one 128-bit vector (16 / sizeof(T) channels of one pixel) per thread step, 32-bit index arithmetic
-// (the scalar kernel above did a 64-bit division per ELEMENT and ran at 0.9 TB/s; YOLOv4 has a DropBlock behind every conv)
+// (the scalar kernel above does a 64-bit division per ELEMENT; YOLOv4 has a DropBlock behind every conv)
 template <typename T>
 __global__ void __launch_bounds__(256) dropblock_apply_nhwc_vec_kernel(const T* x, T* out, const float* __restrict__ mask,
                                                                        const float* __restrict__ kept, unsigned total_vec,

@@ -96,10 +96,10 @@ __global__ void __launch_bounds__(kThreads) dw_bwd_data_kernel(const __nv_bfloat
 
 // ---- 3x3 specialisations: fixed channel group per thread (block = channel groups x pixel lanes, as in the BN
 // kernels), the block's slab of the filter sits in shared memory (float4 reads). The generic kernels above
-// re-read 72 scalar weights per output vector and recompute the channel group of every element: 9x slower than the
-// HBM time on the ReXNet expansions (profiles/r01_rexnet_launches.md).
+// re-read 72 scalar weights per output vector and recompute the channel group of every element: instruction-bound,
+// far from the HBM time on the ReXNet expansions.
 // kStride: 1 or 2 known at compile time (the backward index arithmetic divides by the stride: a runtime divisor costs
-// ~40 instructions per tap and made the data-gradient pass 2.4x slower than the forward one); 0 = runtime stride.
+// ~40 instructions per tap, which makes the data-gradient pass instruction bound); 0 = runtime stride.
 template <bool kBackward, int kStride>
 __global__ void __launch_bounds__(kThreads, 3) dw3x3_kernel(const __nv_bfloat16* __restrict__ src, const float* __restrict__ w,
                                                          const float* __restrict__ bias, __nv_bfloat16* __restrict__ dst,
@@ -173,8 +173,7 @@ __global__ void __launch_bounds__(kThreads, 3) dw3x3_kernel(const __nv_bfloat16*
 
 // ---- four horizontally adjacent outputs per thread ------------------------------------------------------------------
 // The one-output-per-thread kernel above issues 9 vector loads, 72 converts, 18 shared-memory filter reads, two integer
-// divisions and 9 bounds predicates per 8 output values and sat at ~1 TB/s on the ReXNet expansions (instruction-bound,
-// profiles/r02_launches_rexnet1_0x_b256.md). With 4 outputs of one row per thread the 3 input rows are loaded once
+// divisions and 9 bounds predicates per 8 output values and is instruction-bound on the ReXNet expansions. With 4 outputs of one row per thread the 3 input rows are loaded once
 // (3 x (3*S+3) vectors for stride S instead of 36), the filter slab is read once per quad and the index arithmetic is
 // amortised over 32 output values.
 //   forward  (kFlip = 0): y[oh, ow]  = b + sum_{r,s} x[oh*S + r - pad, ow*S + s - pad] * w[r, s]
@@ -261,8 +260,7 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_quad_kernel(const __nv_bflo
 // (h-1)/2); along W the quad {w0..w0+3} reads the three dy columns c0 = w0/2, c0+1, c0+2 in a fixed pattern:
 //   dx[w0]   += dy[c0]   w[.,1]              dx[w0+1] += dy[c0+1] w[.,0] + dy[c0]   w[.,2]
 //   dx[w0+2] += dy[c0+1] w[.,1]              dx[w0+3] += dy[c0+2] w[.,0] + dy[c0+1] w[.,2]
-// 3 - 6 vector loads per 4 outputs; the one-output kernel issued 9 predicated loads per output (0.9 TB/s on ReXNet's four
-// stride-2 blocks, 4.8 % of the step).
+// 3 - 6 vector loads per 4 outputs; the one-output kernel issues 9 predicated loads per output.
 __global__ void __launch_bounds__(kThreads, 2) dw3x3_dgrad_s2_quad_kernel(const __nv_bfloat16* __restrict__ dy,
                                                                         const float* __restrict__ w, __nv_bfloat16* __restrict__ dx,
                                                                         int N, int H, int W, int Ho, int Wo, int C, int cg_t,

@@ -259,7 +259,7 @@ int grid_for(long long work, int per_block) {
 
 // ---- S > 1, K <= 32: register-resident class columns -----------------------------------------------
 // The one-thread-per-position kernels above read a 2- or 4-byte element per load and pass over the K classes two or
-// three times: too few bytes in flight (0.28-0.43 of the HBM rate at [16, 21, 512, 512]). Here a thread owns V = 8 /
+// three times: too few bytes in flight to stream at the HBM rate. Here a thread owns V = 8 /
 // sizeof(T) consecutive positions, issues its K 8-byte loads back to back into registers (KMAX of them, -inf beyond
 // K) and computes max, sum of exponentials, the target logit and - backward - the gradient from those registers:
 // the logits are read from HBM exactly once and every store is a full 8-byte (logits) / 16-byte (fp32 loss) vector.

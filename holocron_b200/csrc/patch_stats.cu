@@ -3,7 +3,7 @@
 // The reference materialises the N x L x (Cin*k*k) im2col tensor (9x the input) and makes two reduction passes over it.
 // Here: one streaming pass reduces every input pixel over its channels (s1 = sum x, s2 = sum x^2), then every output pixel
 // adds the kh*kw window entries of those two maps: mean = S1/K, var = S2/K - mean^2. The convolution itself runs on the
-// tcgen05 kernel with the standardisation folded into its epilogue (hb_conv_args.norm_*).
+// implicit-GEMM tensor-core kernel (conv_fprop.cu) with the standardisation folded into its epilogue (hb_conv_args.norm_*).
 #include "common.cuh"
 
 namespace {

@@ -31,8 +31,8 @@ struct HardMishBwd {
   }
 };
 // kFast (16-bit storage types): MUFU log / reciprocal. The argument is >= 1, where __logf is within 2^-21.4 absolute
-// error, 2^7 times finer than the bf16 / fp16 rounding of the result; IEEE logf made the forward pass instruction bound
-// (0.56 of the HBM rate). fp32 tensors keep logf and IEEE division.
+// error, 2^7 times finer than the bf16 / fp16 rounding of the result; IEEE logf makes the forward pass instruction bound.
+// fp32 tensors keep logf and IEEE division.
 template <bool kFast>
 struct NLReluFwd {
   float beta;

@@ -4,8 +4,7 @@
 //   global average pooling:   y[n,c] = mean_p x[n,p,c]                          (the squeeze; also the classifier heads)
 // NHWC bf16 activations, fp32 gate / accumulation. One CTA per (image, channel slab): the per-image reductions need no
 // atomics (deterministic) and 256 images x slabs CTAs fill the GPU. Replaces, per SE block and step, a broadcast multiply,
-// an activation pass, two multiplies + a reduction in backward and a one-thread-per-(n, 8 channels) pooling walk
-// (profiles/r01_rexnet_launches.md: ~4 ms of a 41 ms ReXNet-1.0x step).
+// an activation pass, two multiplies + a reduction in backward and a one-thread-per-(n, 8 channels) pooling walk.
 #include "common.cuh"
 #include "act.cuh"
 

@@ -1,9 +1,10 @@
-// sm_100a building blocks for the tensor-core kernels: mbarrier, TMA (tiled + im2col), tcgen05
-// (alloc / mma / commit / ld) and shared-memory matrix descriptors. Inline PTX only.
+// sm_90a building blocks for the tensor-core kernels: mbarrier, TMA (tiled + im2col), wgmma fences and
+// shared-memory matrix descriptors. Inline PTX only.
 #pragma once
 #include <cuda.h>
 #include <cuda_runtime.h>
 #include <stdint.h>
+#include "wgmma.cuh"
 
 namespace tc {
 
@@ -81,90 +82,37 @@ __device__ __forceinline__ void tma_load_im2col_4d(const CUtensorMap* m, uint64_
       : "memory");
 }
 
-// ---- tcgen05 --------------------------------------------------------------------------------
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t ncols) {
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(ncols)
-               : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
+// ---- wgmma -----------------------------------------------------------------------------------
+// Ordering of the accumulator registers against the asynchronous warpgroup MMAs (all four are warpgroup-wide).
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator reads / writes across a wgmma wait
+template <int N>
+__device__ __forceinline__ void fence_regs(float (&r)[N]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t ncols) {
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(ncols) : "memory");
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], bf16/f16 inputs, fp32 accumulate; issued by ONE thread.
-__device__ __forceinline__ void umma_f16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, bool accumulate) {
-  uint32_t acc = accumulate ? 1u : 0u;
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(acc)
-      : "memory");
-}
-// Lean issue form: descriptors passed as (lo, hi) 32-bit halves so that the per-MMA work of the single issuing thread is
-// one 32-bit add per operand (the address lives in the low word). The first kernels rebuilt both 64-bit descriptors
-// for every MMA: ~30 dependent ALU instructions = ~190 cycles per tcgen05.mma issued, which made every layer
-// issue-bound regardless of N (measured: 185-250 cycles per MMA for N = 48 ... 256).
-__device__ __forceinline__ void umma_f16_lh(uint32_t tmem_d, uint32_t a_lo, uint32_t a_hi, uint32_t b_lo, uint32_t b_hi,
-                                            uint32_t idesc, uint32_t accumulate) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t.reg .b64 da, db;\n\t"
-      "mov.b64 da, {%1, %2};\n\t"
-      "mov.b64 db, {%3, %4};\n\t"
-      "setp.ne.b32 p, %6, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], da, db, %5, p;\n\t}"
-      ::"r"(tmem_d), "r"(a_lo), "r"(a_hi), "r"(b_lo), "r"(b_hi), "r"(idesc), "r"(accumulate)
-      : "memory");
-}
-// high word of a shared-memory descriptor: SBO>>4 | version 1 (bit 46) | layout (bits 61..63)
-__device__ __forceinline__ uint32_t desc_hi(uint32_t sbo_bytes, uint32_t layout) {
-  return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 14) | ((layout & 7) << 29);
-}
-// low word: start>>4 | LBO>>4 << 16; advancing the start by X bytes = adding X>>4
+// ---- descriptors ----------------------------------------------------------------------------
+// Shared-memory matrix descriptor of wgmma (sm_90):
+//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset | [62,64) layout (1 = 128B swizzle)
+// The 128-byte swizzle is a function of the absolute shared-memory address (the TMA writes it that way), so a
+// descriptor may start at any 128-byte row of a 1024-byte aligned buffer and advancing along K inside a row is a plain
+// address add: the low word carries the address, the high word (SBO, layout) stays fixed.
+//   K-major operand (rows = M or N, 128-byte rows of 64 K elements): SBO = 1024 (8-row atom), LBO unused.
+//   MN-major operand (rows = K, 128-byte rows of 64 M/N elements): SBO = 1024 (next 8 K rows), LBO = distance
+//   between 64-element atoms along M/N.
+__device__ __forceinline__ uint32_t desc_hi(uint32_t sbo_bytes) { return ((sbo_bytes >> 4) & 0x3FFF) | (1u << 30); }
 __device__ __forceinline__ uint32_t desc_lo(uint32_t saddr, uint32_t lbo_bytes) {
   return ((saddr >> 4) & 0x3FFF) | (((lbo_bytes >> 4) & 0x3FFF) << 16);
 }
+__device__ __forceinline__ uint64_t make_desc(uint32_t lo, uint32_t hi) { return ((uint64_t)hi << 32) | lo; }
 
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread have completed.
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: this warp's 32 lanes x 16 consecutive fp32 columns (thread i gets lane i).
-__device__ __forceinline__ void tmem_ld_x16(uint32_t taddr, uint32_t* r) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]), "=r"(r[8]),
-        "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
-
-// ---- descriptors ----------------------------------------------------------------------------
-// Shared-memory matrix descriptor (cute::UMMA::SmemDescriptor bit layout, sm_100 "version 1"):
-//   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [46,48) version=1 | [49,52) base offset | [61,64) layout
-// layout: 0 none, 2 = 128B swizzle, 4 = 64B, 6 = 32B.
-__device__ __forceinline__ uint64_t make_smem_desc(uint32_t saddr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t layout) {
-  uint64_t d = 0;
-  d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-  d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
-  d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(layout & 7) << 61;
-  return d;
-}
-constexpr uint32_t kLayoutSW128 = 2;
-
-// Instruction descriptor for kind::f16 (cute::UMMA::InstrDescriptor): bf16 x bf16 -> fp32.
-//   [4,6) c_format=1 (F32) | [7,10) a_format=1 (BF16) | [10,13) b_format=1 | [15] a_major | [16] b_major
-//   [17,23) N>>3 | [24,29) M>>4         (major: 0 = K-major, 1 = MN-major)
-__host__ __device__ __forceinline__ uint32_t make_idesc_bf16(int M, int N, int a_mn_major, int b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(a_mn_major & 1) << 15) | ((uint32_t)(b_mn_major & 1) << 16) |
-         ((uint32_t)(N >> 3) << 17) | ((uint32_t)(M >> 4) << 24);
-}
+// Accumulator fragment of an m64nN wgmma: register i of thread t holds row  16*(warp of t) + lane/4 (+8 when i & 2)
+// and column  8*(i/4) + 2*(lane%4) + (i & 1)  of the warpgroup's 64-row tile.
+__device__ __forceinline__ int frag_row(int t) { return ((t >> 5) & 3) * 16 + ((t & 31) >> 2); }
+__device__ __forceinline__ int frag_col(int t) { return (t & 3) * 2; }
 
 }  // namespace tc

@@ -1,6 +1,6 @@
 """CUDA-graph capture of a whole training step (forward + loss + backward + gradient all-reduce + optimizer).
 
-The reference has no counterpart (it is eager PyTorch); this is the B200-side answer to the ~650 kernel launches and
+The reference has no counterpart (it is eager PyTorch); this is the device-side answer to the ~650 kernel launches and
 the Python / autograd bookkeeping of one RepVGG step: the step is captured ONCE into a ``torch.cuda.CUDAGraph`` and
 replayed, so the host cost per step is one graph launch. Requirements (all met by this package's ops):
 

@@ -4,7 +4,7 @@ The reference builds every backbone from ``conv_sequence`` lists ``[Conv2d, Batc
 in ``nn.Sequential`` (holocron/models/utils.py:28-86). The model files of this package keep exactly those module trees
 (so ``state_dict`` keys and the init RNG order are unchanged) but use :class:`FusedSequential`, whose ``forward`` walks the
 stack and maps every ``conv -> BN -> act`` run onto
-  * the tcgen05 implicit-GEMM convolution (dense) or the depth-wise kernel (``groups == channels``), and
+  * the wgmma implicit-GEMM convolution (dense) or the depth-wise kernel (``groups == channels``), and
   * ONE fused normalise/(residual)/activate pass (+ one statistics pass in training),
 instead of 3-4 separate library kernels. Anything it does not recognise is simply called.
 """

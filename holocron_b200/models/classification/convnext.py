@@ -4,7 +4,7 @@ LayerScale :44-52, Bottlenext :55-109, ConvNeXt :112-189, factories :223-401).
 Block = 7x7 depth-wise conv (+bias) -> LayerNorm over channels -> 1x1 expand x4 (+bias) -> GELU -> 1x1 project (+bias) ->
 per-channel LayerScale -> stochastic depth -> + identity. What runs where:
   * 7x7 depth-wise: the depth-wise CUDA kernels (`csrc/dwconv.cu`, channels % 8 == 0 - true for every factory);
-  * the two 1x1 convolutions (all of the block's FLOPs) and the 4x4 / 2x2 patchify convolutions: tcgen05 implicit GEMM with
+  * the two 1x1 convolutions (all of the block's FLOPs) and the 4x4 / 2x2 patchify convolutions: wgmma implicit GEMM with
     the bias in the epilogue;
   * LayerNorm, GELU, LayerScale, the residual addition: library element-wise / row kernels on the NHWC tensor (LayerNorm over
     the innermost dimension of a channels_last tensor is a plain row normalisation, no permute copy).

@@ -4,7 +4,7 @@ PointConvBlock :94-147, MobileOneBlock :150-177, MobileOne :180-230, factories :
 The re-parametrisable sibling of RepVGG: a block is ``act(sum of BatchNorm'd depth-wise branches)`` followed by
 ``act(sum of BatchNorm'd 1x1 branches)`` - an identity BatchNorm (when shapes allow), a depth-wise 1x1 "scale" branch and
 ``overparam_factor`` 3x3 / 1x1 branches. Module tree, parameter names and init order are the reference's. Every branch
-convolution runs on the depth-wise / tcgen05 kernels and ALL BatchNorms of a branch sum plus the activation are folded into
+convolution runs on the depth-wise / tensor-core kernels and ALL BatchNorms of a branch sum plus the activation are folded into
 fused passes of at most three branches each (the running sum of the previous pass enters the next one as its residual); the
 reference issues one BatchNorm kernel per branch, ``len(branches) - 1`` additions and the activation.
 ``reparametrize()`` folds every branch into one convolution with a bias exactly like the reference (host-side, fp32)."""

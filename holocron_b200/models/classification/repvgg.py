@@ -1,11 +1,11 @@
-"""RepVGG on the B200 kernels — API mirror of holocron/models/classification/repvgg.py.
+"""RepVGG on the H100 kernels — API mirror of holocron/models/classification/repvgg.py.
 
 Same module tree / ``state_dict`` keys as the reference (``features.<stage>.<block>.branches.{0,1}.{0,1}.*``,
 ``features.<stage>.<block>.branches.2.*`` for the identity BN, ``head.*``; after ``reparametrize()``:
 ``...branches.weight/.bias``), same constructor arguments and the same RNG call order at init, so parameters are
 interchangeable with the reference and ``torch.manual_seed(s)`` gives identical weights.
 
-What differs is the execution: a train-form block is two tcgen05 implicit-GEMM convolutions (3x3 and 1x1) over
+What differs is the execution: a train-form block is two wgmma implicit-GEMM convolutions (3x3 and 1x1) over
 bf16 NHWC activations, one statistics pass and ONE fused pass that normalises the three branches, sums them and
 applies the activation (reference: 2 cuDNN convs + 3 BatchNorm kernels + 2 adds + ReLU). A re-parametrised block
 is a single convolution with bias and ReLU fused in its epilogue.

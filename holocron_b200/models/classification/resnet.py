@@ -5,7 +5,7 @@ Module tree, parameter names and init order are the reference's (``state_dict`` 
 ``conv -> BN -> act`` units (:mod:`holocron_b200.models._blocks`); the shortcut addition and the block's final activation are
 folded into the last unit's normalisation pass, ``act(BN(conv(.)) + identity)`` - the reference's ``out += identity`` and
 activation are two more tensor passes. Grouped 3x3 convolutions (ResNeXt) are a library call, everything else is on the
-tcgen05 kernels; the 7x7 stem takes the implicit-GEMM path, ResNet-D's 3x3 stem the im2col one."""
+tensor-core kernels; the 7x7 stem takes the implicit-GEMM path, ResNet-D's 3x3 stem the im2col one."""
 from collections import OrderedDict
 from typing import Any, Callable, Dict, List, Optional, Type, Union
 

@@ -7,8 +7,8 @@ of 16 channels *between* the fused ops (filters are packed with zero rows/column
 ``scale = shift = 0``): padded channels stay exactly zero through conv, BN, SiLU/ReLU6, the depth-wise conv and the
 partial-channel shortcut, and gradients of the padding never reach a parameter.
 
-Per block: 1x1 expand (tcgen05) -> fused BN+SiLU -> depth-wise 3x3 kernel -> fused BN -> [SE gate from the pooled map]
--> ReLU6 -> 1x1 project (tcgen05) -> fused BN (+ shortcut on the first ``in_channels`` channels, reference rexnet.py:141).
+Per block: 1x1 expand (tensor cores) -> fused BN+SiLU -> depth-wise 3x3 kernel -> fused BN -> [SE gate from the pooled map]
+-> ReLU6 -> 1x1 project (tensor cores) -> fused BN (+ shortcut on the first ``in_channels`` channels, reference rexnet.py:141).
 """
 import functools
 import operator

@@ -4,7 +4,7 @@ Tridentneck :62-134, _tridentnet :137-153, tridentnet50 :156-167).
 The network carries three scale branches side by side on the channel axis (``ChannelRepeat(3)`` behind the stem); a
 ``TridentConv2d`` applies ONE filter to each third of the channels, with dilations 1 / 2 / 3 for the 3x3 layers, and the
 BatchNorm that follows spans all ``3 x width`` channels. Here the dilation-1 chunks (all 1x1 layers and the first branch of
-every 3x3 layer) run on the tcgen05 convolution, the dilated chunks are library calls, and normalisation + activation
+every 3x3 layer) run on the tensor-core convolution, the dilated chunks are library calls, and normalisation + activation
 (+ shortcut) is one fused pass over the concatenated tensor."""
 from typing import Any, Callable, List, Optional
 

@@ -1,7 +1,7 @@
 """YOLOv2 on the fused kernels — API mirror of holocron/models/detection/yolov2.py (YOLOv2 :29-259, yolov2 :287-321).
 
 Module tree / ``state_dict`` / init order are the reference's (``backbone`` = ``DarknetBodyV2`` with the pass-through route,
-``block5``, ``passthrough_layer``, ``block6``, ``head``, buffer ``anchors``). The conv-BN-LeakyReLU units run on the tcgen05
+``block5``, ``passthrough_layer``, ``block6``, ``head``, buffer ``anchors``). The conv-BN-LeakyReLU units run on the tensor-core
 convolution + fused normalise/activate pass; the 125-channel output convolution is zero-padded to 128 channels inside the
 conv binding; the pass-through ``ConcatDownsample2d`` and the channel concatenation are pure data movement. The losses are
 the sync-free per-box formulation of :class:`holocron_b200.models.detection.yolo._YOLO` (classification term over every

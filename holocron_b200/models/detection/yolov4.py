@@ -2,7 +2,7 @@
 
 Module tree / ``state_dict`` / init order are the reference's (backbone = ``DarknetBodyV4``, ``neck.fpn/pan1/pan2``,
 ``head.head1 ... head.yolo3``). All conv-BN-Mish(-DropBlock) units run through :mod:`holocron_b200.models._blocks`
-(tcgen05 convolution + fused normalise/activate pass, DropBlock kernel without host sync); the 255-channel output
+(tensor-core convolution + fused normalise/activate pass, DropBlock kernel without host sync); the 255-channel output
 convolutions are padded to 256 channels inside the conv binding. The YOLO layer's box decoding, target assignment and
 losses follow reference yolov4.py:269-420 using the fused pairwise box kernels of :mod:`holocron_b200.ops.boxes`
 (``ciou_loss`` == DIoU loss, reference quirk; the "ignore" masking of yolov4.py:386 writes to a copy and is therefore

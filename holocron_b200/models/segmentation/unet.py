@@ -2,7 +2,7 @@
 UNetBackbone :104-137, UNet :140-226, UBlock :229-279, DynamicUNet :282-370, factories :373-513).
 
 Same module trees / ``state_dict`` as the reference. Every ``conv3x3 -> [norm] -> act`` unit of the contracting, bridge and
-expansive paths runs on the tcgen05 implicit-GEMM kernel + the fused normalise / activate pass; max-pooling, bilinear / nearest
+expansive paths runs on the wgmma implicit-GEMM kernel + the fused normalise / activate pass; max-pooling, bilinear / nearest
 up-sampling, ``PixelShuffle``, transposed convolutions, cropping and channel concatenation are resampling / data-movement ops
 left to the library (they act on the same bf16 channels_last tensors). ``DynamicUNet`` needs the channel counts of its encoder's
 feature maps at construction time; the reference finds them by running the encoder on a CPU tensor - here the encoder is walked

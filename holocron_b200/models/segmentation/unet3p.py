@@ -1,7 +1,7 @@
 """UNet3+ on the fused kernels — API mirror of holocron/models/segmentation/unet3p.py (+ ``down_path`` of unet.py:36-55).
 
 Same module tree / ``state_dict`` as the reference. Every 3x3 convolution (encoder conv-BN-ReLU pairs, the 64-channel
-branch convolutions of each full-scale aggregation, the 320-channel fusion conv-BN-ReLU) runs on the tcgen05
+branch convolutions of each full-scale aggregation, the 320-channel fusion conv-BN-ReLU) runs on the tensor-core
 implicit-GEMM kernel; max-pooling, bilinear up-sampling and channel concatenation are bandwidth-trivial resampling ops
 left to torch (they operate on the same bf16 channels_last tensors, no layout changes)."""
 from typing import Any, Callable, List, Optional

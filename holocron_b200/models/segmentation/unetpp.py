@@ -3,7 +3,7 @@ factories :193-238).
 
 Nested U-Nets (https://arxiv.org/abs/1912.05074): a triangular grid of ``UpPath`` cells; UNet+ feeds each cell the previous
 cell of its row, UNet++ every previous cell of its row (dense skip connections). Same module trees / ``state_dict`` as the
-reference; all conv units run on the tcgen05 convolution + fused normalise / activate pass (see :mod:`.unet`)."""
+reference; all conv units run on the tensor-core convolution + fused normalise / activate pass (see :mod:`.unet`)."""
 from typing import Any, Callable, List, Optional
 
 from torch import Tensor, nn

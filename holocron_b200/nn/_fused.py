@@ -9,6 +9,7 @@ Reference call sites being replaced: ``nn.Conv2d`` / ``nn.BatchNorm2d`` / activa
 (holocron/models/classification/repvgg.py:71-73).
 """
 import ctypes
+import functools
 import os
 import weakref
 from typing import List, Optional, Sequence, Tuple
@@ -51,16 +52,27 @@ def conv_work(m_out: int, cout: int, k_total: int, in_elems: int, w_elems: int, 
 
 
 # ---- column statistics travelling with a tensor (training-mode BatchNorm without a statistics pass) ----
-CONV_STAT_SLOTS = 2 * 148      # conv epilogues: 2 epilogue groups x (<= one CTA per SM)
-BN_STAT_SLOTS = 4 * 148        # streaming kernels: <= 4 blocks per SM
+@functools.lru_cache(maxsize=None)
+def _sm_count(index: int) -> int:
+    return torch.cuda.get_device_properties(index).multi_processor_count
+
+
+def conv_stat_slots(device) -> int:
+    """Statistics slots of a convolution epilogue: 2 consumer warpgroups x (<= one CTA per SM)."""
+    return 2 * _sm_count(torch.device(device).index or 0)
+
+
+def bn_stat_slots(device) -> int:
+    """Statistics slots of the streaming BatchNorm kernels: <= 4 blocks per SM."""
+    return 4 * _sm_count(torch.device(device).index or 0)
 
 
 def epilogue_stats_pay_off(k_total: int) -> bool:
-    """Whether the convolution epilogue should also produce the BatchNorm statistics of its output. The epilogue
-    warps have slack only on layers whose tile time is set by the tensor pipe (K = R*S*Cin large); on the narrow layers
-    (48 .. 96 channels) the epilogue IS the critical path and the extra shared-memory pass costs more than the stand-alone
-    statistics kernel it replaces (measured on RepVGG-A0, batch 256: +1.7 ms vs -0.5 ms per step when applied to every
-    layer). HB_FORCE_CONV_STATS / HB_DISABLE_CONV_STATS override."""
+    """Whether the convolution epilogue should also produce the BatchNorm statistics of its output. The extra
+    shared-memory pass over the staged tile is cheap next to the main loop only where the tile time is set by the tensor
+    pipe (K = R*S*Cin large); on the narrow layers (48 .. 96 channels) it lengthens the epilogue, which the consumer
+    warpgroups run after their MMAs. The K >= 1024 threshold has not been re-tuned on the H100.
+    HB_FORCE_CONV_STATS / HB_DISABLE_CONV_STATS override."""
     if os.environ.get("HB_DISABLE_CONV_STATS"):
         return False
     if os.environ.get("HB_FORCE_CONV_STATS"):
@@ -361,10 +373,10 @@ def conv2d_forward_raw(x: Tensor, wf: Tensor, cout: int, r: int, s: int, stride:
         a.norm_mean, a.norm_rstd, a.norm_wsum = norm[0].data_ptr(), norm[1].data_ptr(), norm[2].data_ptr()
     st = st2 = None
     if want_stats:
-        st = torch.empty((CONV_STAT_SLOTS, cout, 2), device=x.device, dtype=torch.float32)
+        st = torch.empty((conv_stat_slots(x.device), cout, 2), device=x.device, dtype=torch.float32)
         a.stats = st.data_ptr()
         if w2 is not None:
-            st2 = torch.empty((CONV_STAT_SLOTS, cout, 2), device=x.device, dtype=torch.float32)
+            st2 = torch.empty((conv_stat_slots(x.device), cout, 2), device=x.device, dtype=torch.float32)
             a.stats2 = st2.data_ptr()
     slots = ctypes.c_int(0)
     info = dict(shape=(kind, h, cin_p, cout, r, stride), launches=1,
@@ -372,7 +384,7 @@ def conv2d_forward_raw(x: Tensor, wf: Tensor, cout: int, r: int, s: int, stride:
     check(_timed(kind, info, lambda: lib().hb_conv2d_fused_bf16(ctypes.byref(a), ctypes.byref(slots), stream_ptr())),
           "hb_conv2d_fused_bf16")
     if want_stats:
-        if slots.value > CONV_STAT_SLOTS:
+        if slots.value > st.shape[0]:
             raise RuntimeError("statistics slot capacity exceeded")
         attach_stats(y, st, slots.value)
         if y2 is not None:
@@ -381,7 +393,7 @@ def conv2d_forward_raw(x: Tensor, wf: Tensor, cout: int, r: int, s: int, stride:
 
 
 class _Conv2dFn(torch.autograd.Function):
-    """y = conv2d(x, weight) (+ bias) on the tcgen05 implicit-GEMM kernels; backward = dgrad + wgrad kernels.
+    """y = conv2d(x, weight) (+ bias) on the wgmma implicit-GEMM kernels; backward = dgrad + wgrad kernels.
 
     Channel counts that do not fit the kernels' granularity are zero-padded internally: the input to a multiple of 8
     (or whatever padded width the incoming activation already has), the output to a multiple of 16. With
@@ -398,8 +410,8 @@ class _Conv2dFn(torch.autograd.Function):
         if (cin <= 4 and x.shape[1] == cin and r == 3 and s == 3 and pad == 1 and dil == 1 and not need_dx and x.is_contiguous()
                 and x.dtype in DTYPE_CODE and cout % 16 == 0 and not os.environ.get("HB_DISABLE_STEM_IM2COL")):
             # network stem (3 input channels): one explicit im2col pass (27 -> 32 columns), then a dense 1x1 GEMM over it. The
-            # implicit-GEMM path pads 3 channels to 8-16 and fetches 9 x 32-byte pixels per output through TMA im2col: 1.36 ms
-            # for ReXNet's 224^2 stem at batch 256 (0.27 TB/s), 5 % of its training step.
+            # implicit-GEMM path pads 3 channels to 8-16 and fetches 9 x 32-byte pixels per output through TMA im2col, far below
+            # the HBM rate.
             col, wp = _stem_im2col_single(x, weight, stride)
             y = conv2d_forward_raw(col, wp, cout, 1, 1, 1, 0, 1, _pad_vec(bias, cout),
                                    want_stats=want_stats and epilogue_stats_pay_off(col.shape[1]))
@@ -464,7 +476,7 @@ class _Conv2dFn(torch.autograd.Function):
 
 def conv2d(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, stride: int = 1, padding: int = 0,
            dilation: int = 1, keep_padded: bool = False, want_stats: bool = False) -> Tensor:
-    """Dense (groups=1) 2-D convolution on the sm_100a tensor cores; returns bf16 channels_last."""
+    """Dense (groups=1) 2-D convolution on the sm_90a tensor cores; returns bf16 channels_last."""
     require_cuda(x, weight)
     return _Conv2dFn.apply(x, weight, bias, int(stride), int(padding), int(dilation), bool(keep_padded), bool(want_stats))
 
@@ -557,7 +569,7 @@ def _bn_batch_stats(us: Sequence[Tensor], branches, g32, b32, stats: Tensor, c: 
     for u in us:
         st = get_stats(u)
         if st is None:
-            buf = torch.empty((BN_STAT_SLOTS, c, 2), device=u.device, dtype=torch.float32)
+            buf = torch.empty((bn_stat_slots(u.device), c, 2), device=u.device, dtype=torch.float32)
             sl = ctypes.c_int(0)
             check(_timed("bn_stats", _elem_bytes_info("bn_stats", m, c, 1, 0), lambda: L.hb_bn_stats_partials_bf16(
                 ptr(u), m, c, ptr(buf), ctypes.byref(sl), stream_ptr())), "hb_bn_stats_partials_bf16")
@@ -586,7 +598,7 @@ def _bn_forward_pass(us: Sequence[Tensor], stats: Tensor, res: Optional[Tensor],
     if emit_stats and os.environ.get("HB_DISABLE_BN_OUT_STATS"):    # A/B switch
         emit_stats = False
     out = _empty_cl(n, c, h, w, dev)
-    ost = torch.empty((BN_STAT_SLOTS, c, 2), device=dev, dtype=torch.float32) if emit_stats else None
+    ost = torch.empty((bn_stat_slots(dev), c, 2), device=dev, dtype=torch.float32) if emit_stats else None
     sl = ctypes.c_int(0)
     up = [ptr(us[i]) if i < nb else ptr(None) for i in range(3)]
     check(_timed("bn_fwd", _elem_bytes_info("bn_fwd", m, c, nb + (res is not None), 1), lambda: lib().hb_bn_act_fwd_bf16(
@@ -726,7 +738,7 @@ class _RepBlockFn(torch.autograd.Function):
     """Train-form RepVGG block as ONE autograd node:  out = act(BN3(conv3x3(x)) + BN1(conv1x1(x)) [+ BNid(x)]).
 
     Forward: ONE tensor-core launch computes both branches from a single read of x (the 1x1 branch re-uses the centre-tap
-    loads of the 3x3 branch, second TMEM accumulator) and its epilogue also produces the BatchNorm statistics of both
+    loads of the 3x3 branch into a second accumulator) and its epilogue also produces the BatchNorm statistics of both
     outputs; the identity branch's statistics arrive with x from the previous block's forward pass. Then one C-sized
     finalisation and ONE fused pass that normalises the branches, sums them, applies the activation and accumulates the
     statistics of its own output for the next block (reference: 2 cuDNN convs + 3 BatchNorm kernels + 2 adds + ReLU).
@@ -749,9 +761,9 @@ class _RepBlockFn(torch.autograd.Function):
         if cout % 16 != 0:
             raise NotImplementedError("fused RepBlock needs out_channels % 16 == 0")
         stem = cin <= 4 and x.shape[1] == cin and not need_dx and x.is_contiguous() and x.dtype in DTYPE_CODE
-        # Dual-output launch (x read once, 1x1 branch from the centre-tap loads): correct and tested, but on B200 it loses to
-        # two launches - the second accumulator halves the Cout tile of the wide layers (N = 96 MMAs cost as much as N = 128)
-        # and doubles the per-tile epilogue work of the narrow ones, whose epilogue is the critical path. Opt-in (A/B).
+        # Dual-output launch (x read once, 1x1 branch from the centre-tap loads): correct and tested, opt-in (A/B). The two
+        # accumulators share the 128-column register budget, so each output's Cout tile is capped at 64 columns (twice the
+        # tiles on the wide layers) and every tile runs two epilogues; two launches are the default. Not measured on the H100.
         fused_fwd = bool(os.environ.get("HB_FUSED_FPROP"))
         if stem:
             # network stem: explicit im2col once (27 -> 32 columns), both branches become dense GEMMs over it

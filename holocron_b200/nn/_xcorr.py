@@ -1,13 +1,13 @@
 """norm_conv2d / add2d (holocron/nn/functional.py:322-462).
 
-``norm_conv2d`` is a dense contraction: it runs on the tcgen05 implicit-GEMM convolution (bf16 operands, fp32 accumulation)
+``norm_conv2d`` is a dense contraction: it runs on the wgmma implicit-GEMM convolution (bf16 operands, fp32 accumulation)
 with the per-patch standardisation folded algebraically into the epilogue,
 
     out[m, co] = rstd[m] * (conv(x, w)[m, co] - mean[m] * sum_k w[co, k]) + bias[co],
 
 the patch statistics coming from one streaming pass over x (``hb_patch_stats_bf16``); nothing like the reference's
 ``N x L x Cin*k*k`` im2col tensor exists. ``HB_NORMCONV_FP32=1`` selects the fp32 CUDA-core kernel instead (bit-level
-closeness to the fp32 reference, ~30x slower). ``add2d`` has no multiplications (L1 distance): it stays on the fp32
+closeness to the fp32 reference, far slower). ``add2d`` has no multiplications (L1 distance): it stays on the fp32
 CUDA-core tile kernel of ``csrc/xcorr.cu``; so do the weight gradients of both ops."""
 import ctypes
 import os
@@ -89,7 +89,7 @@ class _XcorrFn(torch.autograd.Function):
 
 def _norm_conv_tensor_cores(x32: Tensor, weight: Tensor, b32: Optional[Tensor], mean: Tensor, rstd: Tensor, stride: int,
                             pad: int, dil: int, eps: float) -> Tensor:
-    """Forward of norm_conv2d on the tcgen05 kernel; fills ``mean`` / ``rstd`` (per output pixel) for the backward pass."""
+    """Forward of norm_conv2d on the tensor-core kernel; fills ``mean`` / ``rstd`` (per output pixel) for the backward pass."""
     from . import _fused as K
     n, cin, h, w = x32.shape
     cout, _, k, _ = weight.shape

@@ -1,6 +1,6 @@
 """Functional API mirroring ``holocron.nn.functional`` (reference holocron/nn/functional.py) for the hot-path ops.
 
-Every function here launches the sm_100a kernels of ``libholocron_b200.so`` through the C ABI; inputs must be CUDA
+Every function here launches the sm_90a kernels of ``libholocron_b200.so`` through the C ABI; inputs must be CUDA
 tensors (there is no CPU fallback — the CPU restatement lives in ``oracle/`` and is test-only).
 """
 from typing import Optional

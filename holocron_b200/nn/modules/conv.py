@@ -63,7 +63,7 @@ class SlimConv2d(nn.Module):
     x*flip(w), a k x k conv on top and a 1x1 + k x k on the bottom, concatenated to 3C/4 channels.
 
     Children ``fc1, bn, fc2, conv_top, conv_bot1, conv_bot2`` as in the reference. The three spatial convolutions run on
-    the tcgen05 implicit-GEMM kernel whenever their channel counts allow it (out_channels % 16 == 0), the squeeze path
+    the wgmma implicit-GEMM kernel whenever their channel counts allow it (out_channels % 16 == 0), the squeeze path
     works on (N, C, 1, 1) tensors and stays in torch.
     """
 
@@ -107,7 +107,7 @@ class PyConv2d(nn.ModuleList):
     """Pyramidal convolution (https://arxiv.org/abs/2006.11538) — reference conv.py:373-438: ``num_levels`` parallel
     convolutions of growing kernel size (k, k + 2, ...) and group count over the same input, concatenated on the channel axis.
     Same children (``state_dict`` keys ``0.weight``, ``1.weight``, ...). The levels run through the conv unit executor: dense
-    levels on the tcgen05 kernel, grouped ones as a library call on the activation dtype."""
+    levels on the tensor-core kernel, grouped ones as a library call on the activation dtype."""
 
     def __init__(self, in_channels: int, out_channels: int, kernel_size: int, num_levels: int = 2, padding: int = 0,
                  groups: Optional[List[int]] = None, **kwargs: Any) -> None:

@@ -1,4 +1,4 @@
-/* holocron_b200 — C ABI of the B200 (sm_100a) kernels behind the holocron.nn / holocron.ops / holocron.optim
+/* holocron_b200 — C ABI of the H100 (sm_90a) kernels behind the holocron.nn / holocron.ops / holocron.optim
  * hot path of frgfm/Holocron.
  *
  * The reference is pure Python/PyTorch and has no FFI of its own (SURVEY.md §8b): every entry point below replaces
@@ -31,7 +31,7 @@ int hb_nl_relu_bwd(const void* x, const void* dy, void* dx, size_t n, float beta
 /* backward of the in-place variant, from the OUTPUT y = log(1 + beta*relu(x)) */
 int hb_nl_relu_bwd_from_out(const void* y, const void* dy, void* dx, size_t n, float beta, int dtype, void* stream);
 
-/* ---- dense convolutions (tcgen05 implicit GEMM): nn.Conv2d call sites of holocron/models/utils.py:71-76
+/* ---- dense convolutions (wgmma implicit GEMM): nn.Conv2d call sites of holocron/models/utils.py:71-76
  *      (conv_sequence), models/classification/repvgg.py:55-73 (RepBlock) and their autograd backward -------- */
 /* y[N,Ho,Wo,Cout] = act(conv(x[N,H,W,Cin], w[Cout,R,S,Cin]) + bias + residual); Cin % 8 == 0, Cout % 16 == 0.
  * bias: fp32 [Cout] or NULL; residual: bf16 like y or NULL; act: 0 none, 1 relu; num_ctas: 0 = one per SM. */

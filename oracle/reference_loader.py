@@ -1,19 +1,20 @@
-"""Imports the UNMODIFIED reference (frgfm/Holocron) from /root/reference as ``holocron.*`` modules.
+"""Imports the UNMODIFIED reference (frgfm/Holocron) as ``holocron.*`` modules from the checkout named by the
+``HOLOCRON_REFERENCE`` environment variable.
 
-Only usable in the build container (the reference tree does not exist on the GPU box). Used by
-``tests/golden/make_golden.py`` to generate the committed golden fixtures, and by the optional
-``tests/test_oracle_vs_reference.py`` cross-check, which skips itself when the tree is absent.
+Used by ``tests/golden/make_golden.py`` to generate the committed golden fixtures (the tests themselves only read those
+fixtures and never need the reference).
 
 ``import holocron`` itself fails in this image (its __init__ pulls matplotlib/fastprogress and a generated
 version.py), so a stub parent package whose __path__ points at the reference is pre-seeded and the needed
 sub-packages are imported directly.
 """
 import importlib
+import os
 import sys
 import types
 from pathlib import Path
 
-REFERENCE_ROOT = Path("/root/reference")
+REFERENCE_ROOT = Path(os.environ.get("HOLOCRON_REFERENCE", "holocron-reference"))
 
 
 def available() -> bool:
@@ -23,7 +24,7 @@ def available() -> bool:
 def load():
     """Returns the stub ``holocron`` package with nn, ops, optim and models imported from the reference."""
     if not available():
-        raise RuntimeError("reference tree not available at /root/reference")
+        raise RuntimeError(f"reference tree not available at {REFERENCE_ROOT} (set HOLOCRON_REFERENCE)")
     existing = sys.modules.get("holocron")
     if existing is not None and getattr(existing, "__holocron_reference__", False):
         return existing

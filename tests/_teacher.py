@@ -2,11 +2,11 @@
 
 A deep random-init network in training mode is ill-conditioned: batch-norm over a handful of samples re-normalises the
 bf16 rounding noise at every layer, and end-to-end outputs of ANY bf16 execution drift from the fp32 fixture (torch's
-own bf16 autocast lands 0.05 - 0.47 rel-L2 away on the Darknet fixtures, see profiles/r01_bf16_conditioning.log). An
+own bf16 autocast lands 0.05 - 0.47 rel-L2 away on the Darknet fixtures). An
 end-to-end tolerance alone therefore says little about kernel correctness. These hooks check, while the model runs,
 EVERY fused launch against fp32 torch library ops applied to the very same input tensors (teacher forcing), so each
 comparison spans exactly one unit and the tolerance can be tight (5e-3 rel-L2; the bf16 output rounding alone
-is ~1.7e-3, which is what every launch of every zoo model measures on B200):
+is ~1.7e-3):
 
   * conv launches   - conv2d_forward_raw (all dense convolutions, incl. the data-gradient launches routed through it)
   * BN/act passes   - bn_act (statistics + normalise + residual + activation)

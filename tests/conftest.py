@@ -12,7 +12,7 @@ GOLDEN = ROOT / "tests" / "golden"
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: test needs a CUDA device (run on the B200 box with `-m gpu`)")
+    config.addinivalue_line("markers", "gpu: test needs a CUDA device (an H100; select with `-m gpu`)")
 
 
 def pytest_collection_modifyitems(config, items):

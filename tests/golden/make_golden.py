@@ -1,12 +1,14 @@
-"""Generates the golden fixtures under tests/golden/ by running the UNMODIFIED reference (frgfm/Holocron,
-mounted read-only at /root/reference) on seeded CPU inputs.  Run in the build container only:
+"""Generates the golden fixtures under tests/golden/ by running the UNMODIFIED reference (frgfm/Holocron, a checkout
+named by the HOLOCRON_REFERENCE environment variable) on seeded CPU inputs:
 
-    python tests/golden/make_golden.py
+    HOLOCRON_REFERENCE=/path/to/Holocron python tests/golden/make_golden.py [--zoo | --ref-modules | ...]
 
 Every fixture is a dict of small tensors (inputs + the reference's outputs / gradients / updated state); the
 tests compare the oracle (CPU) and the CUDA path (GPU) against them.
 """
+import os
 import sys
+import tempfile
 from pathlib import Path
 
 import torch
@@ -331,7 +333,59 @@ if __name__ == "__main__" and "--optim2" in sys.argv:
     print("optim2.pt", (OUT / "optim2.pt").stat().st_size)
 
 
-if __name__ == "__main__" and not any(f in sys.argv for f in ("--zoo", "--zoo-resnet", "--zoo-f3", "--zoo-f3b", "--yolo", "--trainers", "--seg", "--api", "--trainer", "--optim2")):
+def gen_ref_modules():
+    """Outputs of the reference's own modules for the module-level CPU comparisons (tests/test_zoo_wiring_cpu.py,
+    tests/test_host_logic.py, tests/test_formats_cpu.py): PyConv2d / TridentConv2d / ConcatDownsample2d on seeded weights
+    and inputs, Mixup draws, and the parameter layout the reference's hub loader expects for rexnet1_0x."""
+    import importlib.util
+    import types
+    for name in ("matplotlib", "matplotlib.pyplot", "tqdm", "tqdm.auto"):   # plots / progress bars of holocron.utils.misc
+        try:
+            missing = name not in sys.modules and importlib.util.find_spec(name) is None
+        except (ImportError, ValueError):
+            missing = True
+        if missing:
+            stub = types.ModuleType(name)
+            stub.tqdm = lambda it, *a, **k: it
+            sys.modules[name] = stub
+    from holocron.models.classification.tridentnet import TridentConv2d
+    from holocron.utils.data import Mixup
+    d = {"pyconv": [], "trident": []}
+    torch.manual_seed(21)
+    d["pyconv_x"] = torch.rand(2, 8, 16, 16)
+    for kwargs in (dict(num_levels=1), dict(num_levels=2), dict(num_levels=3, groups=[1, 2, 4]), dict(num_levels=4, stride=2)):
+        torch.manual_seed(0)
+        ref = holocron.nn.PyConv2d(8, 16, 3, padding=1, **kwargs)
+        d["pyconv"].append({"kwargs": kwargs, "params": [q.detach().clone() for q in ref.parameters()],
+                            "num_levels": ref.num_levels, "out": ref(d["pyconv_x"]).detach()})
+    torch.manual_seed(22)
+    d["trident_x"] = torch.rand(2, 24, 12, 12)
+    for k, dil in ((1, 1), (3, 3)):
+        torch.manual_seed(1)
+        ref = TridentConv2d(8, 8, k, padding=k // 2, dilation=dil, bias=False)
+        d["trident"].append({"k": k, "dil": dil, "state": ref.state_dict(), "out": ref(d["trident_x"]).detach()})
+    torch.manual_seed(23)
+    d["concat_x"] = torch.rand(2, 6, 8, 12)
+    d["concat_out"] = holocron.nn.ConcatDownsample2d(2)(d["concat_x"])
+    d["mixup"] = []
+    for num_classes, alpha, seed in ((7, 0.2, 0), (7, 1.0, 1), (1, 0.4, 2)):
+        g = torch.Generator().manual_seed(seed)
+        x = torch.rand(6, 3, 5, 5, generator=g)
+        t = torch.randint(0, max(num_classes, 2), (6,), generator=g)
+        torch.manual_seed(100 + seed)
+        xr, tr = Mixup(num_classes, alpha)(x.clone(), t.clone())
+        d["mixup"].append({"num_classes": num_classes, "alpha": alpha, "seed": seed, "x": xr, "t": tr})
+    ref_model = holocron.models.rexnet1_0x(num_classes=10)
+    d["rexnet1_0x_layout"] = [(k, tuple(v.shape), str(v.dtype)) for k, v in ref_model.state_dict().items()]
+    torch.save(d, OUT / "ref_modules.pt")
+
+
+if __name__ == "__main__" and "--ref-modules" in sys.argv:
+    gen_ref_modules()
+    print("ref_modules.pt", (OUT / "ref_modules.pt").stat().st_size)
+
+
+if __name__ == "__main__" and not any(f in sys.argv for f in ("--zoo", "--zoo-resnet", "--zoo-f3", "--zoo-f3b", "--yolo", "--trainers", "--seg", "--api", "--trainer", "--optim2", "--ref-modules")):
     gen_activations()
     gen_losses()
     gen_boxes()
@@ -701,11 +755,12 @@ def gen_trainer():
         "acc2_clip_onecycle": dict(gradient_acc=2, gradient_clip=0.5, skip_nan_loss=False, sched="onecycle", lr=2e-3, nan_at=None),
         "nan_skip_cosine": dict(gradient_acc=1, gradient_clip=None, skip_nan_loss=True, sched="cosine", lr=1e-3, nan_at=3),
     }
+    tmp = tempfile.TemporaryDirectory()
     for tag, cfg in scenarios.items():
         model = tiny()
         data = batches(8, cfg["nan_at"])
         opt = AdaBelief(model.parameters(), lr=1e-3, betas=(0.95, 0.99), eps=1e-6)
-        tr = T(model, data, data, torch.nn.CrossEntropyLoss(), opt, gpu=None, output_file="/tmp/_hb_golden_ckpt.pth", amp=False,
+        tr = T(model, data, data, torch.nn.CrossEntropyLoss(), opt, gpu=None, output_file=os.path.join(tmp.name, "ckpt.pth"), amp=False,
                skip_nan_loss=cfg["skip_nan_loss"], nan_tolerance=5, gradient_acc=cfg["gradient_acc"], gradient_clip=cfg["gradient_clip"])
         losses, lrs, beta1s = [], [], []
         orig = tr._get_loss
@@ -732,6 +787,7 @@ def gen_trainer():
                        bn_eval=[n for n, m in model.named_modules() if isinstance(m, torch.nn.BatchNorm2d) and not m.training])
     norm, other = tutils.split_normalization_params(tiny())
     d["split"] = dict(norm=len(norm), other=len(other), norm_numel=sum(p.numel() for p in norm), other_numel=sum(p.numel() for p in other))
+    tmp.cleanup()
     torch.save(d, OUT / "trainer.pt")
 
 

@@ -2,7 +2,7 @@
 
   * the HF-hub repository layout of reference models/utils.py:146-175 (config.json + pytorch_model.bin), written by
     ``save_hf_hub_folder`` and read back by ``model_from_hf_hub`` through a stubbed ``hf_hub_download`` (no network);
-    the same two files are read by the UNMODIFIED reference's ``model_from_hf_hub`` when /root/reference is mounted;
+    the parameter layout matches what the UNMODIFIED reference's ``model_from_hf_hub`` loads (recorded golden data);
   * ``load_pretrained_params`` (reference models/utils.py:89-113) from a ``file://`` URL incl. key filter / replacement, and
     the factories' ``checkpoint=Checkpoint(...)`` argument;
   * ``clean_checkpoint`` (reference references/clean_checkpoint.py): Trainer checkpoint -> bare legacy-serialised state_dict."""
@@ -16,7 +16,8 @@ import torch
 import holocron_b200 as hb
 from holocron_b200.models import checkpoints as CK
 from holocron_b200.models import utils as U
-from oracle import reference_loader
+
+from conftest import load_golden
 
 
 def _stub_hub(monkeypatch, folder, repo):
@@ -43,25 +44,30 @@ def test_hf_hub_folder_round_trip(tmp_path, monkeypatch):
     assert list(sd) == list(sl) and all(torch.equal(sd[k], sl[k]) for k in sd)
 
 
-@pytest.mark.skipif(not reference_loader.available(), reason="needs /root/reference (build container only)")
 def test_hf_hub_folder_is_readable_by_the_reference(tmp_path, monkeypatch):
-    """Interoperability both ways: a folder written here loads in the unmodified reference (same arch registry key, same
-    parameter names), and a folder holding the reference's state_dict loads here."""
-    holocron = reference_loader.load()
+    """Interoperability both ways: a folder written here holds exactly the parameter names, shapes and dtypes the
+    unmodified reference's ``model_from_hf_hub`` loads into its rexnet1_0x (recorded by tests/golden/make_golden.py
+    --ref-modules) under the same arch registry key, and a folder holding a state_dict of that layout loads here."""
+    layout = load_golden("ref_modules")["rexnet1_0x_layout"]
     torch.manual_seed(4)
     ours = hb.models.rexnet1_0x(num_classes=10)
     classes = [str(i) for i in range(10)]
     folder = U.save_hf_hub_folder(ours, tmp_path / "hub", "rexnet1_0x", classes)
-    ref_utils = holocron.models.utils
-    monkeypatch.setattr(ref_utils, "hf_hub_download", lambda repo_id, filename, **kw: str(folder / filename))
-    ref_model = ref_utils.model_from_hf_hub("frgfm/rexnet1_0x")
-    so, sr = ours.state_dict(), ref_model.state_dict()
-    assert list(so) == list(sr) and all(torch.equal(so[k], sr[k]) for k in so)
-    # and back: the reference's state_dict in the same layout
-    torch.save(ref_model.state_dict(), folder / "pytorch_model.bin")
+    cfg = json.loads((folder / "config.json").read_text())
+    assert cfg["arch"] == "rexnet1_0x"                        # the reference's loader picks the factory by this key ...
+    assert cfg["classes"] == classes and len(cfg["classes"]) == 10   # ... and builds it with num_classes=len(classes)
+    saved = torch.load(folder / "pytorch_model.bin", map_location="cpu")
+    assert [(k, tuple(v.shape), str(v.dtype)) for k, v in saved.items()] == layout
+    so = ours.state_dict()
+    assert all(torch.equal(so[k], saved[k]) for k in so)
+    # and back: a state_dict in the reference's layout (other values) loads into this package's model
+    torch.manual_seed(5)
+    ref_sd = {k: (torch.randn(shape) if "float" in dt else torch.randint(0, 5, shape)).to(getattr(torch, dt.split(".")[1]))
+              for k, shape, dt in layout}
+    torch.save(ref_sd, folder / "pytorch_model.bin")
     _stub_hub(monkeypatch, folder, "frgfm/rexnet1_0x")
     back = U.model_from_hf_hub("frgfm/rexnet1_0x")
-    assert all(torch.equal(v, back.state_dict()[k]) for k, v in sr.items())
+    assert all(torch.equal(v, back.state_dict()[k]) for k, v in ref_sd.items())
 
 
 def _checkpoint(url, arch):

@@ -1,4 +1,4 @@
-"""GPU parity tests for the tcgen05 convolution kernels (fprop / dgrad / wgrad) and the fused BatchNorm/branch-sum/
+"""GPU parity tests for the tensor-core convolution kernels (fprop / dgrad / wgrad) and the fused BatchNorm/branch-sum/
 activation kernels, through the C ABI, against the CPU oracle (torch fp32 on the same bf16-rounded inputs).
 
 Tolerances: outputs stored in bf16 -> relative L2 error < 4e-3 (bf16 rounding, 2^-9 rms) and max-abs < 2 bf16 ulp of the

@@ -30,8 +30,8 @@ def test_norm_conv2d_and_add2d_vs_golden(monkeypatch):
     g = load_golden("convs")
     x, w, b = g["x"].cuda(), g["w"], g["b"]
     for tag, kw in CFGS:
-        # default path: tcgen05 implicit GEMM with the patch standardisation in the epilogue. Operands are rounded to bf16
-        # (2^-9 relative each) and so is the stored output: the bar against the fp32 reference is 1e-2 rel-L2 (measured ~4e-3);
+        # default path: wgmma implicit GEMM with the patch standardisation in the epilogue. Operands are rounded to bf16
+        # (2^-9 relative each) and so is the stored output: the bar against the fp32 reference is 1e-2 rel-L2;
         # the weight gradient comes from the fp32 kernel fed with the bf16-path statistics.
         monkeypatch.delenv("HB_NORMCONV_FP32", raising=False)
         wd = w.cuda().requires_grad_(True); bd = b.cuda().requires_grad_(True)

@@ -78,7 +78,7 @@ def test_train_step_loss_parity_and_update():
     opt = hb.optim.AdaBelief(m.parameters(), lr=1e-3, betas=(0.95, 0.99), eps=1e-6)
     lm = TF.cross_entropy(m(x.cuda()), t.cuda(), label_smoothing=0.1)
     lm.backward()
-    # bf16 forward through 28 blocks: loss within 1e-2 relative of the fp32 oracle (measured 3e-3)
+    # bf16 forward through 28 blocks: loss within 1e-2 relative of the fp32 oracle
     assert abs(lm.item() - lo.item()) / abs(lo.item()) < 1e-2
     assert all(p.grad is not None and torch.isfinite(p.grad).all() for p in m.parameters())
     before = [p.detach().clone() for p in m.parameters()]

@@ -1,4 +1,4 @@
-"""Dev harness (GPU box): checks the tcgen05 conv kernels against torch's conv2d on the same bf16 inputs."""
+"""Dev harness (GPU): checks the wgmma conv kernels against torch's conv2d on the same bf16 inputs."""
 import ctypes
 import sys
 import time

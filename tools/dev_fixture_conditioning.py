@@ -1,4 +1,4 @@
-"""Dev tool (CPU, build container): conditioning of candidate zoo fixtures.
+"""Dev tool (CPU, needs a reference checkout): conditioning of candidate zoo fixtures.
 
 For a reference model and a candidate (batch, size, parameter treatment) prints the rel-L2 distance between the
 reference's fp32 logits and the SAME reference module tree run under CPU bf16 autocast - the error any bf16 execution

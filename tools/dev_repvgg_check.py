@@ -1,4 +1,4 @@
-"""Dev harness (GPU box): RepBlock / RepVGG forward+backward through the CUDA path vs golden fixtures + oracle."""
+"""Dev harness (GPU): RepBlock / RepVGG forward+backward through the CUDA path vs golden fixtures + oracle."""
 import sys
 import time
 

@@ -1,7 +1,7 @@
 """Leaf-kernel micro rows of the hot path (BASELINE.md §3.3, `python bench.py --micro`): every bandwidth-bound kernel
 north_star names, at the configurations' sizes, timed with CUDA events through the PUBLIC Python API (forward, and
 forward+backward where the op is differentiable) and reported as achieved GB/s over the ALGORITHMIC bytes of SURVEY.md
-§8(d) against the measured HBM copy peak. Inputs are larger than the 126 MB L2 or the L2 is flushed between iterations
+§8(d) against the measured HBM copy peak. Inputs are larger than the L2 (50 MB on an H100) or the L2 is flushed between iterations
 (a 256 MB scratch write), stated per row."""
 import torch
 import torch.nn.functional as TF

@@ -1,7 +1,6 @@
-"""Build-container check (needs /root/reference): the UNMODIFIED reference's RepVGG-A0 train step (holocron.models.repvgg_a0 +
-holocron.optim.AdaBelief, CPU fp32) timed beside the oracle port that `bench.py --impl reference` runs on the GPU box
-(oracle.models.RepVGGOracle + oracle.optim.adabelief_step): same step, same batch, same threads. Shows that the port is a fair
-stand-in for the reference arm (the GPU box has no /root/reference)."""
+"""CPU check (needs a reference checkout, HOLOCRON_REFERENCE): the UNMODIFIED reference's RepVGG-A0 train step
+(holocron.models.repvgg_a0 + holocron.optim.AdaBelief, CPU fp32) timed beside the oracle port that `bench.py --impl reference`
+runs, which stands in for the reference arm where no reference checkout exists."""
 import sys
 import time
 
