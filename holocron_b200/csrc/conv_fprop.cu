@@ -41,7 +41,6 @@ struct FpropParams {
   int stride, pad_h, pad_w, dil;
   int R, S;
   int Cin, Cout;
-  int BN;           // Cout tile
   int num_m_tiles, num_n_tiles;
   int cblocks;      // ceil(Cin / 64)
   int ksteps_last;  // 16-channel MMA steps of the last channel block (Cin = 48 -> 3 instead of 4 zero-padded ones)
@@ -53,7 +52,7 @@ struct FpropParams {
   int e_mode, e_cblocks, e_ksteps_last;
   int nout;         // 1, or 2 in dual mode
   int stages;
-  int b_stage_bytes;  // BN*128 rounded up to 1024
+  int b_stage_bytes;  // BN*128 rounded up to 1024 (BN: the Cout tile, a template parameter of the kernel)
   int out_pitch;      // bytes per row of the smem output staging tile (min(BN, 64)*2 + 16)
   int a_mode;         // 0: plain 2-D [M, C] matrix (1x1 s1 p0), 1: im2col
   int act;            // 0 none, 1 relu
@@ -79,8 +78,9 @@ struct FpropParams {
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // kStats: the epilogue also accumulates the output-column statistics (separate instantiation: the plain kernel carries
-// neither the extra registers nor the extra shared-memory pass in its instruction stream)
-template <bool kStats>
+// neither the extra registers nor the extra shared-memory pass in its instruction stream).
+// BN: the Cout tile (a multiple of 16 up to 128, at most 64 in dual mode), the N of every wgmma.
+template <bool kStats, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                   const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2, const FpropParams p) {
@@ -111,7 +111,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int n_tile = blockIdx.x % p.num_n_tiles;
   const int m_first = blockIdx.x / p.num_n_tiles, m_step = gridDim.x / p.num_n_tiles;
   const int kblocks = p.R * p.S * p.cblocks;
-  const uint32_t tx_bytes = kABytes + p.BN * 128;
+  const uint32_t tx_bytes = kABytes + BN * 128;
 
   if (warp < 4) {
     // ================= TMA producer =================
@@ -133,7 +133,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                  (uint16_t)(s * p.dil), (uint16_t)(r * p.dil));
             else
               tma_load_2d(&tmA, &full_bar[stage], sa, cb * kBK, m0);
-            tma_load_3d(&tmB, &full_bar[stage], sb, cb * kBK, tap, n_tile * p.BN);
+            tma_load_3d(&tmB, &full_bar[stage], sb, cb * kBK, tap, n_tile * BN);
             if (++stage == p.stages) { stage = 0; phase ^= 1; }
           }
         }
@@ -149,7 +149,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
                                (uint16_t)((p.S / 2) * p.dil), (uint16_t)((p.R / 2) * p.dil));
           else
             tma_load_2d(&tmA, &full_bar[stage], sa, cb * kBK, m0);
-          tma_load_3d(&tmB2, &full_bar[stage], sb, cb * kBK, 0, n_tile * p.BN);
+          tma_load_3d(&tmB2, &full_bar[stage], sb, cb * kBK, 0, n_tile * BN);
           if (++stage == p.stages) { stage = 0; phase ^= 1; }
         }
       }
@@ -168,64 +168,56 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const uint32_t stage_lo = (uint32_t)stage_bytes >> 4;
   long long* row_off = reinterpret_cast<long long*>(sout + (((size_t)kBM * p.out_pitch + 15) & ~(size_t)15));
   // column groups of <= 64 columns go through the fixed-size staging tile: gpo groups per output, nout outputs
-  const int gpo = (p.BN + 63) >> 6;
+  const int gpo = (BN + 63) >> 6;
   const int ngroups = p.nout * gpo;
   // column statistics: this thread's running (sum0, sum1, sumsq0, sumsq1) of one column PAIR of each group over a fixed
   // subset of its warpgroup's 64 tile rows, kept in registers across all tiles of the CTA
   float st[4][4];
 #pragma unroll
   for (int gi = 0; gi < 4; ++gi) { st[gi][0] = st[gi][1] = st[gi][2] = st[gi][3] = 0.f; }
-  const int col_base = n_tile * p.BN;
-  const int ncols_valid = min(p.BN, p.Cout - col_base);          // multiple of 16
+  const int col_base = n_tile * BN;
+  const int ncols_valid = min(BN, p.Cout - col_base);          // multiple of 16
   float acc[kMaxCols / 2];
   int stage = 0; uint32_t phase = 0;
 
   for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
-    // ---- main loop: one K block in flight while the previous stage is handed back to the producer ----
-    int prev = -1, cb = 0;
-    const int nkb = kblocks + p.e_cblocks;
-    for (int kb = 0; kb < nkb; ++kb) {
+    // ---- main loop: one commit group per K block; one block stays in flight while the stage of the previous one
+    // is handed back to the producer ----
+    int prev = -1;
+    auto next_block = [&](uint32_t& a_lo, uint32_t& b_lo) {
       mbar_wait(&full_bar[stage], phase);
-      const uint32_t a_lo = a_lo0 + (uint32_t)stage * stage_lo;
-      const uint32_t b_lo = desc_lo(smem_u32(smem), 16) + (uint32_t)stage * stage_lo + (kABytes >> 4);
-      wgmma_fence();
-      if (kb < kblocks) {
-        const bool last_cb = ++cb == p.cblocks;
-        const int ks = last_cb ? p.ksteps_last : kBK / kMmaK;
-        if (last_cb) cb = 0;
-#pragma unroll
-        for (int k = 0; k < kBK / kMmaK; ++k)
-          if (k < ks)
-            wgmma_bf16<0, 0>(p.BN, acc, make_desc(a_lo + 2 * k, dhi), make_desc(b_lo + 2 * k, dhi), (uint32_t)(kb | k));
-      } else {
-        // extra K blocks: same accumulator (e_mode 1) or the second accumulator, BN columns further (e_mode 2)
-        const int ecb = kb - kblocks;
-        const int ks = (ecb == p.e_cblocks - 1) ? p.e_ksteps_last : kBK / kMmaK;
-#pragma unroll
-        for (int k = 0; k < kBK / kMmaK; ++k) {
-          if (k < ks) {
-            const uint64_t ad = make_desc(a_lo + 2 * k, dhi), bd = make_desc(b_lo + 2 * k, dhi);
-            if (p.e_mode == 2) {
-              const uint32_t sc = (uint32_t)(ecb | k);
-              // the second accumulator starts at column BN: a constant offset inside every case
-              switch (p.BN) {
-                case 16: wgmma_n16<0, 0>(acc + 8, ad, bd, sc); break;
-                case 32: wgmma_n32<0, 0>(acc + 16, ad, bd, sc); break;
-                case 48: wgmma_n48<0, 0>(acc + 24, ad, bd, sc); break;
-                case 64: wgmma_n64<0, 0>(acc + 32, ad, bd, sc); break;
-                default: break;
-              }
-            } else {
-              wgmma_bf16<0, 0>(p.BN, acc, ad, bd, 1u);
-            }
-          }
-        }
-      }
-      wgmma_commit();
+      a_lo = a_lo0 + (uint32_t)stage * stage_lo;
+      b_lo = desc_lo(smem_u32(smem), 16) + (uint32_t)stage * stage_lo + (kABytes >> 4);
+    };
+    auto retire_prev = [&]() {
       wgmma_wait<1>();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);   // the MMAs that read stage `prev` are done
       prev = stage;
       if (++stage == p.stages) { stage = 0; phase ^= 1; }
+    };
+    for (int kb = 0, cb = 0; kb < kblocks; ++kb) {
+      uint32_t a_lo, b_lo;
+      next_block(a_lo, b_lo);
+      if (++cb == p.cblocks) {
+        cb = 0;
+        wgmma_group_ks<BN, 0, 0>(p.ksteps_last, acc, a_lo, b_lo, 2, dhi, kb != 0);
+      } else {
+        wgmma_group<BN, kBK / kMmaK, 0, 0>(acc, a_lo, b_lo, 2, dhi, kb != 0);
+      }
+      retire_prev();
+    }
+    // extra K blocks: same accumulator (e_mode 1) or the second accumulator, BN columns further (e_mode 2)
+    for (int ecb = 0; ecb < p.e_cblocks; ++ecb) {
+      uint32_t a_lo, b_lo;
+      next_block(a_lo, b_lo);
+      const int ks = (ecb == p.e_cblocks - 1) ? p.e_ksteps_last : kBK / kMmaK;
+      if constexpr (BN <= 64) {
+        if (p.e_mode == 2) wgmma_group_ks<BN, 0, 0>(ks, acc + BN / 2, a_lo, b_lo, 2, dhi, ecb != 0);
+        else wgmma_group_ks<BN, 0, 0>(ks, acc, a_lo, b_lo, 2, dhi, 1u);
+      } else {
+        wgmma_group_ks<BN, 0, 0>(ks, acc, a_lo, b_lo, 2, dhi, 1u);
+      }
+      retire_prev();
     }
     wgmma_wait<0>();
     fence_regs(acc);
@@ -245,10 +237,10 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     for (int gi = 0; gi < ngroups; ++gi) {
       const int o = gi >= gpo ? 1 : 0;                 // output index (dual mode: 0 = RxS conv, 1 = 1x1 conv)
       const int g0 = (gi - o * gpo) * 64;
-      const int gw = min(64, p.BN - g0);
+      const int gw = min(64, BN - g0);
       __nv_bfloat16* yo = o ? p.y2 : p.y;
       const bool first = o == 0;
-      const int cs0 = o * p.BN + g0;                   // first accumulator column of this group
+      const int cs0 = o * BN + g0;                   // first accumulator column of this group
       consumer_sync();   // staging tile free
       if (gi == 0 && et < kBM) {
         // element offset of each output row of the tile (read by every thread in the copy-out below)
@@ -361,7 +353,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       float* so = o ? p.stats2 : p.stats;
       if (!so) continue;
       const int g0 = (gi - o * gpo) * 64;
-      const int gw = min(64, p.BN - g0);
+      const int gw = min(64, BN - g0);
       const int npairs = gw >> 1, rgs = 128 / npairs;
       consumer_sync();
       float4* scratch = reinterpret_cast<float4*>(sout) + wg * 128;   // [2][128] float4, 4 KB <= staging tile
@@ -407,6 +399,29 @@ struct FpropArgs {
   cudaStream_t stream;
 };
 
+// one instantiation per Cout tile width, with and without the statistics epilogue
+template <bool kStats, int BN>
+cudaError_t launch_fprop_kernel(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
+                                const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
+                                const FpropParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    const cudaError_t e =
+        cudaFuncSetAttribute(conv_fprop_kernel<kStats, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  conv_fprop_kernel<kStats, BN><<<grid, kThreads, smem_bytes, stream>>>(tmA, tmB, tmA2, tmB2, p);
+  return cudaSuccess;
+}
+
+template <int BN>
+cudaError_t launch_fprop(bool stats, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
+                         const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2, const FpropParams& p) {
+  return stats ? launch_fprop_kernel<true, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p)
+               : launch_fprop_kernel<false, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p);
+}
+
 int fprop_launch(const FpropArgs& a) {
   const int Cin = a.Cin, Cout = a.Cout, R = a.R, S = a.S;
   const long long m_total_ll = (long long)a.N * a.Ho * a.Wo;
@@ -431,7 +446,6 @@ int fprop_launch(const FpropArgs& a) {
     BN = bn_max;
     for (int c = bn_max; c >= 64; c -= 16) if (Cout % c == 0) { BN = c; break; }
   }
-  p.BN = BN;
   p.nout = dual ? 2 : 1;
   p.num_m_tiles = (p.m_total + kBM - 1) / kBM;
   p.num_n_tiles = (Cout + BN - 1) / BN;
@@ -495,13 +509,6 @@ int fprop_launch(const FpropArgs& a) {
   }
 
   const size_t smem_bytes = (size_t)stages * stage_bytes + out_bytes + 2 * stages * sizeof(uint64_t) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_fprop_kernel<false>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e == cudaSuccess) e = cudaFuncSetAttribute(conv_fprop_kernel<true>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
   // grid: a multiple of num_n_tiles (every CTA keeps one Cout tile), at most one CTA per SM / per tile
   int grid = a.num_ctas > 0 ? a.num_ctas : HB_NUM_SMS;
   if (grid > HB_NUM_SMS * 4) grid = HB_NUM_SMS * 4;
@@ -510,8 +517,20 @@ int fprop_launch(const FpropArgs& a) {
   if (per_n > p.num_m_tiles) per_n = p.num_m_tiles;
   grid = per_n * p.num_n_tiles;
   if (a.stat_slots) *a.stat_slots = 2 * per_n;
-  if (p.stats || p.stats2) conv_fprop_kernel<true><<<grid, kThreads, smem_bytes, a.stream>>>(tmA, tmB, tmA2, tmB2, p);
-  else conv_fprop_kernel<false><<<grid, kThreads, smem_bytes, a.stream>>>(tmA, tmB, tmA2, tmB2, p);
+  const bool stats = p.stats || p.stats2;
+  cudaError_t e;
+  switch (BN) {
+    case 16: e = launch_fprop<16>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 32: e = launch_fprop<32>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 48: e = launch_fprop<48>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 64: e = launch_fprop<64>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 80: e = launch_fprop<80>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 96: e = launch_fprop<96>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 112: e = launch_fprop<112>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 128: e = launch_fprop<128>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    default: return (int)cudaErrorInvalidValue;
+  }
+  if (e != cudaSuccess) return (int)e;
   HB_LAUNCH_CHECK();
   return 0;
 }

@@ -35,7 +35,6 @@ struct RowsParams {
   int TRO;       // output rows per tile = SR * NSUB
   int CB;        // 64-channel blocks
   int ksteps_last;  // k-steps (of 16 channels) in the last channel block
-  int BN;        // = Cout (multiple of 16, <= 128)
   int tiles_per_img, num_tiles;
   int nstages;       // ring slots: 2, or 1 when two tiles' rows do not fit in shared memory
   int stage_bytes;   // CB * (cb_bytes + nextra * ecb_bytes): the main rows and every extra source of one tile
@@ -53,6 +52,8 @@ struct RowsParams {
 
 __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
+// BN = Cout (a multiple of 16 up to 128), the N of every wgmma
+template <int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmW,
                  const __grid_constant__ CUtensorMap tmXe0, const __grid_constant__ CUtensorMap tmWe0,
@@ -83,7 +84,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     if (warp == 0 && lane == 0) {
       prefetch_tmap(&tmXe0); prefetch_tmap(&tmWe0); prefetch_tmap(&tmXe1); prefetch_tmap(&tmWe1);
       // resident filters: 9 taps x CB channel blocks (+ one 1x1 filter per extra source)
-      mbar_arrive_expect_tx(w_bar, (uint32_t)((9 + p.nextra) * p.CB * p.BN * 128));
+      mbar_arrive_expect_tx(w_bar, (uint32_t)((9 + p.nextra) * p.CB * BN * 128));
       for (int tap = 0; tap < 9; ++tap)
         for (int cb = 0; cb < p.CB; ++cb)
           tma_load_3d(&tmW, w_bar, wsm + (size_t)(tap * p.CB + cb) * p.w_tap_bytes, cb * 64, tap, 0);
@@ -125,9 +126,9 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   const uint32_t w_tap_lo = (uint32_t)p.w_tap_bytes >> 4;
   const uint32_t cb_lo = (uint32_t)p.cb_bytes >> 4;
   const uint32_t ecb_lo = (uint32_t)p.ecb_bytes >> 4;
-  const int chunks_per_row = p.BN / 8;
+  const int chunks_per_row = BN / 8;
   // column statistics: thread = (column pair pr, pixel subset rg) over the valid pixels of every sub-tile
-  const int npairs = p.BN >> 1, rgs = kConsumers / npairs;
+  const int npairs = BN >> 1, rgs = kConsumers / npairs;
   const int st_rg = et / npairs, st_pr = et - st_rg * npairs;
   const bool st_on = p.stats != nullptr && st_rg < rgs;
   float st0 = 0.f, st1 = 0.f, sq0 = 0.f, sq1 = 0.f;
@@ -141,8 +142,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     // window start of this warpgroup's 64 rows: 64 pixel rows x 128 B further
     const uint32_t s_lo = desc_lo(smem_u32(stage0 + (size_t)st * p.stage_bytes), 16) + (uint32_t)wg * ((64 * 128) >> 4);
     for (int sub = 0; sub < p.NSUB; ++sub) {
-      wgmma_fence();
-      uint32_t accum = 0;
+      // one commit group per (tap or extra source, channel block), all in flight until the sub-tile's epilogue
 #pragma unroll 1
       for (int tap = 0; tap < 9; ++tap) {
         const int r = tap / 3, s = tap % 3;
@@ -151,13 +151,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         uint32_t b_lo = w_lo0 + (uint32_t)(tap * p.CB) * w_tap_lo;
         for (int cb = 0; cb < p.CB; ++cb) {
           const int ks = (cb == p.CB - 1) ? p.ksteps_last : 4;
-#pragma unroll
-          for (int k = 0; k < 4; ++k) {
-            if (k < ks) {
-              wgmma_bf16<0, 0>(p.BN, acc, make_desc(a_lo + 2 * k, dhi), make_desc(b_lo + 2 * k, dhi), accum);
-              accum = 1;
-            }
-          }
+          wgmma_group_ks<BN, 0, 0>(ks, acc, a_lo, b_lo, 2, dhi, (tap | cb) ? 1u : 0u);
           a_lo += cb_lo;
           b_lo += w_tap_lo;
         }
@@ -168,14 +162,11 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         uint32_t b_lo = w_lo0 + (uint32_t)((9 + e) * p.CB) * w_tap_lo;
         for (int cb = 0; cb < p.CB; ++cb) {
           const int ks = (cb == p.CB - 1) ? p.ksteps_last : 4;
-#pragma unroll
-          for (int k = 0; k < 4; ++k)
-            if (k < ks) wgmma_bf16<0, 0>(p.BN, acc, make_desc(a_lo + 2 * k, dhi), make_desc(b_lo + 2 * k, dhi), 1u);
+          wgmma_group_ks<BN, 0, 0>(ks, acc, a_lo, b_lo, 2, dhi, 1u);
           a_lo += ecb_lo;
           b_lo += w_tap_lo;
         }
       }
-      wgmma_commit();
       wgmma_wait<0>();
       fence_regs(acc);
       if (sub == p.NSUB - 1 && lane == 0) mbar_arrive(&empty_bar[st]);   // ring slot may be refilled
@@ -185,7 +176,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
 #pragma unroll
       for (int j = 0; j < 16; ++j) {
         const int col = 8 * j + fcol;
-        if (col < p.BN) {
+        if (col < BN) {
 #pragma unroll
           for (int h = 0; h < 2; ++h) {
             float f0 = acc[4 * j + 2 * h], f1 = acc[4 * j + 2 * h + 1];
@@ -250,8 +241,8 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     float4* scratch = reinterpret_cast<float4*>(sout);   // [256] float4, 4 KB <= staging tile
     scratch[et] = make_float4(st0, st1, sq0, sq1);
     consumer_sync();
-    if (et < 2 * p.BN) {
-      const int c = et % p.BN, half = et / p.BN;
+    if (et < 2 * BN) {
+      const int c = et % BN, half = et / BN;
       float sv = 0.f, qv = 0.f;
       if (half == 0) {
         const int pr = c >> 1, hi = c & 1;
@@ -264,6 +255,20 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
       *reinterpret_cast<float2*>(p.stats + ((size_t)(blockIdx.x * 2 + half) * p.Cout + c) * 2) = make_float2(sv, qv);
     }
   }
+}
+
+// one instantiation per Cout; false when the kernel's shared-memory limit cannot be raised (nothing launched)
+template <int BN>
+bool launch_rows(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmX, const CUtensorMap& tmW,
+                 const CUtensorMap* tmXe, const CUtensorMap* tmWe, const RowsParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    if (cudaFuncSetAttribute(conv_rows_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
+      return false;
+    attr_set = true;
+  }
+  conv_rows_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(tmX, tmW, tmXe[0], tmWe[0], tmXe[1], tmWe[1], p);
+  return true;
 }
 
 }  // namespace
@@ -281,7 +286,7 @@ int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, c
   const int Wp = W + 2;
   if (Wp > 128 || W < 8 || nextra < 0 || nextra > 2) return -1;
   RowsParams p{};
-  p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.Wp = Wp; p.BN = Cout; p.nextra = nextra;
+  p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.Wp = Wp; p.nextra = nextra;
   p.SR = 128 / Wp;
   p.CB = (Cin + 63) / 64;
   const int last = Cin - (p.CB - 1) * 64;
@@ -343,17 +348,22 @@ int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, c
     }
   }
   const size_t smem_bytes = (size_t)w_bytes + (size_t)p.nstages * p.stage_bytes + out_bytes + 64 + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(conv_rows_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return -1;
-    attr_set = true;
-  }
   if (smem_bytes > 227 * 1024) return -1;
   int grid = num_ctas > 0 ? num_ctas : HB_NUM_SMS;
   if (grid > p.num_tiles) grid = p.num_tiles;
+  bool launched;
+  switch (Cout) {
+    case 16: launched = launch_rows<16>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    case 32: launched = launch_rows<32>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    case 48: launched = launch_rows<48>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    case 64: launched = launch_rows<64>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    case 80: launched = launch_rows<80>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    case 96: launched = launch_rows<96>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    case 112: launched = launch_rows<112>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+    default: launched = launch_rows<128>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
+  }
+  if (!launched) return -1;
   if (stat_slots) *stat_slots = 2 * grid;
-  conv_rows_kernel<<<grid, kThreads, smem_bytes, stream>>>(tmX, tmW, tmXe[0], tmWe[0], tmXe[1], tmWe[1], p);
   g_hb_launches.fetch_add(1, std::memory_order_relaxed);
   return cudaGetLastError() == cudaSuccess ? 0 : -2;
 }

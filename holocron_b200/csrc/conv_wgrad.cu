@@ -32,7 +32,6 @@ struct WgradParams {
   int m_total, Ho, Wo, stride, pad, dil, R, S, Cin, Cout;
   int ci_tile;         // Cin tile (<= 128)
   int ci_chunks;       // ceil(ci_tile / 64)
-  int n_last;          // MMA width of the last 64-channel chunk (ci_tile tail rounded up to 16)
   int taps_per_group;  // taps per unit (1: the accumulators of one tap fill the register budget)
   int num_tap_groups, num_co_tiles, num_ci_tiles, k_splits;
   int kblocks_total;   // ceil(m_total / 64)
@@ -43,8 +42,11 @@ struct WgradParams {
   long long dw_elems;
 };
 
+// CIW: the Cin tile rounded up to 16 (16 ... 128) = the MMA widths of its 64-channel chunks: min(CIW, 64), then CIW - 64
+template <int CIW>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
+  constexpr int kChunks = (CIW + 63) / 64, kNLast = CIW - 64 * (kChunks - 1);
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
@@ -113,7 +115,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
   const int wg = et >> 7;
   const int frow = frag_row(et & 127), fcol = frag_col(et & 127);
   const uint32_t dhi = desc_hi(1024);
-  float acc[64];   // [chunk 0: 32 | chunk 1: 32]
+  float acc[CIW / 2];   // [chunk 0: 32 | chunk 1: kNLast / 2]
   int stage = 0; uint32_t phase = 0;
   for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
     int co_t, ci_t, tg, ks, kb0, kb1;
@@ -133,18 +135,11 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
       for (int k = 0; k < kBKpix / 16; ++k) {
         const uint64_t ad = make_desc(a_lo + k * (2048 >> 4), dhi);
         const uint32_t sc = acc0 | (uint32_t)k;
-        if (p.ci_chunks == 1) {
-          wgmma_bf16<1, 1>(p.n_last, acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
+        if constexpr (kChunks == 1) {
+          wgmma<kNLast, 1, 1>(acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
         } else {
-          wgmma_n64<1, 1>(acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
-          const uint64_t bd = make_desc(b_lo + (kChunkBytes >> 4) + k * (2048 >> 4), dhi);
-          switch (p.n_last) {   // second chunk: accumulators 32.. (a constant offset inside every case)
-            case 16: wgmma_n16<1, 1>(acc + 32, ad, bd, sc); break;
-            case 32: wgmma_n32<1, 1>(acc + 32, ad, bd, sc); break;
-            case 48: wgmma_n48<1, 1>(acc + 32, ad, bd, sc); break;
-            case 64: wgmma_n64<1, 1>(acc + 32, ad, bd, sc); break;
-            default: break;
-          }
+          wgmma<64, 1, 1>(acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
+          wgmma<kNLast, 1, 1>(acc + 32, ad, make_desc(b_lo + (kChunkBytes >> 4) + k * (2048 >> 4), dhi), sc);
         }
       }
       wgmma_commit();
@@ -166,12 +161,11 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
       if (co >= p.Cout) continue;
       float* drow = base + ((size_t)co * RS + tap) * p.Cin;
 #pragma unroll
-      for (int j = 0; j < 16; ++j) {
+      for (int j = 0; j < CIW / 8; ++j) {
         // register block j: chunk j / 8, columns 8 * (j % 8) + fcol of that chunk
         const int c = (j >> 3) * 64 + 8 * (j & 7) + fcol;
         const int ci = ci_t * p.ci_tile + c;
-        const int width = (j >> 3) + 1 < p.ci_chunks ? 64 : p.n_last;
-        if ((j >> 3) >= p.ci_chunks || 8 * (j & 7) >= width || c >= p.ci_tile || ci >= p.Cin) continue;
+        if (c >= p.ci_tile || ci >= p.Cin) continue;
         const float v0 = have ? acc[4 * j + 2 * h] : 0.f, v1 = have ? acc[4 * j + 2 * h + 1] : 0.f;
         if (p.use_atomics == 1) {
           atomicAdd(drow + ci, v0);
@@ -239,6 +233,20 @@ inline void launch_wgrad_reduce(const float* ws, float* dw, long long n, int sli
   wgrad_reduce_kernel<<<blocks, dim3(32, 8), 0, st>>>(ws, dw, n, slices, dw2, n_first, accumulate);
 }
 
+// one instantiation per Cin tile width (rounded up to 16)
+template <int CIW>
+cudaError_t launch_wgrad(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmDY, const CUtensorMap& tmX,
+                         const WgradParams& p) {
+  static bool attr_set = false;
+  if (!attr_set) {
+    const cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<CIW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+    if (e != cudaSuccess) return e;
+    attr_set = true;
+  }
+  conv_wgrad_kernel<CIW><<<grid, kThreads, smem_bytes, stream>>>(tmDY, tmX, p);
+  return cudaSuccess;
+}
+
 struct WgradPlan {
   WgradParams p;
   size_t ws_bytes;
@@ -262,7 +270,6 @@ int plan_wgrad(WgradPlan& plan, int N, int H, int W, int Cin, int Cout, int R, i
   }
   p.ci_tile = ci_tile;
   p.ci_chunks = (ci_tile + 63) / 64;
-  p.n_last = ((ci_tile - (p.ci_chunks - 1) * 64) + 15) & ~15;
   p.taps_per_group = 1;
   p.stage_bytes = kABytes + p.ci_chunks * kChunkBytes;
   p.stages = (200 * 1024) / p.stage_bytes;
@@ -359,15 +366,20 @@ static int wgrad_impl(const void* x, const void* dy, float* dw, float* workspace
     if (rc) return rc;
   }
   const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 2 * p.stages * sizeof(uint64_t) + 1024;
-  static bool attr_set = false;
-  if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return (int)e;
-    attr_set = true;
-  }
   const int num_units = base_units * k_splits;
   int grid = ctas < num_units ? ctas : num_units;
-  conv_wgrad_kernel<<<grid, kThreads, smem_bytes, st>>>(tmDY, tmX, p);
+  cudaError_t e;
+  switch ((p.ci_tile + 15) & ~15) {
+    case 16: e = launch_wgrad<16>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    case 32: e = launch_wgrad<32>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    case 48: e = launch_wgrad<48>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    case 64: e = launch_wgrad<64>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    case 80: e = launch_wgrad<80>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    case 96: e = launch_wgrad<96>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    case 112: e = launch_wgrad<112>(grid, smem_bytes, st, tmDY, tmX, p); break;
+    default: e = launch_wgrad<128>(grid, smem_bytes, st, tmDY, tmX, p); break;
+  }
+  if (e != cudaSuccess) return (int)e;
   HB_LAUNCH_CHECK();
   if (p.use_atomics == 2) {
     const long long n = p.dw_elems;

@@ -41,6 +41,48 @@ struct WRowsParams {
   long long slice_elems; // dw_elems + (has_b1 ? Cout*Cin : 0)
 };
 
+// The MMAs of one tile for the first NT of a warpgroup's TPW tap slots (the others lie past nslots): one commit group
+// per 16-pixel k-step with one wgmma per slot, so every fence -> commit region is straight-line. Each slot's accumulator
+// still takes its k-steps in order. dhi: descriptor high word; `any`: the accumulators already hold earlier tiles.
+template <int NC, int NT, int TPW>
+__device__ __forceinline__ void wrows_tile_mma(float (&acc)[TPW][NC / 2], const WRowsParams& p, int slot0, uint32_t sx,
+                                               uint32_t sy, uint32_t dhi, bool any) {
+  static_assert(NT <= TPW, "slot count");
+  if constexpr (NT > 0) {
+    uint32_t a_lo[NT], b_lo[NT];
+#pragma unroll
+    for (int t = 0; t < NT; ++t) {
+      const int slot = slot0 + t;
+      // slot < 9: tap window (r, s) against dY; slot 9: centre window against dY1
+      const int off = slot < 9 ? (slot / 3) * p.Wp + (slot % 3) : p.Wp + 1;
+      a_lo[t] = desc_lo(sx + off * 128, 16);
+      b_lo[t] = desc_lo(slot < 9 ? sy : sy + p.ybuf_bytes, 16);
+    }
+    for (int k = 0; k < p.KS; ++k) {
+      const uint32_t sc = (any || k > 0) ? 1u : 0u;
+      const uint32_t kofs = (uint32_t)k * (2048 >> 4);
+      wgmma_fence();
+#pragma unroll
+      for (int t = 0; t < NT; ++t)
+        wgmma<NC, 1, 1>(acc[t], make_desc(a_lo[t] + kofs, dhi), make_desc(b_lo[t] + kofs, dhi), sc);
+      wgmma_commit();
+    }
+  }
+}
+
+// Picks the instantiation for the run-time number of active slots nt (0 .. TPW).
+template <int NC, int NT, int TPW>
+__device__ __forceinline__ void wrows_tile_mma_n(int nt, float (&acc)[TPW][NC / 2], const WRowsParams& p, int slot0,
+                                                 uint32_t sx, uint32_t sy, uint32_t dhi, bool any) {
+  if constexpr (NT > 0) {
+    if (nt < NT) {
+      wrows_tile_mma_n<NC, NT - 1, TPW>(nt, acc, p, slot0, sx, sy, dhi, any);
+      return;
+    }
+  }
+  wrows_tile_mma<NC, NT, TPW>(acc, p, slot0, sx, sy, dhi, any);
+}
+
 template <int NC>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant__ CUtensorMap tmDY,
@@ -103,6 +145,7 @@ conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
   const int wg = et >> 7;
   const int slot0 = sg * 2 * TPW + wg * TPW;
   const uint32_t dhi = desc_hi(1024);
+  const int nt = max(0, min(TPW, p.nslots - slot0));   // slots of this warpgroup below nslots
   float acc[TPW][NC / 2];
   bool any = false;
   int it = 0;
@@ -111,25 +154,7 @@ conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
     mbar_wait(&full_bar[st], (it >> 1) & 1);
     const uint32_t sx = smem_u32(smem + (size_t)st * p.stage_bytes);
     const uint32_t sy = sx + p.xbuf_bytes;
-    wgmma_fence();
-#pragma unroll
-    for (int t = 0; t < TPW; ++t) {
-      const int slot = slot0 + t;
-      if (slot >= p.nslots) break;
-      // slot < 9: tap window (r, s) against dY; slot 9: centre window against dY1
-      const int off = slot < 9 ? (slot / 3) * p.Wp + (slot % 3) : p.Wp + 1;
-      const uint32_t a_lo0 = desc_lo(sx + off * 128, 16);
-      const uint32_t b_lo0 = desc_lo(slot < 9 ? sy : sy + p.ybuf_bytes, 16);
-      for (int k = 0; k < p.KS; ++k) {
-        const uint64_t ad = make_desc(a_lo0 + k * (2048 >> 4), dhi), bd = make_desc(b_lo0 + k * (2048 >> 4), dhi);
-        const uint32_t sc = (any || k > 0) ? 1u : 0u;
-        if constexpr (NC == 16) wgmma_n16<1, 1>(acc[t], ad, bd, sc);
-        else if constexpr (NC == 32) wgmma_n32<1, 1>(acc[t], ad, bd, sc);
-        else if constexpr (NC == 48) wgmma_n48<1, 1>(acc[t], ad, bd, sc);
-        else wgmma_n64<1, 1>(acc[t], ad, bd, sc);
-      }
-    }
-    wgmma_commit();
+    wrows_tile_mma_n<NC, TPW, TPW>(nt, acc, p, slot0, sx, sy, dhi, any);
     wgmma_wait<0>();
 #pragma unroll
     for (int t = 0; t < TPW; ++t) fence_regs(acc[t]);

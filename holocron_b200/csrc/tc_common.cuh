@@ -115,4 +115,31 @@ __device__ __forceinline__ uint64_t make_desc(uint32_t lo, uint32_t hi) { return
 __device__ __forceinline__ int frag_row(int t) { return ((t >> 5) & 3) * 16 + ((t & 31) >> 2); }
 __device__ __forceinline__ int frag_col(int t) { return (t & 3) * 2; }
 
+// ---- MMA issue ------------------------------------------------------------------------------
+// One commit group: KS k-steps of width N issued straight-line between a fence and a commit. Every fence -> commit
+// region of a kernel must be such a sequence; a predicate, a loop with a run-time trip count or a branch between
+// different MMAs inside the region makes ptxas serialise all wgmmas of the kernel (notes C7519 / C7520).
+// Descriptor low words advance by `step` per k-step; the first k-step uses `scale_first` (0 = overwrite).
+template <int N, int KS, int TA, int TB>
+__device__ __forceinline__ void wgmma_group(float* d, uint32_t a_lo, uint32_t b_lo, uint32_t step, uint32_t dhi,
+                                            uint32_t scale_first) {
+  wgmma_fence();
+#pragma unroll
+  for (int k = 0; k < KS; ++k)
+    wgmma<N, TA, TB>(d, make_desc(a_lo + k * step, dhi), make_desc(b_lo + k * step, dhi), k ? 1u : scale_first);
+  wgmma_commit();
+}
+// The same for a 64-channel block with a run-time k-step count ks in 1..4 (a partial last channel block): the switch
+// picks a whole region, so each region stays straight-line.
+template <int N, int TA, int TB>
+__device__ __forceinline__ void wgmma_group_ks(int ks, float* d, uint32_t a_lo, uint32_t b_lo, uint32_t step,
+                                               uint32_t dhi, uint32_t scale_first) {
+  switch (ks) {
+    case 1: wgmma_group<N, 1, TA, TB>(d, a_lo, b_lo, step, dhi, scale_first); break;
+    case 2: wgmma_group<N, 2, TA, TB>(d, a_lo, b_lo, step, dhi, scale_first); break;
+    case 3: wgmma_group<N, 3, TA, TB>(d, a_lo, b_lo, step, dhi, scale_first); break;
+    default: wgmma_group<N, 4, TA, TB>(d, a_lo, b_lo, step, dhi, scale_first); break;
+  }
+}
+
 }  // namespace tc
