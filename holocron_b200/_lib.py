@@ -83,6 +83,10 @@ SIGNATURES = {
     "hb_dice_scratch_doubles": "i",
     "hb_dice_fwd": "pppppp" + "iiqffip",
     "hb_dice_bwd": "pppp" + "iiqip",
+    "hb_cce_fwd": "pppppp" + "iiii" + "f" + "ip",
+    "hb_cce_bwd": "pppppp" + "iiii" + "f" + "iip",
+    "hb_mcl_fwd": "p" * 9 + "iiiii" + "f" + "ip",
+    "hb_mcl_bwd": "p" * 10 + "iiiii" + "f" + "iip",
     "hb_optim_chunk_elems": "",
     "hb_adabelief_step": "ppifffffiippp",
     "hb_adamp_step": "ppiifffffifipppp",

@@ -1,5 +1,7 @@
-// Classification / segmentation losses: focal, poly-1 (hard + soft targets) and dice.
-// Reference: holocron/nn/functional.py:59-113 (focal_loss), :540-613 (poly_loss), :503-537 (dice_loss).
+// Classification / segmentation losses: focal, poly-1 (hard + soft targets; with eps = 0 also the multi-label cross
+// entropy), dice, complement cross entropy and the mutual channel loss.
+// Reference: holocron/nn/functional.py:59-113 (focal_loss), :540-613 (poly_loss), :503-537 (dice_loss),
+// :150-191 (multilabel_cross_entropy), :194-255 (complement_cross_entropy), :258-319 (mutual_channel_loss).
 //
 // Logits are [N, K, S] (S = product of the spatial dims, possibly 1); a "position" is one (n, s) pair.
 // The reference runs log_softmax + transpose/flatten/gather + boolean-mask indexing + mean (~10 kernels, 4-6
@@ -659,6 +661,345 @@ int dice_blocks_per_class(long long per_class, int K) {
   return gx < 1 ? 1 : gx;
 }
 
+// ---- losses with three partial sums: complement CE and the mutual channel loss ----------------------
+// partials[3 * block + {0, 1, 2}] = {sum of w_y * ce over the non-ignored positions, sum of their w_y, sum of the second
+// term}; out = {A + coef * C, B, A / B + coef * C / P}: torch's weighted-mean cross entropy plus coef times the plain mean.
+__global__ void finalize3_kernel(const double* partials, int n, double P, float coef, float* out) {
+  if (threadIdx.x == 0 && blockIdx.x == 0) {
+    double a = 0.0, b = 0.0, c = 0.0;
+    for (int i = 0; i < n; ++i) { a += partials[3 * i]; b += partials[3 * i + 1]; c += partials[3 * i + 2]; }
+    out[0] = (float)(a + (double)coef * c);
+    out[1] = (float)b;
+    out[2] = (float)(a / b + (double)coef * c / P);
+  }
+}
+
+__device__ __forceinline__ void store3(double* partials, double a, double b, double c, double* red) {
+  a = block_sum<double>(a, red);
+  b = block_sum<double>(b, red);
+  c = block_sum<double>(c, red);
+  if (threadIdx.x == 0) { partials[3 * blockIdx.x] = a; partials[3 * blockIdx.x + 1] = b; partials[3 * blockIdx.x + 2] = c; }
+}
+
+// {d loss / d (w_y ce), d loss / d (second term)} of one position for the reduction (mean: the first over sum w_y)
+__device__ __forceinline__ void grad_scales(const float* gout, const float* fwd_out, int reduction, long long pos,
+                                            long long P, float& gce, float& g2) {
+  if (reduction == 0) { gce = g2 = gout[pos]; return; }
+  gce = g2 = gout[0];
+  if (reduction == 1) { gce /= fwd_out[1]; g2 /= (float)P; }
+}
+
+// ---- complement cross entropy ---------------------------------------------------------------------
+// per position (target y, A = the classes k != y outside the ignored column):
+//   L = w_y * ce * [y != ignore_index] + gamma * C,   ce = lse - x_y,
+//   C = -1/(K-1) * sum_{k in A} w_k q_k log q_k,    log q_k = x_k - lse_{k != y}
+// (q is the softmax over the non-target classes - the reference's p_k / (1 - p_y) without the cancellation of 1 - p_y).
+//   dC/dx_y = 0,   dC/dx_j = -1/(K-1) * q_j * ([j in A] w_j (1 + log q_j) - sum_{k in A} w_k q_k (1 + log q_k))
+// The CE part follows torch: any ignore_index value drops the row. The complement term drops the ignored column only.
+struct CceParams {
+  const void* x;            // [N, K, S]
+  const long long* target;  // [N, S]
+  const float* weight;      // [K] or null
+  float* loss_pos;          // [N*S]
+  double* partials;         // [grid][3]
+  const float* gout;        // backward: [N*S] (none) or 1 element
+  const float* fwd_out;     // backward: {sum, sum w_y, mean} of the forward
+  void* dx;
+  int N, K, S, ignore_index, reduction;
+  float gamma;
+};
+
+// k-loop shapes: one thread owns a position (S > 1) or a warp does, its lanes striding over the classes (S == 1)
+struct ThreadLanes {
+  static constexpr int kStep = 1;
+  int k0 = 0;
+  __device__ float max(float v) const { return v; }
+  __device__ float sum(float v) const { return v; }
+};
+struct WarpLanes {
+  static constexpr int kStep = 32;
+  int k0;
+  __device__ float max(float v) const { return warp_max(v); }
+  __device__ float sum(float v) const { return warp_sum(v); }
+};
+
+template <typename T, bool kBackward, class Ln>
+__device__ __forceinline__ void cce_position(const CceParams& p, const Ln& ln, const T* xp, T* dp, long long st,
+                                             long long pos, double& sa, double& sb, double& sc) {
+  const int K = p.K;
+  auto x_at = [&](int k) { return to_f(xp[k * st]); };
+  auto w_at = [&](int k) { return p.weight ? p.weight[k] : 1.f; };
+  const long long tl = p.target[pos];
+  const bool inr = tl >= 0 && tl < K;
+  const int t = inr ? (int)tl : -1;
+  const bool comp = p.gamma != 0.f;
+  const int icol = (p.ignore_index >= 0 && p.ignore_index < K) ? p.ignore_index : -1;
+  float mx = -INFINITY, mc = -INFINITY;
+  for (int k = ln.k0; k < K; k += Ln::kStep) {
+    const float v = x_at(k);
+    mx = fmaxf(mx, v);
+    if (k != t) mc = fmaxf(mc, v);
+  }
+  mx = ln.max(mx);
+  mc = ln.max(mc);
+  float s = 0.f, sn = 0.f;
+  for (int k = ln.k0; k < K; k += Ln::kStep) {
+    const float v = x_at(k);
+    s += expf(v - mx);
+    if (comp && k != t) sn += expf(v - mc);
+  }
+  s = ln.sum(s);
+  sn = ln.sum(sn);
+  const float lse = mx + logf(s), lsen = mc + logf(sn);
+  // forward: sum_{k in A} w_k q_k log q_k; backward: sum_{k in A} w_k q_k (1 + log q_k)
+  float acc = 0.f;
+  if (comp && inr) {
+    for (int k = ln.k0; k < K; k += Ln::kStep)
+      if (k != t && k != icol) {
+        const float lq = x_at(k) - lsen;
+        acc += w_at(k) * expf(lq) * (kBackward ? 1.f + lq : lq);
+      }
+    acc = ln.sum(acc);
+  }
+  const float inv = 1.f / (float)(K - 1);
+  if (!kBackward) {
+    float wce = 0.f, wv = 0.f;
+    if (tl != p.ignore_index) {
+      if (inr) { wv = w_at(t); wce = wv * (lse - x_at(t)); } else { wce = NAN; }
+    }
+    const float c = comp ? (inr ? -inv * acc : NAN) : 0.f;
+    if (ln.k0 == 0) {
+      p.loss_pos[pos] = wce + p.gamma * c;
+      sa += wce; sb += wv; sc += c;
+    }
+  } else {
+    float gce, gc;
+    grad_scales(p.gout, p.fwd_out, p.reduction, pos, (long long)p.N * p.S, gce, gc);
+    const float cw = (inr && tl != p.ignore_index) ? gce * w_at(t) : 0.f;
+    const float cc = (comp && inr) ? -p.gamma * gc * inv : 0.f;
+    for (int k = ln.k0; k < K; k += Ln::kStep) {
+      const float v = x_at(k);
+      float d = cw * (expf(v - lse) - (k == t ? 1.f : 0.f));
+      if (comp && inr && k != t) {  // lsen is -inf without the complement term
+        const float lq = v - lsen;
+        d += cc * expf(lq) * ((k != icol ? w_at(k) * (1.f + lq) : 0.f) - acc);
+      }
+      dp[k * st] = from_f<T>(d);
+    }
+  }
+}
+
+template <typename T, bool kBackward>
+__global__ void __launch_bounds__(kThreads) cce_kernel(CceParams p) {
+  __shared__ double red[32];
+  const T* x = (const T*)p.x;
+  T* dx = (T*)p.dx;
+  const long long P = (long long)p.N * p.S;
+  double sa = 0.0, sb = 0.0, sc = 0.0;
+  if (p.S == 1) {
+    const WarpLanes ln{threadIdx.x & 31};
+    const long long warps = (long long)gridDim.x * (kThreads / 32);
+    for (long long pos = (long long)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); pos < P; pos += warps)
+      cce_position<T, kBackward>(p, ln, x + pos * p.K, dx + pos * p.K, 1, pos, sa, sb, sc);
+  } else {
+    const ThreadLanes ln{};
+    const long long stride = (long long)gridDim.x * kThreads;
+    for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
+      const long long off = (pos / p.S) * p.K * p.S + pos % p.S;
+      cce_position<T, kBackward>(p, ln, x + off, dx + off, p.S, pos, sa, sb, sc);
+    }
+  }
+  if (!kBackward) store3(p.partials, sa, sb, sc, red);
+}
+
+// ---- mutual channel loss --------------------------------------------------------------------------
+// x is [N, C = cnum * xi, S]; row r = n * C + ch (one channel of one sample) is a contiguous run of S values.
+//   discriminative part: d_c = max_j (x[c*xi + j] * mask[c][j]) (masked channels enter as 0 * x), torch cross entropy of
+//     d over the cnum classes;
+//   diversity part: per position, the mean over classes of max_j softmax_s(x[c*xi + j])  (softmax over the spatial axis);
+//   L = discr - alpha * diversity.
+// Argmaxes take the first index on ties, as the CPU max does.
+struct McParams {
+  const void* x;
+  const long long* target;      // [N, S]
+  const float* weight;          // [cnum] or null
+  const unsigned char* mask;    // [cnum * xi]
+  const float* row_lse;         // [N * C]: log sum_s exp(x) of every row (pass A)
+  float* loss_pos;              // [N * S]
+  float* lse_d;                 // [N * S]: log-sum-exp of d over the classes (saved for the backward)
+  double* partials;             // [grid][3]
+  const float* gout;
+  const float* fwd_out;
+  float* rdot;                  // [N * C]: sum_s G_s p_s of every row (pass C)
+  void* dx;
+  int N, cnum, xi, S, ignore_index, reduction;
+  float alpha;
+};
+
+// pass A: one block per row, online (max, sum exp) merged across the block in a fixed order
+__device__ __forceinline__ void lse_merge(float& m, float& z, float m2, float z2) {
+  const float mn = fmaxf(m, m2);
+  if (mn == -INFINITY) return;
+  z = z * expf(m - mn) + z2 * expf(m2 - mn);
+  m = mn;
+}
+
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mcl_row_lse_kernel(const T* __restrict__ x, long long S, int vec, float* row_lse) {
+  constexpr int V = Vec16<T>::N;
+  __shared__ float sm[32], sz[32];
+  const T* row = x + (long long)blockIdx.x * S;
+  float m = -INFINITY, z = 0.f;
+  if (vec) {
+    for (long long i = threadIdx.x; i < S / V; i += kThreads) {
+      const Vec16<T> v = ld16_stream(row + i * V);
+      float vm = -INFINITY;
+#pragma unroll
+      for (int j = 0; j < V; ++j) vm = fmaxf(vm, to_f(v.v[j]));
+      float vz = 0.f;
+#pragma unroll
+      for (int j = 0; j < V; ++j) vz += expf(to_f(v.v[j]) - vm);
+      lse_merge(m, z, vm, vz);
+    }
+  } else {
+    for (long long i = threadIdx.x; i < S; i += kThreads) lse_merge(m, z, to_f(row[i]), 1.f);
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    const float m2 = __shfl_xor_sync(0xffffffffu, m, o), z2 = __shfl_xor_sync(0xffffffffu, z, o);
+    lse_merge(m, z, m2, z2);
+  }
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  if (lane == 0) { sm[warp] = m; sz[warp] = z; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    for (int w = 1; w < kThreads / 32; ++w) lse_merge(m, z, sm[w], sz[w]);
+    row_lse[blockIdx.x] = m + logf(z);
+  }
+}
+
+// class c at one position: the masked max (value, channel) and the largest spatial-softmax probability (value, channel)
+template <typename T>
+__device__ __forceinline__ void mcl_class(const McParams& p, const T* xc, const float* lse_c, const unsigned char* mc,
+                                          float& d, int& jd, float& pv, int& jv) {
+  for (int j = 0; j < p.xi; ++j) {
+    const float v = to_f(xc[(long long)j * p.S]);
+    const float dv = v * (float)mc[j];
+    if (j == 0 || dv > d) { d = dv; jd = j; }
+    const float pr = expf(v - lse_c[j]);
+    if (j == 0 || pr > pv) { pv = pr; jv = j; }
+  }
+}
+
+// pass B: one thread per position
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mcl_fwd_kernel(McParams p) {
+  __shared__ double red[32];
+  const T* x = (const T*)p.x;
+  const int C = p.cnum * p.xi;
+  const long long P = (long long)p.N * p.S;
+  double sa = 0.0, sb = 0.0, sc = 0.0;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
+    const long long n = pos / p.S, s = pos % p.S;
+    const T* xp = x + n * C * p.S + s;
+    const float* lse_n = p.row_lse + n * C;
+    const long long tl = p.target[pos];
+    float m = -INFINITY, z = 0.f, dt = NAN, div = 0.f;
+    for (int c = 0; c < p.cnum; ++c) {
+      float d, pv;
+      int jd, jv;
+      mcl_class<T>(p, xp + (long long)c * p.xi * p.S, lse_n + c * p.xi, p.mask + c * p.xi, d, jd, pv, jv);
+      lse_merge(m, z, d, 1.f);
+      if (c == tl) dt = d;
+      div += pv;
+    }
+    const float lse = m + logf(z);
+    float wce = 0.f, wv = 0.f;
+    if (tl != p.ignore_index) {
+      if (tl >= 0 && tl < p.cnum) { wv = p.weight ? p.weight[tl] : 1.f; wce = wv * (lse - dt); } else { wce = NAN; }
+    }
+    div /= (float)p.cnum;
+    p.loss_pos[pos] = wce - p.alpha * div;
+    p.lse_d[pos] = lse;
+    sa += wce; sb += wv; sc += div;
+  }
+  store3(p.partials, sa, sb, sc, red);
+}
+
+// pass C: one block per (sample, class); per row of the class R = sum_s G_s p_s with G_s = -(alpha/cnum) g_s at the
+// positions where the row holds the class' largest probability. Per-thread, per-row sums live in shared memory.
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mcl_rdot_kernel(McParams p) {
+  extern __shared__ float acc[];  // [xi][blockDim.x]
+  __shared__ double red[32];
+  const int n = blockIdx.x / p.cnum, c = blockIdx.x % p.cnum;
+  const int C = p.cnum * p.xi;
+  const long long P = (long long)p.N * p.S;
+  const T* xc = (const T*)p.x + ((long long)n * C + (long long)c * p.xi) * p.S;
+  const float* lse_c = p.row_lse + (long long)n * C + c * p.xi;
+  for (int j = 0; j < p.xi; ++j) acc[j * blockDim.x + threadIdx.x] = 0.f;
+  for (long long s = threadIdx.x; s < p.S; s += blockDim.x) {
+    float gce, g;
+    grad_scales(p.gout, p.fwd_out, p.reduction, n * p.S + s, P, gce, g);
+    float pv = 0.f;
+    int jv = 0;
+    for (int j = 0; j < p.xi; ++j) {
+      const float pr = expf(to_f(xc[(long long)j * p.S + s]) - lse_c[j]);
+      if (j == 0 || pr > pv) { pv = pr; jv = j; }
+    }
+    acc[jv * blockDim.x + threadIdx.x] += g * pv;
+  }
+  const float f = -p.alpha / (float)p.cnum;
+  for (int j = 0; j < p.xi; ++j) {
+    const double r = block_sum<double>((double)acc[j * blockDim.x + threadIdx.x], red);
+    if (threadIdx.x == 0) p.rdot[(long long)n * C + c * p.xi + j] = f * (float)r;
+  }
+}
+
+// pass D: one thread per position; dx = (CE gradient of d_c on its kept argmax channel) + p (G - R)
+template <typename T>
+__global__ void __launch_bounds__(kThreads) mcl_bwd_kernel(McParams p) {
+  const T* x = (const T*)p.x;
+  T* dx = (T*)p.dx;
+  const int C = p.cnum * p.xi;
+  const long long P = (long long)p.N * p.S;
+  const float f = -p.alpha / (float)p.cnum;
+  const long long stride = (long long)gridDim.x * kThreads;
+  for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
+    const long long n = pos / p.S, s = pos % p.S;
+    const long long off = n * C * p.S + s;
+    const float* lse_n = p.row_lse + n * C;
+    const float* rdot_n = p.rdot + n * C;
+    const long long tl = p.target[pos];
+    float gce, gdiv;
+    grad_scales(p.gout, p.fwd_out, p.reduction, pos, P, gce, gdiv);
+    const bool ce_on = tl != p.ignore_index && tl >= 0 && tl < p.cnum;
+    gce = ce_on ? gce * (p.weight ? p.weight[tl] : 1.f) : 0.f;
+    const float lse = p.lse_d[pos];
+    for (int c = 0; c < p.cnum; ++c) {
+      const long long oc = off + (long long)c * p.xi * p.S;
+      float d, pv;
+      int jd, jv;
+      mcl_class<T>(p, x + oc, lse_n + c * p.xi, p.mask + c * p.xi, d, jd, pv, jv);
+      const float dd = gce * (expf(d - lse) - (c == tl ? 1.f : 0.f));
+      for (int j = 0; j < p.xi; ++j) {
+        const int ch = c * p.xi + j;
+        const float pr = expf(to_f(x[oc + (long long)j * p.S]) - lse_n[ch]);
+        float o = pr * ((j == jv ? f * gdiv : 0.f) - rdot_n[ch]);
+        if (j == jd) o += dd * (float)p.mask[ch];
+        dx[oc + (long long)j * p.S] = from_f<T>(o);
+      }
+    }
+  }
+}
+
+// pass C block size: xi per-thread sums (plus the reduction scratch) must fit the default 48 KB of shared memory
+int mcl_rdot_threads(int xi) {
+  int t = (47 * 1024 / (int)sizeof(float) / xi) / 32 * 32;
+  return t > kThreads ? kThreads : t;
+}
+
 }  // namespace
 
 extern "C" {
@@ -836,5 +1177,101 @@ int hb_dice_bwd(const void* target, const float* coef, const float* gout, void* 
   HB_LAUNCH_CHECK();
   return 0;
 }
+
+#define HB_LOSS_DTYPE_SWITCH(dtype, LAUNCH)              \
+  switch (dtype) {                                       \
+    case HB_DTYPE_F32: LAUNCH(float); break;             \
+    case HB_DTYPE_BF16: LAUNCH(__nv_bfloat16); break;    \
+    case HB_DTYPE_F16: LAUNCH(__half); break;            \
+    default: return (int)cudaErrorInvalidValue;          \
+  }
+
+int hb_cce_fwd(const void* x, const long long* target, const float* weight, float* loss_pos, double* partials,
+               float* fwd_out, int N, int K, int S, int ignore_index, float gamma, int dtype, void* stream) {
+  CceParams p{};
+  p.x = x; p.target = target; p.weight = weight; p.loss_pos = loss_pos; p.partials = partials;
+  p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.gamma = gamma;
+  const long long P = (long long)N * S;
+  if (P == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = grid_for(P, S == 1 ? kThreads / 32 : kThreads);
+#define HB_CCE_FWD(T) cce_kernel<T, false><<<grid, kThreads, 0, st>>>(p)
+  HB_LOSS_DTYPE_SWITCH(dtype, HB_CCE_FWD)
+#undef HB_CCE_FWD
+  HB_LAUNCH_CHECK();
+  finalize3_kernel<<<1, 32, 0, st>>>(partials, grid, (double)P, gamma, fwd_out);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+int hb_cce_bwd(const void* x, const long long* target, const float* weight, const float* gout, const float* fwd_out,
+               void* dx, int N, int K, int S, int ignore_index, float gamma, int reduction, int dtype, void* stream) {
+  CceParams p{};
+  p.x = x; p.target = target; p.weight = weight; p.gout = gout; p.fwd_out = fwd_out; p.dx = dx;
+  p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.reduction = reduction; p.gamma = gamma;
+  const long long P = (long long)N * S;
+  if (P == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = grid_for(P, S == 1 ? kThreads / 32 : kThreads);
+#define HB_CCE_BWD(T) cce_kernel<T, true><<<grid, kThreads, 0, st>>>(p)
+  HB_LOSS_DTYPE_SWITCH(dtype, HB_CCE_BWD)
+#undef HB_CCE_BWD
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+int hb_mcl_fwd(const void* x, const long long* target, const float* weight, const unsigned char* mask, float* row_lse,
+               float* loss_pos, float* lse_d, double* partials, float* fwd_out, int N, int cnum, int xi, int S,
+               int ignore_index, float alpha, int dtype, void* stream) {
+  McParams p{};
+  p.x = x; p.target = target; p.weight = weight; p.mask = mask; p.row_lse = row_lse; p.loss_pos = loss_pos;
+  p.lse_d = lse_d; p.partials = partials;
+  p.N = N; p.cnum = cnum; p.xi = xi; p.S = S; p.ignore_index = ignore_index; p.alpha = alpha;
+  const long long P = (long long)N * S, rows = (long long)N * cnum * xi;
+  if (P == 0 || rows == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = grid_for(P, kThreads);
+#define HB_MCL_FWD(T)                                                                                      \
+  {                                                                                                        \
+    const int vec = S % Vec16<T>::N == 0 && aligned16(x);                                                  \
+    mcl_row_lse_kernel<T><<<(unsigned)rows, kThreads, 0, st>>>((const T*)x, S, vec, row_lse);              \
+    HB_LAUNCH_CHECK();                                                                                     \
+    mcl_fwd_kernel<T><<<grid, kThreads, 0, st>>>(p);                                                       \
+  }
+  HB_LOSS_DTYPE_SWITCH(dtype, HB_MCL_FWD)
+#undef HB_MCL_FWD
+  HB_LAUNCH_CHECK();
+  finalize3_kernel<<<1, 32, 0, st>>>(partials, grid, (double)P, -alpha, fwd_out);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+int hb_mcl_bwd(const void* x, const long long* target, const float* weight, const unsigned char* mask,
+               const float* row_lse, const float* lse_d, const float* gout, const float* fwd_out, float* rdot, void* dx,
+               int N, int cnum, int xi, int S, int ignore_index, float alpha, int reduction, int dtype, void* stream) {
+  McParams p{};
+  p.x = x; p.target = target; p.weight = weight; p.mask = mask; p.row_lse = row_lse; p.lse_d = const_cast<float*>(lse_d); p.gout = gout;
+  p.fwd_out = fwd_out; p.rdot = rdot; p.dx = dx;
+  p.N = N; p.cnum = cnum; p.xi = xi; p.S = S; p.ignore_index = ignore_index; p.alpha = alpha; p.reduction = reduction;
+  const long long P = (long long)N * S, groups = (long long)N * cnum;
+  if (P == 0 || groups == 0) return 0;
+  const int rt = mcl_rdot_threads(xi);
+  if (rt < 32) return (int)cudaErrorInvalidValue;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int grid = grid_for(P, kThreads);
+  const size_t smem = (size_t)xi * rt * sizeof(float);
+#define HB_MCL_BWD(T)                                                                                      \
+  {                                                                                                        \
+    mcl_rdot_kernel<T><<<(unsigned)groups, rt, smem, st>>>(p);                                             \
+    HB_LAUNCH_CHECK();                                                                                     \
+    mcl_bwd_kernel<T><<<grid, kThreads, 0, st>>>(p);                                                       \
+  }
+  HB_LOSS_DTYPE_SWITCH(dtype, HB_MCL_BWD)
+#undef HB_MCL_BWD
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+#undef HB_LOSS_DTYPE_SWITCH
 
 }  // extern "C"

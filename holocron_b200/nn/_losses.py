@@ -1,5 +1,7 @@
-"""focal_loss / poly_loss / dice_loss on the fused CUDA kernels (holocron_b200/csrc/losses.cu)."""
+"""focal_loss / poly_loss / dice_loss / multilabel_cross_entropy / complement_cross_entropy / mutual_channel_loss on the
+fused CUDA kernels (holocron_b200/csrc/losses.cu)."""
 import ctypes
+import math
 from typing import Optional
 
 import torch
@@ -99,6 +101,82 @@ class _PolySoftFn(torch.autograd.Function):
         return dx, None, None, None, None, None
 
 
+class _ComplementCEFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x: Tensor, target: Tensor, weight: Optional[Tensor], ignore_index: int, reduction: int,
+                gamma: float) -> Tensor:
+        require_cuda(x, target)
+        xc = x.contiguous()
+        tc = target.contiguous().view(-1)
+        n, k, s = _nks(xc)
+        if tc.numel() != n * s:
+            raise ValueError("target shape does not match the input's (N, ...) dims")
+        L = lib()
+        loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
+        partials = torch.empty(3 * L.hb_loss_max_partials(), device=x.device, dtype=torch.float64)
+        fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
+        check(L.hb_cce_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n, k, s,
+                           int(ignore_index), _cf(gamma), dtype_code(xc), stream_ptr()), "hb_cce_fwd")
+        ctx.save_for_backward(xc, tc, weight, fwd_out)
+        ctx.cfg = (n, k, s, int(ignore_index), reduction, gamma)
+        if reduction == 1:
+            return fwd_out[2].to(x.dtype)
+        if reduction == 2:
+            return fwd_out[0].to(x.dtype)
+        return loss_pos.to(x.dtype).view(x.shape[0], *x.shape[2:])
+
+    @staticmethod
+    def backward(ctx, gout: Tensor):
+        xc, tc, weight, fwd_out = ctx.saved_tensors
+        n, k, s, ignore_index, reduction, gamma = ctx.cfg
+        g = gout.detach().float().contiguous().view(-1)
+        dx = torch.empty_like(xc)
+        check(lib().hb_cce_bwd(ptr(xc), ptr(tc), ptr(weight), ptr(g), ptr(fwd_out), ptr(dx), n, k, s, ignore_index,
+                               _cf(gamma), reduction, dtype_code(xc), stream_ptr()), "hb_cce_bwd")
+        return dx, None, None, None, None, None
+
+
+class _MutualChannelFn(torch.autograd.Function):
+    @staticmethod
+    def forward(ctx, x: Tensor, target: Tensor, weight: Optional[Tensor], mask: Tensor, ignore_index: int,
+                reduction: int, xi: int, alpha: float) -> Tensor:
+        require_cuda(x, target)
+        xc = x.contiguous()
+        tc = target.contiguous().view(-1)
+        n, c, s = _nks(xc)
+        cnum = c // xi
+        if tc.numel() != n * s:
+            raise ValueError("target shape does not match the input's (N, ...) dims")
+        L = lib()
+        row_lse = torch.empty(n * c, device=x.device, dtype=torch.float32)
+        loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
+        lse_d = torch.empty(n * s, device=x.device, dtype=torch.float32)
+        partials = torch.empty(3 * L.hb_loss_max_partials(), device=x.device, dtype=torch.float64)
+        fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
+        check(L.hb_mcl_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(mask), ptr(row_lse), ptr(loss_pos), ptr(lse_d),
+                           ptr(partials), ptr(fwd_out), n, cnum, xi, s, int(ignore_index), _cf(alpha), dtype_code(xc),
+                           stream_ptr()), "hb_mcl_fwd")
+        ctx.save_for_backward(xc, tc, weight, mask, row_lse, lse_d, fwd_out)
+        ctx.cfg = (n, cnum, xi, s, int(ignore_index), reduction, alpha)
+        if reduction == 1:
+            return fwd_out[2].to(x.dtype)
+        if reduction == 2:
+            return fwd_out[0].to(x.dtype)
+        return loss_pos.to(x.dtype).view(x.shape[0], *x.shape[2:])
+
+    @staticmethod
+    def backward(ctx, gout: Tensor):
+        xc, tc, weight, mask, row_lse, lse_d, fwd_out = ctx.saved_tensors
+        n, cnum, xi, s, ignore_index, reduction, alpha = ctx.cfg
+        g = gout.detach().float().contiguous().view(-1)
+        rdot = torch.empty_like(row_lse)
+        dx = torch.empty_like(xc)
+        check(lib().hb_mcl_bwd(ptr(xc), ptr(tc), ptr(weight), ptr(mask), ptr(row_lse), ptr(lse_d), ptr(g), ptr(fwd_out),
+                               ptr(rdot), ptr(dx), n, cnum, xi, s, ignore_index, _cf(alpha), reduction, dtype_code(xc),
+                               stream_ptr()), "hb_mcl_bwd")
+        return dx, None, None, None, None, None, None, None
+
+
 def _check_reduction(reduction: str) -> int:
     # the reference treats every value other than "sum" / "mean" as "none"
     return _RED.get(reduction, 0)
@@ -167,3 +245,73 @@ def dice_loss(x: Tensor, target: Tensor, weight: Optional[Tensor] = None, gamma:
     ``1 - (1 + 1/gamma) * mean_k[(gamma*sum(x*t) + eps) / (sum(x + gamma*t) + eps)]`` with the sums taken jointly over
     batch and space. Two streaming reductions per class in one pass instead of 4 full-tensor temporaries."""
     return _DiceFn.apply(x, target, _weight(weight, x), float(gamma), float(eps))
+
+
+def _torch_reduction(reduction: str) -> int:
+    # the losses built on torch's cross_entropy reject what it rejects
+    if reduction not in _RED:
+        raise ValueError(f"{reduction} is not a valid value for reduction")
+    return _RED[reduction]
+
+
+def multilabel_cross_entropy(x: Tensor, target: Tensor, weight: Optional[Tensor] = None, ignore_index: int = -100,
+                             reduction: str = "mean") -> Tensor:
+    """Cross entropy with multi-label (soft) targets — mirrors holocron/nn/functional.py:150-191:
+    ``-sum_k t_k w_k log_softmax(x)_k`` over the class axis. ``ignore_index`` drops that class column (only inside
+    ``[0, K)``), ``weight`` scales the class axis for any rank, ``'mean'`` averages over the ``N * ...`` positions and
+    ``'none'`` is shaped ``(N, ...)``. The soft-target poly-1 kernels with ``eps = 0``."""
+    if target.shape != x.shape:
+        raise ValueError("invalid target shape")
+    return _PolySoftFn.apply(x, target, _weight(weight, x), ignore_index, _check_reduction(reduction), 0.0)
+
+
+def complement_cross_entropy(x: Tensor, target: Tensor, weight: Optional[Tensor] = None, ignore_index: int = -100,
+                             reduction: str = "mean", gamma: float = -1) -> Tensor:
+    """Complement cross entropy (https://arxiv.org/abs/2009.02189) — mirrors holocron/nn/functional.py:194-255:
+    ``cross_entropy(x, target, weight, ignore_index, reduction) + gamma * C`` with
+    ``C = -1/(K-1) sum_{k != y} w_k q_k log q_k`` and ``q`` the softmax over the non-target classes. The cross-entropy
+    part follows torch (any ``ignore_index`` drops the row, ``'mean'`` divides by the summed target weights); in ``C``
+    ``ignore_index`` drops a class column (only inside ``[0, K)``) and ``'mean'`` averages over every position.
+    ``gamma == 0`` is the cross entropy alone. Out-of-range targets give NaN (the reference raises)."""
+    red = _torch_reduction(reduction)
+    if target.ndim != x.ndim - 1:
+        raise ValueError("complement_cross_entropy expects class-index targets of shape (N, ...)")
+    if gamma != 0 and x.shape[1] == 1:
+        raise ZeroDivisionError("complement_cross_entropy needs at least 2 classes (the term is scaled by 1 / (K - 1))")
+    return _ComplementCEFn.apply(x, target.long(), _weight(weight, x), ignore_index, red, float(gamma))
+
+
+def mutual_channel_mask(cnum: int, xi: int) -> Tensor:
+    """The channel mask of the mutual channel loss, drawn as the reference draws it (holocron/nn/functional.py:290-294):
+    ``ceil(xi / 2)`` ones per class, placed by one ``torch.randperm(xi)`` per class on the default CPU generator.
+    Returns a float32 CPU tensor of shape ``(cnum, xi)``."""
+    base = torch.zeros(xi)
+    base[: math.ceil(xi / 2)] = 1
+    mask = torch.zeros((cnum, xi))
+    for idx in range(cnum):
+        mask[idx] = base[torch.randperm(xi)]
+    return mask
+
+
+def mutual_channel_loss(x: Tensor, target: Tensor, weight: Optional[Tensor] = None, ignore_index: int = -100,
+                        reduction: str = "mean", xi: int = 2, alpha: float = 1.0) -> Tensor:
+    """Mutual channel loss (https://arxiv.org/abs/2002.04264) — mirrors holocron/nn/functional.py:258-319 on
+    ``x`` of shape ``(N, cnum * xi, ...)``: ``discr - alpha * diversity``, where ``discr`` is torch's cross entropy of the
+    per-class maxima of the randomly masked channels (masked channels enter as ``0 * x``) and ``diversity`` the mean over
+    classes of the largest spatial softmax among a class' channels. Each call draws a new mask on the host, consuming the
+    default CPU generator exactly as the reference does, so the loss cannot be captured into a CUDA graph."""
+    b, c = x.shape[:2]
+    cnum = c // xi
+    if c % xi != 0:
+        # what the reference's x.view(b, cnum, xi, -1) raises
+        raise RuntimeError(f"shape '[{b}, {cnum}, {xi}, -1]' is invalid for input of size {x.numel()}")
+    require_cuda(x, target)
+    if torch.cuda.is_current_stream_capturing():
+        raise RuntimeError("mutual_channel_loss draws a new channel mask on the host at every call and cannot run "
+                           "inside CUDA graph capture; keep it out of the captured region (e.g. TrainStep(graph=False))")
+    # pinned + non-blocking: a pageable copy would wait for the work already queued on the stream
+    mask = mutual_channel_mask(cnum, xi).to(torch.uint8).view(-1).pin_memory().to(x.device, non_blocking=True)
+    red = _torch_reduction(reduction)
+    if target.ndim != x.ndim - 1:
+        raise ValueError("mutual_channel_loss expects class-index targets of shape (N, ...)")
+    return _MutualChannelFn.apply(x, target.long(), _weight(weight, x), mask, ignore_index, red, int(xi), float(alpha))

@@ -9,14 +9,15 @@ import torch
 from torch import Tensor
 
 from .._lib import check, dtype_code, lib, ptr, require_cuda, stream_ptr
-from ._losses import dice_loss, focal_loss, poly_loss  # noqa: F401
+from ._losses import (complement_cross_entropy, dice_loss, focal_loss, multilabel_cross_entropy,  # noqa: F401
+                      mutual_channel_loss, poly_loss)
 from ._xcorr import add2d, norm_conv2d  # noqa: F401
 from ._dropblock import dropblock2d  # noqa: F401
 
 import ctypes
 
-__all__ = ["add2d", "concat_downsample2d", "dice_loss", "dropblock2d", "focal_loss", "hard_mish", "nl_relu", "norm_conv2d",
-           "poly_loss"]
+__all__ = ["add2d", "complement_cross_entropy", "concat_downsample2d", "dice_loss", "dropblock2d", "focal_loss", "hard_mish",
+           "multilabel_cross_entropy", "mutual_channel_loss", "nl_relu", "norm_conv2d", "poly_loss"]
 
 _cf = ctypes.c_float
 

@@ -242,6 +242,28 @@ int hb_dice_fwd(const void* x, const void* target, const float* weight, double* 
                 int K, long long S, float gamma, float eps, int dtype, void* stream);
 int hb_dice_bwd(const void* target, const float* coef, const float* gout, void* dx, int N, int K, long long S, int dtype,
                 void* stream);
+/* multilabel_cross_entropy (holocron/nn/functional.py:150-191) is hb_poly_soft_fwd / _bwd with eps = 0. */
+/* complement_cross_entropy: holocron/nn/functional.py:194-255. x [N, K, S], target int64 [N, S]; any ignore_index value
+ * drops the row from the cross-entropy part, one inside [0, K) also drops that class from the complement term.
+ * loss_pos: float[N*S] = w_y * ce + gamma * C; partials: double[3 * hb_loss_max_partials()] scratch;
+ * fwd_out: float[3] = {sum, sum of w_y over the non-ignored rows, mean}. gamma = 0 gives the cross entropy alone. */
+int hb_cce_fwd(const void* x, const long long* target, const float* weight, float* loss_pos, double* partials,
+               float* fwd_out, int N, int K, int S, int ignore_index, float gamma, int dtype, void* stream);
+/* reduction: 0 none (gout[N*S]), 1 mean, 2 sum (gout[1]); fwd_out from hb_cce_fwd; dx like x */
+int hb_cce_bwd(const void* x, const long long* target, const float* weight, const float* gout, const float* fwd_out,
+               void* dx, int N, int K, int S, int ignore_index, float gamma, int reduction, int dtype, void* stream);
+/* mutual_channel_loss: holocron/nn/functional.py:258-319. x [N, cnum*xi, S], target int64 [N, S], weight float[cnum];
+ * mask: uint8[cnum*xi] channel mask drawn by the caller. Outputs: row_lse float[N*cnum*xi] (spatial log-sum-exp of every
+ * (sample, channel) row), loss_pos float[N*S], lse_d float[N*S] (log-sum-exp of the masked class maxima),
+ * partials double[3 * hb_loss_max_partials()] scratch, fwd_out float[3] = {sum, sum of w_y over the non-ignored
+ * positions, mean}. row_lse and lse_d are inputs of hb_mcl_bwd. */
+int hb_mcl_fwd(const void* x, const long long* target, const float* weight, const unsigned char* mask, float* row_lse,
+               float* loss_pos, float* lse_d, double* partials, float* fwd_out, int N, int cnum, int xi, int S,
+               int ignore_index, float alpha, int dtype, void* stream);
+/* rdot: float[N*cnum*xi] scratch. Fails with cudaErrorInvalidValue when xi > 376 (per-row sums in shared memory). */
+int hb_mcl_bwd(const void* x, const long long* target, const float* weight, const unsigned char* mask,
+               const float* row_lse, const float* lse_d, const float* gout, const float* fwd_out, float* rdot, void* dx,
+               int N, int cnum, int xi, int S, int ignore_index, float alpha, int reduction, int dtype, void* stream);
 
 /* ---- optimizers: holocron/optim/adabelief.py:121-167, lamb.py:79-137, tadam.py:160-212 ----------------- */
 /* metas: device table of T records {p, g, m, v, vmax, aux, ext, numel} (8 x 8 bytes each, fp32 tensors);

@@ -3,6 +3,9 @@ north_star names, at the configurations' sizes, timed with CUDA events through t
 forward+backward where the op is differentiable) and reported as achieved GB/s over the ALGORITHMIC bytes of SURVEY.md
 §8(d) against the measured HBM copy peak. Inputs are larger than the L2 (50 MB on an H100) or the L2 is flushed between iterations
 (a 256 MB scratch write), stated per row."""
+import sys
+from pathlib import Path
+
 import torch
 import torch.nn.functional as TF
 
@@ -30,7 +33,10 @@ def _time(fn, flush=None, iters=10, warm=3):
 def run_micro(peaks):
     import holocron_b200 as hb
     from holocron_b200.nn import functional as F
+    from holocron_b200.nn._losses import mutual_channel_mask
     from holocron_b200.ops import boxes as B
+    sys.path.insert(0, str(Path(__file__).resolve().parents[1] / "tests"))
+    import _losses_extra_oracle as OX
     dev = torch.device("cuda", 0)
     flush = torch.empty(256 << 20, device=dev, dtype=torch.uint8)
     rows = []
@@ -62,6 +68,45 @@ def run_micro(peaks):
         xr = x.clone().requires_grad_(True)
         loss = fn(xr, t)
         row(f"{name} bwd", list(x.shape), _time(lambda: torch.autograd.grad(loss, xr, retain_graph=True)), 2 * nk * 4 + npos * 8)
+        del xr, loss
+    # complement and multi-label cross entropy on the same logits, each beside the CPU oracle's eager formulation run on
+    # the same GPU (the `eager` rows: what the reference's torch code costs there)
+    soft = torch.softmax(torch.randn_like(x), 1)
+    for name, fn, tgt, fb, bb in (
+            ("complement_cross_entropy", F.complement_cross_entropy, t, nk * 4 + npos * 8 + 4, 2 * nk * 4 + npos * 8),
+            ("multilabel_cross_entropy", F.multilabel_cross_entropy, soft, 2 * nk * 4 + 4, 3 * nk * 4)):
+        for impl, f in ((name, fn), (f"{name} eager", getattr(OX, name))):
+            row(f"{impl} fwd", list(x.shape), _time(lambda: f(x, tgt)), fb)
+            xr = x.clone().requires_grad_(True)
+            loss = f(xr, tgt)
+            row(f"{impl} bwd", list(x.shape), _time(lambda: torch.autograd.grad(loss, xr, retain_graph=True)), bb)
+            del xr, loss
+    del x, t, soft
+    # ImageNet head: 256 x 1000 logits (1 MB, L2 flushed), one warp per row
+    x = torch.randn(256, 1000, device=dev)
+    t = torch.randint(0, 1000, (256,), device=dev)
+    for impl, f in (("complement_cross_entropy", F.complement_cross_entropy),
+                    ("complement_cross_entropy eager", OX.complement_cross_entropy)):
+        row(f"{impl} fwd", list(x.shape), _time(lambda: f(x, t), flush), x.numel() * 4 + 256 * 8 + 4, l2="L2 flushed")
+        xr = x.clone().requires_grad_(True)
+        loss = f(xr, t)
+        row(f"{impl} bwd", list(x.shape), _time(lambda: torch.autograd.grad(loss, xr, retain_graph=True), flush),
+            2 * x.numel() * 4 + 256 * 8, l2="L2 flushed")
+        del xr, loss
+    del x, t
+    # mutual channel loss: 16 x 63 x 256 x 256 bf16 (132 MB, xi = 3: 21 classes); algorithmic bytes = the features once
+    # and the targets (forward), plus the feature gradient (backward)
+    x = torch.randn(16, 63, 256, 256, device=dev, dtype=torch.bfloat16)
+    t = torch.randint(0, 21, (16, 256, 256), device=dev)
+    nk, npos = x.numel(), t.numel()
+    mask = mutual_channel_mask(21, 3).to(dev)
+    for impl, f in (("mutual_channel_loss", lambda a: F.mutual_channel_loss(a, t, xi=3)),
+                    ("mutual_channel_loss eager", lambda a: OX.mutual_channel_loss(a, t, mask, xi=3))):
+        row(f"{impl} fwd", list(x.shape), _time(lambda: f(x), flush), nk * 2 + npos * 8, l2="L2 flushed")
+        xr = x.clone().requires_grad_(True)
+        loss = f(xr)
+        row(f"{impl} bwd", list(x.shape), _time(lambda: torch.autograd.grad(loss, xr, retain_graph=True), flush),
+            2 * nk * 2 + npos * 8, l2="L2 flushed")
         del xr, loss
     del x, t
     x = torch.softmax(torch.randn(16, 21, 256, 256, device=dev), 1)
