@@ -2,12 +2,13 @@
 // the sm_90a tensor cores: NHWC bf16 activations, KRSC bf16 filters, fp32 accumulation in registers (wgmma).
 //
 // GEMM view:  Y[m, co] = sum_{r,s,ci} X[pix(m) + (r,s), ci] * Wt[co, r, s, ci]
-//   M = N*Ho*Wo output pixels (tile 128 = two 64-row warpgroup MMAs), N = Cout (tile BN <= 128),
+//   M = N*Ho*Wo output pixels (tile 128 = two 64-row warpgroup MMAs), N = Cout (tile BN <= 256),
 //   K = R*S*Cin walked tap by tap in 64-channel blocks.
 // Replaces the cuDNN calls behind nn.Conv2d in holocron.models.utils.conv_sequence
 // (reference holocron/models/utils.py:28-86) and RepBlock (models/classification/repvgg.py:55-73).
 //
-// Pipeline (one persistent CTA per SM, 384 threads):
+// Pipeline (one persistent CTA per SM, 384 threads; the producer warpgroup gives registers to the consumers with
+// setmaxnreg: 40 + 2 x 232 per thread, so that a consumer thread can hold 128 fp32 accumulators of a 256-column tile):
 //   warpgroup 0   TMA producer (one thread): im2col-mode loads of the activation tile (hardware handles padding,
 //                 stride, row/image wrap; out-of-range channels are zero-filled) + tiled loads of the filter slab,
 //                 both landing 128B-swizzled in a multi-stage smem ring (mbarrier complete_tx).
@@ -32,8 +33,10 @@ constexpr int kBK = 64;           // channels per K block (one 128-byte swizzle 
 constexpr int kMmaK = 16;         // K per wgmma for 16-bit inputs
 constexpr int kThreads = 384;     // producer warpgroup + 2 consumer warpgroups
 constexpr int kConsumers = 256;
-constexpr int kMaxCols = 128;     // accumulator columns per thread set (both outputs in dual mode)
+constexpr int kProducerRegs = 40;   // per thread after setmaxnreg: 128 x (40 + 2 x 232) = 64 512 <= 64 K registers
+constexpr int kConsumerRegs = 232;
 constexpr int kABytes = kBM * kBK * 2;  // 16 KiB
+constexpr int kSmemMax = 227 * 1024;    // dynamic shared memory per CTA on sm_90
 
 struct FpropParams {
   int m_total;      // N*Ho*Wo
@@ -79,7 +82,7 @@ __device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;
 
 // kStats: the epilogue also accumulates the output-column statistics (separate instantiation: the plain kernel carries
 // neither the extra registers nor the extra shared-memory pass in its instruction stream).
-// BN: the Cout tile (a multiple of 16 up to 128, at most 64 in dual mode), the N of every wgmma.
+// BN: the Cout tile (a multiple of 16 up to 256, at most 64 in dual mode), the N of every wgmma.
 template <bool kStats, int BN>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
@@ -115,6 +118,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
 
   if (warp < 4) {
     // ================= TMA producer =================
+    regs_release<kProducerRegs>();
     if (warp == 0 && lane == 0) {
       int stage = 0; uint32_t phase = 0;
       for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
@@ -158,6 +162,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   }
 
   // ================= consumers: MMA + epilogue =================
+  regs_acquire<kConsumerRegs>();
   const int et = threadIdx.x - 128;        // 0..255
   const int wg = et >> 7;                  // rows [64*wg, 64*wg + 64) of every tile
   const int wet = et & 127;
@@ -177,7 +182,9 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   for (int gi = 0; gi < 4; ++gi) { st[gi][0] = st[gi][1] = st[gi][2] = st[gi][3] = 0.f; }
   const int col_base = n_tile * BN;
   const int ncols_valid = min(BN, p.Cout - col_base);          // multiple of 16
-  float acc[kMaxCols / 2];
+  // accumulator columns: BN, or 2 x BN for the second output of dual mode (only possible for BN <= 64)
+  constexpr int kCols = BN <= 64 ? 2 * BN : BN;
+  float acc[kCols / 2];
   int stage = 0; uint32_t phase = 0;
 
   for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
@@ -253,7 +260,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         }
       }
 #pragma unroll
-      for (int j = 0; j < kMaxCols / 8; ++j) {
+      for (int j = 0; j < kCols / 8; ++j) {
         const int cs = 8 * j + fcol;                   // accumulator column of registers 4j .. 4j+3
         if (cs >= cs0 && cs < cs0 + gw) {
           const int cl = cs - cs0;                     // column inside the staged group
@@ -407,7 +414,7 @@ cudaError_t launch_fprop_kernel(int grid, size_t smem_bytes, cudaStream_t stream
   static bool attr_set = false;
   if (!attr_set) {
     const cudaError_t e =
-        cudaFuncSetAttribute(conv_fprop_kernel<kStats, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
+        cudaFuncSetAttribute(conv_fprop_kernel<kStats, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
@@ -418,8 +425,13 @@ cudaError_t launch_fprop_kernel(int grid, size_t smem_bytes, cudaStream_t stream
 template <int BN>
 cudaError_t launch_fprop(bool stats, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
                          const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2, const FpropParams& p) {
-  return stats ? launch_fprop_kernel<true, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p)
-               : launch_fprop_kernel<false, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p);
+  if constexpr (BN > 128) {   // wide tiles never carry the statistics epilogue (see fprop_launch)
+    if (stats) return cudaErrorInvalidValue;
+    return launch_fprop_kernel<false, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p);
+  } else {
+    return stats ? launch_fprop_kernel<true, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p)
+                 : launch_fprop_kernel<false, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p);
+  }
 }
 
 int fprop_launch(const FpropArgs& a) {
@@ -438,16 +450,26 @@ int fprop_launch(const FpropArgs& a) {
   p.stride = a.stride; p.pad_h = a.pad_h; p.pad_w = a.pad_w; p.dil = a.dil;
   p.R = R; p.S = S; p.Cin = Cin; p.Cout = Cout;
   p.scatter = a.scatter; p.OH = a.OH; p.OW = a.OW; p.o_step = a.o_step; p.o_a = a.o_a; p.o_b = a.o_b;
-  // Cout tile: whole Cout when it fits the accumulator registers (128 columns, or 64 per output in dual mode), else the
-  // largest multiple of 16 below that limit that divides Cout (falls back to the limit with a masked tail).
+  p.num_m_tiles = (p.m_total + kBM - 1) / kBM;
+  int grid = a.num_ctas > 0 ? a.num_ctas : HB_NUM_SMS;
+  if (grid > HB_NUM_SMS * 4) grid = HB_NUM_SMS * 4;
+  // Cout tile. Narrow rule: whole Cout up to 128 columns (64 per output in dual mode), else the largest multiple of 16
+  // below that limit that divides Cout (falls back to the limit with a masked tail). Wide rule (single output, filters
+  // with more than one tap, no output statistics): whole Cout up to 256, else 256 or 192 when it divides Cout. A wide
+  // tile multiplies each activation tile it loads into twice the columns. It is only taken while there are still at
+  // least as many tiles as CTAs in the grid, so small-M layers keep their parallelism; not for 1x1 filters: their K
+  // loop is short next to the epilogue, and on an H100 their wide tiles measured slower than the narrow ones; and not
+  // with statistics: each (CTA, warpgroup) slot sums the tiles of its CTA in order, so the Cout tile sets which partial
+  // sums the BatchNorm adds up, and the narrow tiles keep those sums, to the bit, as they were.
   const int bn_max = dual ? 64 : 128;
   int BN = Cout;
   if (Cout > bn_max) {
     BN = bn_max;
     for (int c = bn_max; c >= 64; c -= 16) if (Cout % c == 0) { BN = c; break; }
+    const int wide = dual || R * S == 1 || a.stats ? 0 : Cout <= 256 ? Cout : Cout % 256 == 0 ? 256 : Cout % 192 == 0 ? 192 : 0;
+    if (wide && (long long)p.num_m_tiles * (Cout / wide) >= grid) BN = wide;
   }
   p.nout = dual ? 2 : 1;
-  p.num_m_tiles = (p.m_total + kBM - 1) / kBM;
   p.num_n_tiles = (Cout + BN - 1) / BN;
   p.cblocks = (Cin + kBK - 1) / kBK;
   p.ksteps_last = ((Cin - (p.cblocks - 1) * kBK) + kMmaK - 1) / kMmaK;
@@ -459,7 +481,9 @@ int fprop_launch(const FpropArgs& a) {
   p.out_pitch = (BN < 64 ? BN : 64) * 2 + 16;
   const int out_bytes = ((((kBM * p.out_pitch + 15) & ~15) + kBM * 8) + 1023) & ~1023;   // staging tile + row offsets
   const int stage_bytes = kABytes + p.b_stage_bytes;
-  int stages = (204 * 1024 - out_bytes) / stage_bytes;
+  // as many ring stages as the 227 KiB of dynamic shared memory hold next to the staging tile, the barriers and the
+  // 1 KiB alignment slack (BN = 256: 4 stages of 48 KiB)
+  int stages = (kSmemMax - 1024 - out_bytes - 2 * 8 * (int)sizeof(uint64_t)) / stage_bytes;
   if (stages > 8) stages = 8;
   if (stages < 2) return (int)cudaErrorInvalidValue;
   p.stages = stages;
@@ -510,8 +534,6 @@ int fprop_launch(const FpropArgs& a) {
 
   const size_t smem_bytes = (size_t)stages * stage_bytes + out_bytes + 2 * stages * sizeof(uint64_t) + 1024;
   // grid: a multiple of num_n_tiles (every CTA keeps one Cout tile), at most one CTA per SM / per tile
-  int grid = a.num_ctas > 0 ? a.num_ctas : HB_NUM_SMS;
-  if (grid > HB_NUM_SMS * 4) grid = HB_NUM_SMS * 4;
   int per_n = grid / p.num_n_tiles;
   if (per_n < 1) per_n = 1;
   if (per_n > p.num_m_tiles) per_n = p.num_m_tiles;
@@ -528,6 +550,14 @@ int fprop_launch(const FpropArgs& a) {
     case 96: e = launch_fprop<96>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
     case 112: e = launch_fprop<112>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
     case 128: e = launch_fprop<128>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 144: e = launch_fprop<144>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 160: e = launch_fprop<160>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 176: e = launch_fprop<176>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 192: e = launch_fprop<192>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 208: e = launch_fprop<208>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 224: e = launch_fprop<224>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 240: e = launch_fprop<240>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
+    case 256: e = launch_fprop<256>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
     default: return (int)cudaErrorInvalidValue;
   }
   if (e != cudaSuccess) return (int)e;

@@ -95,6 +95,15 @@ __device__ __forceinline__ void fence_regs(float (&r)[N]) {
   for (int i = 0; i < N; ++i) asm volatile("" : "+f"(r[i])::"memory");
 }
 
+// ---- register reallocation between warpgroups ------------------------------------------------
+// Warpgroup-wide (every thread of the warpgroup executes it). A warpgroup that only issues TMA hands registers back to the
+// SM's pool so that the MMA warpgroups of the same CTA can hold wider accumulators. N: a multiple of 8 in [24, 256];
+// the sum over the CTA's warpgroups of 128 * N must fit in the 64 K registers of an SM.
+template <int N>
+__device__ __forceinline__ void regs_release() { asm volatile("setmaxnreg.dec.sync.aligned.u32 %0;" ::"n"(N)); }
+template <int N>
+__device__ __forceinline__ void regs_acquire() { asm volatile("setmaxnreg.inc.sync.aligned.u32 %0;" ::"n"(N)); }
+
 // ---- descriptors ----------------------------------------------------------------------------
 // Shared-memory matrix descriptor of wgmma (sm_90):
 //   [0,14) start>>4 | [16,30) LBO>>4 | [32,46) SBO>>4 | [49,52) base offset | [62,64) layout (1 = 128B swizzle)
