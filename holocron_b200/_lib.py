@@ -63,6 +63,9 @@ SIGNATURES = {
     "hb_dwconv_bwd_data_bf16": "ppp" + "iiiiiiip",
     "hb_dwconv_wgrad_scratch_doubles": "ii",
     "hb_dwconv_bwd_weight_bf16": "ppppp" + "iiiiiiip",
+    "hb_involution_fwd_bf16": "ppp" + "i" * 11 + "p",
+    "hb_involution_bwd_data_bf16": "ppp" + "i" * 11 + "p",
+    "hb_involution_bwd_kernel_bf16": "ppp" + "i" * 11 + "p",
     "hb_gap_fwd_bf16": "ppiiip",
     "hb_gap_bwd_bf16": "ppiiip",
     "hb_gate_act_fwd_bf16": "ppp" + "iiii" + "f" + "p",

@@ -1,5 +1,5 @@
 """Convolution-like modules on the hot path — mirrors holocron/nn/modules/conv.py (NormConv2d :55-147, Add2d :150-248,
-SlimConv2d :251-370, PyConv2d :373-438). Parameter names/shapes are the reference's (state_dict contract)."""
+SlimConv2d :251-370, PyConv2d :373-438, Involution2d :441-499). Parameter names/shapes are the reference's (state_dict contract)."""
 import math
 from typing import Any, List, Optional, Union
 
@@ -11,7 +11,7 @@ from torch.nn.modules.utils import _pair
 
 from .. import functional as F
 
-__all__ = ["Add2d", "NormConv2d", "PyConv2d", "SlimConv2d"]
+__all__ = ["Add2d", "Involution2d", "NormConv2d", "PyConv2d", "SlimConv2d"]
 
 
 class _NormConvNd(_ConvNd):
@@ -133,3 +133,40 @@ class PyConv2d(nn.ModuleList):
         if self.num_levels == 1:
             return conv_bn_act(x, self[0], None, None)
         return torch.cat([conv_bn_act(x, conv, None, None) for conv in self], dim=1)
+
+
+class Involution2d(nn.Module):
+    """Involution (https://arxiv.org/abs/2103.06255): every output pixel applies its own K x K kernel, shared by the
+    channels of a group and generated from the input by ``span(reduce(pool(x)))`` (two 1x1 convolutions with a bias and
+    nothing in between; ``pool`` is an ``AvgPool2d(stride, stride)`` when ``stride > 1`` and ``None`` otherwise).
+
+    Children ``pool, reduce, span, unfold`` as in the reference, created in its order (same seeded init and
+    ``state_dict``); ``unfold`` only carries the configuration. The forward pass runs the average pooling as a library
+    call, both 1x1 convolutions on the tensor-core kernel (``span`` keeps its zero-padded width) and the involution on its
+    own kernels (:mod:`holocron_b200.nn._involution`), which read x once through a shared-memory halo instead of building
+    the N*C*K^2*Ho*Wo unfolded tensor. A bf16 channels_last input takes no layout copy; other dtypes run in bf16 and the
+    output is cast back. Shapes the reference cannot compute raise RuntimeError before any launch; ``kernel_size``
+    outside {1, 3, 5, 7} raises NotImplementedError.
+    """
+
+    def __init__(self, in_channels: int, kernel_size: int, padding: int = 0, stride: int = 1, groups: int = 1,
+                 dilation: int = 1, reduction_ratio: float = 1) -> None:
+        super().__init__()
+        self.groups = groups
+        self.k_size = kernel_size
+        self.pool = nn.AvgPool2d(stride, stride) if stride > 1 else None
+        self.reduce = nn.Conv2d(in_channels, int(in_channels // reduction_ratio), 1)
+        self.span = nn.Conv2d(int(in_channels // reduction_ratio), kernel_size**2 * groups, 1)
+        self.unfold = nn.Unfold(kernel_size, dilation, padding, stride)
+
+    def forward(self, x: Tensor) -> Tensor:
+        from .. import _fused as K
+        from .._involution import check_involution, involution2d
+        u = self.unfold
+        check_involution(x.shape[1], x.shape[2], x.shape[3], self.k_size, u.stride, u.padding, u.dilation, self.groups)
+        xb = K.to_channels_last_bf16(x)
+        kernel = self.pool(xb) if isinstance(self.pool, nn.Module) else xb
+        kernel = K.conv2d(kernel, self.reduce.weight, self.reduce.bias)
+        kernel = K.conv2d(kernel, self.span.weight, self.span.bias, keep_padded=True)
+        y = involution2d(xb, kernel, self.k_size, u.stride, u.padding, u.dilation, self.groups)
+        return y if x.dtype == torch.bfloat16 else y.to(x.dtype)

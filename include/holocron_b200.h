@@ -177,6 +177,19 @@ size_t hb_dwconv_wgrad_scratch_doubles(int C, int K);
 int hb_dwconv_bwd_weight_bf16(const void* x, const void* dy, float* dw, float* db, double* scratch, int N, int H, int W,
                               int C, int K, int stride, int pad, void* stream);
 
+/* ---- involution: holocron/nn/modules/conv.py:441-499 (Involution2d: the unfold, the product with the generated kernel
+ *      and the sum over the taps) -------------------------------------------------------------------------------
+ * x NHWC bf16 [N,H,W,Cp], ker NHWC bf16 [N,Ho,Wo,Kp] with channel g*K*K + t for group g and tap t (Kp >= G*K*K: the
+ * zero-padded span output), y / dy NHWC bf16 [N,Ho,Wo,Cp], Ho = (H + 2*pad - dil*(K-1) - 1) / stride + 1. C % G == 0,
+ * Cp >= C with Cp % 8 == 0 (channels C..Cp-1 of y and dx are written as zeros), K in {1,3,5,7}. dker: every column
+ * of [N,Ho,Wo,Kp] is written, the padding columns G*K*K..Kp-1 as zeros. Deterministic (fixed-order sums, no atomics). */
+int hb_involution_fwd_bf16(const void* x, const void* ker, void* y, int N, int H, int W, int C, int Cp, int Kp, int K,
+                           int G, int stride, int pad, int dil, void* stream);
+int hb_involution_bwd_data_bf16(const void* dy, const void* ker, void* dx, int N, int H, int W, int C, int Cp, int Kp,
+                                int K, int G, int stride, int pad, int dil, void* stream);
+int hb_involution_bwd_kernel_bf16(const void* x, const void* dy, void* dker, int N, int H, int W, int C, int Cp, int Kp,
+                                  int K, int G, int stride, int pad, int dil, void* stream);
+
 /* ---- global average pooling: holocron/nn/modules/downsample.py:58-74 ----------------------------------- */
 int hb_gap_fwd_bf16(const void* x, void* y, int N, int HW, int C, void* stream);
 int hb_gap_bwd_bf16(const void* dy, void* dx, int N, int HW, int C, void* stream);
