@@ -66,6 +66,13 @@ SIGNATURES = {
     "hb_involution_fwd_bf16": "ppp" + "i" * 11 + "p",
     "hb_involution_bwd_data_bf16": "ppp" + "i" * 11 + "p",
     "hb_involution_bwd_kernel_bf16": "ppp" + "i" * 11 + "p",
+    "hb_lambda_content_fwd_bf16": "pppp" + "i" * 12 + "p",
+    "hb_lambda_out_fwd_bf16": "pppppp" + "i" * 12 + "p",
+    "hb_lambda_bwd_content_bf16": "ppppppp" + "i" * 12 + "p",
+    "hb_lambda_dlp_bf16": "ppp" + "i" * 12 + "p",
+    "hb_lambda_bwd_q_bf16": "pppppp" + "i" * 12 + "p",
+    "hb_lambda_bwd_v_bf16": "ppppppp" + "i" * 12 + "p",
+    "hb_lambda_bwd_r_bf16": "pppp" + "i" * 12 + "p",
     "hb_gap_fwd_bf16": "ppiiip",
     "hb_gap_bwd_bf16": "ppiiip",
     "hb_gate_act_fwd_bf16": "ppp" + "iiii" + "f" + "p",

@@ -190,6 +190,36 @@ int hb_involution_bwd_data_bf16(const void* dy, const void* ker, void* dx, int N
 int hb_involution_bwd_kernel_bf16(const void* x, const void* dy, void* dker, int N, int H, int W, int C, int Cp, int Kp,
                                   int K, int G, int stride, int pad, int dil, void* stream);
 
+/* ---- lambda layer: holocron/nn/modules/lambda_layer.py:15-108 (LambdaLayer.forward :70-108: the key softmax :90, the
+ *      content lambda :93-94, the position lambda :97-104 and the output :106-108) ----------------------------------
+ * Every entry takes the same geometry: B samples of H x W positions, dim_k dk in {8,16,32}, dim_u u in 1..4, heads in
+ * 1..8, dim_v dv >= 1, r = the odd local receptive field (1..23, lambda_layer.py:60-64) or 0 for the global variant
+ * (pos_emb, :66-68), and the padded NHWC widths (multiples of 8) of q (channel h*dk+k, Cqp >= heads*dk), k (k*u+u',
+ * Ckp >= dk*u), v (v*u+u', Cvp >= dv*u) and y / dy (h*dv+v, Cop >= heads*dv); every channel past the logical ones of an
+ * output is written as zero. stats [B][dk*u][2] fp32 (row max, sum of exponentials of the key softmax); lc / dlc
+ * [B][dk][dv] fp32; Rt [r*r][u][dk] fp32 (R transposed tap-major); lp [B][HW][dk][dv] fp32 (global only, the GEMM of
+ * pos_emb and v); dlp [B][HW][dk][dvp] bf16, dvp = dv rounded up to 8 (sum_h q * dy, the per-position gradient of lp);
+ * dvpos [B][HW][dv*u] fp32 (global only, pos_emb^T dlp). Deterministic (fixed-order sums, no atomics), no host sync. */
+int hb_lambda_content_fwd_bf16(const void* k, const void* v, float* stats, float* lc, int B, int H, int W, int dk,
+                               int u, int heads, int dv, int r, int Cqp, int Ckp, int Cvp, int Cop, void* stream);
+int hb_lambda_out_fwd_bf16(const void* q, const void* v, const float* Rt, const float* lc, const float* lp, void* y,
+                           int B, int H, int W, int dk, int u, int heads, int dv, int r, int Cqp, int Ckp, int Cvp,
+                           int Cop, void* stream);
+int hb_lambda_bwd_content_bf16(const void* q, const void* k, const void* v, const void* dy, const float* stats,
+                               float* dlc, void* dk_out, int B, int H, int W, int dk, int u, int heads, int dv, int r,
+                               int Cqp, int Ckp, int Cvp, int Cop, void* stream);
+int hb_lambda_dlp_bf16(const void* q, const void* dy, void* dlp, int B, int H, int W, int dk, int u, int heads, int dv,
+                       int r, int Cqp, int Ckp, int Cvp, int Cop, void* stream);
+int hb_lambda_bwd_q_bf16(const void* dy, const void* v, const float* Rt, const float* lc, const float* lp, void* dq,
+                         int B, int H, int W, int dk, int u, int heads, int dv, int r, int Cqp, int Ckp, int Cvp,
+                         int Cop, void* stream);
+int hb_lambda_bwd_v_bf16(const void* k, const float* stats, const float* dlc, const void* dlp, const float* Rt,
+                         const float* dvpos, void* dv_out, int B, int H, int W, int dk, int u, int heads, int dv, int r,
+                         int Cqp, int Ckp, int Cvp, int Cop, void* stream);
+/* dR [dk][u][r*r] fp32 (R's own layout); scratch: B*dk*u*r*r floats of per-sample partials */
+int hb_lambda_bwd_r_bf16(const void* dlp, const void* v, float* scratch, float* dR, int B, int H, int W, int dk, int u,
+                         int heads, int dv, int r, int Cqp, int Ckp, int Cvp, int Cop, void* stream);
+
 /* ---- global average pooling: holocron/nn/modules/downsample.py:58-74 ----------------------------------- */
 int hb_gap_fwd_bf16(const void* x, void* y, int N, int HW, int C, void* stream);
 int hb_gap_bwd_bf16(const void* dy, void* dx, int N, int HW, int C, void* stream);
