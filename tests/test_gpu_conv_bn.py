@@ -2,12 +2,15 @@
 activation kernels, through the C ABI, against the CPU oracle (torch fp32 on the same bf16-rounded inputs).
 
 Tolerances: outputs stored in bf16 -> relative L2 error < 4e-3 (bf16 rounding, 2^-9 rms) and max-abs < 2 bf16 ulp of the
-largest value; fp32 outputs (weight gradients, BN statistics, dgamma/dbeta) -> rel L2 < 1e-3 (north_star)."""
+largest value; fp32 outputs (weight gradients, BN statistics, dgamma/dbeta) -> rel L2 < 1e-3 (north_star). The convolution
+cases also check every element against the per-element bound of tests/_bounds.py."""
 import pytest
 import torch
 import torch.nn.functional as TF
 
 from holocron_b200.nn import _fused as K
+
+from _bounds import FP32_BITS, assert_within, conv_ref, dgrad_ref, wgrad_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -51,6 +54,11 @@ def test_conv2d_forward_backward_vs_oracle(case):
     assert rel_l2(wd.grad, wo.grad) < 1e-3           # fp32 weight gradient
     if cin >= 8:
         assert rel_l2(xd.grad, xo.grad) < 4e-3
+    # per element: fp64 on the same bf16 operands, one ulp of the output type + 1e-5 * sum|terms|
+    assert_within(y, *conv_ref(x, wt, None, stride, pad), "y")
+    assert_within(wd.grad, *wgrad_ref(x, up, k, stride, pad), "dw", bits=FP32_BITS)
+    if cin >= 8:
+        assert_within(xd.grad, *dgrad_ref(x.shape, wt, up, stride, pad), "dx")
 
 
 def test_conv_bias_relu_residual_epilogue():

@@ -8,13 +8,15 @@
 Reference: torch fp32 autograd on the CPU on the same bf16-rounded operands (reference semantics:
 holocron/models/classification/repvgg.py:55-73 = nn.Conv2d 3x3 p1 + nn.Conv2d 1x1 + identity, summed).
 Tolerances: bf16 outputs rel-L2 < 4e-3; fp32 weight gradients < 1e-3 (north_star); deterministic kernels bit-equal
-between two runs."""
+between two runs. Every element also lies within the per-element bound of tests/_bounds.py (fp64 on the same operands)."""
 import numpy as np
 import pytest
 import torch
 import torch.nn.functional as TF
 
 from holocron_b200._lib import lib, ptr, stream_ptr
+
+from _bounds import FP32_BITS, assert_within, dgrad_ref, ulp, wgrad_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -62,6 +64,13 @@ def test_accumulated_block_dgrad(case):
     assert rc == 0, rc
     torch.cuda.synchronize()
     assert rel_l2(out, ref.permute(0, 2, 3, 1)) < 4e-3
+    r, a = dgrad_ref(x.shape, w3, dy3, 1, 1)
+    if nextra >= 1:
+        r1, a1 = dgrad_ref(x.shape, w1, dy1)
+        r, a = r + r1, a + a1
+    if nextra >= 2:
+        r, a = r + dxid.double(), a + dxid.double().abs()
+    assert_within(out.permute(0, 3, 1, 2), r, a, "dX")
 
 
 def test_accum_reports_unsupported_shapes():
@@ -105,6 +114,15 @@ def test_parity_class_stride2_dgrad(case):
     assert rc == 0, rc
     torch.cuda.synchronize()
     assert rel_l2(dx[..., :cin], ref.permute(0, 2, 3, 1)) < 4e-3
+    r, a = dgrad_ref((n, cin, h, w), w3, dy3, 2, 1)
+    slack = None
+    if with1x1:
+        # the 1x1 branch is stored (bf16) first; class (0, 0) of the 3x3 part is rounded to bf16 and added onto it
+        r1, a1 = dgrad_ref((n, cin, h, w), w1, dy1, 2, 0)
+        slack = torch.zeros_like(r)
+        slack[:, :, ::2, ::2] = 0.5 * (ulp(r) + ulp(r1))[:, :, ::2, ::2]
+        r, a = r + r1, a + a1
+    assert_within(dx[..., :cin].permute(0, 3, 1, 2), r, a, "dX", slack=slack)
     assert bool((dx[..., cin:] == 0).all())           # padded channels: written, exactly zero
     assert torch.isfinite(dx.float()).all()            # every element of dx is written by exactly one class
 
@@ -134,6 +152,13 @@ def test_block_wgrad_one_pass(case):
     assert torch.equal(outs[0], outs[1])               # fixed-order reduction: bit-reproducible
     assert rel_l2(outs[0][:cout * 9 * cin].view(cout, 3, 3, cin), g3.permute(0, 2, 3, 1)) < 1e-3
     assert rel_l2(outs[0][cout * 9 * cin:].view(cout, 1, 1, cin), g1.permute(0, 2, 3, 1)) < 1e-3
+    dw = outs[0].cpu()
+    r3, a3 = wgrad_ref(x, dy3, 3, 1, 1)
+    r1, a1 = wgrad_ref(x, dy1, 1)
+    assert_within(dw[:cout * 9 * cin].view(cout, 3, 3, cin), r3.permute(0, 2, 3, 1), a3.permute(0, 2, 3, 1), "dW3",
+                  bits=FP32_BITS)
+    assert_within(dw[cout * 9 * cin:].view(cout, 1, 1, cin), r1.permute(0, 2, 3, 1), a1.permute(0, 2, 3, 1), "dW1",
+                  bits=FP32_BITS)
 
 
 def test_generic_wgrad_is_deterministic_with_workspace():
@@ -156,6 +181,8 @@ def test_generic_wgrad_is_deterministic_with_workspace():
     y = TF.conv2d(x.permute(0, 3, 1, 2).float(), wt, padding=1)
     (g,) = torch.autograd.grad(y, wt, dy.permute(0, 3, 1, 2).float())
     assert rel_l2(outs[0], g.permute(0, 2, 3, 1)) < 1e-3
+    r, a = wgrad_ref(x.permute(0, 3, 1, 2), dy.permute(0, 3, 1, 2), 3, 1, 1)
+    assert_within(outs[0].cpu(), r.permute(0, 2, 3, 1), a.permute(0, 2, 3, 1), "dW", bits=FP32_BITS)
 
 
 def test_multi_tensor_filter_packing_matches_single():

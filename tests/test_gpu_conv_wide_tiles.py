@@ -6,12 +6,15 @@ least one tile per SM, so these shapes are sized for it (2 x 92 x 92 output pixe
 two). Covered: 1x1, 3x3 and stride-2 forward, the stride-1 data gradient with a K extension and an epilogue residual,
 and the parity-class stride-2 data gradient. A launch with output-column statistics keeps the narrow tiles (so the
 partial sums are grouped as before); its output must equal, bit for bit, the same convolution on the wide tiles, and
-its partials must match sums over that output and repeat bit for bit."""
+its partials must match sums over that output and repeat bit for bit. Besides the relative L2 bar, every element must lie
+within the per-element bound of tests/_bounds.py."""
 import pytest
 import torch
 import torch.nn.functional as TF
 
 from holocron_b200.nn import _fused as K
+
+from _bounds import assert_within, conv_ref, dgrad_ref, epilogue_ref, ulp
 
 pytestmark = pytest.mark.gpu
 
@@ -55,6 +58,7 @@ def test_fprop_wide_tiles_vs_oracle(name):
     wf = w.permute(0, 2, 3, 1).contiguous().cuda()
     y = K.conv2d_forward_raw(cl(x), wf, cout, k, k, stride, k // 2, 1, bias.cuda())
     assert rel_l2(y, ref) < 4e-3
+    assert_within(y, *conv_ref(x, w, bias, stride, k // 2), name)
 
 
 @pytest.mark.parametrize("cd", [192, 256])
@@ -69,6 +73,10 @@ def test_dgrad_kext_residual_wide_tiles(cd):
     y = K.conv2d_forward_raw(cl(dy3), wd3.permute(0, 2, 3, 1).contiguous().cuda(), cd, 3, 3, 1, 1, 1, None, cl(dxid),
                              K.ACT_NONE, xe=cl(dy1), we=wd1.permute(0, 2, 3, 1).contiguous().cuda(), kind="dgrad")
     assert rel_l2(y, ref) < 4e-3
+    r3, a3 = conv_ref(dy3, wd3, None, 1, 1)
+    r1, a1 = conv_ref(dy1, wd1)
+    ref, a, slack = epilogue_ref(r3 + r1, a3 + a1, dxid)             # residual added to the bf16-rounded sum
+    assert_within(y, ref, a, "dX", slack=slack)
 
 
 @pytest.mark.parametrize("h", [184, 183, 12])
@@ -88,6 +96,12 @@ def test_dgrad_s2_parity_classes_cd192(h):
     wd1 = w1.permute(1, 2, 3, 0).contiguous().cuda()   # [Cd, 1, 1, C]
     dx = K.dgrad_s2_raw(cl(dy3), torch.nn.Parameter(w3.cuda()), cd, h, h, cl(dy1), wd1)
     assert rel_l2(dx, ref) < 4e-3
+    # the 1x1 branch is stored (bf16) first; class (0, 0) of the 3x3 part is rounded to bf16 and added onto it
+    r3, a3 = dgrad_ref((n, cd, h, h), w3, dy3, 2, 1)
+    r1, a1 = dgrad_ref((n, cd, h, h), w1, dy1, 2, 0)
+    slack = torch.zeros_like(r3)
+    slack[:, :, ::2, ::2] = 0.5 * (ulp(r3) + ulp(r1))[:, :, ::2, ::2]
+    assert_within(dx, r3 + r1, a3 + a1, "dX", slack=slack)
 
 
 @pytest.mark.parametrize("shape", [(2, 92, 192, 192), (2, 42, 128, 1280), (1, 8, 128, 256)])
@@ -107,6 +121,7 @@ def test_stats_launch_matches_wide_tiles(shape):
     # same accumulation order per output element whatever the Cout tile: the plain launch (wide tiles where the layer
     # allows them) gives the statistics launch's output bit for bit
     assert torch.equal(K.conv2d_forward_raw(x, wf, cout, 3, 3, 1, 1, 1), y1)
+    assert_within(y1, *conv_ref(x, wf.permute(0, 3, 1, 2), None, 1, 1), "y")
     yf = y1.double().permute(0, 2, 3, 1).reshape(-1, cout)
     tot = p1.double().sum(0)
     torch.testing.assert_close(tot[:, 0], yf.sum(0), rtol=1e-4, atol=1e-2)

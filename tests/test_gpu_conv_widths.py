@@ -2,12 +2,15 @@
 Cin tile (weight gradient) are template parameters, one kernel instantiation per multiple of 16 up to 128, so each
 width is its own code: run all of them through forward, data gradient and weight gradient, for the generic
 implicit-GEMM kernels (1x1, 3x3 on a grid narrower than 8 pixels, stride 2) and the row-window kernels (3x3 stride 1).
-Tolerances as in test_gpu_conv_bn.py: bf16 outputs rel L2 < 4e-3, fp32 weight gradients rel L2 < 1e-3."""
+Tolerances as in test_gpu_conv_bn.py: bf16 outputs rel L2 < 4e-3, fp32 weight gradients rel L2 < 1e-3, and every element
+within the per-element bound of tests/_bounds.py."""
 import pytest
 import torch
 import torch.nn.functional as TF
 
 from holocron_b200.nn import _fused as K
+
+from _bounds import FP32_BITS, assert_within, conv_ref, dgrad_ref, wgrad_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -45,3 +48,6 @@ def test_conv_every_width_vs_oracle(width, kind):
     assert rel_l2(y, yo) < 4e-3
     assert rel_l2(xd.grad, xo.grad) < 4e-3
     assert rel_l2(wd.grad, wo.grad) < 1e-3
+    assert_within(y, *conv_ref(x, wt, None, stride, pad), "y")
+    assert_within(xd.grad, *dgrad_ref(x.shape, wt, up, stride, pad), "dx")
+    assert_within(wd.grad, *wgrad_ref(x, up, k, stride, pad), "dw", bits=FP32_BITS)

@@ -18,6 +18,8 @@ from holocron_b200.distributed import GradBucket
 from holocron_b200.models.classification.repvgg import RepBlock
 from holocron_b200.nn import _fused as K
 
+from _bounds import assert_within, conv_ref, epilogue_ref
+
 pytestmark = pytest.mark.gpu
 
 
@@ -66,6 +68,8 @@ def test_dual_output_conv_and_epilogue_statistics(case):
     y3, y1 = K.conv2d_forward_raw(_cl(x), wf3, cout, 3, 3, stride, 1, 1, w2=wf1, want_stats=True)
     assert y3.shape == r3.shape and y1.shape == r1.shape
     assert rel_l2(y3, r3) < 4e-3 and rel_l2(y1, r1) < 4e-3
+    assert_within(y3, *conv_ref(x, w3, None, stride, 1), "y3")
+    assert_within(y1, *conv_ref(x, w1, None, stride, 0), "y1")
     # statistics are those of the STORED bf16 tensors
     assert rel_l2(_stats_of(y3), _ref_stats(y3)) < 1e-5
     assert rel_l2(_stats_of(y1), _ref_stats(y1)) < 1e-5
@@ -88,6 +92,7 @@ def test_single_conv_statistics_all_paths(case):
     ref = TF.conv2d(x.float(), wt.float(), None, 1, k // 2)
     y = K.conv2d_forward_raw(_cl(x), wt.permute(0, 2, 3, 1).contiguous().cuda(), cout, k, k, 1, k // 2, 1, want_stats=True)
     assert rel_l2(y, ref) < 4e-3
+    assert_within(y, *conv_ref(x, wt, None, 1, k // 2), "y")
     assert rel_l2(_stats_of(y), _ref_stats(y)) < 1e-5
 
 
@@ -106,6 +111,10 @@ def test_k_extension_with_residual(case):
     y = K.conv2d_forward_raw(_cl(d3), w3.permute(0, 2, 3, 1).contiguous().cuda(), cd, 3, 3, 1, 1, 1, None,
                              _cl(res) if with_res else None, K.ACT_NONE, xe=_cl(d1), we=w1.permute(0, 2, 3, 1).contiguous().cuda())
     assert rel_l2(y, ref) < 4e-3
+    r3, a3 = conv_ref(d3, w3, None, 1, 1)
+    r1, a1 = conv_ref(d1, w1)
+    ref, a, slack = epilogue_ref(r3 + r1, a3 + a1, res if with_res else None)
+    assert_within(y, ref, a, "y", slack=slack)
 
 
 def test_bn_forward_emits_output_statistics_and_is_deterministic():

@@ -10,23 +10,11 @@ from holocron_b200.nn import _fused as K
 from holocron_b200.nn._involution import involution2d
 
 import _involution_oracle as O
+from _bounds import assert_within as _assert_within
 from conftest import load_golden
 
 pytestmark = pytest.mark.gpu
 DEV = torch.device("cuda", 0)
-
-
-def _ulp(ref: torch.Tensor) -> torch.Tensor:
-    """One bf16 ulp at each reference value (8 significant bits)."""
-    a = ref.abs().clamp_min(2.0 ** -126)
-    return torch.exp2(torch.floor(torch.log2(a)) - 7)
-
-
-def _assert_within(got: torch.Tensor, ref: torch.Tensor, abs_sum: torch.Tensor, what: str):
-    err = (got.double() - ref).abs()
-    bound = _ulp(ref) + 1e-5 * abs_sum
-    bad = err > bound
-    assert not bad.any(), f"{what}: {int(bad.sum())} elements off, worst excess {float((err - bound).max()):.3e}"
 
 
 def _cl(t: torch.Tensor) -> torch.Tensor:
