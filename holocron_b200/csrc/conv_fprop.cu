@@ -19,20 +19,17 @@
 //                 128-bit stores (+ residual add in that pass). The producer meanwhile fills the ring for the
 //                 next tile.
 #include <stdlib.h>
-#include "common.cuh"
-#include "tc_common.cuh"
-#include "tmap.cuh"
+#include "conv_common.cuh"
 #include "holocron_b200.h"
 
 namespace {
 
 using namespace tc;
+using namespace conv;
 
 constexpr int kBM = 128;          // output pixels per tile
 constexpr int kBK = 64;           // channels per K block (one 128-byte swizzle row)
 constexpr int kMmaK = 16;         // K per wgmma for 16-bit inputs
-constexpr int kThreads = 384;     // producer warpgroup + 2 consumer warpgroups
-constexpr int kConsumers = 256;
 constexpr int kProducerRegs = 40;   // per thread after setmaxnreg: 128 x (40 + 2 x 232) = 64 512 <= 64 K registers
 constexpr int kConsumerRegs = 232;
 constexpr int kABytes = kBM * kBK * 2;  // 16 KiB
@@ -61,9 +58,8 @@ struct FpropParams {
   int act;            // 0 none, 1 relu
   __nv_bfloat16* y;
   __nv_bfloat16* y2;              // dual mode: second output (same addressing as y)
-  // optional per-channel statistics of the bf16 OUTPUT (what the BatchNorm that follows normalises): float
-  // [slots][Cout][2] = (sum, sum of squares) partials, slot = (blockIdx.x / num_n_tiles) * 2 + consumer warpgroup;
-  // every (slot, channel) is written exactly once and the consumer adds the slots in a fixed order (deterministic)
+  // optional per-channel statistics of the bf16 OUTPUT (what the BatchNorm that follows normalises), in the slot format
+  // of conv_common.cuh, slot = (blockIdx.x / num_n_tiles) * 2 + consumer warpgroup
   float* stats;
   float* stats2;
   const float* bias;              // [Cout] or null
@@ -77,8 +73,6 @@ struct FpropParams {
   // (i*o_step + o_a, j*o_step + o_b) of an OH x OW image (the parity classes of a strided data gradient)
   int scatter, OH, OW, o_step, o_a, o_b;
 };
-
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // kStats: the epilogue also accumulates the output-column statistics (separate instantiation: the plain kernel carries
 // neither the extra registers nor the extra shared-memory pass in its instruction stream).
@@ -120,7 +114,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
     // ================= TMA producer =================
     regs_release<kProducerRegs>();
     if (warp == 0 && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+      Ring ring;
       for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
         const int m0 = m_tile * kBM;
         const int q0 = m0 % p.Wo, p0 = (m0 / p.Wo) % p.Ho, n0 = m0 / (p.Wo * p.Ho);
@@ -128,33 +122,34 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         for (int tap = 0; tap < p.R * p.S; ++tap) {
           const int r = tap / p.S, s = tap % p.S;
           for (int cb = 0; cb < p.cblocks; ++cb) {
-            mbar_wait(&empty_bar[stage], phase ^ 1);
-            uint8_t* sa = smem + (size_t)stage * stage_bytes;
+            uint64_t* bar = &full_bar[ring.stage];
+            mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+            uint8_t* sa = smem + (size_t)ring.stage * stage_bytes;
             uint8_t* sb = sa + kABytes;
-            mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
+            mbar_arrive_expect_tx(bar, tx_bytes);
             if (p.a_mode == 1)
-              tma_load_im2col_4d(&tmA, &full_bar[stage], sa, cb * kBK, base_w, base_h, n0,
-                                 (uint16_t)(s * p.dil), (uint16_t)(r * p.dil));
+              tma_load_im2col_4d(&tmA, bar, sa, cb * kBK, base_w, base_h, n0, (uint16_t)(s * p.dil), (uint16_t)(r * p.dil));
             else
-              tma_load_2d(&tmA, &full_bar[stage], sa, cb * kBK, m0);
-            tma_load_3d(&tmB, &full_bar[stage], sb, cb * kBK, tap, n_tile * BN);
-            if (++stage == p.stages) { stage = 0; phase ^= 1; }
+              tma_load_2d(&tmA, bar, sa, cb * kBK, m0);
+            tma_load_3d(&tmB, bar, sb, cb * kBK, tap, n_tile * BN);
+            ring.next(p.stages);
           }
         }
         for (int cb = 0; cb < p.e_cblocks; ++cb) {
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + (size_t)stage * stage_bytes;
+          uint64_t* bar = &full_bar[ring.stage];
+          mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+          uint8_t* sa = smem + (size_t)ring.stage * stage_bytes;
           uint8_t* sb = sa + kABytes;
-          mbar_arrive_expect_tx(&full_bar[stage], tx_bytes);
+          mbar_arrive_expect_tx(bar, tx_bytes);
           if (p.e_mode == 1)
-            tma_load_2d(&tmA2, &full_bar[stage], sa, cb * kBK, m0);
+            tma_load_2d(&tmA2, bar, sa, cb * kBK, m0);
           else if (p.a_mode == 1)
-            tma_load_im2col_4d(&tmA, &full_bar[stage], sa, cb * kBK, base_w, base_h, n0,
-                               (uint16_t)((p.S / 2) * p.dil), (uint16_t)((p.R / 2) * p.dil));
+            tma_load_im2col_4d(&tmA, bar, sa, cb * kBK, base_w, base_h, n0, (uint16_t)((p.S / 2) * p.dil),
+                               (uint16_t)((p.R / 2) * p.dil));
           else
-            tma_load_2d(&tmA, &full_bar[stage], sa, cb * kBK, m0);
-          tma_load_3d(&tmB2, &full_bar[stage], sb, cb * kBK, 0, n_tile * BN);
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+            tma_load_2d(&tmA, bar, sa, cb * kBK, m0);
+          tma_load_3d(&tmB2, bar, sb, cb * kBK, 0, n_tile * BN);
+          ring.next(p.stages);
         }
       }
     }
@@ -177,30 +172,30 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
   const int ngroups = p.nout * gpo;
   // column statistics: this thread's running (sum0, sum1, sumsq0, sumsq1) of one column PAIR of each group over a fixed
   // subset of its warpgroup's 64 tile rows, kept in registers across all tiles of the CTA
-  float st[4][4];
+  float4 st[4];
 #pragma unroll
-  for (int gi = 0; gi < 4; ++gi) { st[gi][0] = st[gi][1] = st[gi][2] = st[gi][3] = 0.f; }
+  for (int gi = 0; gi < 4; ++gi) st[gi] = make_float4(0.f, 0.f, 0.f, 0.f);
   const int col_base = n_tile * BN;
   const int ncols_valid = min(BN, p.Cout - col_base);          // multiple of 16
   // accumulator columns: BN, or 2 x BN for the second output of dual mode (only possible for BN <= 64)
   constexpr int kCols = BN <= 64 ? 2 * BN : BN;
   float acc[kCols / 2];
-  int stage = 0; uint32_t phase = 0;
+  Ring ring;
 
   for (int m_tile = m_first; m_tile < p.num_m_tiles; m_tile += m_step) {
     // ---- main loop: one commit group per K block; one block stays in flight while the stage of the previous one
     // is handed back to the producer ----
     int prev = -1;
     auto next_block = [&](uint32_t& a_lo, uint32_t& b_lo) {
-      mbar_wait(&full_bar[stage], phase);
-      a_lo = a_lo0 + (uint32_t)stage * stage_lo;
-      b_lo = desc_lo(smem_u32(smem), 16) + (uint32_t)stage * stage_lo + (kABytes >> 4);
+      mbar_wait(&full_bar[ring.stage], ring.phase);
+      a_lo = a_lo0 + (uint32_t)ring.stage * stage_lo;
+      b_lo = desc_lo(smem_u32(smem), 16) + (uint32_t)ring.stage * stage_lo + (kABytes >> 4);
     };
     auto retire_prev = [&]() {
       wgmma_wait<1>();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);   // the MMAs that read stage `prev` are done
-      prev = stage;
-      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      prev = ring.stage;
+      ring.next(p.stages);
     };
     for (int kb = 0, cb = 0; kb < kblocks; ++kb) {
       uint32_t a_lo, b_lo;
@@ -316,15 +311,7 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
           for (int u = 0; u < 4; ++u) {
             if (!ok[u]) continue;
             uint4 val = *reinterpret_cast<const uint4*>(sout + sidx[u]);
-            __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(&val);
-            const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&rv[u]);
-#pragma unroll
-            for (int jj = 0; jj < 4; ++jj) {
-              float2 fa = __bfloat1622float2(a[jj]), fb = __bfloat1622float2(b[jj]);
-              fa.x += fb.x; fa.y += fb.y;
-              if (p.act == 1) { fa.x = hb::relu_nan(fa.x); fa.y = hb::relu_nan(fa.y); }
-              a[jj] = __floats2bfloat162_rn(fa.x, fa.y);
-            }
+            add_residual16(val, rv[u], p.act == 1);
             *reinterpret_cast<uint4*>(yo + off[u]) = val;
           }
         }
@@ -337,20 +324,16 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
         const int row_end = min(64 * wg + 64, rows_valid);
         if (rg < rgs && g0 + pr * 2 < ncols_valid) {
           const uint8_t* sp = sout + pr * 4;
-          float s0 = 0.f, s1 = 0.f, q0 = 0.f, q1 = 0.f;
-          for (int rr = 64 * wg + rg; rr < row_end; rr += rgs) {
-            const float2 f = __bfloat1622float2(*reinterpret_cast<const __nv_bfloat162*>(sp + (size_t)rr * p.out_pitch));
-            s0 += f.x; s1 += f.y; q0 = fmaf(f.x, f.x, q0); q1 = fmaf(f.y, f.y, q1);
-          }
+          float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+          for (int rr = 64 * wg + rg; rr < row_end; rr += rgs) accum_pair(s, sp + (size_t)rr * p.out_pitch);
 #pragma unroll
           for (int g = 0; g < 4; ++g)
-            if (g == gi) { st[g][0] += s0; st[g][1] += s1; st[g][2] += q0; st[g][3] += q1; }
+            if (g == gi) { st[g].x += s.x; st[g].y += s.y; st[g].z += s.z; st[g].w += s.w; }
         }
       }
     }
   }
-  // ---- statistics: fold the row subsets in a fixed order and write this (CTA, warpgroup)'s partial (every slot is
-  // written, zeros included, so the consumer can add all slots without a memset)
+  // ---- statistics: fold the row subsets in a fixed order and write this (CTA, warpgroup)'s partial
   if (kStats && (p.stats || p.stats2)) {
     const int slot = (blockIdx.x / p.num_n_tiles) * 2 + wg;
 #pragma unroll
@@ -364,32 +347,13 @@ conv_fprop_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant
       const int npairs = gw >> 1, rgs = 128 / npairs;
       consumer_sync();
       float4* scratch = reinterpret_cast<float4*>(sout) + wg * 128;   // [2][128] float4, 4 KB <= staging tile
-      scratch[wet] = make_float4(st[gi][0], st[gi][1], st[gi][2], st[gi][3]);
+      scratch[wet] = st[gi];
       consumer_sync();
-      if (wet < gw && g0 + wet < ncols_valid) {
-        const int pr = wet >> 1, hi = wet & 1;
-        float sv = 0.f, qv = 0.f;
-        for (int rg = 0; rg < rgs; ++rg) {
-          const float4 v = scratch[rg * npairs + pr];
-          sv += hi ? v.y : v.x;
-          qv += hi ? v.w : v.z;
-        }
-        float2* dst = reinterpret_cast<float2*>(so + ((size_t)slot * p.Cout + col_base + g0 + wet) * 2);
-        *dst = make_float2(sv, qv);
-      }
+      if (wet < gw && g0 + wet < ncols_valid)
+        store_stats(so, slot, p.Cout, col_base + g0 + wet, fold_stats(scratch, rgs, npairs, wet));
     }
   }
 }
-
-}  // namespace
-
-// conv_rows.cu: shared-memory-reuse kernel for stride-1 3x3 layers whose filter fits in shared memory
-int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, const void* residual, int N, int H, int W,
-                     int Cin, int Cout, int act, int num_ctas, cudaStream_t stream, int nextra = 0,
-                     const void* const* xe = nullptr, const void* const* we = nullptr, float* stats = nullptr,
-                     int* stat_slots = nullptr);
-
-namespace {
 
 struct FpropArgs {
   const void* x; const void* w; void* y; const float* bias; const void* residual;
@@ -405,34 +369,6 @@ struct FpropArgs {
   const float* norm_mean; const float* norm_rstd; const float* norm_wsum;
   cudaStream_t stream;
 };
-
-// one instantiation per Cout tile width, with and without the statistics epilogue
-template <bool kStats, int BN>
-cudaError_t launch_fprop_kernel(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
-                                const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2,
-                                const FpropParams& p) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e =
-        cudaFuncSetAttribute(conv_fprop_kernel<kStats, BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, kSmemMax);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  conv_fprop_kernel<kStats, BN><<<grid, kThreads, smem_bytes, stream>>>(tmA, tmB, tmA2, tmB2, p);
-  return cudaSuccess;
-}
-
-template <int BN>
-cudaError_t launch_fprop(bool stats, int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmA,
-                         const CUtensorMap& tmB, const CUtensorMap& tmA2, const CUtensorMap& tmB2, const FpropParams& p) {
-  if constexpr (BN > 128) {   // wide tiles never carry the statistics epilogue (see fprop_launch)
-    if (stats) return cudaErrorInvalidValue;
-    return launch_fprop_kernel<false, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p);
-  } else {
-    return stats ? launch_fprop_kernel<true, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p)
-                 : launch_fprop_kernel<false, BN>(grid, smem_bytes, stream, tmA, tmB, tmA2, tmB2, p);
-  }
-}
 
 int fprop_launch(const FpropArgs& a) {
   const int Cin = a.Cin, Cout = a.Cout, R = a.R, S = a.S;
@@ -499,38 +435,15 @@ int fprop_launch(const FpropArgs& a) {
   if (p.norm_mean && (!p.norm_rstd || !p.norm_wsum || a.scatter)) return (int)cudaErrorInvalidValue;
 
   CUtensorMap tmA, tmB, tmA2, tmB2;
-  int rc;
-  if (p.a_mode == 0) {
-    uint64_t dims[2] = {(uint64_t)Cin, (uint64_t)p.m_total};
-    uint64_t strides[1] = {(uint64_t)Cin * 2};
-    uint32_t box[2] = {kBK, kBM};
-    rc = tmap::encode_tiled_bf16(&tmA, a.x, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-  } else {
-    rc = tmap::encode_im2col_bf16(&tmA, a.x, a.N, a.H, a.W, Cin, a.pad_h, a.pad_w, R, S, a.dil, a.stride, kBK, kBM,
-                                  CU_TENSOR_MAP_SWIZZLE_128B, a.pad_after_h, a.pad_after_w);
-  }
+  int rc = p.a_mode == 0 ? tmap::encode_matrix(&tmA, a.x, p.m_total, Cin, kBM)
+                         : tmap::encode_im2col_bf16(&tmA, a.x, a.N, a.H, a.W, Cin, a.pad_h, a.pad_w, R, S, a.dil,
+                                                    a.stride, kBK, kBM, CU_TENSOR_MAP_SWIZZLE_128B, a.pad_after_h,
+                                                    a.pad_after_w);
   if (rc) return rc;
-  {
-    uint64_t dims[3] = {(uint64_t)Cin, (uint64_t)(R * S), (uint64_t)Cout};
-    uint64_t strides[2] = {(uint64_t)Cin * 2, (uint64_t)R * S * Cin * 2};
-    uint32_t box[3] = {kBK, 1, (uint32_t)BN};
-    rc = tmap::encode_tiled_bf16(&tmB, a.w, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
+  if ((rc = tmap::encode_krsc_slab(&tmB, a.w, Cout, R * S, Cin, BN))) return rc;
   tmA2 = tmA; tmB2 = tmB;   // unused slots alias the main maps (never dereferenced by the kernel)
-  if (kext) {
-    uint64_t dims[2] = {(uint64_t)a.Ce, (uint64_t)p.m_total};
-    uint64_t strides[1] = {(uint64_t)a.Ce * 2};
-    uint32_t box[2] = {kBK, kBM};
-    if ((rc = tmap::encode_tiled_bf16(&tmA2, a.xe, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B))) return rc;
-  }
-  if (p.e_mode) {
-    uint64_t dims[3] = {(uint64_t)ce, 1, (uint64_t)Cout};
-    uint64_t strides[2] = {(uint64_t)ce * 2, (uint64_t)ce * 2};
-    uint32_t box[3] = {kBK, 1, (uint32_t)BN};
-    if ((rc = tmap::encode_tiled_bf16(&tmB2, kext ? a.we : a.w2, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)))
-      return rc;
-  }
+  if (kext && (rc = tmap::encode_matrix(&tmA2, a.xe, p.m_total, a.Ce, kBM))) return rc;
+  if (p.e_mode && (rc = tmap::encode_krsc_slab(&tmB2, kext ? a.we : a.w2, Cout, 1, ce, BN))) return rc;
 
   const size_t smem_bytes = (size_t)stages * stage_bytes + out_bytes + 2 * stages * sizeof(uint64_t) + 1024;
   // grid: a multiple of num_n_tiles (every CTA keeps one Cout tile), at most one CTA per SM / per tile
@@ -540,29 +453,18 @@ int fprop_launch(const FpropArgs& a) {
   grid = per_n * p.num_n_tiles;
   if (a.stat_slots) *a.stat_slots = 2 * per_n;
   const bool stats = p.stats || p.stats2;
-  cudaError_t e;
-  switch (BN) {
-    case 16: e = launch_fprop<16>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 32: e = launch_fprop<32>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 48: e = launch_fprop<48>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 64: e = launch_fprop<64>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 80: e = launch_fprop<80>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 96: e = launch_fprop<96>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 112: e = launch_fprop<112>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 128: e = launch_fprop<128>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 144: e = launch_fprop<144>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 160: e = launch_fprop<160>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 176: e = launch_fprop<176>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 192: e = launch_fprop<192>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 208: e = launch_fprop<208>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 224: e = launch_fprop<224>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 240: e = launch_fprop<240>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    case 256: e = launch_fprop<256>(stats, grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  if (e != cudaSuccess) return (int)e;
-  HB_LAUNCH_CHECK();
-  return 0;
+  // one instantiation per Cout tile width, with and without the statistics epilogue; wide tiles never carry the
+  // statistics epilogue (see the Cout tile rule above)
+  return (int)dispatch_width<16, 256>(BN, [&](auto bn) {
+    constexpr int kBN = decltype(bn)::value;
+    if constexpr (kBN > 128) {
+      if (stats) return cudaErrorInvalidValue;
+      return launch<conv_fprop_kernel<false, kBN>>(grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p);
+    } else {
+      return stats ? launch<conv_fprop_kernel<true, kBN>>(grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p)
+                   : launch<conv_fprop_kernel<false, kBN>>(grid, smem_bytes, a.stream, tmA, tmB, tmA2, tmB2, p);
+    }
+  });
 }
 
 }  // namespace
@@ -604,8 +506,7 @@ int hb_conv2d_fused_bf16(const hb_conv_args* c, int* stat_slots, void* stream) {
     if (rows_enabled) {
       const int rc = hb_conv_rows_try(c->x, c->w, c->y, c->bias, c->residual, N, H, W, Cin, Cout, c->act, c->num_ctas,
                                       (cudaStream_t)stream, 0, nullptr, nullptr, c->stats, stat_slots);
-      if (rc == 0) return 0;
-      if (rc == -2) return (int)cudaErrorLaunchFailure;
+      if (rc != (int)cudaErrorNotSupported) return rc;
     }
   }
   FpropArgs a{};

@@ -16,16 +16,12 @@
 // Warp roles: one TMA producer warpgroup and two consumer warpgroups (rows 0-63 and 64-127 of every sub-tile) that
 // issue the wgmma chain of a sub-tile and then run its epilogue (accumulator registers -> bf16 staging tile in shared
 // memory -> coalesced 128-bit stores); the producer meanwhile loads the next tile's rows into the other ring slot.
-#include "common.cuh"
-#include "tc_common.cuh"
-#include "tmap.cuh"
+#include "conv_common.cuh"
 
 namespace {
 
 using namespace tc;
-
-constexpr int kThreads = 384;      // producer warpgroup + 2 consumer warpgroups
-constexpr int kConsumers = 256;
+using namespace conv;
 
 struct RowsParams {
   int N, H, W, Cin, Cout;
@@ -47,10 +43,8 @@ struct RowsParams {
   __nv_bfloat16* y;
   const float* bias;
   const __nv_bfloat16* residual;
-  float* stats;      // optional [2 * gridDim.x][Cout][2] (sum, sum of squares) partials of the bf16 output, see conv_fprop.cu
+  float* stats;      // optional statistics of the bf16 output, 2 * gridDim.x slots (conv_common.cuh)
 };
-
-__device__ __forceinline__ void consumer_sync() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // BN = Cout (a multiple of 16 up to 128), the N of every wgmma
 template <int BN>
@@ -92,23 +86,22 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         for (int cb = 0; cb < p.CB; ++cb)
           tma_load_3d(e == 0 ? &tmWe0 : &tmWe1, w_bar, wsm + (size_t)((9 + e) * p.CB + cb) * p.w_tap_bytes, cb * 64, 0, 0);
       const uint32_t tx = (uint32_t)(p.CB * ((p.TRO + 2) + p.nextra * p.TRO) * p.Wp * 128);
-      int it = 0;   // ring slot = it % nstages, phase = (it / nstages) & 1
+      int it = 0;
       for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
         const int n = tile / p.tiles_per_img, p0 = (tile % p.tiles_per_img) * p.TRO;
-        const int st = it % p.nstages;
-        mbar_wait(&empty_bar[st], ((it / p.nstages) & 1) ^ 1);
-        mbar_arrive_expect_tx(&full_bar[st], tx);
+        const Ring ring = Ring::at(it, p.nstages);
+        mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+        mbar_arrive_expect_tx(&full_bar[ring.stage], tx);
         for (int b = 0; b <= p.nextra; ++b) {
           const CUtensorMap* tm = b == 0 ? &tmX : (b == 1 ? &tmXe0 : &tmXe1);
           const int h0 = b == 0 ? p0 - 1 : p0;   // the extra sources need no row halo (centre tap only)
           for (int cb = 0; cb < p.CB; ++cb) {
             // box (64 ch, Wp, rows, 1 image) at (c, w = -1, h0, n): halo and image borders = OOB zero fill
-            asm volatile(
-                "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-                ::"r"(smem_u32(stage0 + (size_t)st * p.stage_bytes + (size_t)p.CB * (b ? p.cb_bytes + (b - 1) * p.ecb_bytes : 0) +
-                               (size_t)cb * (b ? p.ecb_bytes : p.cb_bytes))),
-                  "l"(reinterpret_cast<uint64_t>(tm)), "r"(smem_u32(&full_bar[st])), "r"(cb * 64), "r"(-1), "r"(h0), "r"(n)
-                : "memory");
+            tma_load_4d(tm, &full_bar[ring.stage],
+                        stage0 + (size_t)ring.stage * p.stage_bytes +
+                            (size_t)p.CB * (b ? p.cb_bytes + (b - 1) * p.ecb_bytes : 0) +
+                            (size_t)cb * (b ? p.ecb_bytes : p.cb_bytes),
+                        cb * 64, -1, h0, n);
           }
         }
       }
@@ -131,16 +124,17 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
   const int npairs = BN >> 1, rgs = kConsumers / npairs;
   const int st_rg = et / npairs, st_pr = et - st_rg * npairs;
   const bool st_on = p.stats != nullptr && st_rg < rgs;
-  float st0 = 0.f, st1 = 0.f, sq0 = 0.f, sq1 = 0.f;
+  float4 stat = make_float4(0.f, 0.f, 0.f, 0.f);
   float acc[64];
   mbar_wait(w_bar, 0);
   int it = 0;
   for (int tile = blockIdx.x; tile < p.num_tiles; tile += gridDim.x, ++it) {
-    const int st = it % p.nstages;
     const int n = tile / p.tiles_per_img, p0 = (tile % p.tiles_per_img) * p.TRO;
-    mbar_wait(&full_bar[st], (it / p.nstages) & 1);
+    const Ring ring = Ring::at(it, p.nstages);
+    mbar_wait(&full_bar[ring.stage], ring.phase);
     // window start of this warpgroup's 64 rows: 64 pixel rows x 128 B further
-    const uint32_t s_lo = desc_lo(smem_u32(stage0 + (size_t)st * p.stage_bytes), 16) + (uint32_t)wg * ((64 * 128) >> 4);
+    const uint32_t s_lo =
+        desc_lo(smem_u32(stage0 + (size_t)ring.stage * p.stage_bytes), 16) + (uint32_t)wg * ((64 * 128) >> 4);
     for (int sub = 0; sub < p.NSUB; ++sub) {
       // one commit group per (tap or extra source, channel block), all in flight until the sub-tile's epilogue
 #pragma unroll 1
@@ -169,7 +163,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
       }
       wgmma_wait<0>();
       fence_regs(acc);
-      if (sub == p.NSUB - 1 && lane == 0) mbar_arrive(&empty_bar[st]);   // ring slot may be refilled
+      if (sub == p.NSUB - 1 && lane == 0) mbar_arrive(&empty_bar[ring.stage]);   // ring slot may be refilled
 
       // ---- epilogue of this sub-tile ----
       consumer_sync();   // staging tile free
@@ -203,15 +197,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         const size_t off = ((size_t)(n * p.H + row0 + i) * p.W + q) * p.Cout + c8 * 8;
         if (p.residual) {
           const uint4 rv = *reinterpret_cast<const uint4*>(p.residual + off);
-          __nv_bfloat162* a = reinterpret_cast<__nv_bfloat162*>(&val);
-          const __nv_bfloat162* b = reinterpret_cast<const __nv_bfloat162*>(&rv);
-#pragma unroll
-          for (int jj = 0; jj < 4; ++jj) {
-            float2 fa = __bfloat1622float2(a[jj]), fb = __bfloat1622float2(b[jj]);
-            fa.x += fb.x; fa.y += fb.y;
-            if (p.act == 1) { fa.x = hb::relu_nan(fa.x); fa.y = hb::relu_nan(fa.y); }
-            a[jj] = __floats2bfloat162_rn(fa.x, fa.y);
-          }
+          add_residual16(val, rv, p.act == 1);
         }
         *reinterpret_cast<uint4*>(p.y + off) = val;
         c8 += dc; q += dq; i += di;
@@ -225,9 +211,7 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
         const int sdi = rgs / p.W, sdq = rgs - sdi * p.W;
         const uint8_t* sp = sout + st_pr * 4;
         for (int v = st_rg; v < npix; v += rgs) {
-          const float2 f = __bfloat1622float2(
-              *reinterpret_cast<const __nv_bfloat162*>(sp + (size_t)(si * p.Wp + sq) * p.out_pitch));
-          st0 += f.x; st1 += f.y; sq0 = fmaf(f.x, f.x, sq0); sq1 = fmaf(f.y, f.y, sq1);
+          accum_pair(stat, sp + (size_t)(si * p.Wp + sq) * p.out_pitch);
           sq += sdq; si += sdi;
           if (sq >= p.W) { sq -= p.W; ++si; }
         }
@@ -239,52 +223,27 @@ conv_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_constant_
     // (slot, channel) is written)
     consumer_sync();
     float4* scratch = reinterpret_cast<float4*>(sout);   // [256] float4, 4 KB <= staging tile
-    scratch[et] = make_float4(st0, st1, sq0, sq1);
+    scratch[et] = stat;
     consumer_sync();
     if (et < 2 * BN) {
       const int c = et % BN, half = et / BN;
-      float sv = 0.f, qv = 0.f;
-      if (half == 0) {
-        const int pr = c >> 1, hi = c & 1;
-        for (int rg = 0; rg < rgs; ++rg) {
-          const float4 v = scratch[rg * npairs + pr];
-          sv += hi ? v.y : v.x;
-          qv += hi ? v.w : v.z;
-        }
-      }
-      *reinterpret_cast<float2*>(p.stats + ((size_t)(blockIdx.x * 2 + half) * p.Cout + c) * 2) = make_float2(sv, qv);
+      store_stats(p.stats, blockIdx.x * 2 + half, p.Cout, c,
+                  half == 0 ? fold_stats(scratch, rgs, npairs, c) : make_float2(0.f, 0.f));
     }
   }
 }
 
-// one instantiation per Cout; false when the kernel's shared-memory limit cannot be raised (nothing launched)
-template <int BN>
-bool launch_rows(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmX, const CUtensorMap& tmW,
-                 const CUtensorMap* tmXe, const CUtensorMap* tmWe, const RowsParams& p) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(conv_rows_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return false;
-    attr_set = true;
-  }
-  conv_rows_kernel<BN><<<grid, kThreads, smem_bytes, stream>>>(tmX, tmW, tmXe[0], tmWe[0], tmXe[1], tmWe[1], p);
-  return true;
-}
-
 }  // namespace
 
-// Returns 0 and launches when the shape is eligible; returns -1 (nothing launched) when the caller should use the
-// generic implicit-GEMM kernel instead. Not part of the public C ABI (called from hb_conv2d_fprop_bf16 and
-// hb_conv3x3_accum_bf16). xe/we: up to two extra [N,H,W,Cin] sources with [Cout,1,1,Cin] filters accumulated into the
-// same output:  y = conv3x3(x, w) + sum_e conv1x1(xe[e], we[e]).
+// Called from hb_conv2d_fused_bf16 and hb_conv3x3_accum_bf16 (declared in conv_common.cuh).
 int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, const void* residual, int N, int H, int W,
-                     int Cin, int Cout, int act, int num_ctas, cudaStream_t stream, int nextra = 0,
-                     const void* const* xe = nullptr, const void* const* we = nullptr, float* stats = nullptr,
-                     int* stat_slots = nullptr) {
-  if (stats && (residual || !stat_slots)) return -1;
-  if (Cout % 16 != 0 || Cout > 128 || Cin % 8 != 0 || Cin > 128) return -1;
+                     int Cin, int Cout, int act, int num_ctas, cudaStream_t stream, int nextra, const void* const* xe,
+                     const void* const* we, float* stats, int* stat_slots) {
+  constexpr int kNo = (int)cudaErrorNotSupported;
+  if (stats && (residual || !stat_slots)) return kNo;
+  if (Cout % 16 != 0 || Cout > 128 || Cin % 8 != 0 || Cin > 128) return kNo;
   const int Wp = W + 2;
-  if (Wp > 128 || W < 8 || nextra < 0 || nextra > 2) return -1;
+  if (Wp > 128 || W < 8 || nextra < 0 || nextra > 2) return kNo;
   RowsParams p{};
   p.N = N; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.Wp = Wp; p.nextra = nextra;
   p.SR = 128 / Wp;
@@ -315,7 +274,7 @@ int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, c
       }
     }
   }
-  if (nsub < 1) return -1;
+  if (nsub < 1) return kNo;
   p.NSUB = nsub;
   p.TRO = nsub * p.SR;
   p.stage_bytes = p.CB * (p.cb_bytes + nextra * p.ecb_bytes);
@@ -326,46 +285,26 @@ int hb_conv_rows_try(const void* x, const void* w, void* y, const float* bias, c
   p.stats = stats;
 
   CUtensorMap tmX, tmW, tmXe[2], tmWe[2];
-  {
-    uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-    uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-    uint32_t box[4] = {64, (uint32_t)Wp, (uint32_t)(p.TRO + 2), 1};
-    if (tmap::encode_tiled_bf16(&tmX, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-    uint64_t wdims[3] = {(uint64_t)Cin, 9, (uint64_t)Cout};
-    uint64_t wstrides[2] = {(uint64_t)Cin * 2, (uint64_t)9 * Cin * 2};
-    uint32_t wbox[3] = {64, 1, (uint32_t)Cout};
-    if (tmap::encode_tiled_bf16(&tmW, w, 3, wdims, wstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-    uint32_t ebox[4] = {64, (uint32_t)Wp, (uint32_t)p.TRO, 1};
-    uint64_t ewdims[3] = {(uint64_t)Cin, 1, (uint64_t)Cout};
-    uint64_t ewstrides[2] = {(uint64_t)Cin * 2, (uint64_t)Cin * 2};
-    for (int e = 0; e < 2; ++e) {
-      // unused slots alias the main tensors (never dereferenced by the kernel)
-      const void* xs = e < nextra ? xe[e] : x;
-      const void* ws = e < nextra ? we[e] : w;
-      if (!hb::aligned16(xs) || !hb::aligned16(ws)) return -1;
-      if (tmap::encode_tiled_bf16(&tmXe[e], xs, 4, dims, strides, ebox, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-      if (tmap::encode_tiled_bf16(&tmWe[e], ws, 3, ewdims, ewstrides, wbox, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-    }
+  if (tmap::encode_nhwc_box(&tmX, x, N, H, W, Cin, Wp, p.TRO + 2)) return kNo;
+  if (tmap::encode_krsc_slab(&tmW, w, Cout, 9, Cin, Cout)) return kNo;
+  for (int e = 0; e < 2; ++e) {
+    // unused slots alias the main tensors (never dereferenced by the kernel)
+    const void* xs = e < nextra ? xe[e] : x;
+    const void* ws = e < nextra ? we[e] : w;
+    if (!hb::aligned16(xs) || !hb::aligned16(ws)) return kNo;
+    if (tmap::encode_nhwc_box(&tmXe[e], xs, N, H, W, Cin, Wp, p.TRO)) return kNo;
+    if (tmap::encode_krsc_slab(&tmWe[e], ws, Cout, 1, Cin, Cout)) return kNo;
   }
   const size_t smem_bytes = (size_t)w_bytes + (size_t)p.nstages * p.stage_bytes + out_bytes + 64 + 1024;
-  if (smem_bytes > 227 * 1024) return -1;
+  if (smem_bytes > 227 * 1024) return kNo;
   int grid = num_ctas > 0 ? num_ctas : HB_NUM_SMS;
   if (grid > p.num_tiles) grid = p.num_tiles;
-  bool launched;
-  switch (Cout) {
-    case 16: launched = launch_rows<16>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    case 32: launched = launch_rows<32>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    case 48: launched = launch_rows<48>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    case 64: launched = launch_rows<64>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    case 80: launched = launch_rows<80>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    case 96: launched = launch_rows<96>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    case 112: launched = launch_rows<112>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-    default: launched = launch_rows<128>(grid, smem_bytes, stream, tmX, tmW, tmXe, tmWe, p); break;
-  }
-  if (!launched) return -1;
   if (stat_slots) *stat_slots = 2 * grid;
-  g_hb_launches.fetch_add(1, std::memory_order_relaxed);
-  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+  // one instantiation per Cout
+  return (int)dispatch_width<16, 128>(Cout, [&](auto bn) {
+    return launch<conv_rows_kernel<decltype(bn)::value>>(grid, smem_bytes, stream, tmX, tmW, tmXe[0], tmWe[0], tmXe[1],
+                                                          tmWe[1], p);
+  });
 }
 
 extern "C" {
@@ -375,16 +314,14 @@ extern "C" {
 //   dX = dgrad3x3(dY3) + dgrad1x1(dY1) + I * dX_identity
 // (reference: the three autograd contributions of models/classification/repvgg.py:71-73 summed by two add kernels).
 // Returns cudaErrorNotSupported (801) without launching when the shape does not fit the shared-memory-resident scheme;
-// callers then fall back to separate convolutions.
+// callers then fall back to separate convolutions. Otherwise 0, or the launch's error.
 int hb_conv3x3_accum_bf16(const void* x, const void* w, const void* xe0, const void* we0, const void* xe1, const void* we1,
                           int nextra, void* y, int N, int H, int W, int Cin, int Cout, int num_ctas, void* stream) {
   const void* xe[2] = {xe0, xe1};
   const void* we[2] = {we0, we1};
   if (!hb::aligned16(x) || !hb::aligned16(w) || !hb::aligned16(y)) return (int)cudaErrorMisalignedAddress;
-  const int rc = hb_conv_rows_try(x, w, y, nullptr, nullptr, N, H, W, Cin, Cout, 0, num_ctas, (cudaStream_t)stream, nextra,
-                                  xe, we);
-  if (rc == 0) return 0;
-  return rc == -1 ? (int)cudaErrorNotSupported : (int)cudaErrorLaunchFailure;
+  return hb_conv_rows_try(x, w, y, nullptr, nullptr, N, H, W, Cin, Cout, 0, num_ctas, (cudaStream_t)stream, nextra, xe, we,
+                          nullptr, nullptr);
 }
 
 }  // extern "C"

@@ -14,17 +14,14 @@
 // This replaces cuDNN's wgrad behind autograd for nn.Conv2d in the reference
 // (holocron/models/utils.py:71, models/classification/repvgg.py:55-62).
 #include <cstdlib>
-#include "common.cuh"
-#include "tc_common.cuh"
-#include "tmap.cuh"
+#include "conv_common.cuh"
 
 namespace {
 
 using namespace tc;
+using namespace conv;
 
 constexpr int kBKpix = 64;     // pixels (reduction) per stage
-constexpr int kThreads = 384;  // producer warpgroup + 2 consumer warpgroups
-constexpr int kConsumers = 256;
 constexpr int kChunkBytes = kBKpix * 128;  // one 64px x 64ch box = 8 KiB
 constexpr int kABytes = 2 * kChunkBytes;   // 128 co
 
@@ -79,7 +76,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
 
   if (warp < 4) {
     if (warp == 0 && lane == 0) {
-      int stage = 0; uint32_t phase = 0;
+      Ring ring;
       for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         int co_t, ci_t, tg, ks, kb0, kb1;
         decode(unit, co_t, ci_t, tg, ks);
@@ -91,19 +88,20 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
           const int m0 = kb * kBKpix;
           const int q0 = m0 % p.Wo, p0 = (m0 / p.Wo) % p.Ho, n0 = m0 / (p.Wo * p.Ho);
           const int base_w = q0 * p.stride - p.pad, base_h = p0 * p.stride - p.pad;
-          mbar_wait(&empty_bar[stage], phase ^ 1);
-          uint8_t* sa = smem + (size_t)stage * p.stage_bytes;
-          mbar_arrive_expect_tx(&full_bar[stage], tx);
-          tma_load_2d(&tmDY, &full_bar[stage], sa, co_t * 128, m0);
-          tma_load_2d(&tmDY, &full_bar[stage], sa + kChunkBytes, co_t * 128 + 64, m0);
+          uint64_t* bar = &full_bar[ring.stage];
+          mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+          uint8_t* sa = smem + (size_t)ring.stage * p.stage_bytes;
+          mbar_arrive_expect_tx(bar, tx);
+          tma_load_2d(&tmDY, bar, sa, co_t * 128, m0);
+          tma_load_2d(&tmDY, bar, sa + kChunkBytes, co_t * 128 + 64, m0);
           for (int t = 0; t < ntaps; ++t) {
             const int tap = tap0 + t, r = tap / p.S, s = tap % p.S;
             uint8_t* sb = sa + kABytes + t * b_tap_bytes;
             for (int c = 0; c < p.ci_chunks; ++c)
-              tma_load_im2col_4d(&tmX, &full_bar[stage], sb + c * kChunkBytes, ci_t * p.ci_tile + c * 64, base_w, base_h,
-                                 n0, (uint16_t)(s * p.dil), (uint16_t)(r * p.dil));
+              tma_load_im2col_4d(&tmX, bar, sb + c * kChunkBytes, ci_t * p.ci_tile + c * 64, base_w, base_h, n0,
+                                 (uint16_t)(s * p.dil), (uint16_t)(r * p.dil));
           }
-          if (++stage == p.stages) { stage = 0; phase ^= 1; }
+          ring.next(p.stages);
         }
       }
     }
@@ -116,7 +114,7 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
   const int frow = frag_row(et & 127), fcol = frag_col(et & 127);
   const uint32_t dhi = desc_hi(1024);
   float acc[CIW / 2];   // [chunk 0: 32 | chunk 1: kNLast / 2]
-  int stage = 0; uint32_t phase = 0;
+  Ring ring;
   for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
     int co_t, ci_t, tg, ks, kb0, kb1;
     decode(unit, co_t, ci_t, tg, ks);
@@ -124,9 +122,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     const int tap = tg * p.taps_per_group;
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
-      mbar_wait(&full_bar[stage], phase);
+      mbar_wait(&full_bar[ring.stage], ring.phase);
       // 16 pixels = two 8-row swizzle atoms (SBO 1024 B), i.e. 2048 B per k-step
-      const uint32_t s_lo = desc_lo(smem_u32(smem + (size_t)stage * p.stage_bytes), 16);
+      const uint32_t s_lo = desc_lo(smem_u32(smem + (size_t)ring.stage * p.stage_bytes), 16);
       const uint32_t a_lo = s_lo + (uint32_t)wg * (kChunkBytes >> 4);
       const uint32_t b_lo = s_lo + (kABytes >> 4);
       const uint32_t acc0 = kb > kb0 ? 1u : 0u;
@@ -145,8 +143,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
       wgmma_commit();
       wgmma_wait<1>();
       if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
-      prev = stage;
-      if (++stage == p.stages) { stage = 0; phase ^= 1; }
+      prev = ring.stage;
+      ring.next(p.stages);
     }
     wgmma_wait<0>();
     fence_regs(acc);
@@ -233,20 +231,6 @@ inline void launch_wgrad_reduce(const float* ws, float* dw, long long n, int sli
   wgrad_reduce_kernel<<<blocks, dim3(32, 8), 0, st>>>(ws, dw, n, slices, dw2, n_first, accumulate);
 }
 
-// one instantiation per Cin tile width (rounded up to 16)
-template <int CIW>
-cudaError_t launch_wgrad(int grid, size_t smem_bytes, cudaStream_t stream, const CUtensorMap& tmDY, const CUtensorMap& tmX,
-                         const WgradParams& p) {
-  static bool attr_set = false;
-  if (!attr_set) {
-    const cudaError_t e = cudaFuncSetAttribute(conv_wgrad_kernel<CIW>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024);
-    if (e != cudaSuccess) return e;
-    attr_set = true;
-  }
-  conv_wgrad_kernel<CIW><<<grid, kThreads, smem_bytes, stream>>>(tmDY, tmX, p);
-  return cudaSuccess;
-}
-
 struct WgradPlan {
   WgradParams p;
   size_t ws_bytes;
@@ -293,12 +277,6 @@ int plan_wgrad(WgradPlan& plan, int N, int H, int W, int Cin, int Cout, int R, i
 
 }  // namespace
 
-// conv_wgrad_rows.cu: row-window variant for stride-1 3x3 layers with few channels
-size_t hb_wgrad_rows_workspace_bytes(int N, int H, int W, int Cin, int Cout, int R, int S, int stride, int pad, int dil,
-                                     int num_ctas, int has_b1);
-int hb_wgrad_rows_try(const void* x, const void* dy, const void* dy1, float* ws, size_t ws_bytes, int N, int H, int W, int Cin,
-                      int Cout, int num_ctas, cudaStream_t stream, int* slices_out);
-
 extern "C" {
 
 // Bytes of fp32 scratch hb_conv2d_wgrad_bf16 wants for this shape (0 when a single pixel range is used). With a
@@ -330,7 +308,7 @@ static int wgrad_impl(const void* x, const void* dy, float* dw, float* workspace
       HB_LAUNCH_CHECK();
       return 0;
     }
-    if (rc == -2) return (int)cudaErrorLaunchFailure;
+    if (rc != (int)cudaErrorNotSupported) return rc;
   }
   WgradPlan plan{};
   if (int rc = plan_wgrad(plan, N, H, W, Cin, Cout, R, S, stride, pad, dil, num_ctas)) return rc;
@@ -355,32 +333,18 @@ static int wgrad_impl(const void* x, const void* dy, float* dw, float* workspace
   }
 
   CUtensorMap tmDY, tmX;
-  {
-    uint64_t dims[2] = {(uint64_t)Cout, (uint64_t)p.m_total};
-    uint64_t strides[1] = {(uint64_t)Cout * 2};
-    uint32_t box[2] = {64, (uint32_t)kBKpix};
-    int rc = tmap::encode_tiled_bf16(&tmDY, dy, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-    rc = tmap::encode_im2col_bf16(&tmX, x, N, H, W, Cin, pad, pad, R, S, dil, stride, 64, kBKpix,
-                                  CU_TENSOR_MAP_SWIZZLE_128B);
-    if (rc) return rc;
-  }
+  if (int rc = tmap::encode_matrix(&tmDY, dy, p.m_total, Cout, kBKpix)) return rc;
+  if (int rc = tmap::encode_im2col_bf16(&tmX, x, N, H, W, Cin, pad, pad, R, S, dil, stride, 64, kBKpix,
+                                        CU_TENSOR_MAP_SWIZZLE_128B))
+    return rc;
   const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 2 * p.stages * sizeof(uint64_t) + 1024;
   const int num_units = base_units * k_splits;
   int grid = ctas < num_units ? ctas : num_units;
-  cudaError_t e;
-  switch ((p.ci_tile + 15) & ~15) {
-    case 16: e = launch_wgrad<16>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    case 32: e = launch_wgrad<32>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    case 48: e = launch_wgrad<48>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    case 64: e = launch_wgrad<64>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    case 80: e = launch_wgrad<80>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    case 96: e = launch_wgrad<96>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    case 112: e = launch_wgrad<112>(grid, smem_bytes, st, tmDY, tmX, p); break;
-    default: e = launch_wgrad<128>(grid, smem_bytes, st, tmDY, tmX, p); break;
-  }
+  // one instantiation per Cin tile width (rounded up to 16)
+  const cudaError_t e = dispatch_width<16, 128>((p.ci_tile + 15) & ~15, [&](auto ciw) {
+    return launch<conv_wgrad_kernel<decltype(ciw)::value>>(grid, smem_bytes, st, tmDY, tmX, p);
+  });
   if (e != cudaSuccess) return (int)e;
-  HB_LAUNCH_CHECK();
   if (p.use_atomics == 2) {
     const long long n = p.dw_elems;
     launch_wgrad_reduce(workspace, dw, n, k_splits, st, nullptr, -1, accumulate);
@@ -420,9 +384,8 @@ static int repvgg_wgrad_impl(const void* x, const void* dy3, const void* dy1, fl
     return (int)cudaErrorMisalignedAddress;
   cudaStream_t st = (cudaStream_t)stream;
   int slices = 0;
-  const int rc = hb_wgrad_rows_try(x, dy3, dy1, workspace, workspace_bytes, N, H, W, Cin, Cout, num_ctas, st, &slices);
-  if (rc == -1) return (int)cudaErrorNotSupported;
-  if (rc != 0) return (int)cudaErrorLaunchFailure;
+  if (int rc = hb_wgrad_rows_try(x, dy3, dy1, workspace, workspace_bytes, N, H, W, Cin, Cout, num_ctas, st, &slices))
+    return rc;
   const long long n = (long long)Cout * 10 * Cin;
   launch_wgrad_reduce(workspace, dw, n, slices, st, dw1, dw1 ? (long long)Cout * 9 * Cin : -1, accumulate);
   HB_LAUNCH_CHECK();

@@ -15,16 +15,12 @@
 // (deterministic). Channels and slots beyond one CTA's registers are split into (64-input-channel, <= 64-output-channel,
 // slot range) groups; the CTAs of a group share the tiles between them, each group owns a disjoint part of dW.
 // The generic kernel (conv_wgrad.cu) re-reads X nine times from L2 (one im2col load per tap).
-#include "common.cuh"
-#include "tc_common.cuh"
-#include "tmap.cuh"
+#include "conv_common.cuh"
 
 namespace {
 
 using namespace tc;
-
-constexpr int kThreads = 384;   // producer warpgroup + 2 consumer warpgroups
-constexpr int kConsumers = 256;
+using namespace conv;
 
 struct WRowsParams {
   int N, H, W, Cin, Cout;
@@ -117,24 +113,15 @@ conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
       if (p.has_b1) prefetch_tmap(&tmDY1);
       int it = 0;
       for (int tile = member; tile < p.num_tiles; tile += members, ++it) {
-        const int st = it & 1;
         const int n = tile / p.tiles_per_img, p0 = (tile % p.tiles_per_img) * p.TRO;
-        mbar_wait(&empty_bar[st], ((it >> 1) & 1) ^ 1);
-        mbar_arrive_expect_tx(&full_bar[st], tx);
-        uint8_t* sx = smem + (size_t)st * p.stage_bytes;
-        asm volatile(
-            "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-            ::"r"(smem_u32(sx)), "l"(reinterpret_cast<uint64_t>(&tmX)), "r"(smem_u32(&full_bar[st])), "r"(ci0), "r"(-1),
-              "r"(p0 - 1), "r"(n) : "memory");
-        asm volatile(
-            "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-            ::"r"(smem_u32(sx + p.xbuf_bytes)), "l"(reinterpret_cast<uint64_t>(&tmDY)),
-              "r"(smem_u32(&full_bar[st])), "r"(co0), "r"(0), "r"(p0), "r"(n) : "memory");
-        if (p.has_b1)
-          asm volatile(
-              "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
-              ::"r"(smem_u32(sx + p.xbuf_bytes + p.ybuf_bytes)), "l"(reinterpret_cast<uint64_t>(&tmDY1)),
-                "r"(smem_u32(&full_bar[st])), "r"(co0), "r"(0), "r"(p0), "r"(n) : "memory");
+        const Ring ring = Ring::at(it, 2);
+        uint64_t* bar = &full_bar[ring.stage];
+        mbar_wait(&empty_bar[ring.stage], ring.phase ^ 1);
+        mbar_arrive_expect_tx(bar, tx);
+        uint8_t* sx = smem + (size_t)ring.stage * p.stage_bytes;
+        tma_load_4d(&tmX, bar, sx, ci0, -1, p0 - 1, n);
+        tma_load_4d(&tmDY, bar, sx + p.xbuf_bytes, co0, 0, p0, n);
+        if (p.has_b1) tma_load_4d(&tmDY1, bar, sx + p.xbuf_bytes + p.ybuf_bytes, co0, 0, p0, n);
       }
     }
     return;
@@ -150,16 +137,16 @@ conv_wgrad_rows_kernel(const __grid_constant__ CUtensorMap tmX, const __grid_con
   bool any = false;
   int it = 0;
   for (int tile = member; tile < p.num_tiles; tile += members, ++it) {
-    const int st = it & 1;
-    mbar_wait(&full_bar[st], (it >> 1) & 1);
-    const uint32_t sx = smem_u32(smem + (size_t)st * p.stage_bytes);
+    const Ring ring = Ring::at(it, 2);
+    mbar_wait(&full_bar[ring.stage], ring.phase);
+    const uint32_t sx = smem_u32(smem + (size_t)ring.stage * p.stage_bytes);
     const uint32_t sy = sx + p.xbuf_bytes;
     wrows_tile_mma_n<NC, TPW, TPW>(nt, acc, p, slot0, sx, sy, dhi, any);
     wgmma_wait<0>();
 #pragma unroll
     for (int t = 0; t < TPW; ++t) fence_regs(acc[t]);
     any = true;
-    if (lane == 0) mbar_arrive(&empty_bar[st]);
+    if (lane == 0) mbar_arrive(&empty_bar[ring.stage]);
   }
 
   // ================= single epilogue per CTA =================
@@ -245,45 +232,24 @@ size_t hb_wgrad_rows_workspace_bytes(int N, int H, int W, int Cin, int Cout, int
   return (size_t)pl.members * pl.p.slice_elems * sizeof(float);
 }
 
-// launches the partial-sum kernel; *slices_out = number of partial slices written to ws (each slice_elems floats:
-// dW3 [Cout,3,3,Cin] then, with dy1, dW1 [Cout,Cin]). Returns 0 / -1 (not eligible) / -2 (launch failure).
+// Called from the weight-gradient entry points of conv_wgrad.cu (declared in conv_common.cuh).
 int hb_wgrad_rows_try(const void* x, const void* dy, const void* dy1, float* ws, size_t ws_bytes, int N, int H, int W, int Cin,
                       int Cout, int num_ctas, cudaStream_t stream, int* slices_out) {
+  constexpr int kNo = (int)cudaErrorNotSupported;
   WRowsPlan pl{};
   const int has_b1 = dy1 != nullptr;
-  if (!plan_wrows(pl, N, H, W, Cin, Cout, num_ctas, has_b1)) return -1;
+  if (!plan_wrows(pl, N, H, W, Cin, Cout, num_ctas, has_b1)) return kNo;
   WRowsParams& p = pl.p;
-  if (!ws || ws_bytes < (size_t)pl.members * p.slice_elems * sizeof(float)) return -1;
+  if (!ws || ws_bytes < (size_t)pl.members * p.slice_elems * sizeof(float)) return kNo;
   p.ws = ws;
   CUtensorMap tmX, tmDY, tmDY1;
-  {
-    uint64_t dims[4] = {(uint64_t)Cin, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-    uint64_t strides[3] = {(uint64_t)Cin * 2, (uint64_t)W * Cin * 2, (uint64_t)H * W * Cin * 2};
-    uint32_t box[4] = {64, (uint32_t)p.Wp, (uint32_t)(p.TRO + 2), 1};
-    if (tmap::encode_tiled_bf16(&tmX, x, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-    uint64_t ydims[4] = {(uint64_t)Cout, (uint64_t)W, (uint64_t)H, (uint64_t)N};
-    uint64_t ystrides[3] = {(uint64_t)Cout * 2, (uint64_t)W * Cout * 2, (uint64_t)H * W * Cout * 2};
-    uint32_t ybox[4] = {64, (uint32_t)p.Wp, (uint32_t)p.TRO, 1};
-    if (tmap::encode_tiled_bf16(&tmDY, dy, 4, ydims, ystrides, ybox, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-    if (tmap::encode_tiled_bf16(&tmDY1, has_b1 ? dy1 : dy, 4, ydims, ystrides, ybox, CU_TENSOR_MAP_SWIZZLE_128B)) return -1;
-  }
-  static bool attr_set = false;
-  if (!attr_set) {
-    if (cudaFuncSetAttribute(conv_wgrad_rows_kernel<16>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-        cudaFuncSetAttribute(conv_wgrad_rows_kernel<32>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-        cudaFuncSetAttribute(conv_wgrad_rows_kernel<48>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess ||
-        cudaFuncSetAttribute(conv_wgrad_rows_kernel<64>, cudaFuncAttributeMaxDynamicSharedMemorySize, 227 * 1024) != cudaSuccess)
-      return -1;
-    attr_set = true;
-  }
-  if (pl.smem > 227 * 1024) return -1;
-  switch (p.co_group) {
-    case 16: conv_wgrad_rows_kernel<16><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
-    case 32: conv_wgrad_rows_kernel<32><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
-    case 48: conv_wgrad_rows_kernel<48><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
-    default: conv_wgrad_rows_kernel<64><<<pl.grid, kThreads, pl.smem, stream>>>(tmX, tmDY, tmDY1, p); break;
-  }
-  g_hb_launches.fetch_add(1, std::memory_order_relaxed);
+  if (tmap::encode_nhwc_box(&tmX, x, N, H, W, Cin, p.Wp, p.TRO + 2)) return kNo;
+  if (tmap::encode_nhwc_box(&tmDY, dy, N, H, W, Cout, p.Wp, p.TRO)) return kNo;
+  if (tmap::encode_nhwc_box(&tmDY1, has_b1 ? dy1 : dy, N, H, W, Cout, p.Wp, p.TRO)) return kNo;
+  if (pl.smem > 227 * 1024) return kNo;
   *slices_out = pl.members;
-  return cudaGetLastError() == cudaSuccess ? 0 : -2;
+  // one instantiation per output-channel group width
+  return (int)dispatch_width<16, 64>(p.co_group, [&](auto nc) {
+    return launch<conv_wgrad_rows_kernel<decltype(nc)::value>>(pl.grid, pl.smem, stream, tmX, tmDY, tmDY1, p);
+  });
 }

@@ -49,6 +49,30 @@ inline int encode_tiled_bf16(CUtensorMap* out, const void* base, int rank, const
   return r == CUDA_SUCCESS ? 0 : (int)cudaErrorInvalidValue;
 }
 
+// The tiled maps of the tensor-core convolutions. Every box is 64 channels wide (one 128-byte swizzle row).
+// NHWC tensor [N, H, W, C]: box of box_w pixels x box_h rows of one image.
+inline int encode_nhwc_box(CUtensorMap* out, const void* base, int N, int H, int W, int C, uint32_t box_w,
+                           uint32_t box_h) {
+  const uint64_t dims[4] = {(uint64_t)C, (uint64_t)W, (uint64_t)H, (uint64_t)N};
+  const uint64_t strides[3] = {(uint64_t)C * 2, (uint64_t)W * C * 2, (uint64_t)H * W * C * 2};
+  const uint32_t box[4] = {64, box_w, box_h, 1};
+  return encode_tiled_bf16(out, base, 4, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+// KRSC filter [K, taps, C]: the slab of one tap for box_k filters.
+inline int encode_krsc_slab(CUtensorMap* out, const void* base, int K, int taps, int C, uint32_t box_k) {
+  const uint64_t dims[3] = {(uint64_t)C, (uint64_t)taps, (uint64_t)K};
+  const uint64_t strides[2] = {(uint64_t)C * 2, (uint64_t)taps * C * 2};
+  const uint32_t box[3] = {64, 1, box_k};
+  return encode_tiled_bf16(out, base, 3, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+// Row-major matrix [M, C]: box of box_m rows.
+inline int encode_matrix(CUtensorMap* out, const void* base, int M, int C, uint32_t box_m) {
+  const uint64_t dims[2] = {(uint64_t)C, (uint64_t)M};
+  const uint64_t strides[1] = {(uint64_t)C * 2};
+  const uint32_t box[2] = {64, box_m};
+  return encode_tiled_bf16(out, base, 2, dims, strides, box, CU_TENSOR_MAP_SWIZZLE_128B);
+}
+
 // im2col map over an NHWC bf16 activation tensor (TMA dims C, W, H, N).
 //   lower corner = -pad, upper corner = pad - (k-1)*dil  (the box the filter's top-left tap may visit);
 //   traversal stride = conv stride. channels/pixels per load = the smem tile (64 x 128 here).
