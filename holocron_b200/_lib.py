@@ -75,6 +75,12 @@ SIGNATURES = {
     "hb_lambda_bwd_r_bf16": "pppp" + "i" * 12 + "p",
     "hb_gap_fwd_bf16": "ppiiip",
     "hb_gap_bwd_bf16": "ppiiip",
+    "hb_blurpool_fwd": "ppp" + "i" * 8 + "p",
+    "hb_blurpool_bwd": "ppp" + "i" * 8 + "p",
+    "hb_pool_mid_fwd": "ppp" + "i" * 7 + "p",
+    "hb_pool_mid_bwd": "ppp" + "i" * 7 + "p",
+    "hb_pool_last_fwd": "ppp" + "iiii" + "p",
+    "hb_pool_last_bwd": "ppp" + "iiii" + "p",
     "hb_gate_act_fwd_bf16": "ppp" + "iiii" + "f" + "p",
     "hb_gate_act_bwd_bf16": "ppppp" + "iiii" + "f" + "p",
     "hb_box_pairwise": "pppiiip",

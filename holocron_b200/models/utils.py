@@ -36,7 +36,8 @@ def conv_sequence(
     """Builds ``[conv(bias = norm is None), norm, act, attention, drop(inplace=True)]`` with the reference's ordering
     and bias rule. ``blurpool`` is outside the hot path and not supported here."""
     if blurpool:
-        raise NotImplementedError("BlurPool2d is outside the H100 hot path (SURVEY.md §2 row 5)")
+        raise NotImplementedError("conv_sequence(blurpool=True) is not supported: no model here builds a blur-pooled "
+                                  "block; use holocron_b200.nn.BlurPool2d directly")
     if conv_layer is None:
         conv_layer = nn.Conv2d
     if bn_channels is None:

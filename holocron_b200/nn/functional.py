@@ -13,11 +13,12 @@ from ._losses import (complement_cross_entropy, dice_loss, focal_loss, multilabe
                       mutual_channel_loss, poly_loss)
 from ._xcorr import add2d, norm_conv2d  # noqa: F401
 from ._dropblock import dropblock2d  # noqa: F401
+from ._pooling import z_pool  # noqa: F401
 
 import ctypes
 
 __all__ = ["add2d", "complement_cross_entropy", "concat_downsample2d", "dice_loss", "dropblock2d", "focal_loss", "hard_mish",
-           "multilabel_cross_entropy", "mutual_channel_loss", "nl_relu", "norm_conv2d", "poly_loss"]
+           "multilabel_cross_entropy", "mutual_channel_loss", "nl_relu", "norm_conv2d", "poly_loss", "z_pool"]
 
 _cf = ctypes.c_float
 

@@ -224,6 +224,34 @@ int hb_lambda_bwd_r_bf16(const void* dlp, const void* v, float* scratch, float* 
 int hb_gap_fwd_bf16(const void* x, void* y, int N, int HW, int C, void* stream);
 int hb_gap_bwd_bf16(const void* dy, void* dx, int N, int HW, int C, void* stream);
 
+/* ---- blur pooling: holocron/nn/modules/downsample.py:106-151 (BlurPool2d: ReflectionPad2d(p) then a depth-wise
+ *      conv2d with the binomial filter, :148-151) ------------------------------------------------------------------
+ * x / dx NHWC [N,H,W,Cp], y / dy NHWC [N,Ho,Wo,Cp] of dtype 0 (fp32) or 1 (bf16), fp32 accumulation; Cp >= C with
+ * Cp * sizeof(dtype) % 16 == 0 (channels C..Cp-1 of y and dx are written as zeros). taps: HOST pointer to the K*K
+ * filter (row-major fp32 values, copied into the launch), K in 2..7, stride >= 1, p = ((stride-1) + (K-1)) / 2 < H, W
+ * (ReflectionPad2d's limit), Ho = (H + 2p - K) / stride + 1. The reflection is folded into the indices (no padded
+ * copy); the backward pass is the gather-form adjoint (each dx element written once). */
+int hb_blurpool_fwd(const void* x, void* y, const float* taps, int N, int H, int W, int C, int Cp, int K, int stride,
+                    int dtype, void* stream);
+int hb_blurpool_bwd(const void* dy, void* dx, const float* taps, int N, int H, int W, int C, int Cp, int K, int stride,
+                    int dtype, void* stream);
+
+/* ---- max / mean reductions: holocron/nn/modules/downsample.py:80-99 (GlobalMaxPool2d), :170-183 (ZPool) and
+ *      holocron/nn/functional.py:139-147 (z_pool: cat(max(dim), mean(dim))) -------------------------------------
+ * mid: x [A,L,M] reduced over L (GlobalMaxPool2d: A=N, L=H*W, M=Cp; z_pool dim 2: A=N, L=H, M=W*Cp; dim 3: A=N*H,
+ * L=W, M=Cp); y [A][1 + with_mean][M] holds the max plane, then the mean plane when with_mean; idx int32 [A,M] the
+ * index along L of the max. last: x [R,Cp] reduced over its first C channels (z_pool dim 1: R=N*H*W); y [R][2] =
+ * (max, mean), idx int32 [R]. Index order: NaN first, then larger, then lower index (torch's max(dim).indices).
+ * Backward: dx = dmax at the saved index + dmean / L (L = C for last), each element written once. dtype 0 (fp32) or 1
+ * (bf16), Cp * sizeof(dtype) % 16 == 0, M % Cp == 0; channels C..Cp-1 of y, idx and dx are written as zeros.
+ * Deterministic (fixed-order combination, no atomics), no host sync. */
+int hb_pool_mid_fwd(const void* x, void* y, int* idx, int A, int L, int M, int C, int Cp, int with_mean, int dtype,
+                    void* stream);
+int hb_pool_mid_bwd(const void* dy, const int* idx, void* dx, int A, int L, int M, int C, int Cp, int with_mean,
+                    int dtype, void* stream);
+int hb_pool_last_fwd(const void* x, void* y, int* idx, int R, int C, int Cp, int dtype, void* stream);
+int hb_pool_last_bwd(const void* dy, const int* idx, void* dx, int R, int C, int Cp, int dtype, void* stream);
+
 /* ---- squeeze-excite gate: SEBlock.forward `x * y` followed by the block's activation,
  *      holocron/models/classification/rexnet.py:63-66, 125-131 --------------------------------------------- */
 /* out[n,p,c] = act(x[n,p,c] * gate[n,c]);  x/out [N,HW,C] bf16, gate fp32 [N,C]; act codes as hb_bn_act_fwd_bf16 (0-6) */
