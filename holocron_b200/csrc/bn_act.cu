@@ -859,7 +859,8 @@ int hb_bn_act_fwd_bf16(const void* u0, const void* u1, const void* u2, int B, co
     }                                                                                                      \
     if (occ_debug) fprintf(stderr, "[hb] bn_act_fwd_kernel<%d,%d> smem %zu: %d resident blocks/SM\n", NBV, (int)STATS, smem, occ); \
     const int fixed = (B + (residual != nullptr) >= 3) ? 3 : 4;                                            \
-    const int per_sm = per_sm_env > 0 ? per_sm_env : (use_occ ? (occ < 4 ? occ : 4) : fixed);              \
+    /* <= 4 blocks per SM: the caller's out_stats buffer has 4 x SMs slots (bn_stat_slots) */             \
+    const int per_sm = per_sm_env > 0 ? (per_sm_env < 4 ? per_sm_env : 4) : (use_occ ? (occ < 4 ? occ : 4) : fixed); \
     const dim3 grid = make_grid(g, M, 1, per_sm);                                                          \
     if (out_stat_slots) *out_stat_slots = (int)grid.x;                                                     \
     bn_act_fwd_kernel<NBV, STATS><<<grid, kThreads, smem, st>>>(p, g);                                     \

@@ -535,7 +535,7 @@ def conv2d_bias_act(x: Tensor, weight: Tensor, bias: Optional[Tensor], stride: i
 # ------------------------------------------------------------------------------------------------------
 class BNBranch:
     """Non-tensor view of one BatchNorm2d's buffers/hyper-parameters handed to the fused function."""
-    __slots__ = ("running_mean", "running_var", "eps", "momentum", "num_batches_tracked")
+    __slots__ = ("running_mean", "running_var", "eps", "momentum", "num_batches_tracked", "track_running_stats")
 
     def __init__(self, bn: nn.BatchNorm2d) -> None:
         self.running_mean = bn.running_mean
@@ -543,6 +543,8 @@ class BNBranch:
         self.eps = bn.eps
         self.momentum = bn.momentum
         self.num_batches_tracked = bn.num_batches_tracked
+        # nn.BatchNorm2d updates its buffers in training only while the flag is set (trainer.freeze_bn clears it)
+        self.track_running_stats = bn.track_running_stats and bn.running_mean is not None
 
 
 def _arr3(ts: Sequence[Optional[Tensor]]):
@@ -563,6 +565,8 @@ def _bn_batch_stats(us: Sequence[Tensor], branches, g32, b32, stats: Tensor, c: 
 
     Every input normally arrives with its (sum, sum of squares) partials attached by its producer (convolution epilogue,
     previous block's forward pass); only tensors that come without them get a stand-alone statistics pass."""
+    if m == 1:   # what F.batch_norm raises in training: the variance of one value is undefined
+        raise ValueError(f"Expected more than 1 value per channel when training, got input size {us[0].shape}")
     L = lib()
     nb = len(us)
     parts, slots = [], []
@@ -579,15 +583,15 @@ def _bn_batch_stats(us: Sequence[Tensor], branches, g32, b32, stats: Tensor, c: 
     eps, mom = branches[0].eps, branches[0].momentum
     if any(b.eps != eps or b.momentum != mom for b in branches):
         raise NotImplementedError("branches with different eps/momentum")
-    if mom is None:
+    track = [b.track_running_stats for b in branches]
+    if mom is None and any(track):
         raise NotImplementedError("cumulative moving average (momentum=None)")
-    track = branches[0].running_mean is not None
     check(L.hb_bn_finalize(_arr3(parts), _I3(*(slots + [0] * (3 - nb))), _arr3(g32), _arr3(b32),
-                           _arr3([b.running_mean for b in branches]) if track else None,
-                           _arr3([b.running_var for b in branches]) if track else None,
-                           _arr3([b.num_batches_tracked for b in branches]) if track else None,
+                           _arr3([b.running_mean if t else None for b, t in zip(branches, track)]),
+                           _arr3([b.running_var if t else None for b, t in zip(branches, track)]),
+                           _arr3([b.num_batches_tracked if t else None for b, t in zip(branches, track)]),
                            ptr(stats[0]), ptr(stats[1]), ptr(stats[2]), ptr(stats[3]), nb, c, c_log, m, _c_float(eps),
-                           _c_float(mom), stream_ptr()), "hb_bn_finalize")
+                           _c_float(0.0 if mom is None else mom), stream_ptr()), "hb_bn_finalize")
 
 
 def _bn_forward_pass(us: Sequence[Tensor], stats: Tensor, res: Optional[Tensor], m: int, c: int, act: int, slope: float,

@@ -91,3 +91,16 @@ def epilogue_ref(acc: torch.Tensor, abs_sum: torch.Tensor, residual: Optional[to
     if relu:
         ref = ref.clamp_min(0)
     return ref, abs_sum, slack
+
+
+def check_stats(y, parts, slots, what):
+    """The first ``slots`` partials are all written and add up (fp64) to the per-channel sum and sum of squares of the
+    stored output within 1e-5 of the sums of their absolute values."""
+    c = y.shape[-1]
+    p = parts[:slots].double().cpu()
+    assert not torch.isnan(p).any(), f"{what}: unwritten statistics slot"
+    tot = p.sum(0)
+    yf = y.double().cpu().reshape(-1, c)
+    for j, v in enumerate((yf, yf * yf)):
+        err = (tot[:, j] - v.sum(0)).abs()
+        assert bool((err <= 1e-5 * v.abs().sum(0)).all()), f"{what}: statistics {j} off by {float(err.max()):.3e}"

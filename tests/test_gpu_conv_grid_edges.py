@@ -19,7 +19,7 @@ import torch
 
 from holocron_b200._lib import ConvArgs, lib, ptr, stream_ptr
 
-from _bounds import FP32_BITS, assert_within, conv_ref, dgrad_ref, epilogue_ref, ulp, wgrad_ref
+from _bounds import FP32_BITS, assert_within, check_stats, conv_ref, dgrad_ref, epilogue_ref, ulp, wgrad_ref
 
 pytestmark = pytest.mark.gpu
 GRIDS = [0, 1, 2, 3, 7]          # 0 = one CTA per SM, run first: the other grids must reproduce its bits
@@ -94,19 +94,6 @@ def narrow_n_tiles(cout, dual=False):
 def fprop_slots(num_ctas, n_tiles, m_tiles):
     grid = min(num_ctas if num_ctas > 0 else _sms(), 4 * _sms())
     return 2 * min(max(grid // n_tiles, 1), m_tiles)
-
-
-def check_stats(y, parts, slots, what):
-    """The first ``slots`` partials are all written and add up (fp64) to the per-channel sum and sum of squares of the
-    stored output within 1e-5 of the sums of their absolute values."""
-    c = y.shape[-1]
-    p = parts[:slots].double().cpu()
-    assert not torch.isnan(p).any(), f"{what}: unwritten statistics slot"
-    tot = p.sum(0)
-    yf = y.double().cpu().reshape(-1, c)
-    for j, v in enumerate((yf, yf * yf)):
-        err = (tot[:, j] - v.sum(0)).abs()
-        assert bool((err <= 1e-5 * v.abs().sum(0)).all()), f"{what}: statistics {j} off by {float(err.max()):.3e}"
 
 
 # ---------------------------------------------------------------------------------------------------------------------
