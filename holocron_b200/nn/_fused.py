@@ -17,7 +17,7 @@ from typing import List, Optional, Sequence, Tuple
 import torch
 from torch import Tensor, nn
 
-from .._lib import DTYPE_CODE, ConvArgs, check, lib, ptr, require_cuda, stream_ptr
+from .._lib import DTYPE_CODE, ConvArgs, check, dtype_code, lib, ptr, require_cuda, stream_ptr
 
 ACT_NONE, ACT_RELU, ACT_RELU6, ACT_SILU, ACT_LEAKY, ACT_MISH, ACT_HARDMISH, ACT_FRELU = range(8)
 
@@ -142,7 +142,6 @@ def to_channels_last_bf16(x: Tensor, c_pad: Optional[int] = None) -> Tensor:
         return x
     no_grad = not (x.requires_grad and torch.is_grad_enabled())   # the raw kernel is invisible to autograd
     if no_grad and x.is_contiguous() and x.dtype in (torch.float32, torch.bfloat16, torch.float16) and (cp != c or c < 8):
-        from .._lib import dtype_code
         out = torch.empty((n, cp, h, w), device=x.device, dtype=torch.bfloat16).contiguous(memory_format=torch.channels_last)
         check(lib().hb_nchw_to_nhwc_pad_bf16(ptr(x), ptr(out), n, c, h, w, cp, dtype_code(x), stream_ptr()),
               "hb_nchw_to_nhwc_pad_bf16")
@@ -412,63 +411,42 @@ class _Conv2dFn(torch.autograd.Function):
             # network stem (3 input channels): one explicit im2col pass (27 -> 32 columns), then a dense 1x1 GEMM over it. The
             # implicit-GEMM path pads 3 channels to 8-16 and fetches 9 x 32-byte pixels per output through TMA im2col, far below
             # the HBM rate.
-            col, wp = _stem_im2col_single(x, weight, stride)
+            col, wp, _ = _stem_im2col(x, weight, stride)
             y = conv2d_forward_raw(col, wp, cout, 1, 1, 1, 0, 1, _pad_vec(bias, cout),
                                    want_stats=want_stats and epilogue_stats_pay_off(col.shape[1]))
             ctx.save_for_backward(col, weight)
             ctx.cfg = ("stem", bias is not None)
             return y
-        pk = pack_filter(weight, need_dx, round_up(x.shape[1], 8))
-        xb = to_channels_last_bf16(x, pk.cin_p)
-        y = conv2d_forward_raw(xb, pk.wf, pk.cout_p, r, s, stride, pad, dil, _pad_vec(bias, pk.cout_p),
-                               want_stats=want_stats and epilogue_stats_pay_off(r * s * pk.cin_p))
+        y, pk, xb = _packed_conv(x, weight, bias, stride, pad, dil, need_dgrad=need_dx, keep_padded=keep_padded,
+                                 want_stats=want_stats)
         ctx.save_for_backward(xb, weight)
         ctx.cfg = (stride, pad, dil, pk.wd, bias is not None, x.shape[1], pk.cout_p, pk.cin_d)
-        return y if (keep_padded or pk.cout_p == cout) else y[:, :cout]
+        return y
 
     @staticmethod
     def backward(ctx, dy: Tensor):
         xb, weight = ctx.saved_tensors
         if ctx.cfg[0] == "stem":
-            cout, cin = weight.shape[0], weight.shape[1]
+            cout = weight.shape[0]
             dyb = to_channels_last_bf16(dy, cout)
             dw = db = None
             if ctx.needs_input_grad[1]:
-                dw = wgrad_raw(xb, dyb, cout, 1, 1, 0).view(cout, -1)[:, :9 * cin].view(cout, 3, 3, cin).permute(0, 3, 1, 2)
+                dw = _stem_wgrad(xb, dyb, weight)
             if ctx.cfg[1] and ctx.needs_input_grad[2]:
                 db = dyb.float().sum((0, 2, 3))
             return None, dw, db, None, None, None, None, None
         stride, pad, dil, wd, has_bias, cin_x, cout_p, cin_d = ctx.cfg
-        cout, cin, r, s = weight.shape
-        n, cin_p, h, w = xb.shape
+        cout = weight.shape[0]
+        h, w = xb.shape[2], xb.shape[3]
         dyb = to_channels_last_bf16(dy, cout_p)
-        ho, wo = dyb.shape[2], dyb.shape[3]
-        L = lib()
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
             if dil != 1:
                 raise NotImplementedError("dgrad with dilation > 1")
-            if stride == 2 and r == 3 and s == 3 and pad == 1 and h >= 2 and w >= 2:
-                dxp = dgrad_s2_raw(dyb, weight, cin_d, h, w)
-            else:
-                src = dyb
-                if stride > 1:
-                    src = _empty_cl(n, cout_p, h, w, dyb.device)
-                    check(L.hb_zero_insert_bf16(ptr(dyb), ptr(src), n, ho, wo, h, w, cout_p, stride, stream_ptr()),
-                          "hb_zero_insert_bf16")
-                dxp = conv2d_forward_raw(src, wd, cin_d, r, s, 1, (r - 1) * dil - pad, 1, kind="dgrad")
+            dxp = _dgrad(dyb, weight, wd, cin_d, h, w, stride, pad)
             dx = dxp if cin_d == cin_x else dxp[:, :cin_x]
         if ctx.needs_input_grad[1]:
-            if r != s:
-                raise NotImplementedError("non-square filters")
-            g = direct_grad(weight, krsc=True) if (cin_p == cin and cout_p == cout) else None
-            if g is not None and wgrad_raw(xb, dyb, cout_p, r, stride, pad, dil, acc_into=g) is None:
-                dw = None                                  # added to weight.grad by the reduction kernel
-            else:
-                dwp = wgrad_raw(xb, dyb, cout_p, r, stride, pad, dil)
-                dw = dwp.permute(0, 3, 1, 2)
-                if cin_p != cin or cout_p != cout:
-                    dw = dw[:cout, :cin].contiguous(memory_format=torch.channels_last)
+            dw = _wgrad(xb, dyb, weight, stride, pad, dil)
         if has_bias and ctx.needs_input_grad[2]:
             db = dyb[:, :cout].float().sum((0, 2, 3))
         return dx, dw, db, None, None, None, None, None
@@ -511,6 +489,69 @@ def wgrad_raw(xb: Tensor, dyb: Tensor, cout: int, k: int, stride: int, pad: int,
     return dwp
 
 
+def _packed_conv(x: Tensor, weight: Tensor, bias: Optional[Tensor], stride: int, pad: int, dil: int, act: int = ACT_NONE,
+                 *, need_dgrad: bool = False, keep_padded: bool = False, want_stats: bool = False, norm=None):
+    """Packs ``weight``, converts ``x`` to the packed channel width and runs one convolution -> ``(y, pk, xb)``, ``y``
+    sliced to Cout unless ``keep_padded``. ``norm(xb, pk)`` returns the (mean, rstd, wsum) of NormConv2d's epilogue."""
+    cout, _, r, s = weight.shape
+    pk = pack_filter(weight, need_dgrad, round_up(x.shape[1], 8))
+    xb = to_channels_last_bf16(x, pk.cin_p)
+    nrm = None if norm is None else norm(xb, pk)
+    y = conv2d_forward_raw(xb, pk.wf, pk.cout_p, r, s, stride, pad, dil, _pad_vec(bias, pk.cout_p), None, act,
+                           want_stats=want_stats and epilogue_stats_pay_off(r * s * pk.cin_p), norm=nrm)
+    return (y if (keep_padded or pk.cout_p == cout) else y[:, :cout]), pk, xb
+
+
+def _zero_insert(t: Tensor, h: int, w: int, stride: int) -> Tensor:
+    """[N, C, h, w] with the pixels of ``t`` at every ``stride``-th position and zeros between them."""
+    n, c, ho, wo = t.shape
+    out = _empty_cl(n, c, h, w, t.device)
+    check(lib().hb_zero_insert_bf16(ptr(t), ptr(out), n, ho, wo, h, w, c, stride, stream_ptr()), "hb_zero_insert_bf16")
+    return out
+
+
+def _dgrad(dyb: Tensor, weight: Tensor, wd: Tensor, cin_d: int, h: int, w: int, stride: int, pad: int,
+           dy1: Optional[Tensor] = None, wd1: Optional[Tensor] = None) -> Tensor:
+    """dx [N, cin_d, h, w] of a convolution (``weight``, packed for the data gradient as ``wd``) plus that of a RepVGG 1x1
+    branch (``dy1``, ``wd1``): parity classes for stride-2 3x3 pad-1 filters, else zero insertion and a convolution with
+    the flipped filter (the 1x1 branch convolved at the low resolution, then zero-inserted)."""
+    r, s = weight.shape[2], weight.shape[3]
+    if stride == 2 and r == 3 and s == 3 and pad == 1 and h >= 2 and w >= 2:
+        return dgrad_s2_raw(dyb, weight, cin_d, h, w, dy1, wd1)
+    dxa = None
+    if dy1 is not None:
+        dxa = conv2d_forward_raw(dy1, wd1, cin_d, 1, 1, 1, 0, 1, kind="dgrad")
+        if stride > 1:
+            dxa = _zero_insert(dxa, h, w, stride)
+    src = _zero_insert(dyb, h, w, stride) if stride > 1 else dyb
+    dxp = conv2d_forward_raw(src, wd, cin_d, r, s, 1, r - 1 - pad, 1, kind="dgrad")
+    if dxa is not None:
+        dxp.add_(dxa)
+    return dxp
+
+
+def _wgrad_to_param(dwp: Tensor, weight: Tensor) -> Tensor:
+    """KRSC [cout_p, k, k, cin_p] weight gradient -> ``weight``'s (Cout, Cin, k, k), channel padding sliced off."""
+    cout, cin = weight.shape[0], weight.shape[1]
+    dw = dwp.permute(0, 3, 1, 2)
+    if dw.shape[0] != cout or dw.shape[1] != cin:
+        dw = dw[:cout, :cin].contiguous(memory_format=torch.channels_last)
+    return dw
+
+
+def _wgrad(xb: Tensor, dyb: Tensor, weight: Tensor, stride: int, pad: int, dil: int = 1) -> Optional[Tensor]:
+    """Weight gradient of one filter from the (channel-padded) input and output gradient: ``None`` when the reduction
+    kernel added it into the parameter's gradient buffer (:func:`direct_grad`), otherwise in the parameter's shape."""
+    cout, cin, r, s = weight.shape
+    if r != s:
+        raise NotImplementedError("non-square filters")
+    cout_p, cin_p = dyb.shape[1], xb.shape[1]
+    g = direct_grad(weight, krsc=True) if (cin_p == cin and cout_p == cout) else None
+    if g is not None and wgrad_raw(xb, dyb, cout_p, r, stride, pad, dil, acc_into=g) is None:
+        return None
+    return _wgrad_to_param(wgrad_raw(xb, dyb, cout_p, r, stride, pad, dil), weight)
+
+
 def conv2d_bias_act(x: Tensor, weight: Tensor, bias: Optional[Tensor], stride: int, padding: int, act: int = ACT_NONE,
                     slope: float = 0.0) -> Tensor:
     """conv + bias + activation. Without autograd (inference) bias and ReLU are fused in the conv epilogue;
@@ -519,11 +560,7 @@ def conv2d_bias_act(x: Tensor, weight: Tensor, bias: Optional[Tensor], stride: i
     needs_grad = torch.is_grad_enabled() and (x.requires_grad or weight.requires_grad or
                                               (bias is not None and bias.requires_grad))
     if not needs_grad and act in (ACT_NONE, ACT_RELU):
-        cout, cin, r, s = weight.shape
-        pk = pack_filter(weight, False, round_up(x.shape[1], 8))
-        xb = to_channels_last_bf16(x, pk.cin_p)
-        y = conv2d_forward_raw(xb, pk.wf, pk.cout_p, r, s, stride, padding, 1, _pad_vec(bias, pk.cout_p), None, act)
-        return y if pk.cout_p == cout else y[:, :cout]
+        return _packed_conv(x, weight, bias, stride, padding, 1, act)[0]
     if act == ACT_NONE:
         return _Conv2dFn.apply(x, weight, bias, int(stride), int(padding), 1, False, False)
     # the activation pass needs channels % 8 == 0: run it on the zero-padded output (filter rows and bias of the padding are
@@ -634,12 +671,33 @@ def _bn_backward_pass(dob: Tensor, us: Sequence[Tensor], stats: Tensor, res: Opt
         stream_ptr())), "hb_bn_act_bwd_bf16")
 
 
-def _param_grad_targets(params_g: Sequence[Tensor], params_b: Sequence[Tensor]):
-    """(gacc, bacc, all_direct): gradient buffers of the BatchNorm weights / biases the kernel may add into."""
-    gacc = [direct_grad(p) for p in params_g]
-    bacc = [direct_grad(p) for p in params_b]
-    all_direct = all(g is not None for g in gacc) and all(b is not None for b in bacc)
-    return gacc, bacc, all_direct
+def _bn_setup(us: Sequence[Tensor], branches, gammas: Sequence[Tensor], betas: Sequence[Tensor], training: bool, c: int,
+              c_log: int, m: int, dev) -> Tensor:
+    """[4, max(nb, 1), c] fp32 mean / rstd / scale / shift rows of the branches: batch statistics in training, the
+    running statistics otherwise. ``c_log``: the parameters' channel count (<= c, the activation's padded width)."""
+    stats = torch.empty((4, max(len(branches), 1), c), device=dev, dtype=torch.float32)
+    g32 = [g.detach().float() for g in gammas]
+    b32 = [b.detach().float() for b in betas]
+    if not branches:
+        return stats
+    if training:
+        _bn_batch_stats(us, branches, g32, b32, stats, c, c_log, m)
+        return stats
+    for i, b in enumerate(branches):
+        check(lib().hb_bn_eval_affine(ptr(g32[i]), ptr(b32[i]), ptr(b.running_mean), ptr(b.running_var), _c_float(b.eps), c,
+                                      c_log, ptr(stats[2][i]), ptr(stats[3][i]), ptr(stats[0][i]), ptr(stats[1][i]),
+                                      stream_ptr()), "hb_bn_eval_affine")
+    return stats
+
+
+def _bn_grad_targets(gammas: Sequence[Tensor], betas: Sequence[Tensor], c: int, dev):
+    """(gacc, bacc, dgb) of the BatchNorm weights / biases: their gradient buffers when the kernel may add into all of
+    them (``dgb`` None), otherwise a [2, nb, c] fp32 buffer the kernel writes the gradients to (``gacc``, ``bacc`` None)."""
+    gacc = [direct_grad(p) for p in gammas]
+    bacc = [direct_grad(p) for p in betas]
+    if all(g is not None for g in gacc) and all(b is not None for b in bacc):
+        return gacc, bacc, None
+    return None, None, torch.empty((2, len(gammas), c), device=dev, dtype=torch.float32)
 
 
 class _BNActFn(torch.autograd.Function):
@@ -658,20 +716,8 @@ class _BNActFn(torch.autograd.Function):
             raise NotImplementedError("fused BN kernels need channels % 8 == 0")
         m = n * h * w
         dev = us[0].device if nb else res.device
-        L = lib()
-        stats = torch.empty((4, max(nb, 1), c), device=dev, dtype=torch.float32)  # mean, rstd, scale, shift
-        g32 = [g.detach().float() for g in gammas]
-        b32 = [b.detach().float() for b in betas]
-        c_log = g32[0].numel() if nb else c   # parameters may be narrower than a zero-padded activation
-        if nb == 0:
-            pass
-        elif training:
-            _bn_batch_stats(us, branches, g32, b32, stats, c, c_log, m)
-        else:
-            for i, b in enumerate(branches):
-                check(L.hb_bn_eval_affine(ptr(g32[i]), ptr(b32[i]), ptr(b.running_mean), ptr(b.running_var),
-                                          _c_float(b.eps), c, c_log, ptr(stats[2][i]), ptr(stats[3][i]), ptr(stats[0][i]),
-                                          ptr(stats[1][i]), stream_ptr()), "hb_bn_eval_affine")
+        c_log = gammas[0].numel() if nb else c   # parameters may be narrower than a zero-padded activation
+        stats = _bn_setup(us, branches, gammas, betas, training, c, c_log, m, dev)
         out = _bn_forward_pass(us, stats, res, m, c, act, slope, int(res_after), (n, c, h, w), emit_stats)
         ctx.save_for_backward(stats, *us, *([res] if has_res else []), *gammas, *betas)
         ctx.cfg = (nb, act, slope, training, has_res, c_log, int(res_after))
@@ -694,13 +740,7 @@ class _BNActFn(torch.autograd.Function):
         need_res = has_res and ctx.needs_input_grad[1 + 3 * nb]
         dus = [_empty_cl(n, c, h, w, dev) if need_u[i] else None for i in range(nb)]
         dres = _empty_cl(n, c, h, w, dev) if need_res else None
-        gacc = bacc = dgb = None
-        direct = False
-        if need_gb:
-            gacc, bacc, direct = _param_grad_targets(gammas, betas)
-            if not direct:
-                gacc = bacc = None
-                dgb = torch.empty((2, nb, c), device=dev, dtype=torch.float32)
+        gacc, bacc, dgb = _bn_grad_targets(gammas, betas, c, dev) if need_gb else (None, None, None)
         _bn_backward_pass(dob, us, stats, res, dus, dres, dgb, gacc, bacc, c_log, m, c, act, slope, training, res_after)
         grads: List[Optional[Tensor]] = [None]
         grads += dus
@@ -765,51 +805,36 @@ class _RepBlockFn(torch.autograd.Function):
         if cout % 16 != 0:
             raise NotImplementedError("fused RepBlock needs out_channels % 16 == 0")
         stem = cin <= 4 and x.shape[1] == cin and not need_dx and x.is_contiguous() and x.dtype in DTYPE_CODE
-        # Dual-output launch (x read once, 1x1 branch from the centre-tap loads): correct and tested, opt-in (A/B). The two
-        # accumulators share the 128-column register budget, so each output's Cout tile is capped at 64 columns (twice the
-        # tiles on the wide layers) and every tile runs two epilogues; two launches are the default. Not measured on the H100.
-        fused_fwd = bool(os.environ.get("HB_FUSED_FPROP"))
         if stem:
-            # network stem: explicit im2col once (27 -> 32 columns), both branches become dense GEMMs over it
-            xb, w3p, w1p = _stem_im2col(x, w3, w1, stride)
-            if fused_fwd:
-                y3, y1 = conv2d_forward_raw(xb, w3p, cout, 1, 1, 1, 0, 1, w2=w1p,
-                                            want_stats=training and epilogue_stats_pay_off(xb.shape[1]))
-            else:
-                st = training and epilogue_stats_pay_off(xb.shape[1])
-                y3 = conv2d_forward_raw(xb, w3p, cout, 1, 1, 1, 0, 1, want_stats=st)
-                y1 = conv2d_forward_raw(xb, w1p, cout, 1, 1, 1, 0, 1, want_stats=st)
-            pk3 = pk1 = None
+            # network stem: explicit im2col once (27 -> 32 columns), both branches become dense 1x1 GEMMs over it
+            xb, wf3, wf1 = _stem_im2col(x, w3, stride, w1)
+            k3, conv_stride, pad3 = 1, 1, 0
+            wd3 = wd1 = None
         else:
             pk3 = pack_filter(w3, need_dx, round_up(x.shape[1], 8))
             pk1 = pack_filter(w1, need_dx, round_up(x.shape[1], 8))
             xb = to_channels_last_bf16(x, pk3.cin_p)
-            if fused_fwd:
-                y3, y1 = conv2d_forward_raw(xb, pk3.wf, cout, 3, 3, stride, 1, 1, w2=pk1.wf,
-                                            want_stats=training and epilogue_stats_pay_off(9 * pk3.cin_p))
-            else:
-                y3 = conv2d_forward_raw(xb, pk3.wf, cout, 3, 3, stride, 1, 1,
-                                        want_stats=training and epilogue_stats_pay_off(9 * pk3.cin_p))
-                y1 = conv2d_forward_raw(xb, pk1.wf, cout, 1, 1, stride, 0, 1,
-                                        want_stats=training and epilogue_stats_pay_off(pk3.cin_p))
+            wf3, wf1, wd3, wd1 = pk3.wf, pk1.wf, pk3.wd, pk1.wd
+            k3, conv_stride, pad3 = 3, stride, 1
+        kx = xb.shape[1]
+        # Dual-output launch (x read once, 1x1 branch from the centre-tap loads): correct and tested, opt-in (A/B). The two
+        # accumulators share the 128-column register budget, so each output's Cout tile is capped at 64 columns (twice the
+        # tiles on the wide layers) and every tile runs two epilogues; two launches are the default. Not measured on the H100.
+        if os.environ.get("HB_FUSED_FPROP"):
+            y3, y1 = conv2d_forward_raw(xb, wf3, cout, k3, k3, conv_stride, pad3, 1, w2=wf1,
+                                        want_stats=training and epilogue_stats_pay_off(k3 * k3 * kx))
+        else:
+            y3 = conv2d_forward_raw(xb, wf3, cout, k3, k3, conv_stride, pad3, 1,
+                                    want_stats=training and epilogue_stats_pay_off(k3 * k3 * kx))
+            y1 = conv2d_forward_raw(xb, wf1, cout, 1, 1, conv_stride, 0, 1,
+                                    want_stats=training and epilogue_stats_pay_off(kx))
         us = [y3, y1] + ([xb] if nb == 3 else [])
         n, c, h, w = y3.shape
         m = n * h * w
-        dev = y3.device
-        L = lib()
-        stats = torch.empty((4, nb, c), device=dev, dtype=torch.float32)
-        g32 = [g.detach().float() for g in gammas]
-        b32 = [b.detach().float() for b in betas]
-        if training:
-            _bn_batch_stats(us, branches, g32, b32, stats, c, c, m)
-        else:
-            for i, b in enumerate(branches):
-                check(L.hb_bn_eval_affine(ptr(g32[i]), ptr(b32[i]), ptr(b.running_mean), ptr(b.running_var),
-                                          _c_float(b.eps), c, c, ptr(stats[2][i]), ptr(stats[3][i]), ptr(stats[0][i]),
-                                          ptr(stats[1][i]), stream_ptr()), "hb_bn_eval_affine")
+        stats = _bn_setup(us, branches, gammas, betas, training, c, c, m, y3.device)
         out = _bn_forward_pass(us, stats, None, m, c, act, slope, 0, (n, c, h, w), emit_stats=training)
         ctx.save_for_backward(stats, xb, y3, y1, w3, w1, *gammas, *betas)
-        ctx.cfg = (nb, act, slope, training, stride, None if stem else pk3.wd, None if stem else pk1.wd, x.shape[1], stem)
+        ctx.cfg = (nb, act, slope, training, stride, wd3, wd1, x.shape[1], stem)
         return out
 
     @staticmethod
@@ -826,11 +851,7 @@ class _RepBlockFn(torch.autograd.Function):
         need_dx = ctx.needs_input_grad[1]
         dy3, dy1 = _empty_cl(n, c, ho, wo, dev), _empty_cl(n, c, ho, wo, dev)
         dxid = _empty_cl(n, c, ho, wo, dev) if (nb == 3 and need_dx) else None
-        gacc, bacc, direct_bn = _param_grad_targets(gammas, betas)
-        dgb = None
-        if not direct_bn:
-            gacc = bacc = None
-            dgb = torch.empty((2, nb, c), device=dev, dtype=torch.float32)
+        gacc, bacc, dgb = _bn_grad_targets(gammas, betas, c, dev)
         us = [y3, y1] + ([xb] if nb == 3 else [])
         _bn_backward_pass(dob, us, stats, None, [dy3, dy1] + ([dxid] if nb == 3 else []), None, dgb, gacc, bacc, c, m, c, act,
                           slope, training, 0)
@@ -839,10 +860,7 @@ class _RepBlockFn(torch.autograd.Function):
         dx = None
         if need_dx:
             cin_d = wd3.shape[0]
-            if stride == 2 and h >= 2 and w >= 2 and wd3.shape[3] == c:
-                # parity-class data gradient of the stride-2 3x3 branch; the 1x1 branch lands in class (0, 0)
-                dxp = dgrad_s2_raw(dy3, w3, cin_d, h, w, dy1, wd1)
-            elif stride == 1 and wd3.shape[3] == c and (dxid is None or cin_d == c):
+            if stride == 1 and wd3.shape[3] == c and (dxid is None or cin_d == c):
                 dxp = None
                 if not os.environ.get("HB_DISABLE_CONV_ROWS"):
                     # shared-memory-resident filter variant (C <= 64): all three contributions in the K loop
@@ -863,28 +881,14 @@ class _RepBlockFn(torch.autograd.Function):
                     # in the epilogue
                     dxp = conv2d_forward_raw(dy3, wd3, cin_d, 3, 3, 1, 1, 1, None, dxid, ACT_NONE, xe=dy1, we=wd1, kind="dgrad")
             else:
-                # general composition (channel-padded or odd shapes)
-                if stride == 1:
-                    src3 = dy3
-                    dxa = conv2d_forward_raw(dy1, wd1, cin_d, 1, 1, 1, 0, 1, kind="dgrad")
-                else:
-                    lo = conv2d_forward_raw(dy1, wd1, cin_d, 1, 1, 1, 0, 1, kind="dgrad")
-                    dxa = _empty_cl(n, cin_d, h, w, dev)
-                    check(L.hb_zero_insert_bf16(ptr(lo), ptr(dxa), n, ho, wo, h, w, cin_d, stride, stream_ptr()),
-                          "hb_zero_insert_bf16")
-                    src3 = _empty_cl(n, c, h, w, dev)
-                    check(L.hb_zero_insert_bf16(ptr(dy3), ptr(src3), n, ho, wo, h, w, c, stride, stream_ptr()),
-                          "hb_zero_insert_bf16")
-                dxp = conv2d_forward_raw(src3, wd3, cin_d, 3, 3, 1, 1, 1, kind="dgrad")
-                dxp.add_(dxa)
+                # stride 2: parity classes, the 1x1 branch landing in class (0, 0); otherwise (channel-padded or odd
+                # shapes) the general composition
+                dxp = _dgrad(dy3, w3, wd3, cin_d, h, w, stride, 1, dy1, wd1)
                 if dxid is not None:
                     dxp[:, :c].add_(dxid)
             dx = dxp if cin_d == cin_x else dxp[:, :cin_x]
         if stem:
-            cin = w3.shape[1]
-            g3 = wgrad_raw(xb, dy3, c, 1, 1, 0).view(c, -1)[:, :9 * cin].view(c, 3, 3, cin).permute(0, 3, 1, 2)
-            g1 = wgrad_raw(xb, dy1, c, 1, 1, 0).view(c, -1)[:, 4 * cin:5 * cin].reshape(c, cin, 1, 1)
-            return (None, None, g3, g1, *g_gamma, *g_beta)
+            return (None, None, _stem_wgrad(xb, dy3, w3), _stem_wgrad(xb, dy1, w1), *g_gamma, *g_beta)
         grads_w: List[Optional[Tensor]] = [None, None]
         done = [False, False]
         no_pad = cin_p == w3.shape[1]
@@ -910,23 +914,14 @@ class _RepBlockFn(torch.autograd.Function):
                     rc = _timed("wgrad", info, lambda: L.hb_repvgg_wgrad_bf16(
                         ptr(xb), ptr(dy3), ptr(dy1), ptr(dwcat), ptr(ws), ws_bytes, n, h, w, cin_p, c, 0, stream_ptr()))
                     if rc == 0:
-                        for i, dwp in enumerate((dwcat[:c * 9 * cin_p].view(c, 3, 3, cin_p), dwcat[c * 9 * cin_p:].view(c, 1, 1, cin_p))):
-                            dw = dwp.permute(0, 3, 1, 2)
-                            if not no_pad:
-                                dw = dw[:, :w3.shape[1]].contiguous(memory_format=torch.channels_last)
-                            grads_w[i] = dw
+                        grads_w = [_wgrad_to_param(dwcat[:c * 9 * cin_p].view(c, 3, 3, cin_p), w3),
+                                   _wgrad_to_param(dwcat[c * 9 * cin_p:].view(c, 1, 1, cin_p), w1)]
                         done = [True, True]
                     elif rc != 801:
                         check(rc, "hb_repvgg_wgrad_bf16")
-        for i, (wt, dy, k, pad, gdst) in enumerate(((w3, dy3, 3, 1, gw3), (w1, dy1, 1, 0, gw1))):
-            if done[i]:
-                continue
-            if gdst is not None and wgrad_raw(xb, dy, c, k, stride, pad, acc_into=gdst) is None:
-                continue
-            dw = wgrad_raw(xb, dy, c, k, stride, pad).permute(0, 3, 1, 2)
-            if not no_pad:
-                dw = dw[:, :wt.shape[1]].contiguous(memory_format=torch.channels_last)
-            grads_w[i] = dw
+        for i, (wt, dy, pad) in enumerate(((w3, dy3, 1), (w1, dy1, 0))):
+            if not done[i]:
+                grads_w[i] = _wgrad(xb, dy, wt, stride, pad)
         return (None, dx, grads_w[0], grads_w[1], *g_gamma, *g_beta)
 
 
@@ -941,26 +936,10 @@ def _identity_filter(rows: int, cols: int, device) -> Tensor:
     return _eye_cache[key]
 
 
-def _stem_im2col_single(x: Tensor, w3: Tensor, stride: int):
-    """im2col matrix of a 3x3 / pad-1 convolution over <= 4 input channels as a channels_last (N, 32, Ho, Wo) bf16 tensor and
-    the filter re-expressed as a [Cout, 1, 1, 32] row over its columns (k = (r*3 + s)*C + c)."""
-    from .._lib import dtype_code
-    n, cin, h, w = x.shape
-    cout = w3.shape[0]
-    kp = round_up(9 * cin, 32)
-    ho, wo = conv_out_size(h, 3, stride, 1, 1), conv_out_size(w, 3, stride, 1, 1)
-    col = _empty_cl(n, kp, ho, wo, x.device)
-    check(lib().hb_im2col_smallc_bf16(ptr(x), ptr(col), n, cin, h, w, 3, 3, stride, 1, kp, dtype_code(x), stream_ptr()),
-          "hb_im2col_smallc_bf16")
-    wp = torch.zeros((cout, 1, 1, kp), device=x.device, dtype=torch.bfloat16)
-    wp.view(cout, kp)[:, :9 * cin] = w3.detach().permute(0, 2, 3, 1).reshape(cout, 9 * cin)
-    return col, wp
-
-
-def _stem_im2col(x: Tensor, w3: Tensor, w1: Tensor, stride: int):
-    """x (N, C<=4, H, W) NCHW -> im2col matrix as a channels_last (N, 32, Ho, Wo) bf16 tensor, plus the two branch
-    filters re-expressed over its 32 columns (k = (r*3 + s)*C + c; the 1x1 branch only touches the centre tap)."""
-    from .._lib import dtype_code
+def _stem_im2col(x: Tensor, w3: Tensor, stride: int, w1: Optional[Tensor] = None):
+    """x (N, C<=4, H, W) NCHW -> im2col matrix of a 3x3 / pad-1 convolution as a channels_last (N, 32, Ho, Wo) bf16
+    tensor, plus the filter and, for a RepVGG block, its 1x1 branch ``w1`` re-expressed as [Cout, 1, 1, 32] rows over its
+    columns (k = (r*3 + s)*C + c; the 1x1 branch only touches the centre tap). Returns (col, w3p, w1p or None)."""
     n, cin, h, w = x.shape
     cout = w3.shape[0]
     kp = round_up(9 * cin, 32)
@@ -970,9 +949,21 @@ def _stem_im2col(x: Tensor, w3: Tensor, w1: Tensor, stride: int):
           "hb_im2col_smallc_bf16")
     w3p = torch.zeros((cout, 1, 1, kp), device=x.device, dtype=torch.bfloat16)
     w3p.view(cout, kp)[:, :9 * cin] = w3.detach().permute(0, 2, 3, 1).reshape(cout, 9 * cin)
-    w1p = torch.zeros((cout, 1, 1, kp), device=x.device, dtype=torch.bfloat16)
-    w1p.view(cout, kp)[:, 4 * cin:5 * cin] = w1.detach().reshape(cout, cin)
+    w1p = None
+    if w1 is not None:
+        w1p = torch.zeros((cout, 1, 1, kp), device=x.device, dtype=torch.bfloat16)
+        w1p.view(cout, kp)[:, 4 * cin:5 * cin] = w1.detach().reshape(cout, cin)
     return col, w3p, w1p
+
+
+def _stem_wgrad(col: Tensor, dyb: Tensor, weight: Tensor) -> Tensor:
+    """Gradient of a stem filter (3x3, or a RepVGG 1x1 branch at the centre tap) from the im2col columns it was applied
+    to: one 1x1 weight gradient over the columns, sliced back to the filter."""
+    cout, cin, k = weight.shape[0], weight.shape[1], weight.shape[2]
+    g = wgrad_raw(col, dyb, cout, 1, 1, 0).view(cout, -1)
+    if k == 1:
+        return g[:, 4 * cin:5 * cin].reshape(cout, cin, 1, 1)
+    return g[:, :9 * cin].view(cout, 3, 3, cin).permute(0, 3, 1, 2)
 
 
 def repblock(x: Tensor, w3: Tensor, w1: Tensor, bns: Sequence[nn.BatchNorm2d], stride: int, act: int, slope: float,

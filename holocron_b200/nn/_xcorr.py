@@ -92,16 +92,16 @@ def _norm_conv_tensor_cores(x32: Tensor, weight: Tensor, b32: Optional[Tensor], 
     """Forward of norm_conv2d on the tensor-core kernel; fills ``mean`` / ``rstd`` (per output pixel) for the backward pass."""
     from . import _fused as K
     n, cin, h, w = x32.shape
-    cout, _, k, _ = weight.shape
-    pk = K.pack_filter(weight, False, K.round_up(cin, 8))          # bf16 KRSC, rows padded to 16, channels to 8
-    xb = K.to_channels_last_bf16(x32, pk.cin_p)                     # NHWC bf16 (zero-padded channels)
-    scratch = torch.empty(2 * n * h * w, device=x32.device, dtype=torch.float32)
-    check(lib().hb_patch_stats_bf16(ptr(xb), ptr(mean), ptr(rstd), ptr(scratch), n, h, w, pk.cin_p, k, k, stride, pad, dil,
-                                    cin * k * k, _cf(eps), stream_ptr()), "hb_patch_stats_bf16")
-    wsum = pk.wf.float().sum((1, 2, 3))                             # sum of the SAME bf16 filter values the MMAs read
-    bias = None if b32 is None else K._pad_vec(b32, pk.cout_p)
-    y = K.conv2d_forward_raw(xb, pk.wf, pk.cout_p, k, k, stride, pad, dil, bias, norm=(mean, rstd, wsum))
-    return y[:, :cout].float().contiguous()
+    k = weight.shape[2]
+
+    def patch_norm(xb: Tensor, pk):
+        scratch = torch.empty(2 * n * h * w, device=x32.device, dtype=torch.float32)
+        check(lib().hb_patch_stats_bf16(ptr(xb), ptr(mean), ptr(rstd), ptr(scratch), n, h, w, pk.cin_p, k, k, stride, pad,
+                                        dil, cin * k * k, _cf(eps), stream_ptr()), "hb_patch_stats_bf16")
+        return mean, rstd, pk.wf.float().sum((1, 2, 3))             # sum of the SAME bf16 filter values the MMAs read
+
+    y, _, _ = K._packed_conv(x32, weight, b32, stride, pad, dil, norm=patch_norm)
+    return y.float().contiguous()
 
 
 def norm_conv2d(x: Tensor, weight: Tensor, bias: Optional[Tensor] = None, stride: Union[int, Tuple[int, int]] = 1,

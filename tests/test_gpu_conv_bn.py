@@ -29,6 +29,7 @@ CONV_CASES = [
     (2, 28, 28, 48, 96, 1, 2, 0),
     (1, 7, 7, 192, 1280, 3, 2, 1),      # ragged M tile (16 pixels) + 5 N tiles
     (2, 9, 11, 16, 32, 3, 1, 1),        # odd spatial sizes, M tail
+    (2, 1, 9, 32, 48, 3, 2, 1),         # stride 2 on a one-pixel side: data gradient by zero insertion, no parity classes
     (2, 32, 32, 3, 48, 3, 2, 1),        # stem: 3 input channels (padded to 8 internally)
     (1, 1, 1, 1280, 1008, 1, 1, 0),     # GEMV-like
 ]

@@ -178,6 +178,54 @@ def test_repblock_direct_gradients_match_autograd_accumulation(cfg):
         assert p1.grad is not None and rel_l2(p1.grad, p0.grad) < 1e-5, n0
 
 
+REPBLOCK_DX_CASES = [
+    # Cin, Cout, stride, H, W
+    (32, 64, 2, 1, 7),       # stride 2 on a one-pixel side: zero insertion + convolution instead of parity classes
+    (32, 64, 2, 6, 1),
+    (24, 48, 2, 1, 5),       # the same with the input channels padded to 32
+    (3, 32, 1, 12, 12),      # padded input channels and an input that needs its gradient: no im2col stem
+    (3, 32, 2, 12, 12),
+    (24, 48, 1, 10, 10),
+    (24, 48, 2, 10, 10),
+]
+
+
+@pytest.mark.parametrize("case", REPBLOCK_DX_CASES)
+def test_repblock_input_gradient_paths_vs_fp32(case):
+    """Input-gradient paths of the fused RepBlock that the RepVGG widths never take: output, input gradient and parameter
+    gradients against the same block in fp32 torch ops, on bf16-representable inputs and filters. The reference's ReLU
+    takes the fused block's mask, so that a pre-activation rounding to the other side of zero in bf16 (a full upstream
+    gradient switched on or off) is not counted as an error. Tolerances as in test_gpu_repvgg.py's golden block."""
+    from oracle.models import RepBlockOracle
+    cin, cout, stride, h, w = case
+    torch.manual_seed(7)
+    blk = RepBlock(cin, cout, stride, False).train()
+    with torch.no_grad():
+        for p in blk.parameters():
+            if p.ndim == 1:
+                torch.nn.init.uniform_(p, 0.5, 1.5)
+            else:
+                p.copy_(p.bfloat16().float())
+    ref = RepBlockOracle(cin, cout, stride, False).train()
+    ref.load_state_dict(blk.state_dict())
+    x = torch.randn(4, cin, h, w).bfloat16().float()
+    blk = blk.cuda()
+    xd = x.cuda().requires_grad_(True)
+    y = blk(xd)
+    up = torch.randn(y.shape)
+    (y.float() * up.cuda()).sum().backward()
+    xo = x.clone().requires_grad_(True)
+    z = sum(b(xo) for b in ref.branches)
+    yo = z.relu()
+    (z * (y.float().cpu() > 0) * up).sum().backward()
+    assert y.shape == yo.shape
+    assert rel_l2(y, yo) < 6e-3
+    assert rel_l2(xd.grad, xo.grad) < 2e-2
+    ref_params = dict(ref.named_parameters())
+    for name, p in blk.named_parameters():
+        assert p.grad is not None and rel_l2(p.grad, ref_params[name].grad) < 2e-2, name
+
+
 def test_repblock_two_forward_backward_runs_are_bit_identical():
     torch.manual_seed(6)
     blk = RepBlock(96, 96, 1, True).cuda().to(memory_format=torch.channels_last).train()
