@@ -81,6 +81,18 @@ SIGNATURES = {
     "hb_pool_mid_bwd": "ppp" + "i" * 7 + "p",
     "hb_pool_last_fwd": "ppp" + "iiii" + "p",
     "hb_pool_last_bwd": "ppp" + "iiii" + "p",
+    "hb_sam_bwd_slots": "iiii",
+    "hb_sam_fwd": "ppppp" + "iiii" + "p",
+    "hb_sam_bwd": "ppppppp" + "iiii" + "p",
+    "hb_triplet_row_block": "iiii",
+    "hb_triplet_pool_fwd": "p" * 10 + "i" * 6 + "p",
+    "hb_triplet_pool_bwd": "p" * 6 + "i" * 6 + "p",
+    "hb_triplet_conv_fwd": "p" * 7 + "i" + "p",
+    "hb_triplet_gate": "p" * 5 + "i" + "p",
+    "hb_triplet_bn_bwd": "p" * 10 + "i" + "f" + "i" + "p",
+    "hb_triplet_conv_bwd": "p" * 8 + "i" + "p",
+    "hb_triplet_apply": "p" * 5 + "i" * 6 + "p",
+    "hb_triplet_dx": "p" * 11 + "i" * 6 + "p",
     "hb_gate_act_fwd_bf16": "ppp" + "iiii" + "f" + "p",
     "hb_gate_act_bwd_bf16": "ppppp" + "iiii" + "f" + "p",
     "hb_box_pairwise": "pppiiip",

@@ -16,6 +16,7 @@
 // index", so ties and NaNs route the gradient as torch's max(dim).indices does. Partial results are combined in a
 // fixed order (no atomics): every run gives the same bits. Nothing here synchronises with the host.
 #include "common.cuh"
+#include "zpool.cuh"
 
 namespace {
 
@@ -31,26 +32,6 @@ struct BlurParams {
 };
 
 __device__ __forceinline__ int reflect(int t, int n) { return t < 0 ? -t : (t >= n ? 2 * (n - 1) - t : t); }
-
-// fp32 -> T for a value that was read from a T: the bits come back unchanged (a NaN keeps its sign and payload, which
-// a rounding conversion would replace by the canonical NaN)
-template <typename T> __device__ __forceinline__ T same_bits(float f);
-template <> __device__ __forceinline__ float same_bits<float>(float f) { return f; }
-template <> __device__ __forceinline__ bf16 same_bits<bf16>(float f) {
-  return __ushort_as_bfloat16((unsigned short)(__float_as_uint(f) >> 16));
-}
-
-// V fp32 values -> one vector of T, lanes c0 + l >= C written as zeros; kExact for values read from a T (the max)
-template <typename T, bool kExact = false>
-__device__ __forceinline__ Vec16<T> pack(const float* f, int c0, int C) {
-  Vec16<T> v;
-#pragma unroll
-  for (int l = 0; l < Vec16<T>::N; ++l) {
-    const float x = c0 + l < C ? f[l] : 0.f;
-    v.v[l] = kExact ? same_bits<T>(x) : from_f<T>(x);
-  }
-  return v;
-}
 
 // One CTA per output row (n, oy); its threads walk the Wo x Cp/V vectors of that row.
 template <typename T, int K>
@@ -136,16 +117,6 @@ __global__ void __launch_bounds__(kThreads) blur_bwd_kernel(const T* __restrict_
     st16(dxr + (size_t)w * p.Cp + cvec * V, pack<T>(acc, cvec * V, p.C));
   }
 }
-
-// (v, i) replaces (cur, ci): NaN first (the lowest-index NaN), then the larger value, then the lower index. The state
-// (-inf, INT_MAX) loses to every element, -inf included.
-__device__ __forceinline__ bool better(float v, int i, float cur, int ci) {
-  if (cur != cur) return v != v && i < ci;
-  if (v != v || v > cur) return true;
-  return v == cur && i < ci;
-}
-
-constexpr int kNoIndex = 0x7fffffff;
 
 struct MidParams {
   int A, L, M, C, Cp, with_mean;
@@ -324,12 +295,6 @@ __global__ void __launch_bounds__(kThreads) last_bwd_kernel(const T* __restrict_
     for (int l = 0; l < V; ++l) g[l] = c0 + l == hit ? gmax + gmean : gmean;
     st16(dx + (size_t)e * V, pack<T>(g, c0, C));
   }
-}
-
-int pow2_at_least(int v, int cap) {
-  int g = 1;
-  while (g < v && g < cap) g <<= 1;
-  return g;
 }
 
 bool bad_dtype(int dtype) { return dtype != HB_DTYPE_F32 && dtype != HB_DTYPE_BF16; }

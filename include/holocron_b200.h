@@ -252,6 +252,53 @@ int hb_pool_mid_bwd(const void* dy, const int* idx, void* dx, int A, int L, int 
 int hb_pool_last_fwd(const void* x, void* y, int* idx, int R, int C, int Cp, int dtype, void* stream);
 int hb_pool_last_bwd(const void* dy, const int* idx, void* dx, int R, int C, int Cp, int dtype, void* stream);
 
+/* ---- attention: holocron/nn/modules/attention.py:17-30 (SAM: x * sigmoid(conv1x1(x))), :33-56 (DimAttention: x gated by
+ *      sigmoid(BN(conv7x7(z_pool(x)))) along one dim), :59-77 (TripletAttention: the mean of the C, H and W branches) -
+ * x / y / dy / dx NHWC [N,H,W,Cp] of dtype 0 (fp32) or 1 (bf16), Cp * sizeof(dtype) % 16 == 0; channels C..Cp-1 are
+ * never read into a result and are written as zeros. Gates, planes, statistics and parameter gradients are fp32.
+ * Deterministic (fixed-order partial sums, no atomics), no host sync: graph-capturable. */
+/* SAM over R = N*H*W pixel rows, C <= 128 vectors of 16 bytes. w fp32 [C], b fp32 [1]; gate fp32 [R] (saved for the
+ * backward pass). Backward: part fp32 [hb_sam_bwd_slots()][Cp + 1] scratch; dwdb fp32 [C + 1] = (dw, db). */
+int hb_sam_bwd_slots(int R, int C, int Cp, int dtype);
+int hb_sam_fwd(const void* x, const float* w, const float* b, void* y, float* gate, int R, int C, int Cp, int dtype,
+               void* stream);
+int hb_sam_bwd(const void* x, const void* dy, const float* w, const float* gate, void* dx, float* part, float* dwdb,
+               int R, int C, int Cp, int dtype, void* stream);
+/* Triplet pool, Cp <= 2048: one read of x gives the z_pool planes of the branches whose pointers are set: pc [N][2][H][W]
+ * (max, mean over C) + ic [N][H][W]; pw [N][2][H][C] (over W) + iw [N][H][C]; ph [N][2][C][W] (over H) + ih [N][C][W],
+ * through the row-block partials hp_* [N][nHB][W][C], nHB = ceil(H / hb_triplet_row_block()). Indices follow
+ * max(dim).indices (NaN first, then larger, then lower index). Backward: the same traversal of x and dy gives the sums
+ * of dy * x over C (dgc [N][H][W]), W (dgw [N][H][C]) and H (dgh [N][C][W], through hp_sum). */
+int hb_triplet_row_block(int H, int C, int Cp, int dtype);
+int hb_triplet_pool_fwd(const void* x, float* pc, int* ic, float* pw, int* iw, float* hp_max, float* hp_sum,
+                        int* hp_idx, float* ph, int* ih, int N, int H, int W, int C, int Cp, int dtype, void* stream);
+int hb_triplet_pool_bwd(const void* x, const void* dy, float* dgc, float* dgw, float* hp_sum, float* dgh, int N, int H,
+                        int W, int C, int Cp, int dtype, void* stream);
+/* Per-branch planes: HOST arrays of 3 entries (device pointers, NULL = branch disabled; rows / cols = R / S of each
+ * [N][R][S] plane). conv: z = conv2d(plane [N][2][R][S], weight [2][7][7], padding 3) and parts [slots][2] = per-CTA
+ * (sum z, sum z^2) for hb_bn_finalize (slots: HOST int[3] out). gate: g = sigmoid(z * stats[2] + stats[3]), stats =
+ * (mean, rstd, scale, shift) as hb_bn_finalize / hb_bn_eval_affine write them. bn_bwd: dz = (dg * inv_nb) g (1 - g)
+ * through the BatchNorm (batch statistics when train, else the affine map), dgamma / dbeta fp32 [1] written; parts
+ * [slots][2] scratch. conv_bwd: dplane [N][2][R][S] (gather form) and dweight [2][7][7]; parts [slots][98] scratch. */
+int hb_triplet_conv_fwd(const float* const* plane, const float* const* weight, float* const* z, float* const* parts,
+                        int* slots, const int* rows, const int* cols, int N, void* stream);
+int hb_triplet_gate(const float* const* z, const float* const* stats, float* const* gate, const int* rows,
+                    const int* cols, int N, void* stream);
+int hb_triplet_bn_bwd(const float* const* dg, const float* const* z, const float* const* gate,
+                      const float* const* stats, float* const* dz, float* const* parts, float* const* dgamma,
+                      float* const* dbeta, const int* rows, const int* cols, int N, float inv_nb, int train,
+                      void* stream);
+int hb_triplet_conv_bwd(const float* const* plane, const float* const* weight, const float* const* dz,
+                        float* const* dplane, float* const* parts, float* const* dweight, const int* rows,
+                        const int* cols, int N, void* stream);
+/* y = (x g_c + x g_h + x g_w) / (number of set gates), in that order; gates fp32 [N][H][W], [N][C][W], [N][H][C].
+ * dx = dy (g_c + g_h + g_w) / nb + per branch: the plane's dmax at the saved index + dmean / (reduced length). */
+int hb_triplet_apply(const void* x, void* y, const float* gc, const float* gh, const float* gw, int N, int H, int W,
+                     int C, int Cp, int dtype, void* stream);
+int hb_triplet_dx(const void* dy, void* dx, const float* gc, const float* gh, const float* gw, const float* dpc,
+                  const float* dph, const float* dpw, const int* ic, const int* ih, const int* iw, int N, int H, int W,
+                  int C, int Cp, int dtype, void* stream);
+
 /* ---- squeeze-excite gate: SEBlock.forward `x * y` followed by the block's activation,
  *      holocron/models/classification/rexnet.py:63-66, 125-131 --------------------------------------------- */
 /* out[n,p,c] = act(x[n,p,c] * gate[n,c]);  x/out [N,HW,C] bf16, gate fp32 [N,C]; act codes as hb_bn_act_fwd_bf16 (0-6) */
