@@ -18,14 +18,17 @@
 // that keeps the thread's channel group fixed, so per-channel parameters live in registers.
 #include <cstdio>
 #include <cstdlib>
+#include <type_traits>
+#include <utility>
 #include "common.cuh"
 #include "act.cuh"
+#include "slab.cuh"
 
 namespace {
 
 using namespace hb;
 
-constexpr int kThreads = 256;
+constexpr int kThreads = kSlabThreads;
 constexpr int kMaxBranches = 3;
 
 struct Branches {
@@ -33,44 +36,21 @@ struct Branches {
   int n;
 };
 
-// thread geometry shared by all kernels: tx = channel group inside the block's channel slab, ty = row lane
-struct Geo {
-  int cg_total;  // C / 8
-  int cg_t;      // channel groups per block (<= 32)
-  int rows_t;    // row lanes per block
-  __host__ static Geo make(int C) {
-    Geo g;
-    g.cg_total = C / 8;
-    // balanced channel slabs: 38 groups -> 2 x 19 rather than 32 + 6 (the ragged last slab kept 80 % of its block's
-    // threads idle on ReXNet's widths: 300, 366, 432, 576, ... channels)
-    const int slabs = (g.cg_total + 31) / 32;
-    g.cg_t = (g.cg_total + slabs - 1) / slabs;
-    g.rows_t = kThreads / g.cg_t;
-    return g;
-  }
-};
-
-__device__ __forceinline__ void load8(const __nv_bfloat16* p, float* f) {
-  Vec16<__nv_bfloat16> v = ld16_stream(p);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) f[j] = __bfloat162float(v.v[j]);
-}
-__device__ __forceinline__ void store8(__nv_bfloat16* p, const float* f) {
-  Vec16<__nv_bfloat16> v;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v.v[j] = __float2bfloat16_rn(f[j]);
-  st16(p, v);
+// (sum, sum of squares) partials of this block's rows, from the [2][kThreads * 8] lane values in red: parts[blockIdx.x][c]
+// as one float2 per channel ([slots][C][2], the layout hb_bn_finalize reads)
+__device__ __forceinline__ void fold_stat_partials(const SlabGeo& g, const float* red, int C, float* parts) {
+  fold_row_lanes<double, 2>(g, red, [&](int c, const double (&a)[2]) {
+    *reinterpret_cast<float2*>(parts + ((size_t)blockIdx.x * C + c) * 2) = make_float2((float)a[0], (float)a[1]);
+  });
 }
 
 // ---------------------------------------------------------------------------------------------------
 // stand-alone statistics pass: parts[blockIdx.x][c] = (sum, sum of squares) of this block's rows of u [M, C]
 // grid = (row blocks = slots, channel slabs)
-__global__ void __launch_bounds__(kThreads) bn_stats_partials_kernel(const __nv_bfloat16* __restrict__ u, int M, int C, Geo g,
-                                                                     float* __restrict__ parts) {
+__global__ void __launch_bounds__(kThreads) bn_stats_partials_kernel(const __nv_bfloat16* __restrict__ u, int M, int C,
+                                                                     SlabGeo g, float* __restrict__ parts) {
   __shared__ float red[2][kThreads * 8];
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  const bool active = ty < g.rows_t && cg < g.cg_total;
+  const auto [tx, ty, cg, active] = g.thread();
   float s[8], q[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { s[j] = 0.f; q[j] = 0.f; }
@@ -80,14 +60,14 @@ __global__ void __launch_bounds__(kThreads) bn_stats_partials_kernel(const __nv_
     // two rows in flight per trip
     for (; m + row_stride < (size_t)M; m += 2 * row_stride) {
       float a[8], b[8];
-      load8(u + m * C + cg * 8, a);
-      load8(u + (m + row_stride) * C + cg * 8, b);
+      unpack8(ld16_stream(u + m * C + cg * 8), a);
+      unpack8(ld16_stream(u + (m + row_stride) * C + cg * 8), b);
 #pragma unroll
       for (int j = 0; j < 8; ++j) { s[j] += a[j] + b[j]; q[j] += a[j] * a[j] + b[j] * b[j]; }
     }
     if (m < (size_t)M) {
       float a[8];
-      load8(u + m * C + cg * 8, a);
+      unpack8(ld16_stream(u + m * C + cg * 8), a);
 #pragma unroll
       for (int j = 0; j < 8; ++j) { s[j] += a[j]; q[j] += a[j] * a[j]; }
     }
@@ -95,19 +75,7 @@ __global__ void __launch_bounds__(kThreads) bn_stats_partials_kernel(const __nv_
 #pragma unroll
   for (int j = 0; j < 8; ++j) { red[0][threadIdx.x * 8 + j] = s[j]; red[1][threadIdx.x * 8 + j] = q[j]; }
   __syncthreads();
-  // threads 0 .. cg_t*8-1 each own one channel of the slab: sum over row lanes in a fixed order
-  const int nch = g.cg_t * 8;
-  for (int ch = threadIdx.x; ch < nch; ch += kThreads) {
-    const int ctx = ch / 8, j = ch % 8;
-    const int gcg = blockIdx.y * g.cg_t + ctx;
-    if (gcg >= g.cg_total) continue;
-    double a = 0.0, b = 0.0;
-    for (int r = 0; r < g.rows_t; ++r) {
-      a += (double)red[0][(r * g.cg_t + ctx) * 8 + j];
-      b += (double)red[1][(r * g.cg_t + ctx) * 8 + j];
-    }
-    *reinterpret_cast<float2*>(parts + ((size_t)blockIdx.x * C + gcg * 8 + j) * 2) = make_float2((float)a, (float)b);
-  }
+  fold_stat_partials(g, &red[0][0], C, parts);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -134,48 +102,79 @@ struct FinalizeParams {
 // 8 dependent L2 round trips and C / 32 blocks - two blocks for a 48-channel layer - is latency bound.)
 constexpr int kFinCh = 8, kFinLanes = 32;
 
-__global__ void __launch_bounds__(kFinCh * kFinLanes) bn_finalize_kernel(FinalizeParams p) {
-  __shared__ double red[2][kFinLanes][kFinCh];
-  const int c = blockIdx.x * kFinCh + threadIdx.x;
-  const int b = blockIdx.y;
-  double s = 0.0, q = 0.0;
-  if (c < p.C_logical) {
-    const float* pp = p.parts[b] + (size_t)c * 2;
-    const size_t row = (size_t)p.C * 2;
-    const int n = p.slots[b];
+// The fold of both finalize kernels: NS sums of n slots (of which the first `live` are used), read by load(k, v) as the NS
+// values of slot k. Returns the totals in the threads with threadIdx.y == 0; every thread must call it (it synchronises).
+template <int NS, typename Load>
+__device__ __forceinline__ void fold_slots(bool has_slots, int n, int live, Load load, double (&tot)[NS]) {
+  __shared__ double red[NS][kFinLanes][kFinCh];
+  double acc[NS];
+#pragma unroll
+  for (int i = 0; i < NS; ++i) acc[i] = 0.0;
+  if (has_slots) {
     int k = threadIdx.y;
     for (; k + 3 * kFinLanes < n; k += 4 * kFinLanes) {
-      float2 v[4];
+      double v[4][NS];
 #pragma unroll
-      for (int u = 0; u < 4; ++u) v[u] = *reinterpret_cast<const float2*>(pp + (size_t)(k + u * kFinLanes) * row);
+      for (int u = 0; u < 4; ++u) load(k + u * kFinLanes, v[u]);
 #pragma unroll
-      for (int u = 0; u < 4; ++u) { s += (double)v[u].x; q += (double)v[u].y; }
+      for (int u = 0; u < 4; ++u)
+#pragma unroll
+        for (int i = 0; i < NS; ++i)
+          if (i < live) acc[i] += v[u][i];
     }
     for (; k < n; k += kFinLanes) {
-      const float2 v = *reinterpret_cast<const float2*>(pp + (size_t)k * row);
-      s += (double)v.x; q += (double)v.y;
+      double v[NS];
+      load(k, v);
+#pragma unroll
+      for (int i = 0; i < NS; ++i)
+        if (i < live) acc[i] += v[i];
     }
   }
-  red[0][threadIdx.y][threadIdx.x] = s;
-  red[1][threadIdx.y][threadIdx.x] = q;
+#pragma unroll
+  for (int i = 0; i < NS; ++i) red[i][threadIdx.y][threadIdx.x] = acc[i];
   __syncthreads();
   if (threadIdx.y < 4) {
-    s = 0.0; q = 0.0;
 #pragma unroll
-    for (int j = 0; j < 8; ++j) { s += red[0][threadIdx.y * 8 + j][threadIdx.x]; q += red[1][threadIdx.y * 8 + j][threadIdx.x]; }
+    for (int i = 0; i < NS; ++i) {
+      double t = 0.0;
+#pragma unroll
+      for (int j = 0; j < 8; ++j) t += red[i][threadIdx.y * 8 + j][threadIdx.x];
+      acc[i] = t;
+    }
   }
   __syncthreads();
-  if (threadIdx.y < 4) { red[0][threadIdx.y][threadIdx.x] = s; red[1][threadIdx.y][threadIdx.x] = q; }
+  if (threadIdx.y < 4) {
+#pragma unroll
+    for (int i = 0; i < NS; ++i) red[i][threadIdx.y][threadIdx.x] = acc[i];
+  }
   __syncthreads();
+  if (threadIdx.y != 0) return;
+#pragma unroll
+  for (int i = 0; i < NS; ++i) {
+    double t = 0.0;
+#pragma unroll
+    for (int j = 0; j < 4; ++j) t += red[i][j][threadIdx.x];
+    tot[i] = t;
+  }
+}
+
+__global__ void __launch_bounds__(kFinCh * kFinLanes) bn_finalize_kernel(FinalizeParams p) {
+  const int c = blockIdx.x * kFinCh + threadIdx.x;
+  const int b = blockIdx.y;
+  const float* pp = p.parts[b] + (size_t)c * 2;
+  const size_t row = (size_t)p.C * 2;
+  double tot[2];
+  fold_slots<2>(c < p.C_logical, p.slots[b], 2, [&](int k, double (&v)[2]) {
+    const float2 f = *reinterpret_cast<const float2*>(pp + (size_t)k * row);
+    v[0] = (double)f.x; v[1] = (double)f.y;
+  }, tot);
   if (threadIdx.y != 0 || c >= p.C) return;
   const size_t o = (size_t)b * p.C + c;
   if (c >= p.C_logical) {
     p.mean[o] = 0.f; p.rstd[o] = 0.f; p.scale[o] = 0.f; p.shift[o] = 0.f;
     return;
   }
-  s = 0.0; q = 0.0;
-#pragma unroll
-  for (int j = 0; j < 4; ++j) { s += red[0][j][threadIdx.x]; q += red[1][j][threadIdx.x]; }
+  const double s = tot[0], q = tot[1];
   const double mean = s / p.M;
   double var = q / p.M - mean * mean;
   if (var < 0) var = 0;
@@ -231,12 +230,12 @@ struct FwdParams {
 };
 using RawVec = Vec16<__nv_bfloat16>;
 
-__device__ __forceinline__ void unpack8(const RawVec& v, float* f) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) f[j] = __bfloat162float(v.v[j]);
+// 8 floats of a per-channel constant in shared memory, as two float4
+__device__ __forceinline__ void lds8(const float* p, float* f) {
+  const float4 a = *reinterpret_cast<const float4*>(p);
+  const float4 b = *reinterpret_cast<const float4*>(p + 4);
+  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
-
-__device__ __forceinline__ void lds8(const float* p, float* f);
 
 // ---- per-thread cp.async ring ---------------------------------------------------------------------
 // Every thread streams ITS OWN 16-byte vectors (one per input tensor and row) global -> shared with cp.async, kDepth rows
@@ -263,7 +262,8 @@ __device__ __forceinline__ RawVec lds16(uint32_t saddr) {
 }
 __device__ __forceinline__ uint32_t smem_addr(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
 
-// Walks the rows m = m0, m0 + stride, ... < M of one thread. NT input tensors; `src(t)` gives tensor t's base pointer.
+// Walks the rows m = m0, m0 + stride, ... < M of one thread. NT input tensors; src[t] is tensor t's base pointer (set by
+// the kernel after init; a null source is not streamed).
 template <int NT>
 struct RowRing {
   static constexpr int kDepth = ring_depth(NT);
@@ -273,6 +273,10 @@ struct RowRing {
   size_t col_off;      // element offset of the thread's 8 channels inside a row
   int C;
   const __nv_bfloat16* src[NT > 0 ? NT : 1];
+  __device__ __forceinline__ void init(uint8_t* smem, size_t m0_, size_t stride_, int M_, int C_, size_t col_off_) {
+    base = smem_addr(smem) + threadIdx.x * 16;
+    m0 = m0_; stride = stride_; M = (size_t)M_; col_off = col_off_; C = C_;
+  }
   // slot s, tensor t of this thread
   __device__ __forceinline__ uint32_t addr(int s, int t) const { return base + (uint32_t)((s * NT + t) * kThreads * 16); }
   __device__ __forceinline__ bool valid(size_t k) const { return m0 + k * stride < M; }
@@ -300,11 +304,9 @@ struct RowRing {
 // the 16 extra accumulators the 3-branch kernel would drop from 3 to 2 resident blocks per SM, so the statistics variant is
 // compiled for 3 blocks explicitly)
 template <int NB, bool kStats>
-__global__ void __launch_bounds__(kThreads, 3) bn_act_fwd_kernel(FwdParams p, Geo g) {
+__global__ void __launch_bounds__(kThreads, 3) bn_act_fwd_kernel(FwdParams p, SlabGeo g) {
   extern __shared__ __align__(16) uint8_t ring_smem[];
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  const bool active = ty < g.rows_t && cg < g.cg_total;
+  const auto [tx, ty, cg, active] = g.thread();
   float os[8], oq[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) { os[j] = 0.f; oq[j] = 0.f; }
@@ -330,12 +332,7 @@ __global__ void __launch_bounds__(kThreads, 3) bn_act_fwd_kernel(FwdParams p, Ge
   if (active) {
     const bool has_res = p.residual != nullptr;
     RowRing<NB + 1> ring;
-    ring.base = smem_addr(ring_smem) + threadIdx.x * 16;
-    ring.m0 = (size_t)blockIdx.x * g.rows_t + ty;
-    ring.stride = (size_t)gridDim.x * g.rows_t;
-    ring.M = (size_t)p.M;
-    ring.col_off = (size_t)cg * 8;
-    ring.C = p.C;
+    ring.init(ring_smem, (size_t)blockIdx.x * g.rows_t + ty, (size_t)gridDim.x * g.rows_t, p.M, p.C, (size_t)cg * 8);
 #pragma unroll
     for (int b = 0; b < NB; ++b) ring.src[b] = p.br.u[b];
     ring.src[NB] = p.residual;
@@ -399,18 +396,7 @@ __global__ void __launch_bounds__(kThreads, 3) bn_act_fwd_kernel(FwdParams p, Ge
     red[kThreads * 8 + threadIdx.x * 8 + j] = active ? oq[j] : 0.f;
   }
   __syncthreads();
-  const int nch = g.cg_t * 8;
-  for (int ch = threadIdx.x; ch < nch; ch += kThreads) {
-    const int ctx = ch / 8, j = ch % 8;
-    const int gcg = blockIdx.y * g.cg_t + ctx;
-    if (gcg >= g.cg_total) continue;
-    double a = 0.0, b = 0.0;
-    for (int r = 0; r < g.rows_t; ++r) {
-      a += (double)red[(r * g.cg_t + ctx) * 8 + j];
-      b += (double)red[kThreads * 8 + (r * g.cg_t + ctx) * 8 + j];
-    }
-    *reinterpret_cast<float2*>(p.out_stats + ((size_t)blockIdx.x * p.C + gcg * 8 + j) * 2) = make_float2((float)a, (float)b);
-  }
+  fold_stat_partials(g, red, p.C, p.out_stats);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -446,7 +432,7 @@ struct SlabConsts {
 };
 
 template <int NB>
-__device__ __forceinline__ void load_slab_consts(SlabConsts& k, const BwdParams& p, const Geo& g, bool with_means) {
+__device__ __forceinline__ void load_slab_consts(SlabConsts& k, const BwdParams& p, const SlabGeo& g, bool with_means) {
   const int nch = g.cg_t * 8;
   const double invM = 1.0 / (double)p.M;
   for (int ch = threadIdx.x; ch < nch; ch += kThreads) {
@@ -474,12 +460,6 @@ __device__ __forceinline__ void load_slab_consts(SlabConsts& k, const BwdParams&
     k.shift[ch] = sh;
   }
   __syncthreads();
-}
-
-__device__ __forceinline__ void lds8(const float* p, float* f) {
-  const float4 a = *reinterpret_cast<const float4*>(p);
-  const float4 b = *reinterpret_cast<const float4*>(p + 4);
-  f[0] = a.x; f[1] = a.y; f[2] = a.z; f[3] = a.w; f[4] = b.x; f[5] = b.y; f[6] = b.z; f[7] = b.w;
 }
 
 // dz = d out / d z (z = normalised branch sum [+ residual]); dr = gradient reaching the residual input
@@ -524,14 +504,9 @@ __device__ __forceinline__ void recompute_dz(const BwdParams& p, const SlabConst
 }
 
 template <int NB>
-__device__ __forceinline__ void init_bwd_ring(RowRing<NB + 2>& ring, const BwdParams& p, const Geo& g, uint8_t* ring_smem,
+__device__ __forceinline__ void init_bwd_ring(RowRing<NB + 2>& ring, const BwdParams& p, const SlabGeo& g, uint8_t* ring_smem,
                                               int ty, int cg) {
-  ring.base = smem_addr(ring_smem) + threadIdx.x * 16;
-  ring.m0 = (size_t)blockIdx.x * g.rows_t + ty;
-  ring.stride = (size_t)gridDim.x * g.rows_t;
-  ring.M = (size_t)p.M;
-  ring.col_off = (size_t)cg * 8;
-  ring.C = p.C;
+  ring.init(ring_smem, (size_t)blockIdx.x * g.rows_t + ty, (size_t)gridDim.x * g.rows_t, p.M, p.C, (size_t)cg * 8);
 #pragma unroll
   for (int b = 0; b < NB; ++b) ring.src[b] = p.br.u[b];
   ring.src[NB] = (p.residual && !p.res_after) ? p.residual : nullptr;   // its value only matters inside act()
@@ -540,15 +515,13 @@ __device__ __forceinline__ void init_bwd_ring(RowRing<NB + 2>& ring, const BwdPa
 
 // pass 1: part[blk][0][c] = sum_m dz, part[blk][1+b][c] = sum_m dz * u_b over the rows of this block (no atomics)
 template <int NB>
-__global__ void __launch_bounds__(kThreads, 2) bn_act_bwd_reduce_kernel(BwdParams p, Geo g) {
+__global__ void __launch_bounds__(kThreads, 2) bn_act_bwd_reduce_kernel(BwdParams p, SlabGeo g) {
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   SlabConsts& k = *reinterpret_cast<SlabConsts*>(dyn_smem);
   float* red = reinterpret_cast<float*>(dyn_smem + sizeof(SlabConsts));   // [kThreads * 8]
   uint8_t* ring_smem = dyn_smem + sizeof(SlabConsts) + kThreads * 8 * sizeof(float);
   load_slab_consts<NB>(k, p, g, false);
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  const bool active = ty < g.rows_t && cg < g.cg_total;
+  const auto [tx, ty, cg, active] = g.thread();
   float acc[1 + NB][8];
 #pragma unroll
   for (int i = 0; i < 1 + NB; ++i)
@@ -578,34 +551,27 @@ __global__ void __launch_bounds__(kThreads, 2) bn_act_bwd_reduce_kernel(BwdParam
       }
     }
   }
-  const int nch = g.cg_t * 8;
 #pragma unroll
   for (int i = 0; i < 1 + NB; ++i) {
     __syncthreads();
 #pragma unroll
     for (int j = 0; j < 8; ++j) red[threadIdx.x * 8 + j] = acc[i][j];
     __syncthreads();
-    for (int ch = threadIdx.x; ch < nch; ch += kThreads) {
-      const int ctx = ch / 8, j = ch % 8;
-      const int gcg = blockIdx.y * g.cg_t + ctx;
-      if (gcg >= g.cg_total) continue;
-      double a = 0.0;
-      for (int r = 0; r < g.rows_t; ++r) a += (double)red[(r * g.cg_t + ctx) * 8 + j];
-      p.part[((size_t)blockIdx.x * (1 + NB) + i) * p.C + gcg * 8 + j] = a;
-    }
+    fold_row_lanes<double, 1>(g, red, [&](int c, const double (&a)[1]) {
+      p.part[((size_t)blockIdx.x * (1 + NB) + i) * p.C + c] = a[0];
+    });
   }
 }
 
 // pass 2: du_b = scale_b * dz + cu_b * u_b + c0_b, dres = dr
 template <int NB>
-__global__ void __launch_bounds__(kThreads, 2) bn_act_bwd_apply_kernel(BwdParams p, Geo g) {
+__global__ void __launch_bounds__(kThreads, 2) bn_act_bwd_apply_kernel(BwdParams p, SlabGeo g) {
   extern __shared__ __align__(16) uint8_t dyn_smem[];
   SlabConsts& k = *reinterpret_cast<SlabConsts*>(dyn_smem);
   uint8_t* ring_smem = dyn_smem + sizeof(SlabConsts);
   load_slab_consts<NB>(k, p, g, true);
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  if (ty >= g.rows_t || cg >= g.cg_total) return;
+  const auto [tx, ty, cg, active] = g.thread();
+  if (!active) return;
   RowRing<NB + 2> ring;
   init_bwd_ring<NB>(ring, p, g, ring_smem, ty, cg);
   ring.prologue();
@@ -649,60 +615,15 @@ struct BwdFinalizeParams {
 };
 // same block shape as bn_finalize_kernel: 8 channels x 32 row-block lanes, four independent rows in flight, fixed order
 __global__ void __launch_bounds__(kFinCh * kFinLanes) bn_bwd_finalize_kernel(BwdFinalizeParams p) {
-  __shared__ double red[1 + kMaxBranches][kFinLanes][kFinCh];
   const int c = blockIdx.x * kFinCh + threadIdx.x;
-  double acc[1 + kMaxBranches];
-#pragma unroll
-  for (int i = 0; i <= kMaxBranches; ++i) acc[i] = 0.0;
-  if (c < p.C) {
-    const size_t row = (size_t)(1 + p.B) * p.C;
-    int k = threadIdx.y;
-    for (; k + 3 * kFinLanes < p.nblocks; k += 4 * kFinLanes) {
-      double v[4][1 + kMaxBranches];
-#pragma unroll
-      for (int u = 0; u < 4; ++u)
-#pragma unroll
-        for (int i = 0; i <= kMaxBranches; ++i)
-          if (i <= p.B) v[u][i] = p.part[(size_t)(k + u * kFinLanes) * row + (size_t)i * p.C + c];
-#pragma unroll
-      for (int u = 0; u < 4; ++u)
-#pragma unroll
-        for (int i = 0; i <= kMaxBranches; ++i)
-          if (i <= p.B) acc[i] += v[u][i];
-    }
-    for (; k < p.nblocks; k += kFinLanes) {
-#pragma unroll
-      for (int i = 0; i <= kMaxBranches; ++i)
-        if (i <= p.B) acc[i] += p.part[(size_t)k * row + (size_t)i * p.C + c];
-    }
-  }
-#pragma unroll
-  for (int i = 0; i <= kMaxBranches; ++i) red[i][threadIdx.y][threadIdx.x] = acc[i];
-  __syncthreads();
-  if (threadIdx.y < 4) {
-#pragma unroll
-    for (int i = 0; i <= kMaxBranches; ++i) {
-      double t = 0.0;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) t += red[i][threadIdx.y * 8 + j][threadIdx.x];
-      acc[i] = t;
-    }
-  }
-  __syncthreads();
-  if (threadIdx.y < 4) {
-#pragma unroll
-    for (int i = 0; i <= kMaxBranches; ++i) red[i][threadIdx.y][threadIdx.x] = acc[i];
-  }
-  __syncthreads();
-  if (threadIdx.y != 0 || c >= p.C) return;
+  const size_t row = (size_t)(1 + p.B) * p.C;
   double tot[1 + kMaxBranches];
+  fold_slots<1 + kMaxBranches>(c < p.C, p.nblocks, 1 + p.B, [&](int k, double (&v)[1 + kMaxBranches]) {
 #pragma unroll
-  for (int i = 0; i <= kMaxBranches; ++i) {
-    double t = 0.0;
-#pragma unroll
-    for (int j = 0; j < 4; ++j) t += red[i][j][threadIdx.x];
-    tot[i] = t;
-  }
+    for (int i = 0; i <= kMaxBranches; ++i)
+      if (i <= p.B) v[i] = p.part[(size_t)k * row + (size_t)i * p.C + c];
+  }, tot);
+  if (threadIdx.y != 0 || c >= p.C) return;
   for (int i = 0; i <= p.B; ++i) p.sums[(size_t)i * p.C + c] = tot[i];
   for (int b = 0; b < p.B; ++b) {
     const size_t o = (size_t)b * p.C + c;
@@ -718,15 +639,14 @@ __global__ void __launch_bounds__(kFinCh * kFinLanes) bn_bwd_finalize_kernel(Bwd
 }
 
 // persistent grid: `per_sm` blocks per SM, grid-stride over rows
-inline dim3 make_grid(const Geo& g, int M, int z, int per_sm = 4, int min_rows = 4) {
-  const int slabs = (g.cg_total + g.cg_t - 1) / g.cg_t;
+inline dim3 make_grid(const SlabGeo& g, int M, int z, int per_sm = 4, int min_rows = 4) {
   long long row_blocks = ((long long)M + g.rows_t - 1) / g.rows_t;
-  long long cap = (HB_NUM_SMS * per_sm) / slabs;
+  long long cap = (HB_NUM_SMS * per_sm) / g.slabs;
   if (cap < 1) cap = 1;
   long long want = (row_blocks + min_rows - 1) / min_rows;   // at least ~min_rows rows per lane when there is enough work
   if (want < 1) want = 1;
   if (want > cap) want = cap;
-  return dim3((unsigned)want, (unsigned)slabs, (unsigned)z);
+  return dim3((unsigned)want, (unsigned)g.slabs, (unsigned)z);
 }
 
 inline int env_int(const char* name, int dflt) {
@@ -734,53 +654,39 @@ inline int env_int(const char* name, int dflt) {
   return v ? atoi(v) : dflt;
 }
 
-template <typename K>
-inline cudaError_t allow_smem(K kernel, size_t bytes) {
-  return cudaFuncSetAttribute(kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-}
-
-// Resident blocks per SM of one kernel instantiation with SMEM dynamic bytes, asked from the runtime once. The grids are
-// persistent (every block walks M / gridDim.x rows), so a grid of 4 blocks per SM of a kernel that only fits 3 runs as one
-// full wave plus a one-third-occupied second wave, which streams markedly slower than a grid of exactly the resident blocks.
+// Resident blocks per SM of one kernel instantiation with SMEM dynamic bytes. The grids are persistent (every block walks
+// M / gridDim.x rows), so a grid of 4 blocks per SM of a kernel that only fits 3 runs as one full wave plus a one-third-occupied
+// second wave, which streams markedly slower than a grid of exactly the resident blocks.
 template <typename K>
 inline int resident_blocks(K kernel, size_t smem) {
   int n = 0;
   if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&n, kernel, kThreads, smem) != cudaSuccess || n < 1) n = 1;
   return n;
 }
-#define HB_BN_OCC(KERNEL, NB, SMEM, OUT)                                                     \
-  {                                                                                          \
-    static int cached_occ_ = 0;                                                              \
-    if (!cached_occ_) {                                                                      \
-      if (allow_smem(KERNEL<NB>, 200 * 1024) != cudaSuccess) return (int)cudaErrorInvalidValue; \
-      cached_occ_ = resident_blocks(KERNEL<NB>, SMEM);                                       \
-    }                                                                                        \
-    OUT = cached_occ_;                                                                       \
-  }
-#define HB_BN_OCC_DISPATCH(KERNEL, B, SMEM, OUT)                                             \
-  switch (B) {                                                                               \
-    case 0: HB_BN_OCC(KERNEL, 0, SMEM, OUT) break;                                           \
-    case 1: HB_BN_OCC(KERNEL, 1, SMEM, OUT) break;                                           \
-    case 2: HB_BN_OCC(KERNEL, 2, SMEM, OUT) break;                                           \
-    default: HB_BN_OCC(KERNEL, 3, SMEM, OUT) break;                                          \
-  }
 
-#define HB_BN_LAUNCH(KERNEL, NB, GRID, SMEM, ST, ...)                                        \
-  {                                                                                          \
-    static bool ready = false;                                                               \
-    if (!ready) {                                                                            \
-      if (allow_smem(KERNEL<NB>, 200 * 1024) != cudaSuccess) return (int)cudaErrorInvalidValue; \
-      ready = true;                                                                          \
-    }                                                                                        \
-    KERNEL<NB><<<GRID, kThreads, SMEM, ST>>>(__VA_ARGS__);                                   \
+// One kernel instantiation, ready to launch with SMEM dynamic bytes, and its resident blocks per SM (0: its dynamic
+// shared-memory limit could not be raised). Both are set up on the first call only. The cache is keyed on the kernel pointer,
+// not its type: every bn_act_fwd_kernel<NB, kStats> has the same function type, and one of them must not use another's count.
+template <auto Kernel>
+std::pair<decltype(Kernel), int> instance(size_t smem) {
+  static int occ = 0;
+  if (!occ) {
+    if (cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 200 * 1024) != cudaSuccess) return {Kernel, 0};
+    occ = resident_blocks(Kernel, smem);
   }
-#define HB_BN_DISPATCH(KERNEL, B, GRID, SMEM, ST, ...)                                       \
-  switch (B) {                                                                               \
-    case 0: HB_BN_LAUNCH(KERNEL, 0, GRID, SMEM, ST, __VA_ARGS__) break;                      \
-    case 1: HB_BN_LAUNCH(KERNEL, 1, GRID, SMEM, ST, __VA_ARGS__) break;                      \
-    case 2: HB_BN_LAUNCH(KERNEL, 2, GRID, SMEM, ST, __VA_ARGS__) break;                      \
-    default: HB_BN_LAUNCH(KERNEL, 3, GRID, SMEM, ST, __VA_ARGS__) break;                     \
+  return {Kernel, occ};
+}
+
+// pick(std::integral_constant<int, NB>{}) for NB = B normalised branches (0 .. kMaxBranches, checked by the entry points)
+template <typename F>
+auto with_nb(int B, F pick) {
+  switch (B) {
+    case 0: return pick(std::integral_constant<int, 0>{});
+    case 1: return pick(std::integral_constant<int, 1>{});
+    case 2: return pick(std::integral_constant<int, 2>{});
+    default: return pick(std::integral_constant<int, 3>{});
   }
+}
 
 inline size_t ring_bytes(int tensors) { return (size_t)(ring_depth(tensors) + 1) * tensors * kThreads * 16; }
 
@@ -791,7 +697,7 @@ extern "C" {
 // Stand-alone statistics pass over u [M, C] bf16 -> parts float [*slots][C][2] (capacity hb_bn_stat_slots_max()).
 int hb_bn_stats_partials_bf16(const void* u, int M, int C, float* parts, int* slots, void* stream) {
   if (C % 8 != 0 || !slots) return (int)cudaErrorInvalidValue;
-  Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   static const int min_rows = env_int("HB_BN_STATS_ROWS", 16);
   const dim3 grid = make_grid(g, M, 1, 4, min_rows);
   *slots = (int)grid.x;
@@ -844,40 +750,25 @@ int hb_bn_act_fwd_bf16(const void* u0, const void* u1, const void* u2, int B, co
   p.M = M; p.C = C; p.act = act; p.slope = slope; p.res_after = res_after;
   if (out_stats && !out_stat_slots) return (int)cudaErrorInvalidValue;
   p.out_stats = out_stats;
-  Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   static const int per_sm_env = env_int("HB_BN_CAP_FWD", 0);
   static const bool use_occ = env_int("HB_BN_USE_OCC", 1) != 0, occ_debug = env_int("HB_BN_DEBUG", 0) != 0;
   cudaStream_t st = (cudaStream_t)stream;
   const size_t smem = ring_bytes(B + 1);
+  const auto [kernel, occ] = with_nb(B, [&](auto nb) {
+    constexpr int NB = decltype(nb)::value;
+    return out_stats ? instance<bn_act_fwd_kernel<NB, true>>(smem) : instance<bn_act_fwd_kernel<NB, false>>(smem);
+  });
+  if (!occ) return (int)cudaErrorInvalidValue;
+  if (occ_debug)
+    fprintf(stderr, "[hb] bn_act_fwd_kernel<%d,%d> smem %zu: %d resident blocks/SM\n", B, (int)(out_stats != nullptr), smem, occ);
   // grid = min(4, resident blocks of this instantiation) per SM: registers (launch bound 3) and the ring (48 - 64 KB) decide
-#define HB_FWD_GO(NBV, STATS)                                                                              \
-  {                                                                                                        \
-    static int occ = 0;                                                                                    \
-    if (!occ) {                                                                                            \
-      if (allow_smem(bn_act_fwd_kernel<NBV, STATS>, 200 * 1024) != cudaSuccess) return (int)cudaErrorInvalidValue; \
-      occ = resident_blocks(bn_act_fwd_kernel<NBV, STATS>, smem);                                          \
-    }                                                                                                      \
-    if (occ_debug) fprintf(stderr, "[hb] bn_act_fwd_kernel<%d,%d> smem %zu: %d resident blocks/SM\n", NBV, (int)STATS, smem, occ); \
-    const int fixed = (B + (residual != nullptr) >= 3) ? 3 : 4;                                            \
-    /* <= 4 blocks per SM: the caller's out_stats buffer has 4 x SMs slots (bn_stat_slots) */             \
-    const int per_sm = per_sm_env > 0 ? (per_sm_env < 4 ? per_sm_env : 4) : (use_occ ? (occ < 4 ? occ : 4) : fixed); \
-    const dim3 grid = make_grid(g, M, 1, per_sm);                                                          \
-    if (out_stat_slots) *out_stat_slots = (int)grid.x;                                                     \
-    bn_act_fwd_kernel<NBV, STATS><<<grid, kThreads, smem, st>>>(p, g);                                     \
-  }
-#define HB_FWD_CASE(NBV)                                                                                   \
-  case NBV:                                                                                                \
-    if (out_stats) HB_FWD_GO(NBV, true) else HB_FWD_GO(NBV, false)                                         \
-    break;
-  switch (B) {
-    HB_FWD_CASE(0)
-    HB_FWD_CASE(1)
-    HB_FWD_CASE(2)
-    default:
-    HB_FWD_CASE(3)
-  }
-#undef HB_FWD_GO
-#undef HB_FWD_CASE
+  const int fixed = (B + (residual != nullptr) >= 3) ? 3 : 4;
+  // <= 4 blocks per SM: the caller's out_stats buffer has 4 x SMs slots (bn_stat_slots)
+  const int per_sm = per_sm_env > 0 ? (per_sm_env < 4 ? per_sm_env : 4) : (use_occ ? (occ < 4 ? occ : 4) : fixed);
+  const dim3 grid = make_grid(g, M, 1, per_sm);
+  if (out_stat_slots) *out_stat_slots = (int)grid.x;
+  kernel<<<grid, kThreads, smem, st>>>(p, g);
   HB_LAUNCH_CHECK();
   return 0;
 }
@@ -887,7 +778,7 @@ int hb_bn_act_fwd_bf16(const void* u0, const void* u1, const void* u2, int B, co
 // dgamma/dbeta: fp32 [B][C] outputs (optional); gamma_grad_acc / beta_grad_acc: optional HOST arrays of B device pointers
 // (entries may be NULL) to fp32 [C_logical] gradient buffers that dgamma_b / dbeta_b are ADDED to.
 size_t hb_bn_bwd_scratch_doubles(int M, int C, int B) {
-  Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   const dim3 grid = make_grid(g, M, 1, 3);   // upper bound of the reduction pass' row blocks (cap <= 3 per SM)
   return (size_t)(1 + B) * C * (1 + (size_t)grid.x);
 }
@@ -906,7 +797,7 @@ int hb_bn_act_bwd_bf16(const void* dout, const void* u0, const void* u1, const v
   p.du[0] = (__nv_bfloat16*)du0; p.du[1] = (__nv_bfloat16*)du1; p.du[2] = (__nv_bfloat16*)du2;
   p.dres = (__nv_bfloat16*)dres;
   p.M = M; p.C = C; p.act = act; p.slope = slope; p.train = train; p.res_after = res_after;
-  Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   cudaStream_t st = (cudaStream_t)stream;
   static const int cap_red_env = env_int("HB_BN_CAP_RED", 0), cap_app_env = env_int("HB_BN_CAP_APPLY", 0);
   static const bool use_occ = env_int("HB_BN_USE_OCC", 1) != 0, occ_debug = env_int("HB_BN_DEBUG", 0) != 0;
@@ -917,11 +808,11 @@ int hb_bn_act_bwd_bf16(const void* dout, const void* u0, const void* u1, const v
   const bool want_params = (dgamma && dbeta) || gamma_grad_acc || beta_grad_acc;
   if (train || want_params) {
     const size_t smem = sizeof(SlabConsts) + kThreads * 8 * sizeof(float) + ring_bytes(B + 2);
-    int occ = 1;
-    HB_BN_OCC_DISPATCH(bn_act_bwd_reduce_kernel, B, smem, occ)
+    const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_reduce_kernel<decltype(nb)::value>>(smem); });
+    if (!occ) return (int)cudaErrorInvalidValue;
     if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_reduce_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_red);
     const dim3 grid = make_grid(g, M, 1, (use_occ && occ < cap_red) ? occ : cap_red);
-    HB_BN_DISPATCH(bn_act_bwd_reduce_kernel, B, grid, smem, st, p, g)
+    kernel<<<grid, kThreads, smem, st>>>(p, g);
     HB_LAUNCH_CHECK();
     BwdFinalizeParams f{};
     f.part = p.part; f.sums = p.sums; f.mean = mean; f.rstd = rstd; f.dgamma = dgamma; f.dbeta = dbeta;
@@ -935,11 +826,11 @@ int hb_bn_act_bwd_bf16(const void* dout, const void* u0, const void* u1, const v
   }
   {
     const size_t smem = sizeof(SlabConsts) + ring_bytes(B + 2);
-    int occ = 1;
-    HB_BN_OCC_DISPATCH(bn_act_bwd_apply_kernel, B, smem, occ)
+    const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_apply_kernel<decltype(nb)::value>>(smem); });
+    if (!occ) return (int)cudaErrorInvalidValue;
     if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_apply_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_app);
     const dim3 grid = make_grid(g, M, 1, (use_occ && occ < cap_app) ? occ : cap_app);
-    HB_BN_DISPATCH(bn_act_bwd_apply_kernel, B, grid, smem, st, p, g)
+    kernel<<<grid, kThreads, smem, st>>>(p, g);
     HB_LAUNCH_CHECK();
   }
   return 0;

@@ -71,6 +71,19 @@ template <typename T> __device__ __forceinline__ void st16(T* p, const Vec16<T>&
   *reinterpret_cast<uint4*>(p) = v.raw;
 }
 
+// 8 bf16 <-> 8 fp32. There is deliberately no load8: each caller picks its cache hint (unpack8(ld16_stream(p), f) for
+// read-once streams, unpack8(ld16(p), f) for data neighbouring threads re-read through L1).
+__device__ __forceinline__ void unpack8(const Vec16<__nv_bfloat16>& v, float* f) {
+#pragma unroll
+  for (int j = 0; j < 8; ++j) f[j] = __bfloat162float(v.v[j]);
+}
+__device__ __forceinline__ void store8(__nv_bfloat16* p, const float* f) {
+  Vec16<__nv_bfloat16> v;
+#pragma unroll
+  for (int j = 0; j < 8; ++j) v.v[j] = __float2bfloat16_rn(f[j]);
+  st16(p, v);
+}
+
 __host__ __device__ __forceinline__ bool aligned16(const void* p) { return (reinterpret_cast<uintptr_t>(p) & 15) == 0; }
 
 // ---- NaN-propagating clamps -------------------------------------------------------------

@@ -12,17 +12,8 @@ using namespace hb;
 
 constexpr int kThreads = 256;
 
-__device__ __forceinline__ void load8(const __nv_bfloat16* p, float* f) {
-  Vec16<__nv_bfloat16> v = ld16(p);
-#pragma unroll
-  for (int j = 0; j < 8; ++j) f[j] = __bfloat162float(v.v[j]);
-}
-__device__ __forceinline__ void store8(__nv_bfloat16* p, const float* f) {
-  Vec16<__nv_bfloat16> v;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v.v[j] = __float2bfloat16_rn(f[j]);
-  st16(p, v);
-}
+// neighbouring threads re-read the same taps: the L1-allocating load
+__device__ __forceinline__ void load8(const __nv_bfloat16* p, float* f) { unpack8(ld16(p), f); }
 
 struct DwParams {
   int N, H, W, C, Ho, Wo, K, stride, pad;

@@ -23,13 +23,6 @@ struct InvParams {
   int N, H, W, C, Cp, Ho, Wo, Kp, G, stride, pad, dil;
 };
 
-__device__ __forceinline__ void store8(bf16* p, const float* f) {
-  Vec16<bf16> v;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v.v[j] = __float2bfloat16_rn(f[j]);
-  st16(p, v);
-}
-
 __device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
   const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
   asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(valid ? 16 : 0));

@@ -7,44 +7,20 @@
 // an activation pass, two multiplies + a reduction in backward and a one-thread-per-(n, 8 channels) pooling walk.
 #include "common.cuh"
 #include "act.cuh"
+#include "slab.cuh"
 
 namespace {
 
 using namespace hb;
 
-constexpr int kThreads = 256;
-
-struct Geo {
-  int cv, cg_t, rows_t, slabs;
-  __host__ static Geo make(int C) {
-    Geo g;
-    g.cv = C / 8;
-    const int nslab = (g.cv + 31) / 32;
-    g.cg_t = (g.cv + nslab - 1) / nslab;
-    g.rows_t = kThreads / g.cg_t;
-    g.slabs = (g.cv + g.cg_t - 1) / g.cg_t;
-    return g;
-  }
-};
-
-__device__ __forceinline__ void unpack8(const Vec16<__nv_bfloat16>& v, float* f) {
-#pragma unroll
-  for (int j = 0; j < 8; ++j) f[j] = __bfloat162float(v.v[j]);
-}
-__device__ __forceinline__ void store8(__nv_bfloat16* p, const float* f) {
-  Vec16<__nv_bfloat16> v;
-#pragma unroll
-  for (int j = 0; j < 8; ++j) v.v[j] = __float2bfloat16_rn(f[j]);
-  st16(p, v);
-}
+constexpr int kThreads = kSlabThreads;
 
 // grid = (1, slabs, N)
 __global__ void __launch_bounds__(kThreads) gate_act_fwd_kernel(const __nv_bfloat16* __restrict__ x, const float* __restrict__ gate,
                                                                __nv_bfloat16* __restrict__ out, int HW, int C, int act,
-                                                               float slope, Geo g) {
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  if (ty >= g.rows_t || cg >= g.cv) return;
+                                                               float slope, SlabGeo g) {
+  const auto [tx, ty, cg, active] = g.thread();
+  if (!active) return;
   const size_t n = blockIdx.z;
   float gt[8];
 #pragma unroll
@@ -74,11 +50,9 @@ __global__ void __launch_bounds__(kThreads) gate_act_bwd_kernel(const __nv_bfloa
                                                                const __nv_bfloat16* __restrict__ x,
                                                                const float* __restrict__ gate, __nv_bfloat16* __restrict__ dx,
                                                                float* __restrict__ dgate, int HW, int C, int act, float slope,
-                                                               Geo g) {
+                                                               SlabGeo g) {
   __shared__ float red[kThreads * 8];
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  const bool active = ty < g.rows_t && cg < g.cv;
+  const auto [tx, ty, cg, active] = g.thread();
   const size_t n = blockIdx.z;
   float acc[8];
 #pragma unroll
@@ -104,23 +78,14 @@ __global__ void __launch_bounds__(kThreads) gate_act_bwd_kernel(const __nv_bfloa
 #pragma unroll
   for (int j = 0; j < 8; ++j) red[threadIdx.x * 8 + j] = acc[j];
   __syncthreads();
-  for (int ch = threadIdx.x; ch < g.cg_t * 8; ch += kThreads) {
-    const int ctx = ch / 8, j = ch % 8;
-    const int gcg = blockIdx.y * g.cg_t + ctx;
-    if (gcg >= g.cv) continue;
-    float a = 0.f;
-    for (int r = 0; r < g.rows_t; ++r) a += red[(r * g.cg_t + ctx) * 8 + j];
-    dgate[n * C + gcg * 8 + j] = a;
-  }
+  fold_row_lanes<float, 1>(g, red, [&](int c, const float (&a)[1]) { dgate[n * C + c] = a[0]; });
 }
 
 // y[n, c] = mean over the HW rows of image n; grid = (1, slabs, N)
 __global__ void __launch_bounds__(kThreads) gap_fwd_kernel(const __nv_bfloat16* __restrict__ x, __nv_bfloat16* __restrict__ y,
-                                                          int HW, int C, Geo g) {
+                                                          int HW, int C, SlabGeo g) {
   __shared__ float red[kThreads * 8];
-  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
-  const int cg = blockIdx.y * g.cg_t + tx;
-  const bool active = ty < g.rows_t && cg < g.cv;
+  const auto [tx, ty, cg, active] = g.thread();
   const size_t n = blockIdx.z;
   float acc[8];
 #pragma unroll
@@ -143,14 +108,7 @@ __global__ void __launch_bounds__(kThreads) gap_fwd_kernel(const __nv_bfloat16* 
   for (int j = 0; j < 8; ++j) red[threadIdx.x * 8 + j] = acc[j];
   __syncthreads();
   const float inv = 1.f / (float)HW;
-  for (int ch = threadIdx.x; ch < g.cg_t * 8; ch += kThreads) {
-    const int ctx = ch / 8, j = ch % 8;
-    const int gcg = blockIdx.y * g.cg_t + ctx;
-    if (gcg >= g.cv) continue;
-    float a = 0.f;
-    for (int r = 0; r < g.rows_t; ++r) a += red[(r * g.cg_t + ctx) * 8 + j];
-    y[n * C + gcg * 8 + j] = __float2bfloat16_rn(a * inv);
-  }
+  fold_row_lanes<float, 1>(g, red, [&](int c, const float (&a)[1]) { y[n * C + c] = __float2bfloat16_rn(a[0] * inv); });
 }
 
 }  // namespace
@@ -161,7 +119,7 @@ int hb_gate_act_fwd_bf16(const void* x, const float* gate, void* out, int N, int
                          void* stream) {
   if (C % 8 != 0 || act == ACT_FRELU) return (int)cudaErrorInvalidValue;
   if (N <= 0 || HW <= 0) return 0;
-  const Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   gate_act_fwd_kernel<<<dim3(1, g.slabs, N), kThreads, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)x, gate, (__nv_bfloat16*)out, HW, C, act, slope, g);
   HB_LAUNCH_CHECK();
@@ -172,7 +130,7 @@ int hb_gate_act_bwd_bf16(const void* dout, const void* x, const float* gate, voi
                          int act, float slope, void* stream) {
   if (C % 8 != 0 || act == ACT_FRELU) return (int)cudaErrorInvalidValue;
   if (N <= 0 || HW <= 0) return 0;
-  const Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   gate_act_bwd_kernel<<<dim3(1, g.slabs, N), kThreads, 0, (cudaStream_t)stream>>>(
       (const __nv_bfloat16*)dout, (const __nv_bfloat16*)x, gate, (__nv_bfloat16*)dx, dgate, HW, C, act, slope, g);
   HB_LAUNCH_CHECK();
@@ -182,7 +140,7 @@ int hb_gate_act_bwd_bf16(const void* dout, const void* x, const float* gate, voi
 int hb_gap_fwd_bf16(const void* x, void* y, int N, int HW, int C, void* stream) {
   if (C % 8 != 0) return (int)cudaErrorInvalidValue;
   if (N <= 0 || HW <= 0) return 0;
-  const Geo g = Geo::make(C);
+  const SlabGeo g = SlabGeo::make(C);
   gap_fwd_kernel<<<dim3(1, g.slabs, N), kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, HW, C, g);
   HB_LAUNCH_CHECK();
   return 0;

@@ -75,7 +75,7 @@ def batch_stats(u: torch.Tensor):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# geometry (Geo::make, make_grid and RowRing of bn_act.cu)
+# geometry (SlabGeo::make of slab.cuh, make_grid and RowRing of bn_act.cu)
 # ---------------------------------------------------------------------------------------------------------------------
 class Geo(NamedTuple):
     cg_total: int   # 8-channel groups
