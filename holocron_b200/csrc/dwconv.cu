@@ -575,11 +575,16 @@ inline void dw_wgrad_geo(int C, int& cg_t, int& rows_t, int& slabs, int& gx_max)
   if (gx_max < 1) gx_max = 1;
 }
 
-DwParams make_params(int N, int H, int W, int C, int K, int stride, int pad) {
-  DwParams p{N, H, W, C, 0, 0, K, stride, pad};
-  p.Ho = (H + 2 * pad - K) / stride + 1;
-  p.Wo = (W + 2 * pad - K) / stride + 1;
-  return p;
+// 0 when the geometry is supported (fills p), otherwise cudaErrorInvalidValue, before any launch or device query:
+// N, H, W, C, K, stride >= 1, pad >= 0, C % 8 == 0 and a filter that fits the padded input (Ho, Wo >= 1). Integer
+// division truncates towards zero, so H + 2 * pad - K is checked for a negative value itself: (H + 2 * pad - K) / stride + 1
+// alone gives Ho = 1 for a filter up to stride - 1 pixels too large.
+int make_params(DwParams& p, int N, int H, int W, int C, int K, int stride, int pad) {
+  if (N < 1 || H < 1 || W < 1 || C < 1 || C % 8 != 0 || K < 1 || stride < 1 || pad < 0) return (int)cudaErrorInvalidValue;
+  const long long h = (long long)H + 2LL * pad - K, w = (long long)W + 2LL * pad - K;
+  if (h < 0 || w < 0 || h / stride >= 0x7fffffffLL || w / stride >= 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  p = DwParams{N, H, W, C, (int)(h / stride + 1), (int)(w / stride + 1), K, stride, pad};
+  return 0;
 }
 
 }  // namespace
@@ -589,10 +594,9 @@ extern "C" {
 // y[N,Ho,Wo,C] = dwconv(x[N,H,W,C], w fp32 [C,K,K]) + bias; C % 8 == 0
 int hb_dwconv_fwd_bf16(const void* x, const float* w, const float* bias, void* y, int N, int H, int W, int C, int K,
                        int stride, int pad, void* stream) {
-  if (C % 8 != 0) return (int)cudaErrorInvalidValue;
-  DwParams p = make_params(N, H, W, C, K, stride, pad);
+  DwParams p;
+  if (int rc = make_params(p, N, H, W, C, K, stride, pad)) return rc;
   const long long total = (long long)N * p.Ho * p.Wo * (C / 8);
-  if (total <= 0) return 0;
   if (K == 3 && (long long)N * p.Ho * p.Wo < 0x7fffffffLL) {
     int cg_t, rows_t;
     const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
@@ -622,10 +626,9 @@ int hb_dwconv_fwd_bf16(const void* x, const float* w, const float* bias, void* y
 
 int hb_dwconv_bwd_data_bf16(const void* dy, const float* w, void* dx, int N, int H, int W, int C, int K, int stride,
                             int pad, void* stream) {
-  if (C % 8 != 0) return (int)cudaErrorInvalidValue;
-  DwParams p = make_params(N, H, W, C, K, stride, pad);
+  DwParams p;
+  if (int rc = make_params(p, N, H, W, C, K, stride, pad)) return rc;
   const long long total = (long long)N * H * W * (C / 8);
-  if (total <= 0) return 0;
   if (K == 3 && (long long)N * H * W < 0x7fffffffLL) {
     int cg_t, rows_t;
     const __nv_bfloat16* dyb = (const __nv_bfloat16*)dy;
@@ -660,9 +663,10 @@ int hb_dwconv_bwd_data_bf16(const void* dy, const float* w, void* dx, int N, int
   return 0;
 }
 
-// doubles of scratch hb_dwconv_bwd_weight_bf16 needs for C channels and a K x K filter (per-block partial sums)
+// doubles of scratch hb_dwconv_bwd_weight_bf16 needs for C channels and a K x K filter (per-block partial sums); 0 for
+// the shapes it refuses (K outside {1, 3, 5, 7})
 size_t hb_dwconv_wgrad_scratch_doubles(int C, int K) {
-  if (C <= 0 || C % 8 != 0) return 0;
+  if (C <= 0 || C % 8 != 0 || (K != 1 && K != 3 && K != 5 && K != 7)) return 0;
   int cg_t, rows_t, slabs, gx_max;
   dw_wgrad_geo(C, cg_t, rows_t, slabs, gx_max);
   return (size_t)gx_max * C * (K * K + 1);
@@ -671,9 +675,10 @@ size_t hb_dwconv_wgrad_scratch_doubles(int C, int K) {
 // dw fp32 [C,K,K], db fp32 [C] (or NULL); scratch: double[hb_dwconv_wgrad_scratch_doubles(C, K)]. K in {1, 3, 5, 7}.
 int hb_dwconv_bwd_weight_bf16(const void* x, const void* dy, float* dw, float* db, double* scratch, int N, int H, int W,
                               int C, int K, int stride, int pad, void* stream) {
-  if (C % 8 != 0) return (int)cudaErrorInvalidValue;
+  DwParams p;
+  if (int rc = make_params(p, N, H, W, C, K, stride, pad)) return rc;
+  if (K != 1 && K != 3 && K != 5 && K != 7) return (int)cudaErrorInvalidValue;
   cudaStream_t st = (cudaStream_t)stream;
-  DwParams p = make_params(N, H, W, C, K, stride, pad);
   const int KK = K * K;
   int cg_t, rows_t, slabs, gx_max;
   dw_wgrad_geo(C, cg_t, rows_t, slabs, gx_max);

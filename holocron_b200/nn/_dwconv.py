@@ -23,8 +23,9 @@ class _DwConvFn(torch.autograd.Function):
         w32 = weight.detach().float().contiguous()
         b32 = None if bias is None else bias.detach().float().contiguous()
         y = K._empty_cl(n, c, ho, wo, xb.device)
-        check(lib().hb_dwconv_fwd_bf16(ptr(xb), ptr(w32), ptr(b32), ptr(y), n, h, w, c, k, stride, pad, stream_ptr()),
-              "hb_dwconv_fwd_bf16")
+        if n > 0:       # an empty batch launches nothing: the C ABI refuses N < 1
+            check(lib().hb_dwconv_fwd_bf16(ptr(xb), ptr(w32), ptr(b32), ptr(y), n, h, w, c, k, stride, pad, stream_ptr()),
+                  "hb_dwconv_fwd_bf16")
         ctx.save_for_backward(xb, w32)
         ctx.cfg = (stride, pad, bias is not None)
         return y
@@ -40,11 +41,17 @@ class _DwConvFn(torch.autograd.Function):
         dx = dw = db = None
         if ctx.needs_input_grad[0]:
             dx = K._empty_cl(n, c, h, w, dyb.device)
-            check(L.hb_dwconv_bwd_data_bf16(ptr(dyb), ptr(w32), ptr(dx), n, h, w, c, k, stride, pad, stream_ptr()),
-                  "hb_dwconv_bwd_data_bf16")
+            if n > 0:
+                check(L.hb_dwconv_bwd_data_bf16(ptr(dyb), ptr(w32), ptr(dx), n, h, w, c, k, stride, pad, stream_ptr()),
+                      "hb_dwconv_bwd_data_bf16")
         if ctx.needs_input_grad[1] or (has_bias and ctx.needs_input_grad[2]):
             dw = torch.empty((c, 1, k, k), device=dyb.device, dtype=torch.float32)
             db = torch.empty(c, device=dyb.device, dtype=torch.float32) if has_bias else None
+            if n == 0:
+                dw.zero_()
+                if db is not None:
+                    db.zero_()
+                return dx, dw, db, None, None
             sums = torch.empty(L.hb_dwconv_wgrad_scratch_doubles(c, k), device=dyb.device, dtype=torch.float64)
             check(L.hb_dwconv_bwd_weight_bf16(ptr(xb), ptr(dyb), ptr(dw), ptr(db), ptr(sums), n, h, w, c, k, stride, pad,
                                               stream_ptr()), "hb_dwconv_bwd_weight_bf16")

@@ -166,7 +166,10 @@ int hb_bn_act_bwd_bf16(const void* dout, const void* u0, const void* u1, const v
                        float slope, int train, int res_after, void* stream);
 
 /* ---- depth-wise k x k convolution (NHWC bf16; weights fp32 [C,K,K]): FReLU's conv (activation.py:71-73) and the
- *      ReXNet depth-wise stage (holocron/models/classification/rexnet.py:112-125) ------------------------- */
+ *      ReXNet depth-wise stage (holocron/models/classification/rexnet.py:112-125) -------------------------
+ * Ho = (H + 2*pad - K) / stride + 1, Wo likewise. All three entry points return cudaErrorInvalidValue, before any launch
+ * or device query, unless N, H, W, C, K, stride >= 1, pad >= 0, C % 8 == 0 and K <= H + 2*pad, K <= W + 2*pad (so
+ * Ho, Wo >= 1). hb_dwconv_wgrad_scratch_doubles returns 0 for C < 1, C % 8 != 0 or K outside {1,3,5,7}. */
 int hb_dwconv_fwd_bf16(const void* x, const float* w, const float* bias, void* y, int N, int H, int W, int C, int K,
                        int stride, int pad, void* stream);
 int hb_dwconv_bwd_data_bf16(const void* dy, const float* w, void* dx, int N, int H, int W, int C, int K, int stride,

@@ -40,7 +40,7 @@ def excess(got: torch.Tensor, ref: torch.Tensor, abs_sum: torch.Tensor, rel: flo
 def assert_within(got: torch.Tensor, ref: torch.Tensor, abs_sum: torch.Tensor, what: str, rel: float = 1e-5,
                   bits: int = BF16_BITS, slack: Optional[torch.Tensor] = None) -> None:
     ex = excess(got, ref, abs_sum, rel, bits, slack)
-    bad = ex > 0
+    bad = ~(ex <= 0)        # NaN fails too: an element left unwritten in a NaN-filled output
     if bad.any():
         first = tuple(int(i) for i in bad.nonzero()[0])
         raise AssertionError(f"{what}: {int(bad.sum())} of {bad.numel()} elements off, worst excess {float(ex.max()):.3e}, "
@@ -48,34 +48,37 @@ def assert_within(got: torch.Tensor, ref: torch.Tensor, abs_sum: torch.Tensor, w
                              f"ref {float(ref.cpu()[first]):.6g}")
 
 
-def _f64(t: torch.Tensor) -> torch.Tensor:
-    return t.detach().cpu().double()
+def _f64(t: torch.Tensor, device="cpu") -> torch.Tensor:
+    return t.detach().to(device, torch.float64)
 
 
 def conv_ref(x: torch.Tensor, w: torch.Tensor, bias: Optional[torch.Tensor] = None, stride: int = 1, padding: int = 0,
-             dilation: int = 1):
-    """(fp64 conv2d, the same conv2d on |x| and |w|) of NCHW ``x`` and OIHW ``w``, on the CPU."""
-    x64, w64 = _f64(x), _f64(w)
-    b64 = None if bias is None else _f64(bias)
-    ref = TF.conv2d(x64, w64, b64, stride, padding, dilation)
-    abs_sum = TF.conv2d(x64.abs(), w64.abs(), None if b64 is None else b64.abs(), stride, padding, dilation)
+             dilation: int = 1, groups: int = 1, device="cpu"):
+    """(fp64 conv2d, the same conv2d on |x| and |w|) of NCHW ``x`` and OIHW ``w`` (``[Cout, Cin / groups, k, k]``), on
+    ``device`` (the CPU by default)."""
+    x64, w64 = _f64(x, device), _f64(w, device)
+    b64 = None if bias is None else _f64(bias, device)
+    ref = TF.conv2d(x64, w64, b64, stride, padding, dilation, groups)
+    abs_sum = TF.conv2d(x64.abs(), w64.abs(), None if b64 is None else b64.abs(), stride, padding, dilation, groups)
     return ref, abs_sum
 
 
-def dgrad_ref(input_shape, w: torch.Tensor, dy: torch.Tensor, stride: int = 1, padding: int = 0, dilation: int = 1):
+def dgrad_ref(input_shape, w: torch.Tensor, dy: torch.Tensor, stride: int = 1, padding: int = 0, dilation: int = 1,
+              groups: int = 1, device="cpu"):
     """(fp64 data gradient of a conv2d with filter ``w`` (OIHW) and output gradient ``dy``, the same on |w| and |dy|)."""
-    d64, w64 = _f64(dy), _f64(w)
-    return (conv2d_input(input_shape, w64, d64, stride, padding, dilation),
-            conv2d_input(input_shape, w64.abs(), d64.abs(), stride, padding, dilation))
+    d64, w64 = _f64(dy, device), _f64(w, device)
+    return (conv2d_input(input_shape, w64, d64, stride, padding, dilation, groups),
+            conv2d_input(input_shape, w64.abs(), d64.abs(), stride, padding, dilation, groups))
 
 
-def wgrad_ref(x: torch.Tensor, dy: torch.Tensor, k: int, stride: int = 1, padding: int = 0, dilation: int = 1):
-    """(fp64 weight gradient [Cout, Cin, k, k], the same on |x| and |dy|) of a conv2d with NCHW input ``x`` and output
-    gradient ``dy``."""
-    x64, d64 = _f64(x), _f64(dy)
-    shape = (dy.shape[1], x.shape[1], k, k)
-    return (conv2d_weight(x64, shape, d64, stride, padding, dilation),
-            conv2d_weight(x64.abs(), shape, d64.abs(), stride, padding, dilation))
+def wgrad_ref(x: torch.Tensor, dy: torch.Tensor, k: int, stride: int = 1, padding: int = 0, dilation: int = 1,
+              groups: int = 1, device="cpu"):
+    """(fp64 weight gradient [Cout, Cin / groups, k, k], the same on |x| and |dy|) of a conv2d with NCHW input ``x`` and
+    output gradient ``dy``."""
+    x64, d64 = _f64(x, device), _f64(dy, device)
+    shape = (dy.shape[1], x.shape[1] // groups, k, k)
+    return (conv2d_weight(x64, shape, d64, stride, padding, dilation, groups),
+            conv2d_weight(x64.abs(), shape, d64.abs(), stride, padding, dilation, groups))
 
 
 def epilogue_ref(acc: torch.Tensor, abs_sum: torch.Tensor, residual: Optional[torch.Tensor] = None, relu: bool = False):

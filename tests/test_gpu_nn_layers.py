@@ -183,7 +183,7 @@ def test_depthwise_conv_vs_oracle(stride, c):
 @pytest.mark.parametrize("shape", [(2, 96, 37, 29, 1, 1, False), (2, 40, 16, 16, 2, 1, True), (3, 176, 14, 14, 1, 1, False),
                                    (2, 24, 9, 7, 2, 1, False), (1, 8, 5, 4, 1, 1, True), (2, 32, 8, 8, 1, 0, False),
                                    (2, 16, 6, 3, 1, 1, False)])
-def test_depthwise_quad_kernel_edges(shape, monkeypatch):
+def test_depthwise_quad_kernel_edges(shape):
     """Four-outputs-per-thread depth-wise kernel (forward stride 1 / 2, data gradient stride 1 as a flipped correlation): ragged
     widths (W % 4 != 0), padding 0 and 1, widths below one quad (falls back to the one-output kernel), bias."""
     from holocron_b200.nn._dwconv import dwconv2d

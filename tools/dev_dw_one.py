@@ -15,7 +15,7 @@ for (N, H, W, C, stride) in [(256, 112, 112, 96, 2), (256, 56, 56, 176, 1)]:
     y = torch.empty(N, Ho, Wo, C, device="cuda", dtype=torch.bfloat16)
     dx = torch.empty_like(x)
     dw = torch.empty(C, 3, 3, device="cuda")
-    sums = torch.empty(C * 10, device="cuda", dtype=torch.float64)
+    sums = torch.empty(L.hb_dwconv_wgrad_scratch_doubles(C, 3), device="cuda", dtype=torch.float64)
     for _ in range(2):
         L.hb_dwconv_fwd_bf16(ptr(x), ptr(w), ptr(None), ptr(y), N, H, W, C, 3, stride, 1, stream_ptr())
         L.hb_dwconv_bwd_data_bf16(ptr(dy), ptr(w), ptr(dx), N, H, W, C, 3, stride, 1, stream_ptr())
