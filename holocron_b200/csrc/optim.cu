@@ -1,12 +1,31 @@
 // Multi-tensor optimizer steps: AdaBelief, LAMB, TAdam, AdamP, Adan, AdEMAMix, LARS, RaLars and the Lookahead weight
 // synchronisation (reference holocron/optim/{adabelief,lamb,tadam,adamp,adan,ademamix,lars,ralars,wrapper}.py).
 //
-// The reference loops over parameter tensors in Python and issues ~9-14 ATen kernels per tensor (plus, for LAMB,
-// two host synchronisations per tensor). Here a whole parameter group is updated by 1 (AdaBelief) or 2-3
-// (LAMB / TAdam: a per-tensor reduction has to complete before the update) launches: a device-resident table
-// describes every tensor (pointers + numel) and a chunk list maps each CTA to a 4096-element slice of one tensor,
-// so the kernels are pure 128-bit-vectorised HBM streams (AdaBelief: 28 B/param algorithmic traffic).
-// All state is fp32; per-tensor reductions are accumulated in fp64 atomics (order-insensitive at fp32 precision).
+// The reference loops over parameter tensors in Python and issues ~9-16 ATen kernels per tensor (plus, for LAMB, LARS,
+// RaLars and AdamP, host synchronisations per tensor). Here a device-resident table describes every tensor of a parameter
+// group (pointers + numel) and a chunk list maps each CTA to a 4096-element slice of one tensor, so a whole group is
+// updated by a fixed number of launches that are 128-bit-vectorised HBM streams (AdaBelief: 28 B/param algorithmic traffic),
+// with a scalar path for a tensor any of whose pointers is not 16-byte aligned:
+//
+//   family      launches                                     per-tensor reduction (scratch doubles)   control block
+//   AdaBelief   1                                            -                                         read
+//   LAMB        2  moments + norms, apply                    ||p||^2, ||update||^2          [2T]      -
+//   TAdam       3  reduce, apply, W_t update                 sum (g - m)^2 / (v + eps)      [T]       -
+//   AdamP       2  moments + sums, apply                     <p,g>, ||p||^2, ||g||^2, <p,pt> [4T]     read (both passes)
+//   Adan        1                                            -                                         read
+//   AdEMAMix    1                                            -                                         read
+//   LARS        2  norms, apply                              ||p||^2, ||g||^2               [2T]      -
+//   RaLars      2  moments + norms, apply                    ||p||^2, ||update||^2          [2T]      -
+//   Lookahead   1  (weight synchronisation)                  -                                         -
+//
+// A reduction has to complete before the update that uses it, hence the extra launches. Parameters, gradients and every
+// state tensor are fp32: two moments per tensor, plus the amsgrad maximum (AdaBelief, TAdam, AdamP, Adan), a third moment
+// (Adan's exp_avg_delta, AdEMAMix's exp_avg_slow), Adan's prev_grad, the LARS momentum buffer, the Lookahead slow weights,
+// and one fp32 scalar per tensor for TAdam's W_t and the LAMB / RaLars trust ratio. Per-tensor reductions are fp32 within a
+// thread (at most 16 terms), fp64 from the block reduction on, and added across CTAs with fp64 atomics (order-insensitive
+// at fp32 precision). "Control block": the kernel takes the learning rate (and beta1 when >= 0) from the device block of a
+// captured training step and does nothing while its skip flag is set (apply_ctl below); the step counter of the families
+// that keep one on the device (AdaBelief, AdamP, Adan) does not advance either.
 #include "common.cuh"
 
 namespace {

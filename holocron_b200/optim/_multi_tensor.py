@@ -13,6 +13,17 @@ def effective_strides(t: Tensor):
     return tuple(s for s, n in zip(t.stride(), t.shape) if n != 1)
 
 
+def _dense(t: Tensor) -> bool:
+    """Non-overlapping and dense: some permutation of the dims is contiguous, so the storage is one flat run of numel
+    elements and an element-wise kernel may walk it in memory order."""
+    expect = 1
+    for stride, n in sorted((s, n) for s, n in zip(t.stride(), t.shape) if n != 1):
+        if stride != expect:
+            return False
+        expect *= n
+    return True
+
+
 def _same_dense_layout(ts: Sequence[Optional[Tensor]]) -> bool:
     ref = next(t for t in ts if t is not None)
     for t in ts:
@@ -20,8 +31,7 @@ def _same_dense_layout(ts: Sequence[Optional[Tensor]]) -> bool:
             continue
         if t.shape != ref.shape or effective_strides(t) != effective_strides(ref):
             return False
-    return ref.is_contiguous() or (ref.ndim == 4 and ref.is_contiguous(memory_format=torch.channels_last)) or \
-        ref.is_non_overlapping_and_dense()
+    return _dense(ref)
 
 
 class TensorTable:
@@ -36,6 +46,7 @@ class TensorTable:
         self.num_chunks = 0
         self.num_tensors = 0
         self.scratch: Optional[Tensor] = None
+        self.held = None
 
     def update(self, params: List[Tensor], grads: Optional[List[Tensor]], ms: Optional[List[Tensor]],
                vs: Optional[List[Tensor]], vmaxs: Optional[List[Tensor]], auxs: Optional[List[Tensor]],
@@ -45,6 +56,10 @@ class TensorTable:
         ``ext`` (a third full-size state tensor: Adan's ``exp_avg_delta``, AdEMAMix's ``exp_avg_slow``)."""
         none = [None] * len(params)
         cols = [params, grads or none, ms or none, vs or none, vmaxs or none, auxs or none, exts or none]
+        # the kernels read these through raw pointers: a gradient copied into the parameter's layout for this call only
+        # must stay allocated until the next call, or the caller's next allocation (AdamP's scratch, a device step counter)
+        # lands in its memory before the launch has read it
+        self.held = cols
         key = tuple(0 if t is None else t.data_ptr() for col in cols for t in col)
         if key == self.key:
             return
@@ -71,6 +86,14 @@ class TensorTable:
         self.num_tensors = len(params)
         self.scratch = torch.zeros(2 * max(1, len(params)), device=dev, dtype=torch.float64)
         self.key = key
+
+
+def table_key(gi: int, step: int, by_step) -> tuple:
+    """Key of the table (and device step counter) of the parameters of group ``gi`` that sit at ``step``. Parameters of one
+    group at different step counts (a parameter whose gradient appeared later) are keyed by their distance from the group's
+    lowest count, which stays the same from call to call; keyed by the count itself the caches would grow by one entry
+    per call."""
+    return (gi, step - min(by_step) if len(by_step) > 1 else -1)
 
 
 def bump_versions(params: Sequence[Tensor]) -> None:

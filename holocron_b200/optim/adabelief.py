@@ -7,7 +7,7 @@ from torch import Tensor
 from torch.optim import Adam
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions, effective_strides
+from ._multi_tensor import TensorTable, bump_versions, table_key, effective_strides
 
 __all__ = ["AdaBelief", "adabelief"]
 
@@ -92,14 +92,14 @@ class AdaBelief(Adam):
                 by_step.setdefault(state["step"], []).append(p)
             beta1, beta2 = group["betas"]
             for step, plist in by_step.items():
-                table = self._tables.setdefault((gi, step if len(by_step) > 1 else -1), TensorTable())
+                table = self._tables.setdefault(table_key(gi, step, by_step), TensorTable())
                 grads = [_as_layout(p.grad, p) for p in plist]
                 table.update([p.data for p in plist], grads, [self.state[p]["exp_avg"] for p in plist],
                              [self.state[p]["exp_avg_sq"] for p in plist],
                              [self.state[p]["max_exp_avg_sq"] for p in plist] if group["amsgrad"] else None, None)
                 step_dev = None
                 if group.get("capturable"):
-                    key = (gi, step if len(by_step) > 1 else -1)
+                    key = table_key(gi, step, by_step)
                     step_dev = self._step_dev.get(key)
                     if step_dev is None:
                         step_dev = torch.full((1,), step - 1, device=plist[0].device, dtype=torch.int32)

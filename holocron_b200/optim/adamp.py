@@ -8,7 +8,7 @@ from torch import Tensor
 from torch.optim import Adam
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions
+from ._multi_tensor import TensorTable, bump_versions, table_key
 from .adabelief import _as_layout
 
 __all__ = ["AdamP", "adamp"]
@@ -75,7 +75,7 @@ class AdamP(Adam):
                 by_step.setdefault(state["step"], []).append(p)
             beta1, beta2 = group["betas"]
             for step, plist in by_step.items():
-                key = (gi, step if len(by_step) > 1 else -1)
+                key = table_key(gi, step, by_step)
                 table = self._tables.setdefault(key, TensorTable())
                 table.update([p.data for p in plist], [_as_layout(p.grad, p) for p in plist],
                              [self.state[p]["exp_avg"] for p in plist], [self.state[p]["exp_avg_sq"] for p in plist],

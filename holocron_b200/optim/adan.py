@@ -7,7 +7,7 @@ from torch import Tensor
 from torch.optim import Adam
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions
+from ._multi_tensor import TensorTable, bump_versions, table_key
 from .adabelief import _as_layout
 
 __all__ = ["Adan", "adan"]
@@ -71,7 +71,7 @@ class Adan(Adam):
                 by_step.setdefault(state["step"], []).append(p)
             beta1, beta2, beta3 = group["betas"]
             for step, plist in by_step.items():
-                key = (gi, step if len(by_step) > 1 else -1)
+                key = table_key(gi, step, by_step)
                 table = self._tables.setdefault(key, TensorTable())
                 st = [self.state[p] for p in plist]
                 table.update([p.data for p in plist], [_as_layout(p.grad, p) for p in plist], [s["exp_avg"] for s in st],

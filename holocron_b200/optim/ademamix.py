@@ -7,7 +7,7 @@ from torch import Tensor
 from torch.optim import Optimizer
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions
+from ._multi_tensor import TensorTable, bump_versions, table_key
 from .adabelief import _as_layout
 
 __all__ = ["AdEMAMix", "ademamix"]
@@ -69,7 +69,7 @@ class AdEMAMix(Optimizer):
                 by_step.setdefault(state["step"], []).append(p)
             beta1, beta2, beta3 = group["betas"]
             for step, plist in by_step.items():
-                table = self._tables.setdefault((gi, step if len(by_step) > 1 else -1), TensorTable())
+                table = self._tables.setdefault(table_key(gi, step, by_step), TensorTable())
                 st = [self.state[p] for p in plist]
                 table.update([p.data for p in plist], [_as_layout(p.grad, p) for p in plist], [s["exp_avg"] for s in st],
                              [s["exp_avg_sq"] for s in st], None, None, [s["exp_avg_slow"] for s in st])

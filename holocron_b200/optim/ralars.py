@@ -7,7 +7,7 @@ import torch
 from torch.optim import Optimizer
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions
+from ._multi_tensor import TensorTable, bump_versions, table_key
 from .adabelief import _as_layout
 
 __all__ = ["RaLars"]
@@ -80,7 +80,7 @@ class RaLars(Optimizer):
                     r_t = math.sqrt((sma_t - 4) * (sma_t - 2) * sma_inf / ((sma_inf - 4) * (sma_inf - 2) * sma_t))
                 else:
                     mode, r_t = (1 if self.force_adaptive_momentum else 2), 1.0
-                table = self._tables.setdefault((gi, step if len(by_step) > 1 else -1), TensorTable())
+                table = self._tables.setdefault(table_key(gi, step, by_step), TensorTable())
                 st = [self.state[p] for p in plist]
                 table.update([p.data for p in plist], [_as_layout(p.grad, p) for p in plist], [s["exp_avg"] for s in st],
                              [s["exp_avg_sq"] for s in st], None, [s["local_lr"] for s in st])

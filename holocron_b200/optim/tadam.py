@@ -7,7 +7,7 @@ from torch import Tensor
 from torch.optim import Optimizer
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions
+from ._multi_tensor import TensorTable, bump_versions, table_key
 from .adabelief import _as_layout
 
 __all__ = ["TAdam", "tadam"]
@@ -76,7 +76,7 @@ class TAdam(Optimizer):
                 state["step"] += 1
                 by_step.setdefault(state["step"], []).append(p)
             for step, plist in by_step.items():
-                table = self._tables.setdefault((gi, step if len(by_step) > 1 else -1), TensorTable())
+                table = self._tables.setdefault(table_key(gi, step, by_step), TensorTable())
                 table.update([p.data for p in plist], [_as_layout(p.grad, p) for p in plist],
                              [self.state[p]["exp_avg"] for p in plist], [self.state[p]["exp_avg_sq"] for p in plist],
                              [self.state[p]["max_exp_avg_sq"] for p in plist] if group["amsgrad"] else None,
