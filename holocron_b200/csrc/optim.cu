@@ -5,7 +5,7 @@
 // RaLars and AdamP, host synchronisations per tensor). Here a device-resident table describes every tensor of a parameter
 // group (pointers + numel) and a chunk list maps each CTA to a 4096-element slice of one tensor, so a whole group is
 // updated by a fixed number of launches that are 128-bit-vectorised HBM streams (AdaBelief: 28 B/param algorithmic traffic),
-// with a scalar path for a tensor any of whose pointers is not 16-byte aligned:
+// with a scalar path for a tensor any of whose pointers the launch reads or writes is not 16-byte aligned:
 //
 //   family      launches                                     per-tensor reduction (scratch doubles)   control block
 //   AdaBelief   1                                            -                                         read
@@ -26,6 +26,9 @@
 // at fp32 precision). "Control block": the kernel takes the learning rate (and beta1 when >= 0) from the device block of a
 // captured training step and does nothing while its skip flag is set (apply_ctl below); the step counter of the families
 // that keep one on the device (AdaBelief, AdamP, Adan) does not advance either.
+//
+// Every kernel is a prologue (control block, table lookup, bias corrections), a list of streams, one element function that
+// for_chunk calls on the values of each element, and for the reducing passes chunk_sums.
 #include "common.cuh"
 
 namespace {
@@ -84,38 +87,67 @@ __device__ __forceinline__ void bias_corrections(const Hyper& h, float& bc1, flo
   }
 }
 
-// Generic chunk walker: calls f(i) for each element index of this CTA's chunk, 4 at a time when aligned.
-template <typename F4, typename F1>
-__device__ __forceinline__ void for_chunk(const TensorMeta& t, int chunk, bool vec_ok, F4 f4, F1 f1) {
+// One tensor the element function sees: each element's value is read from `in` (0 when null) and, after the function
+// has run, written to `out` (not at all when null). `v` holds the values in flight, one per lane on the vector path.
+struct Stream {
+  const float* in;
+  float* out;
+  float4 v;
+
+  __device__ __forceinline__ bool vec_ok() const { return aligned16(in) && aligned16(out); }
+  __device__ __forceinline__ void load4(long long i) {
+    v = in ? *reinterpret_cast<const float4*>(in + i) : make_float4(0.f, 0.f, 0.f, 0.f);
+  }
+  __device__ __forceinline__ void store4(long long i) const { if (out) *reinterpret_cast<float4*>(out + i) = v; }
+  __device__ __forceinline__ void load1(long long i) { v.x = in ? in[i] : 0.f; }
+  __device__ __forceinline__ void store1(long long i) const { if (out) out[i] = v.x; }
+};
+
+__device__ __forceinline__ Stream rd(const float* t) { return {t, nullptr}; }
+__device__ __forceinline__ Stream rw(float* t) { return {t, t}; }
+
+// Chunk walker: calls f with one float& per stream, in the order the streams are given, for each element of this CTA's
+// chunk. Four elements at a time (lanes x, y, z, w in that order) when every non-null pointer of the streams is 16-byte
+// aligned, one at a time otherwise and for the tail.
+template <typename F, typename... S>
+__device__ __forceinline__ void for_chunk(long long numel, int chunk, F f, S... s) {
   const long long base = (long long)chunk * kChunk;
-  const long long end = min(base + (long long)kChunk, t.numel);
-  if (vec_ok) {
+  const long long end = min(base + (long long)kChunk, numel);
+  long long i = base + threadIdx.x;
+  if ((s.vec_ok() && ...)) {
     const long long end4 = base + ((end - base) & ~3LL);
-    for (long long i = base + threadIdx.x * 4; i < end4; i += kThreads * 4) f4(i);
-    for (long long i = end4 + threadIdx.x; i < end; i += kThreads) f1(i);
-  } else {
-    for (long long i = base + threadIdx.x; i < end; i += kThreads) f1(i);
+    for (long long j = base + threadIdx.x * 4; j < end4; j += kThreads * 4) {
+      (s.load4(j), ...);
+      f(s.v.x...);
+      f(s.v.y...);
+      f(s.v.z...);
+      f(s.v.w...);
+      (s.store4(j), ...);
+    }
+    i = end4 + threadIdx.x;
+  }
+  for (; i < end; i += kThreads) {
+    (s.load1(i), ...);
+    f(s.v.x...);
+    (s.store1(i), ...);
   }
 }
 
-__device__ __forceinline__ bool meta_vec_ok(const TensorMeta& t) {
-  return aligned16(t.p) && aligned16(t.g) && aligned16(t.m) && aligned16(t.v) && (t.vmax == nullptr || aligned16(t.vmax));
+// Per-tensor sums of this CTA: K block reductions in fp64, then thread 0 adds them into row[0..K) with fp64 atomics.
+template <int K>
+__device__ __forceinline__ void chunk_sums(const float (&acc)[K], double* row) {
+  __shared__ double red[32];
+  double tot[K];
+#pragma unroll
+  for (int k = 0; k < K; ++k) tot[k] = block_sum<double>((double)acc[k], red);
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int k = 0; k < K; ++k) atomicAdd(&row[k], tot[k]);
+  }
 }
 
 // ---------------------------------------------------------------------------------------------------
 // AdaBelief  (reference adabelief.py:121-167; NB no +eps inside the belief EMA)
-__device__ __forceinline__ void adabelief_elem(float& p, float g, float& m, float& s, float* smax, const Hyper& h,
-                                               float step_size, float inv_sqrt_bc2) {
-  if (h.wd != 0.f) g = fmaf(h.wd, p, g);
-  m = fmaf(1.f - h.beta1, g, h.beta1 * m);
-  const float r = g - m;
-  s = fmaf(1.f - h.beta2, r * r, h.beta2 * s);
-  float sec = s;
-  if (smax) { *smax = fmaxf(*smax, s); sec = *smax; }
-  const float denom = sqrtf(sec) * inv_sqrt_bc2 + h.eps;
-  p = p - step_size * (m / denom);
-}
-
 __global__ void __launch_bounds__(kThreads) adabelief_kernel(const TensorMeta* __restrict__ metas,
                                                              const int2* __restrict__ chunks, Hyper h) {
   if (!apply_ctl(h)) return;
@@ -126,29 +158,17 @@ __global__ void __launch_bounds__(kThreads) adabelief_kernel(const TensorMeta* _
   const float step_size = h.lr / bc1;
   const float inv_sqrt_bc2 = 1.f / sqrtf(bc2);
   const bool ams = h.amsgrad && t.vmax;
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 m = *reinterpret_cast<float4*>(t.m + i);
-        float4 s = *reinterpret_cast<float4*>(t.v + i);
-        float4 x = ams ? *reinterpret_cast<float4*>(t.vmax + i) : make_float4(0, 0, 0, 0);
-        adabelief_elem(p.x, g.x, m.x, s.x, ams ? &x.x : nullptr, h, step_size, inv_sqrt_bc2);
-        adabelief_elem(p.y, g.y, m.y, s.y, ams ? &x.y : nullptr, h, step_size, inv_sqrt_bc2);
-        adabelief_elem(p.z, g.z, m.z, s.z, ams ? &x.z : nullptr, h, step_size, inv_sqrt_bc2);
-        adabelief_elem(p.w, g.w, m.w, s.w, ams ? &x.w : nullptr, h, step_size, inv_sqrt_bc2);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-        *reinterpret_cast<float4*>(t.m + i) = m;
-        *reinterpret_cast<float4*>(t.v + i) = s;
-        if (ams) *reinterpret_cast<float4*>(t.vmax + i) = x;
-      },
-      [&](long long i) {
-        float p = t.p[i], m = t.m[i], s = t.v[i];
-        float x = ams ? t.vmax[i] : 0.f;
-        adabelief_elem(p, t.g[i], m, s, ams ? &x : nullptr, h, step_size, inv_sqrt_bc2);
-        t.p[i] = p; t.m[i] = m; t.v[i] = s;
-        if (ams) t.vmax[i] = x;
-      });
+  auto one = [&](float& p, float g, float& m, float& s, float& x) {
+    if (h.wd != 0.f) g = fmaf(h.wd, p, g);
+    m = fmaf(1.f - h.beta1, g, h.beta1 * m);
+    const float r = g - m;
+    s = fmaf(1.f - h.beta2, r * r, h.beta2 * s);
+    float sec = s;
+    if (ams) { x = fmaxf(x, s); sec = x; }
+    const float denom = sqrtf(sec) * inv_sqrt_bc2 + h.eps;
+    p = p - step_size * (m / denom);
+  };
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.g), rw(t.m), rw(t.v), rw(ams ? t.vmax : nullptr));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -157,7 +177,6 @@ __global__ void __launch_bounds__(kThreads) adabelief_kernel(const TensorMeta* _
 __global__ void __launch_bounds__(kThreads) lamb_moments_kernel(const TensorMeta* __restrict__ metas,
                                                                 const int2* __restrict__ chunks, Hyper h,
                                                                 double* __restrict__ norms /*[T][2]*/) {
-  __shared__ double red[32];
   const int2 c = chunks[blockIdx.x];
   const TensorMeta t = metas[c.x];
   float pn = 0.f, un = 0.f;   // <= 16 elements per thread: fp32 partials, fp64 from the block reduction on
@@ -169,27 +188,8 @@ __global__ void __launch_bounds__(kThreads) lamb_moments_kernel(const TensorMeta
     pn = fmaf(p, p, pn);
     un = fmaf(u, u, un);
   };
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        const float4 p = *reinterpret_cast<const float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 m = *reinterpret_cast<float4*>(t.m + i);
-        float4 v = *reinterpret_cast<float4*>(t.v + i);
-        one(p.x, g.x, m.x, v.x); one(p.y, g.y, m.y, v.y); one(p.z, g.z, m.z, v.z); one(p.w, g.w, m.w, v.w);
-        *reinterpret_cast<float4*>(t.m + i) = m;
-        *reinterpret_cast<float4*>(t.v + i) = v;
-      },
-      [&](long long i) {
-        float m = t.m[i], v = t.v[i];
-        one(t.p[i], t.g[i], m, v);
-        t.m[i] = m; t.v[i] = v;
-      });
-  const double pd = block_sum<double>((double)pn, red);
-  const double ud = block_sum<double>((double)un, red);
-  if (threadIdx.x == 0) {
-    atomicAdd(&norms[2 * c.x + 0], pd);
-    atomicAdd(&norms[2 * c.x + 1], ud);
-  }
+  for_chunk(t.numel, c.y, one, rd(t.p), rd(t.g), rw(t.m), rw(t.v));
+  chunk_sums<2>({pn, un}, norms + 2 * c.x);
 }
 
 __global__ void __launch_bounds__(kThreads) lamb_apply_kernel(const TensorMeta* __restrict__ metas,
@@ -203,20 +203,12 @@ __global__ void __launch_bounds__(kThreads) lamb_apply_kernel(const TensorMeta* 
   const float local_lr = (phi == 0.f || u_norm == 0.f) ? 1.f : phi / u_norm;
   if (c.y == 0 && threadIdx.x == 0 && t.aux) *t.aux = local_lr;
   const float a = h.lr * local_lr;
-  auto one = [&](float p, float m, float v) {
+  auto one = [&](float& p, float m, float v) {
     float u = m / (sqrtf(v) + h.eps);
     if (h.wd != 0.f) u = fmaf(h.wd, p, u);
-    return p - a * u;
+    p = p - a * u;
   };
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 m = *reinterpret_cast<const float4*>(t.m + i);
-        const float4 v = *reinterpret_cast<const float4*>(t.v + i);
-        p.x = one(p.x, m.x, v.x); p.y = one(p.y, m.y, v.y); p.z = one(p.z, m.z, v.z); p.w = one(p.w, m.w, v.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-      },
-      [&](long long i) { t.p[i] = one(t.p[i], t.m[i], t.v[i]); });
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.m), rd(t.v));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -232,7 +224,6 @@ __device__ __forceinline__ float adamp_pt(float m, float v, float vmax_or_neg, f
 __global__ void __launch_bounds__(kThreads) adamp_moments_kernel(const TensorMeta* __restrict__ metas,
                                                                  const int2* __restrict__ chunks, Hyper h,
                                                                  double* __restrict__ sums /*[T][4]*/) {
-  __shared__ double red[32];
   if (!apply_ctl(h)) return;
   const int2 c = chunks[blockIdx.x];
   const TensorMeta t = metas[c.x];
@@ -249,30 +240,8 @@ __global__ void __launch_bounds__(kThreads) adamp_moments_kernel(const TensorMet
     const float pt = adamp_pt(m, v, ams ? x : -1.f, bc1, inv_sqrt_bc2, h.eps);
     s_pg = fmaf(p, g, s_pg); s_pp = fmaf(p, p, s_pp); s_gg = fmaf(g, g, s_gg); s_ppt = fmaf(p, pt, s_ppt);
   };
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        const float4 p = *reinterpret_cast<const float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 m = *reinterpret_cast<float4*>(t.m + i);
-        float4 v = *reinterpret_cast<float4*>(t.v + i);
-        float4 x = ams ? *reinterpret_cast<float4*>(t.vmax + i) : make_float4(0, 0, 0, 0);
-        one(p.x, g.x, m.x, v.x, x.x); one(p.y, g.y, m.y, v.y, x.y); one(p.z, g.z, m.z, v.z, x.z); one(p.w, g.w, m.w, v.w, x.w);
-        *reinterpret_cast<float4*>(t.m + i) = m;
-        *reinterpret_cast<float4*>(t.v + i) = v;
-        if (ams) *reinterpret_cast<float4*>(t.vmax + i) = x;
-      },
-      [&](long long i) {
-        float m = t.m[i], v = t.v[i], x = ams ? t.vmax[i] : 0.f;
-        one(t.p[i], t.g[i], m, v, x);
-        t.m[i] = m; t.v[i] = v;
-        if (ams) t.vmax[i] = x;
-      });
-  const double a = block_sum<double>((double)s_pg, red), b = block_sum<double>((double)s_pp, red);
-  const double cc = block_sum<double>((double)s_gg, red), d = block_sum<double>((double)s_ppt, red);
-  if (threadIdx.x == 0) {
-    atomicAdd(&sums[4 * c.x + 0], a); atomicAdd(&sums[4 * c.x + 1], b);
-    atomicAdd(&sums[4 * c.x + 2], cc); atomicAdd(&sums[4 * c.x + 3], d);
-  }
+  for_chunk(t.numel, c.y, one, rd(t.p), rd(t.g), rw(t.m), rw(t.v), rw(ams ? t.vmax : nullptr));
+  chunk_sums<4>({s_pg, s_pp, s_gg, s_ppt}, sums + 4 * c.x);
 }
 
 __global__ void __launch_bounds__(kThreads) adamp_apply_kernel(const TensorMeta* __restrict__ metas,
@@ -291,21 +260,12 @@ __global__ void __launch_bounds__(kThreads) adamp_apply_kernel(const TensorMeta*
   const bool project = cosv < h.delta / sqrtf((float)t.numel);
   const float inv = 1.f / (pn + h.eps);
   const float k = project ? (float)sums[4 * c.x + 3] * inv * inv : 0.f;   // <p_hat, pt> / (||p|| + eps)
-  auto one = [&](float p, float m, float v, float x) {
+  auto one = [&](float& p, float m, float v, float x) {
     float pt = adamp_pt(m, v, ams ? x : -1.f, bc1, inv_sqrt_bc2, h.eps);
     pt = fmaf(-k, p, pt);
-    return fmaf(-h.lr, pt, p);
+    p = fmaf(-h.lr, pt, p);
   };
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 m = *reinterpret_cast<const float4*>(t.m + i);
-        const float4 v = *reinterpret_cast<const float4*>(t.v + i);
-        const float4 x = ams ? *reinterpret_cast<const float4*>(t.vmax + i) : make_float4(0, 0, 0, 0);
-        p.x = one(p.x, m.x, v.x, x.x); p.y = one(p.y, m.y, v.y, x.y); p.z = one(p.z, m.z, v.z, x.z); p.w = one(p.w, m.w, v.w, x.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-      },
-      [&](long long i) { t.p[i] = one(t.p[i], t.m[i], t.v[i], ams ? t.vmax[i] : 0.f); });
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.m), rd(t.v), rd(ams ? t.vmax : nullptr));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -313,7 +273,6 @@ __global__ void __launch_bounds__(kThreads) adamp_apply_kernel(const TensorMeta*
 __global__ void __launch_bounds__(kThreads) tadam_reduce_kernel(const TensorMeta* __restrict__ metas,
                                                                 const int2* __restrict__ chunks, Hyper h,
                                                                 double* __restrict__ sums /*[T]*/) {
-  __shared__ double red[32];
   const int2 c = chunks[blockIdx.x];
   const TensorMeta t = metas[c.x];
   float acc = 0.f;
@@ -322,18 +281,8 @@ __global__ void __launch_bounds__(kThreads) tadam_reduce_kernel(const TensorMeta
     const float d = g - m;
     acc += (d * d) / (v + h.eps);
   };
-  const bool need_p = h.wd != 0.f;
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        const float4 m = *reinterpret_cast<const float4*>(t.m + i);
-        const float4 v = *reinterpret_cast<const float4*>(t.v + i);
-        const float4 p = need_p ? *reinterpret_cast<const float4*>(t.p + i) : make_float4(0, 0, 0, 0);
-        one(p.x, g.x, m.x, v.x); one(p.y, g.y, m.y, v.y); one(p.z, g.z, m.z, v.z); one(p.w, g.w, m.w, v.w);
-      },
-      [&](long long i) { one(need_p ? t.p[i] : 0.f, t.g[i], t.m[i], t.v[i]); });
-  const double tot = block_sum<double>((double)acc, red);
-  if (threadIdx.x == 0) atomicAdd(&sums[c.x], tot);
+  for_chunk(t.numel, c.y, one, rd(h.wd != 0.f ? t.p : nullptr), rd(t.g), rd(t.m), rd(t.v));
+  chunk_sums<1>({acc}, sums + c.x);
 }
 
 __device__ __forceinline__ float tadam_wt(const TensorMeta& t, const Hyper& h, double sum) {
@@ -364,25 +313,7 @@ __global__ void __launch_bounds__(kThreads) tadam_apply_kernel(const TensorMeta*
     const float denom = sqrtf(sec) * inv_sqrt_bc2 + h.eps;
     p = p - step_size * (m / denom);
   };
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 m = *reinterpret_cast<float4*>(t.m + i);
-        float4 v = *reinterpret_cast<float4*>(t.v + i);
-        float4 x = ams ? *reinterpret_cast<float4*>(t.vmax + i) : make_float4(0, 0, 0, 0);
-        one(p.x, g.x, m.x, v.x, x.x); one(p.y, g.y, m.y, v.y, x.y); one(p.z, g.z, m.z, v.z, x.z); one(p.w, g.w, m.w, v.w, x.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-        *reinterpret_cast<float4*>(t.m + i) = m;
-        *reinterpret_cast<float4*>(t.v + i) = v;
-        if (ams) *reinterpret_cast<float4*>(t.vmax + i) = x;
-      },
-      [&](long long i) {
-        float p = t.p[i], m = t.m[i], v = t.v[i], x = ams ? t.vmax[i] : 0.f;
-        one(p, t.g[i], m, v, x);
-        t.p[i] = p; t.m[i] = m; t.v[i] = v;
-        if (ams) t.vmax[i] = x;
-      });
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.g), rw(t.m), rw(t.v), rw(ams ? t.vmax : nullptr));
 }
 
 // W_t <- W_t * (2 beta1 - 1) / beta1 + w_t   (after every CTA of the apply pass has read the old W_t)
@@ -425,30 +356,7 @@ __global__ void __launch_bounds__(kThreads) adan_kernel(const TensorMeta* __rest
     p = fmaf(-h.lr, pt, p);
     if (h.wd != 0.f) p = p / shrink;
   };
-  const bool vec = meta_vec_ok(t) && aligned16(t.aux) && aligned16(t.ext);
-  for_chunk(t, c.y, vec,
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        const float4 pg = *reinterpret_cast<const float4*>(t.aux + i);
-        float4 m = *reinterpret_cast<float4*>(t.m + i);
-        float4 v = *reinterpret_cast<float4*>(t.v + i);
-        float4 n = *reinterpret_cast<float4*>(t.ext + i);
-        float4 x = ams ? *reinterpret_cast<float4*>(t.vmax + i) : make_float4(0, 0, 0, 0);
-        one(p.x, g.x, pg.x, m.x, v.x, n.x, x.x); one(p.y, g.y, pg.y, m.y, v.y, n.y, x.y);
-        one(p.z, g.z, pg.z, m.z, v.z, n.z, x.z); one(p.w, g.w, pg.w, m.w, v.w, n.w, x.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-        *reinterpret_cast<float4*>(t.m + i) = m;
-        *reinterpret_cast<float4*>(t.v + i) = v;
-        *reinterpret_cast<float4*>(t.ext + i) = n;
-        if (ams) *reinterpret_cast<float4*>(t.vmax + i) = x;
-      },
-      [&](long long i) {
-        float p = t.p[i], m = t.m[i], v = t.v[i], n = t.ext[i], x = ams ? t.vmax[i] : 0.f;
-        one(p, t.g[i], t.aux[i], m, v, n, x);
-        t.p[i] = p; t.m[i] = m; t.v[i] = v; t.ext[i] = n;
-        if (ams) t.vmax[i] = x;
-      });
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.g), rd(t.aux), rw(t.m), rw(t.v), rw(t.ext), rw(ams ? t.vmax : nullptr));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -470,63 +378,24 @@ __global__ void __launch_bounds__(kThreads) ademamix_kernel(const TensorMeta* __
     const float denom = sqrtf(nu) * inv_sqrt_bc2 + h.eps;
     p = fmaf(-h.lr, fmaf(h.alpha, m2, m1 / bc1) / denom, p);
   };
-  const bool vec = meta_vec_ok(t) && aligned16(t.ext);
-  for_chunk(t, c.y, vec,
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 m1 = *reinterpret_cast<float4*>(t.m + i);
-        float4 m2 = *reinterpret_cast<float4*>(t.ext + i);
-        float4 nu = *reinterpret_cast<float4*>(t.v + i);
-        one(p.x, g.x, m1.x, m2.x, nu.x); one(p.y, g.y, m1.y, m2.y, nu.y);
-        one(p.z, g.z, m1.z, m2.z, nu.z); one(p.w, g.w, m1.w, m2.w, nu.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-        *reinterpret_cast<float4*>(t.m + i) = m1;
-        *reinterpret_cast<float4*>(t.ext + i) = m2;
-        *reinterpret_cast<float4*>(t.v + i) = nu;
-      },
-      [&](long long i) {
-        float p = t.p[i], m1 = t.m[i], m2 = t.ext[i], nu = t.v[i];
-        one(p, t.g[i], m1, m2, nu);
-        t.p[i] = p; t.m[i] = m1; t.ext[i] = m2; t.v[i] = nu;
-      });
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.g), rw(t.m), rw(t.ext), rw(t.v));
 }
 
 // ---------------------------------------------------------------------------------------------------
-// Per-tensor sums of squares of two streams (fp64 atomics per CTA): norms[2t] += sum a^2, norms[2t+1] += sum b^2
-template <typename FA, typename FB>
-__device__ __forceinline__ void two_norms(const TensorMeta& t, int chunk, bool vec, FA a_at4, FB b_at4, double* norms, int ti,
-                                          double* red) {
-  float an = 0.f, bn = 0.f;
-  for_chunk(t, chunk, vec,
-      [&](long long i) {
-        const float4 a = a_at4(i, true), b = b_at4(i, true);
-        an = fmaf(a.x, a.x, fmaf(a.y, a.y, fmaf(a.z, a.z, fmaf(a.w, a.w, an))));
-        bn = fmaf(b.x, b.x, fmaf(b.y, b.y, fmaf(b.z, b.z, fmaf(b.w, b.w, bn))));
-      },
-      [&](long long i) {
-        const float4 a = a_at4(i, false), b = b_at4(i, false);
-        an = fmaf(a.x, a.x, an);
-        bn = fmaf(b.x, b.x, bn);
-      });
-  const double ad = block_sum<double>((double)an, red);
-  const double bd = block_sum<double>((double)bn, red);
-  if (threadIdx.x == 0) { atomicAdd(&norms[2 * ti], ad); atomicAdd(&norms[2 * ti + 1], bd); }
-}
-
 // LARS (reference lars.py:91-135): local_lr = ||p|| / (||g|| + wd ||p||) (1 when either is 0; `scale_clip` is stored but never
 // applied by the reference); d_p = g + wd * p is written back INTO THE GRADIENT like the reference's in-place add_;
 // SGD momentum with dampening / Nesterov, the first buffer being a copy of d_p. m = momentum_buffer (may be null).
 __global__ void __launch_bounds__(kThreads) lars_norms_kernel(const TensorMeta* __restrict__ metas,
                                                               const int2* __restrict__ chunks, double* __restrict__ norms) {
-  __shared__ double red[32];
   const int2 c = chunks[blockIdx.x];
   const TensorMeta t = metas[c.x];
-  const bool vec = aligned16(t.p) && aligned16(t.g);
-  two_norms(t, c.y, vec,
-      [&](long long i, bool v4) { return v4 ? *reinterpret_cast<const float4*>(t.p + i) : make_float4(t.p[i], 0, 0, 0); },
-      [&](long long i, bool v4) { return v4 ? *reinterpret_cast<const float4*>(t.g + i) : make_float4(t.g[i], 0, 0, 0); },
-      norms, c.x, red);
+  float pn = 0.f, gn = 0.f;
+  auto one = [&](float p, float g) {
+    pn = fmaf(p, p, pn);
+    gn = fmaf(g, g, gn);
+  };
+  for_chunk(t.numel, c.y, one, rd(t.p), rd(t.g));
+  chunk_sums<2>({pn, gn}, norms + 2 * c.x);
 }
 
 __global__ void __launch_bounds__(kThreads) lars_apply_kernel(const TensorMeta* __restrict__ metas,
@@ -539,7 +408,6 @@ __global__ void __launch_bounds__(kThreads) lars_apply_kernel(const TensorMeta* 
   if (h.wd != 0.f) denom = fmaf(h.wd, p_norm, denom);
   const float local_lr = (p_norm == 0.f || denom == 0.f) ? 1.f : p_norm / denom;
   const float a = h.lr * local_lr;
-  float* gw = const_cast<float*>(t.g);
   const bool mom = h.momentum != 0.f && t.m != nullptr;
   auto one = [&](float& p, float& g, float& b) {
     if (h.wd != 0.f) g = fmaf(h.wd, p, g);
@@ -550,24 +418,9 @@ __global__ void __launch_bounds__(kThreads) lars_apply_kernel(const TensorMeta* 
     }
     p = fmaf(-a, d, p);
   };
-  const bool vec = aligned16(t.p) && aligned16(t.g) && (!mom || aligned16(t.m));
-  for_chunk(t, c.y, vec,
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 b = (mom && !h.first) ? *reinterpret_cast<float4*>(t.m + i) : make_float4(0, 0, 0, 0);
-        one(p.x, g.x, b.x); one(p.y, g.y, b.y); one(p.z, g.z, b.z); one(p.w, g.w, b.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-        if (h.wd != 0.f) *reinterpret_cast<float4*>(gw + i) = g;
-        if (mom) *reinterpret_cast<float4*>(t.m + i) = b;
-      },
-      [&](long long i) {
-        float p = t.p[i], g = t.g[i], b = (mom && !h.first) ? t.m[i] : 0.f;
-        one(p, g, b);
-        t.p[i] = p;
-        if (h.wd != 0.f) gw[i] = g;
-        if (mom) t.m[i] = b;
-      });
+  const Stream grad{t.g, h.wd != 0.f ? const_cast<float*>(t.g) : nullptr};
+  const Stream buf{mom && !h.first ? t.m : nullptr, mom ? t.m : nullptr};
+  for_chunk(t.numel, c.y, one, rw(t.p), grad, buf);
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -581,10 +434,10 @@ __device__ __forceinline__ float ralars_update(float p, float m, float v, const 
   return u;
 }
 
-__global__ void __launch_bounds__(kThreads) ralars_moments_kernel(const TensorMeta* __restrict__ metas,
-                                                                  const int2* __restrict__ chunks, Hyper h,
-                                                                  double* __restrict__ norms) {
-  __shared__ double red[32];
+// 6 CTAs per SM (<= 40 registers): left to itself ptxas takes 46 (nvcc 12.9), which leaves room for 5
+__global__ void __launch_bounds__(kThreads, 6) ralars_moments_kernel(const TensorMeta* __restrict__ metas,
+                                                                     const int2* __restrict__ chunks, Hyper h,
+                                                                     double* __restrict__ norms) {
   const int2 c = chunks[blockIdx.x];
   const TensorMeta t = metas[c.x];
   float pn = 0.f, un = 0.f;
@@ -595,24 +448,8 @@ __global__ void __launch_bounds__(kThreads) ralars_moments_kernel(const TensorMe
     pn = fmaf(p, p, pn);
     un = fmaf(u, u, un);
   };
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        const float4 p = *reinterpret_cast<const float4*>(t.p + i);
-        const float4 g = *reinterpret_cast<const float4*>(t.g + i);
-        float4 m = *reinterpret_cast<float4*>(t.m + i);
-        float4 v = *reinterpret_cast<float4*>(t.v + i);
-        one(p.x, g.x, m.x, v.x); one(p.y, g.y, m.y, v.y); one(p.z, g.z, m.z, v.z); one(p.w, g.w, m.w, v.w);
-        *reinterpret_cast<float4*>(t.m + i) = m;
-        *reinterpret_cast<float4*>(t.v + i) = v;
-      },
-      [&](long long i) {
-        float m = t.m[i], v = t.v[i];
-        one(t.p[i], t.g[i], m, v);
-        t.m[i] = m; t.v[i] = v;
-      });
-  const double pd = block_sum<double>((double)pn, red);
-  const double ud = block_sum<double>((double)un, red);
-  if (threadIdx.x == 0) { atomicAdd(&norms[2 * c.x + 0], pd); atomicAdd(&norms[2 * c.x + 1], ud); }
+  for_chunk(t.numel, c.y, one, rd(t.p), rd(t.g), rw(t.m), rw(t.v));
+  chunk_sums<2>({pn, un}, norms + 2 * c.x);
 }
 
 __global__ void __launch_bounds__(kThreads) ralars_apply_kernel(const TensorMeta* __restrict__ metas,
@@ -626,18 +463,8 @@ __global__ void __launch_bounds__(kThreads) ralars_apply_kernel(const TensorMeta
   const float local_lr = (phi == 0.f || u_norm == 0.f) ? 1.f : phi / u_norm;
   if (c.y == 0 && threadIdx.x == 0 && t.aux) *t.aux = local_lr;
   const float a = h.lr * local_lr;
-  for_chunk(t, c.y, meta_vec_ok(t),
-      [&](long long i) {
-        float4 p = *reinterpret_cast<float4*>(t.p + i);
-        const float4 m = *reinterpret_cast<const float4*>(t.m + i);
-        const float4 v = *reinterpret_cast<const float4*>(t.v + i);
-        p.x = fmaf(-a, ralars_update(p.x, m.x, v.x, h, h.bc1, h.bc2), p.x);
-        p.y = fmaf(-a, ralars_update(p.y, m.y, v.y, h, h.bc1, h.bc2), p.y);
-        p.z = fmaf(-a, ralars_update(p.z, m.z, v.z, h, h.bc1, h.bc2), p.z);
-        p.w = fmaf(-a, ralars_update(p.w, m.w, v.w, h, h.bc1, h.bc2), p.w);
-        *reinterpret_cast<float4*>(t.p + i) = p;
-      },
-      [&](long long i) { t.p[i] = fmaf(-a, ralars_update(t.p[i], t.m[i], t.v[i], h, h.bc1, h.bc2), t.p[i]); });
+  auto one = [&](float& p, float m, float v) { p = fmaf(-a, ralars_update(p, m, v, h, h.bc1, h.bc2), p); };
+  for_chunk(t.numel, c.y, one, rw(t.p), rd(t.m), rd(t.v));
 }
 
 // ---------------------------------------------------------------------------------------------------
@@ -647,19 +474,11 @@ __global__ void __launch_bounds__(kThreads) lookahead_sync_kernel(const TensorMe
                                                                   const int2* __restrict__ chunks, float rate) {
   const int2 c = chunks[blockIdx.x];
   const TensorMeta t = metas[c.x];
-  auto one = [&](float f, float s) { return rate > 0.f ? fmaf(rate, f - s, s) : s; };
-  for_chunk(t, c.y, aligned16(t.p) && aligned16(t.m),
-      [&](long long i) {
-        const float4 f = *reinterpret_cast<const float4*>(t.p + i);
-        float4 s = *reinterpret_cast<float4*>(t.m + i);
-        s.x = one(f.x, s.x); s.y = one(f.y, s.y); s.z = one(f.z, s.z); s.w = one(f.w, s.w);
-        *reinterpret_cast<float4*>(t.m + i) = s;
-        *reinterpret_cast<float4*>(t.p + i) = s;
-      },
-      [&](long long i) {
-        const float s = one(t.p[i], t.m[i]);
-        t.m[i] = s; t.p[i] = s;
-      });
+  auto one = [&](float& f, float& s) {
+    s = rate > 0.f ? fmaf(rate, f - s, s) : s;
+    f = s;
+  };
+  for_chunk(t.numel, c.y, one, rw(t.p), rw(t.m));
 }
 
 __global__ void step_increment_kernel(int* step, const int* ctl) { if (!ctl || ctl[2] == 0) *step += 1; }

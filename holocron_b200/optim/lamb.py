@@ -6,8 +6,7 @@ import torch
 from torch.optim import Optimizer
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions
-from .adabelief import _as_layout
+from ._multi_tensor import TensorTable, as_layout, bump_versions, collect_step, device_local_lr
 
 __all__ = ["LAMB"]
 
@@ -46,27 +45,14 @@ class LAMB(Optimizer):
             with torch.enable_grad():
                 loss = closure()
         for gi, group in enumerate(self.param_groups):
-            plist = []
-            for p in group["params"]:
-                if p.grad is None:
-                    continue
-                if p.grad.is_sparse:
-                    raise RuntimeError(f"{self.__class__.__name__} does not support sparse gradients")
-                state = self.state[p]
-                if len(state) == 0:
-                    state["step"] = 0
-                    state["exp_avg"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)
-                    state["exp_avg_sq"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)
-                if not isinstance(state.get("local_lr"), torch.Tensor):
-                    state["local_lr"] = torch.ones((), device=p.device, dtype=torch.float32)
-                state["step"] += 1
-                plist.append(p)
+            plist = collect_step(self, group)
             if not plist:
                 continue
+            states = [self.state[p] for p in plist]
+            device_local_lr(states)
             table = self._tables.setdefault(gi, TensorTable())
-            table.update([p.data for p in plist], [_as_layout(p.grad, p) for p in plist],
-                         [self.state[p]["exp_avg"] for p in plist], [self.state[p]["exp_avg_sq"] for p in plist], None,
-                         [self.state[p]["local_lr"] for p in plist])
+            table.update([p.data for p in plist], [as_layout(p.grad, p) for p in plist], ms=[s["exp_avg"] for s in states],
+                         vs=[s["exp_avg_sq"] for s in states], auxs=[s["local_lr"] for s in states])
             beta1, beta2 = group["betas"]
             check(lib().hb_lamb_step(ptr(table.metas), ptr(table.chunks), table.num_chunks, table.num_tensors,
                                      _cf(group["lr"]), _cf(beta1), _cf(beta2), _cf(group["eps"]),
@@ -74,3 +60,7 @@ class LAMB(Optimizer):
                                      ptr(table.scratch), stream_ptr()), "hb_lamb_step")
             bump_versions(plist)
         return loss
+
+    def _init_state(self, p: torch.Tensor, state: dict, group: dict) -> None:
+        state["exp_avg"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)
+        state["exp_avg_sq"] = torch.zeros_like(p.data, memory_format=torch.preserve_format)

@@ -6,7 +6,7 @@ import torch
 from torch.optim import Optimizer
 
 from .._lib import check, lib, ptr, stream_ptr
-from ._multi_tensor import TensorTable, bump_versions, effective_strides
+from ._multi_tensor import TensorTable, as_layout, bump_versions
 
 __all__ = ["LARS"]
 
@@ -55,14 +55,10 @@ class LARS(Optimizer):
             for p in group["params"]:
                 if p.grad is None:
                     continue
-                g = p.grad
-                if g.is_sparse:
+                if p.grad.is_sparse:
                     raise RuntimeError(f"{self.__class__.__name__} does not support sparse gradients")
-                if g.dtype != torch.float32 or g.shape != p.shape or effective_strides(g) != effective_strides(p):
-                    # the kernel updates the gradient in place (weight decay): give it the parameter's layout for good
-                    fixed = torch.empty_like(p)
-                    fixed.copy_(g)
-                    p.grad = g = fixed
+                # the kernel updates the gradient in place (weight decay): give it the parameter's layout for good
+                p.grad = as_layout(p.grad, p)
                 if momentum != 0 and "momentum_buffer" not in self.state[p]:
                     self.state[p]["momentum_buffer"] = torch.empty_like(p, memory_format=torch.preserve_format)
                     fresh.append(p)
@@ -73,7 +69,7 @@ class LARS(Optimizer):
                     continue
                 table = self._tables.setdefault((gi, first), TensorTable())
                 table.update([p.data for p in plist], [p.grad for p in plist],
-                             [self.state[p]["momentum_buffer"] for p in plist] if momentum != 0 else None, None, None, None)
+                             ms=[self.state[p]["momentum_buffer"] for p in plist] if momentum != 0 else None)
                 check(lib().hb_lars_step(ptr(table.metas), ptr(table.chunks), table.num_chunks, table.num_tensors,
                                          _cf(group["lr"]), _cf(momentum), _cf(group["dampening"]), _cf(group["weight_decay"]),
                                          int(bool(group["nesterov"])), first, ptr(table.scratch), stream_ptr()), "hb_lars_step")

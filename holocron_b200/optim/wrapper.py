@@ -94,7 +94,7 @@ class Lookahead(Optimizer):
             if not fast:
                 continue
             table = self._tables.setdefault(gi, TensorTable())
-            table.update(fast, None, [p.data for p in slow_group["params"]], None, None, None)
+            table.update(fast, None, ms=[p.data for p in slow_group["params"]])
             check(lib().hb_lookahead_sync(ptr(table.metas), ptr(table.chunks), table.num_chunks, ctypes.c_float(sync_rate),
                                           stream_ptr()), "hb_lookahead_sync")
             bump_versions(fast_group["params"])
