@@ -272,11 +272,13 @@ __device__ __forceinline__ float exp_mufu(float x) {
   return y;
 }
 
-// exp(x - m) for x <= m as ex2(x * log2e - m * log2e): one FFMA + one MUFU (ml = m * log2e is per position)
+// exp(x - m) for x <= m as ex2((x - m) * log2e): x - m is exact wherever the term matters (Sterbenz), so the argument's
+// error scales with |x - m| as in expf(x - m). Folding m into an FFMA, ex2(x * log2e - m * log2e), saves one instruction
+// but rounds m * log2e, an error that grows with the largest logit: 4e-5 relative at logits near 1000.
 constexpr float kLog2e = 1.4426950408889634f;
-__device__ __forceinline__ float exp_shift(float x, float ml) {
+__device__ __forceinline__ float exp_shift(float x, float m) {
   float y;
-  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"(fmaf(x, kLog2e, -ml)));
+  asm("ex2.approx.ftz.f32 %0, %1;" : "=f"(y) : "f"((x - m) * kLog2e));
   return y;
 }
 template <typename T> __device__ __forceinline__ T neg_inf();
@@ -352,13 +354,10 @@ __global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossBwdParams b) {
         xt[v] = t[v] == k ? f : xt[v];
       }
     }
-    float ml[V];
-#pragma unroll
-    for (int v = 0; v < V; ++v) ml[v] = mx[v] * kLog2e;
 #pragma unroll
     for (int k = 0; k < KMAX; ++k) {
 #pragma unroll
-      for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), ml[v]);
+      for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), mx[v]);
     }
     if (!kBackward) {
 #pragma unroll
@@ -378,8 +377,6 @@ __global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossBwdParams b) {
         if (t[v] >= 0) c[v] = g * hard_dloss(p, xt[v] - lse[v], p.weight ? p.weight[t[v]] : 1.f);
       }
       T* dp = dx + n * K * S + s0;
-#pragma unroll
-      for (int v = 0; v < V; ++v) lse[v] *= kLog2e;
 #pragma unroll
       for (int k = 0; k < KMAX; ++k) {
         Vec8<T> o;
@@ -444,15 +441,10 @@ __global__ void __launch_bounds__(kThreads) poly_soft_vec_kernel(LossBwdParams b
 #pragma unroll
       for (int v = 0; v < V; ++v) mx[v] = fmaxf(mx[v], to_f(r[k].v[v]));
     }
-    {
-      float ml[V];
 #pragma unroll
-      for (int v = 0; v < V; ++v) ml[v] = mx[v] * kLog2e;
+    for (int k = 0; k < KMAX; ++k) {
 #pragma unroll
-      for (int k = 0; k < KMAX; ++k) {
-#pragma unroll
-        for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), ml[v]);
-      }
+      for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), mx[v]);
     }
 #pragma unroll
     for (int v = 0; v < V; ++v) lse[v] = mx[v] + logf(sum[v]);
@@ -1000,6 +992,12 @@ int mcl_rdot_threads(int xi) {
   return t > kThreads ? kThreads : t;
 }
 
+// The shape checks of the entry points, before any launch or device query. N = 0 is an empty batch (nothing to do);
+// K < 1 or S < 1 describe no class or no position of a non-empty tensor.
+bool bad_nks(int N, int K, long long S) { return N < 0 || K < 1 || S < 1; }
+// mcl_rdot_threads(xi) >= 32 for xi <= 376
+bool bad_mcl(int N, int cnum, int xi, int S) { return bad_nks(N, cnum, S) || xi < 1 || mcl_rdot_threads(xi) < 32; }
+
 }  // namespace
 
 extern "C" {
@@ -1011,6 +1009,7 @@ int hb_loss_max_partials(void) { return HB_NUM_SMS * 8; }
 int hb_cls_loss_hard_fwd(const void* x, const long long* target, const float* weight, float* loss_pos, double* partials,
                          float* fwd_out, int N, int K, int S, int ignore_index, int kind, float gamma, float eps,
                          int dtype, void* stream) {
+  if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
   LossParams p{};
   p.x = x; p.target = target; p.weight = weight; p.loss_pos = loss_pos; p.partials = partials;
   p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.kind = kind; p.gamma = gamma; p.eps = eps;
@@ -1044,6 +1043,7 @@ int hb_cls_loss_hard_fwd(const void* x, const long long* target, const float* we
 int hb_cls_loss_hard_bwd(const void* x, const long long* target, const float* weight, const float* gout,
                          const float* fwd_out, void* dx, int N, int K, int S, int ignore_index, int kind, float gamma,
                          float eps, int reduction, int dtype, void* stream) {
+  if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
   LossBwdParams b{};
   b.f.x = x; b.f.target = target; b.f.weight = weight;
   b.f.N = N; b.f.K = K; b.f.S = S; b.f.ignore_index = ignore_index; b.f.kind = kind; b.f.gamma = gamma; b.f.eps = eps;
@@ -1072,6 +1072,7 @@ int hb_cls_loss_hard_bwd(const void* x, const long long* target, const float* we
 
 int hb_poly_soft_fwd(const void* x, const void* soft, const float* weight, float* loss_pos, double* partials,
                      float* fwd_out, int N, int K, int S, int ignore_index, float eps, int dtype, void* stream) {
+  if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
   LossBwdParams b{};
   b.f.x = x; b.f.soft = soft; b.f.weight = weight; b.f.loss_pos = loss_pos; b.f.partials = partials;
   b.f.N = N; b.f.K = K; b.f.S = S; b.f.ignore_index = ignore_index; b.f.kind = POLY; b.f.eps = eps;
@@ -1101,6 +1102,7 @@ int hb_poly_soft_fwd(const void* x, const void* soft, const float* weight, float
 
 int hb_poly_soft_bwd(const void* x, const void* soft, const float* weight, const float* gout, void* dx, int N, int K,
                      int S, int ignore_index, float eps, int reduction, int dtype, void* stream) {
+  if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
   LossBwdParams b{};
   b.f.x = x; b.f.soft = soft; b.f.weight = weight;
   b.f.N = N; b.f.K = K; b.f.S = S; b.f.ignore_index = ignore_index; b.f.kind = POLY; b.f.eps = eps;
@@ -1133,7 +1135,7 @@ size_t hb_dice_scratch_doubles(int K) { return 2 * ((size_t)HB_NUM_SMS * 16 + (s
 int hb_dice_fwd(const void* x, const void* target, const float* weight, double* scratch, float* out, float* coef, int N,
                 int K, long long S, float gamma, float eps, int dtype, void* stream) {
   cudaStream_t st = (cudaStream_t)stream;
-  if (K <= 0 || K > 65535) return (int)cudaErrorInvalidValue;
+  if (bad_nks(N, K, S) || K > 65535) return (int)cudaErrorInvalidValue;
   const int gx = dice_blocks_per_class((long long)N * S, K);
   double* part = scratch;
   double* sums = scratch + 2 * (size_t)gx * K;
@@ -1158,6 +1160,7 @@ int hb_dice_fwd(const void* x, const void* target, const float* weight, double* 
 
 int hb_dice_bwd(const void* target, const float* coef, const float* gout, void* dx, int N, int K, long long S, int dtype,
                 void* stream) {
+  if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
   const long long total = (long long)N * K * S;
   if (total == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
@@ -1188,6 +1191,7 @@ int hb_dice_bwd(const void* target, const float* coef, const float* gout, void* 
 
 int hb_cce_fwd(const void* x, const long long* target, const float* weight, float* loss_pos, double* partials,
                float* fwd_out, int N, int K, int S, int ignore_index, float gamma, int dtype, void* stream) {
+  if (bad_nks(N, K, S) || (gamma != 0.f && K < 2)) return (int)cudaErrorInvalidValue;  // C divides by K - 1
   CceParams p{};
   p.x = x; p.target = target; p.weight = weight; p.loss_pos = loss_pos; p.partials = partials;
   p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.gamma = gamma;
@@ -1206,6 +1210,7 @@ int hb_cce_fwd(const void* x, const long long* target, const float* weight, floa
 
 int hb_cce_bwd(const void* x, const long long* target, const float* weight, const float* gout, const float* fwd_out,
                void* dx, int N, int K, int S, int ignore_index, float gamma, int reduction, int dtype, void* stream) {
+  if (bad_nks(N, K, S) || (gamma != 0.f && K < 2)) return (int)cudaErrorInvalidValue;  // C divides by K - 1
   CceParams p{};
   p.x = x; p.target = target; p.weight = weight; p.gout = gout; p.fwd_out = fwd_out; p.dx = dx;
   p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.reduction = reduction; p.gamma = gamma;
@@ -1223,6 +1228,7 @@ int hb_cce_bwd(const void* x, const long long* target, const float* weight, cons
 int hb_mcl_fwd(const void* x, const long long* target, const float* weight, const unsigned char* mask, float* row_lse,
                float* loss_pos, float* lse_d, double* partials, float* fwd_out, int N, int cnum, int xi, int S,
                int ignore_index, float alpha, int dtype, void* stream) {
+  if (bad_mcl(N, cnum, xi, S)) return (int)cudaErrorInvalidValue;
   McParams p{};
   p.x = x; p.target = target; p.weight = weight; p.mask = mask; p.row_lse = row_lse; p.loss_pos = loss_pos;
   p.lse_d = lse_d; p.partials = partials;
@@ -1249,6 +1255,7 @@ int hb_mcl_fwd(const void* x, const long long* target, const float* weight, cons
 int hb_mcl_bwd(const void* x, const long long* target, const float* weight, const unsigned char* mask,
                const float* row_lse, const float* lse_d, const float* gout, const float* fwd_out, float* rdot, void* dx,
                int N, int cnum, int xi, int S, int ignore_index, float alpha, int reduction, int dtype, void* stream) {
+  if (bad_mcl(N, cnum, xi, S)) return (int)cudaErrorInvalidValue;
   McParams p{};
   p.x = x; p.target = target; p.weight = weight; p.mask = mask; p.row_lse = row_lse; p.lse_d = const_cast<float*>(lse_d); p.gout = gout;
   p.fwd_out = fwd_out; p.rdot = rdot; p.dx = dx;
@@ -1256,7 +1263,6 @@ int hb_mcl_bwd(const void* x, const long long* target, const float* weight, cons
   const long long P = (long long)N * S, groups = (long long)N * cnum;
   if (P == 0 || groups == 0) return 0;
   const int rt = mcl_rdot_threads(xi);
-  if (rt < 32) return (int)cudaErrorInvalidValue;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(P, kThreads);
   const size_t smem = (size_t)xi * rt * sizeof(float);
