@@ -55,10 +55,14 @@ SIGNATURES = {
     "hb_bn_stats_partials_bf16": "piippp",
     "hb_bn_stat_slots_max": "",
     "hb_bn_finalize": "ppppppp" + "pppp" + "iiiiffp",
+    "hb_bn_partials_sums": "ppiiiipp",
+    "hb_bn_finalize_sums": "p" * 10 + "iiiffp",
     "hb_bn_eval_affine": "ppppfiippppp",
     "hb_bn_act_fwd_bf16": "pppipppp" + "iiifi" + "ppp",
     "hb_bn_bwd_scratch_doubles": "iii",
     "hb_bn_act_bwd_bf16": "ppppi" + "pppppp" + "pppppp" + "pp" + "iiiifiip",
+    "hb_bn_act_bwd_reduce_bf16": "ppppi" + "pppppp" + "pppp" + "iiiifip",
+    "hb_bn_act_bwd_apply_bf16": "ppppi" + "pppppp" + "ppppp" + "iiifip",
     "hb_dwconv_fwd_bf16": "pppp" + "iiiiiiip",
     "hb_dwconv_bwd_data_bf16": "ppp" + "iiiiiiip",
     "hb_dwconv_wgrad_scratch_doubles": "ii",

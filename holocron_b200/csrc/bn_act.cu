@@ -95,6 +95,8 @@ struct FinalizeParams {
   int B, C, M;
   int C_logical;  // channels >= C_logical are padding: scale = shift = 0, no parameter / running-stat access
   float eps, momentum;
+  double* sums;   // [B][C][2] (sum, sum of squares) + the row count: written by bn_partials_sums_kernel, read by
+                  // bn_finalize_sums_kernel (a synchronised BatchNorm all-reduces it in between)
 };
 // block = 8 channels (threadIdx.x: one 64-byte run of the [slot][C][2] partials) x 32 slot lanes (threadIdx.y). A lane adds
 // slots L, L + 32, ... with four independent loads in flight, the 32 lane sums are then combined 8-by-8 in lane order: a
@@ -158,25 +160,17 @@ __device__ __forceinline__ void fold_slots(bool has_slots, int n, int live, Load
   }
 }
 
-__global__ void __launch_bounds__(kFinCh * kFinLanes) bn_finalize_kernel(FinalizeParams p) {
-  const int c = blockIdx.x * kFinCh + threadIdx.x;
-  const int b = blockIdx.y;
-  const float* pp = p.parts[b] + (size_t)c * 2;
-  const size_t row = (size_t)p.C * 2;
-  double tot[2];
-  fold_slots<2>(c < p.C_logical, p.slots[b], 2, [&](int k, double (&v)[2]) {
-    const float2 f = *reinterpret_cast<const float2*>(pp + (size_t)k * row);
-    v[0] = (double)f.x; v[1] = (double)f.y;
-  }, tot);
-  if (threadIdx.y != 0 || c >= p.C) return;
+// Branch b, channel c of the finalisation from the fp64 (sum, sum of squares) s, q over n rows: mean / rstd / scale / shift,
+// the running statistics (unbiased variance over n) and num_batches_tracked. n is the local row count (hb_bn_finalize) or
+// the count summed over the ranks of a synchronised BatchNorm (hb_bn_finalize_sums); for an integer n both read the same.
+__device__ __forceinline__ void finalize_channel(const FinalizeParams& p, int b, int c, double s, double q, double n) {
   const size_t o = (size_t)b * p.C + c;
   if (c >= p.C_logical) {
     p.mean[o] = 0.f; p.rstd[o] = 0.f; p.scale[o] = 0.f; p.shift[o] = 0.f;
     return;
   }
-  const double s = tot[0], q = tot[1];
-  const double mean = s / p.M;
-  double var = q / p.M - mean * mean;
+  const double mean = s / n;
+  double var = q / n - mean * mean;
   if (var < 0) var = 0;
   const float rstd = (float)(1.0 / sqrt(var + (double)p.eps));
   const float g = p.gamma[b] ? p.gamma[b][c] : 1.f;
@@ -188,10 +182,53 @@ __global__ void __launch_bounds__(kFinCh * kFinLanes) bn_finalize_kernel(Finaliz
   p.shift[o] = be - (float)mean * sc;
   if (c == 0 && p.num_batches_tracked[b]) *p.num_batches_tracked[b] += 1;
   if (p.running_mean[b]) {
-    const double unbiased = p.M > 1 ? var * ((double)p.M / (double)(p.M - 1)) : var;
+    const double unbiased = n > 1.0 ? var * (n / (n - 1.0)) : var;
     p.running_mean[b][c] = (1.f - p.momentum) * p.running_mean[b][c] + p.momentum * (float)mean;
     p.running_var[b][c] = (1.f - p.momentum) * p.running_var[b][c] + p.momentum * (float)unbiased;
   }
+}
+
+// (sum, sum of squares) of branch b, channel c over the branch's partial slots, in the fixed order of fold_slots; returned in
+// the threads with threadIdx.y == 0 (every thread of the block must call it)
+__device__ __forceinline__ void fold_partials(const FinalizeParams& p, int b, int c, double (&tot)[2]) {
+  const float* pp = p.parts[b] + (size_t)c * 2;
+  const size_t row = (size_t)p.C * 2;
+  fold_slots<2>(c < p.C_logical, p.slots[b], 2, [&](int k, double (&v)[2]) {
+    const float2 f = *reinterpret_cast<const float2*>(pp + (size_t)k * row);
+    v[0] = (double)f.x; v[1] = (double)f.y;
+  }, tot);
+}
+
+__global__ void __launch_bounds__(kFinCh * kFinLanes) bn_finalize_kernel(FinalizeParams p) {
+  const int c = blockIdx.x * kFinCh + threadIdx.x;
+  const int b = blockIdx.y;
+  double tot[2];
+  fold_partials(p, b, c, tot);
+  if (threadIdx.y != 0 || c >= p.C) return;
+  finalize_channel(p, b, c, tot[0], tot[1], (double)p.M);
+}
+
+// synchronised BatchNorm, step 1: the same fixed-order fold, written out as sums[b][c] = (sum, sum of squares) and
+// sums[B][0][0] = M (a double, so that the count adds up over ranks with the sums)
+__global__ void __launch_bounds__(kFinCh * kFinLanes) bn_partials_sums_kernel(FinalizeParams p) {
+  const int c = blockIdx.x * kFinCh + threadIdx.x;
+  const int b = blockIdx.y;
+  double tot[2];
+  fold_partials(p, b, c, tot);
+  if (threadIdx.y != 0 || c >= p.C) return;
+  const size_t o = ((size_t)b * p.C + c) * 2;
+  p.sums[o] = tot[0];
+  p.sums[o + 1] = tot[1];
+  if (b == 0 && c == 0) p.sums[(size_t)p.B * p.C * 2] = (double)p.M;
+}
+
+// synchronised BatchNorm, step 2: finalisation from the all-reduced sums and count
+__global__ void bn_finalize_sums_kernel(FinalizeParams p) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  const int b = blockIdx.y;
+  if (c >= p.C) return;
+  const size_t o = ((size_t)b * p.C + c) * 2;
+  finalize_channel(p, b, c, p.sums[o], p.sums[o + 1], p.sums[(size_t)p.B * p.C * 2]);
 }
 
 // eval-mode affine from running statistics: scale = gamma / sqrt(var + eps), shift = beta - mean * scale
@@ -411,6 +448,8 @@ struct BwdParams {
   const float* rstd;
   double* sums;        // [1 + B][C]: sum dz, sum dz*u_b (final, written by bn_bwd_finalize_kernel)
   double* part;        // [row blocks][1 + B][C]: per-block partials of the above (pass 1), summed in a fixed order
+  const double* count; // row count the sums are over (device scalar: summed over the ranks of a synchronised BatchNorm);
+                       // null: M
   __nv_bfloat16* du[kMaxBranches];
   __nv_bfloat16* dres;  // may be null
   int M, C, act;
@@ -434,7 +473,7 @@ struct SlabConsts {
 template <int NB>
 __device__ __forceinline__ void load_slab_consts(SlabConsts& k, const BwdParams& p, const SlabGeo& g, bool with_means) {
   const int nch = g.cg_t * 8;
-  const double invM = 1.0 / (double)p.M;
+  const double invM = 1.0 / (p.count ? *p.count : (double)p.M);
   for (int ch = threadIdx.x; ch < nch; ch += kThreads) {
     const int c = blockIdx.y * nch + ch;
     const bool ok = c < p.C;
@@ -690,6 +729,90 @@ auto with_nb(int B, F pick) {
 
 inline size_t ring_bytes(int tensors) { return (size_t)(ring_depth(tensors) + 1) * tensors * kThreads * 16; }
 
+// FinalizeParams of the per-branch host arrays (entries other than parts may be null)
+inline int finalize_params(FinalizeParams& p, const float* const* parts, const int* slots, const float* const* gamma,
+                           const float* const* beta, float* const* running_mean, float* const* running_var,
+                           long long* const* num_batches_tracked, int B) {
+  if (B < 1 || B > kMaxBranches) return (int)cudaErrorInvalidValue;
+  for (int b = 0; b < B; ++b) {
+    if (parts) {
+      if (!parts[b] || !slots || slots[b] < 1) return (int)cudaErrorInvalidValue;
+      p.parts[b] = parts[b];
+      p.slots[b] = slots[b];
+    }
+    p.gamma[b] = gamma ? gamma[b] : nullptr;
+    p.beta[b] = beta ? beta[b] : nullptr;
+    p.running_mean[b] = running_mean ? running_mean[b] : nullptr;
+    p.running_var[b] = running_var ? running_var[b] : nullptr;
+    p.num_batches_tracked[b] = num_batches_tracked ? num_batches_tracked[b] : nullptr;
+  }
+  p.B = B;
+  return 0;
+}
+
+// Backward parameters; scratch = [1+B][C] sums followed by the reduction pass' per-block partials (apply reads the sums only)
+inline BwdParams bwd_params(const void* dout, const void* u0, const void* u1, const void* u2, int B, const float* scale,
+                            const float* shift, const float* mean, const float* rstd, const void* residual, double* scratch,
+                            const double* count, void* du0, void* du1, void* du2, void* dres, int M, int C, int act,
+                            float slope, int train, int res_after) {
+  BwdParams p{};
+  p.br = Branches{{(const __nv_bfloat16*)u0, (const __nv_bfloat16*)u1, (const __nv_bfloat16*)u2}, B};
+  p.dout = (const __nv_bfloat16*)dout; p.residual = (const __nv_bfloat16*)residual;
+  p.scale = scale; p.shift = shift; p.mean = mean; p.rstd = rstd;
+  p.sums = scratch; p.part = scratch + (size_t)(1 + B) * C; p.count = count;
+  p.du[0] = (__nv_bfloat16*)du0; p.du[1] = (__nv_bfloat16*)du1; p.du[2] = (__nv_bfloat16*)du2;
+  p.dres = (__nv_bfloat16*)dres;
+  p.M = M; p.C = C; p.act = act; p.slope = slope; p.train = train; p.res_after = res_after;
+  return p;
+}
+
+// reduction pass + bn_bwd_finalize_kernel: p.sums = (sum dz, sum dz*u_b) over these M rows, parameter gradients written /
+// added from them
+inline int launch_bwd_reduce(const BwdParams& p, float* dgamma, float* dbeta, float* const* gamma_grad_acc,
+                             float* const* beta_grad_acc, int C_logical, cudaStream_t st) {
+  const int B = p.br.n, C = p.C;
+  const SlabGeo g = SlabGeo::make(C);
+  static const int cap_red_env = env_int("HB_BN_CAP_RED", 0);
+  static const bool use_occ = env_int("HB_BN_USE_OCC", 1) != 0, occ_debug = env_int("HB_BN_DEBUG", 0) != 0;
+  // one branch (Darknet / ReXNet / UNet blocks): ~70 registers and a 48 KB ring -> three resident blocks per SM
+  int cap_red = cap_red_env > 0 ? cap_red_env : (B <= 1 ? 3 : 2);
+  if (cap_red > 3) cap_red = 3;   // hb_bn_bwd_scratch_doubles sizes the partials for <= 3 blocks per SM
+  const size_t smem = sizeof(SlabConsts) + kThreads * 8 * sizeof(float) + ring_bytes(B + 2);
+  const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_reduce_kernel<decltype(nb)::value>>(smem); });
+  if (!occ) return (int)cudaErrorInvalidValue;
+  if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_reduce_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_red);
+  const dim3 grid = make_grid(g, p.M, 1, (use_occ && occ < cap_red) ? occ : cap_red);
+  kernel<<<grid, kThreads, smem, st>>>(p, g);
+  HB_LAUNCH_CHECK();
+  BwdFinalizeParams f{};
+  f.part = p.part; f.sums = p.sums; f.mean = p.mean; f.rstd = p.rstd; f.dgamma = dgamma; f.dbeta = dbeta;
+  for (int b = 0; b < B; ++b) {
+    f.gacc[b] = gamma_grad_acc ? gamma_grad_acc[b] : nullptr;
+    f.bacc[b] = beta_grad_acc ? beta_grad_acc[b] : nullptr;
+  }
+  f.nblocks = (int)grid.x; f.B = B; f.C = C; f.C_logical = C_logical > 0 ? C_logical : C;
+  bn_bwd_finalize_kernel<<<(C + kFinCh - 1) / kFinCh, dim3(kFinCh, kFinLanes), 0, st>>>(f);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+// apply pass: input gradients from p.sums (and p.count)
+inline int launch_bwd_apply(const BwdParams& p, cudaStream_t st) {
+  const int B = p.br.n;
+  const SlabGeo g = SlabGeo::make(p.C);
+  static const int cap_app_env = env_int("HB_BN_CAP_APPLY", 0);
+  static const bool use_occ = env_int("HB_BN_USE_OCC", 1) != 0, occ_debug = env_int("HB_BN_DEBUG", 0) != 0;
+  const int cap_app = cap_app_env > 0 ? cap_app_env : (B <= 2 ? 3 : 2);   // further limited by the measured occupancy
+  const size_t smem = sizeof(SlabConsts) + ring_bytes(B + 2);
+  const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_apply_kernel<decltype(nb)::value>>(smem); });
+  if (!occ) return (int)cudaErrorInvalidValue;
+  if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_apply_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_app);
+  const dim3 grid = make_grid(g, p.M, 1, (use_occ && occ < cap_app) ? occ : cap_app);
+  kernel<<<grid, kThreads, smem, st>>>(p, g);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
 }  // namespace
 
 extern "C" {
@@ -712,21 +835,40 @@ int hb_bn_finalize(const float* const* parts, const int* slots, const float* con
                    float* const* running_mean, float* const* running_var, long long* const* num_batches_tracked,
                    float* mean, float* rstd, float* scale, float* shift, int B, int C, int C_logical, int M, float eps,
                    float momentum, void* stream) {
-  if (B < 1 || B > kMaxBranches || !parts || !slots) return (int)cudaErrorInvalidValue;
   FinalizeParams p{};
-  for (int b = 0; b < B; ++b) {
-    if (!parts[b] || slots[b] < 1) return (int)cudaErrorInvalidValue;
-    p.parts[b] = parts[b];
-    p.slots[b] = slots[b];
-    p.gamma[b] = gamma ? gamma[b] : nullptr;
-    p.beta[b] = beta ? beta[b] : nullptr;
-    p.running_mean[b] = running_mean ? running_mean[b] : nullptr;
-    p.running_var[b] = running_var ? running_var[b] : nullptr;
-    p.num_batches_tracked[b] = num_batches_tracked ? num_batches_tracked[b] : nullptr;
-  }
+  if (!parts) return (int)cudaErrorInvalidValue;
+  if (const int rc = finalize_params(p, parts, slots, gamma, beta, running_mean, running_var, num_batches_tracked, B))
+    return rc;
   p.mean = mean; p.rstd = rstd; p.scale = scale; p.shift = shift;
-  p.B = B; p.C = C; p.M = M; p.C_logical = C_logical; p.eps = eps; p.momentum = momentum;
+  p.C = C; p.M = M; p.C_logical = C_logical; p.eps = eps; p.momentum = momentum;
   bn_finalize_kernel<<<dim3((C + kFinCh - 1) / kFinCh, B), dim3(kFinCh, kFinLanes), 0, (cudaStream_t)stream>>>(p);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+int hb_bn_partials_sums(const float* const* parts, const int* slots, int B, int C, int C_logical, int M, double* sums,
+                        void* stream) {
+  FinalizeParams p{};
+  if (!parts || !sums) return (int)cudaErrorInvalidValue;
+  if (const int rc = finalize_params(p, parts, slots, nullptr, nullptr, nullptr, nullptr, nullptr, B)) return rc;
+  p.C = C; p.C_logical = C_logical; p.M = M; p.sums = sums;
+  bn_partials_sums_kernel<<<dim3((C + kFinCh - 1) / kFinCh, B), dim3(kFinCh, kFinLanes), 0, (cudaStream_t)stream>>>(p);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+int hb_bn_finalize_sums(const double* sums, const float* const* gamma, const float* const* beta,
+                        float* const* running_mean, float* const* running_var, long long* const* num_batches_tracked,
+                        float* mean, float* rstd, float* scale, float* shift, int B, int C, int C_logical, float eps,
+                        float momentum, void* stream) {
+  FinalizeParams p{};
+  if (!sums) return (int)cudaErrorInvalidValue;
+  if (const int rc = finalize_params(p, nullptr, nullptr, gamma, beta, running_mean, running_var, num_batches_tracked, B))
+    return rc;
+  p.sums = const_cast<double*>(sums);
+  p.mean = mean; p.rstd = rstd; p.scale = scale; p.shift = shift;
+  p.C = C; p.C_logical = C_logical; p.eps = eps; p.momentum = momentum;
+  bn_finalize_sums_kernel<<<dim3((C + 127) / 128, B), 128, 0, (cudaStream_t)stream>>>(p);
   HB_LAUNCH_CHECK();
   return 0;
 }
@@ -789,51 +931,35 @@ int hb_bn_act_bwd_bf16(const void* dout, const void* u0, const void* u1, const v
                        float* const* gamma_grad_acc, float* const* beta_grad_acc, int C_logical, int M, int C, int act,
                        float slope, int train, int res_after, void* stream) {
   if (C % 8 != 0 || B < 0 || B > kMaxBranches) return (int)cudaErrorInvalidValue;
-  BwdParams p{};
-  p.br = Branches{{(const __nv_bfloat16*)u0, (const __nv_bfloat16*)u1, (const __nv_bfloat16*)u2}, B};
-  p.dout = (const __nv_bfloat16*)dout; p.residual = (const __nv_bfloat16*)residual;
-  p.scale = scale; p.shift = shift; p.mean = mean; p.rstd = rstd;
-  p.sums = scratch; p.part = scratch + (size_t)(1 + B) * C;
-  p.du[0] = (__nv_bfloat16*)du0; p.du[1] = (__nv_bfloat16*)du1; p.du[2] = (__nv_bfloat16*)du2;
-  p.dres = (__nv_bfloat16*)dres;
-  p.M = M; p.C = C; p.act = act; p.slope = slope; p.train = train; p.res_after = res_after;
-  const SlabGeo g = SlabGeo::make(C);
-  cudaStream_t st = (cudaStream_t)stream;
-  static const int cap_red_env = env_int("HB_BN_CAP_RED", 0), cap_app_env = env_int("HB_BN_CAP_APPLY", 0);
-  static const bool use_occ = env_int("HB_BN_USE_OCC", 1) != 0, occ_debug = env_int("HB_BN_DEBUG", 0) != 0;
-  // one branch (Darknet / ReXNet / UNet blocks): ~70 registers and a 48 KB ring -> three resident blocks per SM
-  int cap_red = cap_red_env > 0 ? cap_red_env : (B <= 1 ? 3 : 2);
-  if (cap_red > 3) cap_red = 3;   // hb_bn_bwd_scratch_doubles sizes the partials for <= 3 blocks per SM
-  const int cap_app = cap_app_env > 0 ? cap_app_env : (B <= 2 ? 3 : 2);   // further limited by the measured occupancy
+  const BwdParams p = bwd_params(dout, u0, u1, u2, B, scale, shift, mean, rstd, residual, scratch, nullptr, du0, du1, du2,
+                                 dres, M, C, act, slope, train, res_after);
   const bool want_params = (dgamma && dbeta) || gamma_grad_acc || beta_grad_acc;
   if (train || want_params) {
-    const size_t smem = sizeof(SlabConsts) + kThreads * 8 * sizeof(float) + ring_bytes(B + 2);
-    const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_reduce_kernel<decltype(nb)::value>>(smem); });
-    if (!occ) return (int)cudaErrorInvalidValue;
-    if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_reduce_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_red);
-    const dim3 grid = make_grid(g, M, 1, (use_occ && occ < cap_red) ? occ : cap_red);
-    kernel<<<grid, kThreads, smem, st>>>(p, g);
-    HB_LAUNCH_CHECK();
-    BwdFinalizeParams f{};
-    f.part = p.part; f.sums = p.sums; f.mean = mean; f.rstd = rstd; f.dgamma = dgamma; f.dbeta = dbeta;
-    for (int b = 0; b < B; ++b) {
-      f.gacc[b] = gamma_grad_acc ? gamma_grad_acc[b] : nullptr;
-      f.bacc[b] = beta_grad_acc ? beta_grad_acc[b] : nullptr;
-    }
-    f.nblocks = (int)grid.x; f.B = B; f.C = C; f.C_logical = C_logical > 0 ? C_logical : C;
-    bn_bwd_finalize_kernel<<<(C + kFinCh - 1) / kFinCh, dim3(kFinCh, kFinLanes), 0, st>>>(f);
-    HB_LAUNCH_CHECK();
+    const int rc = launch_bwd_reduce(p, dgamma, dbeta, gamma_grad_acc, beta_grad_acc, C_logical, (cudaStream_t)stream);
+    if (rc) return rc;
   }
-  {
-    const size_t smem = sizeof(SlabConsts) + ring_bytes(B + 2);
-    const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_apply_kernel<decltype(nb)::value>>(smem); });
-    if (!occ) return (int)cudaErrorInvalidValue;
-    if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_apply_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_app);
-    const dim3 grid = make_grid(g, M, 1, (use_occ && occ < cap_app) ? occ : cap_app);
-    kernel<<<grid, kThreads, smem, st>>>(p, g);
-    HB_LAUNCH_CHECK();
-  }
-  return 0;
+  return launch_bwd_apply(p, (cudaStream_t)stream);
+}
+
+int hb_bn_act_bwd_reduce_bf16(const void* dout, const void* u0, const void* u1, const void* u2, int B, const float* scale,
+                              const float* shift, const float* mean, const float* rstd, const void* residual,
+                              double* scratch, float* dgamma, float* dbeta, float* const* gamma_grad_acc,
+                              float* const* beta_grad_acc, int C_logical, int M, int C, int act, float slope, int res_after,
+                              void* stream) {
+  if (C % 8 != 0 || B < 0 || B > kMaxBranches || !scratch) return (int)cudaErrorInvalidValue;
+  const BwdParams p = bwd_params(dout, u0, u1, u2, B, scale, shift, mean, rstd, residual, scratch, nullptr, nullptr, nullptr,
+                                 nullptr, nullptr, M, C, act, slope, 1, res_after);
+  return launch_bwd_reduce(p, dgamma, dbeta, gamma_grad_acc, beta_grad_acc, C_logical, (cudaStream_t)stream);
+}
+
+int hb_bn_act_bwd_apply_bf16(const void* dout, const void* u0, const void* u1, const void* u2, int B, const float* scale,
+                             const float* shift, const float* mean, const float* rstd, const void* residual,
+                             const double* sums, const double* count, void* du0, void* du1, void* du2, void* dres, int M,
+                             int C, int act, float slope, int res_after, void* stream) {
+  if (C % 8 != 0 || B < 0 || B > kMaxBranches || !sums || !count) return (int)cudaErrorInvalidValue;
+  const BwdParams p = bwd_params(dout, u0, u1, u2, B, scale, shift, mean, rstd, residual, const_cast<double*>(sums), count,
+                                 du0, du1, du2, dres, M, C, act, slope, 1, res_after);
+  return launch_bwd_apply(p, (cudaStream_t)stream);
 }
 
 }  // extern "C"

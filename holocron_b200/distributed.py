@@ -4,7 +4,8 @@ optimizer step over NVLink/NVSwitch.
 The reference has no distributed code at all (SURVEY.md §2.1: a single ``gpu`` argument in
 holocron/trainer/core.py:52, 90-104). The path shards by batch: every rank runs the same fused kernels on its shard,
 BatchNorm statistics stay per-GPU (the reference uses plain ``nn.BatchNorm2d``), and the only exchange is the mean of the
-parameter gradients. ``torch.distributed`` (backend ``nccl`` on GPUs, ``gloo`` in the CPU tests) is the plumbing.
+parameter gradients. A model converted with ``nn.SyncBatchNorm.convert_sync_batchnorm`` also all-reduces the statistics of
+each BatchNorm step (``nn/_fused.py``, DESIGN.md §6). ``torch.distributed`` (backend ``nccl`` on GPUs, ``gloo`` in the CPU tests) is the plumbing.
 
 Design: all ``.grad`` tensors are views into ONE contiguous fp32 bucket (allocated once, laid out in reverse
 registration order = roughly the order backward produces them), so

@@ -110,7 +110,7 @@ def run_fused(mods: Sequence[nn.Module], x: Tensor, residual: Optional[Tensor] =
         if isinstance(m, nn.Conv2d):
             j = i + 1
             bn = act = None
-            if j < len(mods) and isinstance(mods[j], nn.BatchNorm2d):
+            if j < len(mods) and K.is_batch_norm(mods[j]):
                 bn = mods[j]; j += 1
             if j < len(mods) and _is_act(mods[j]):
                 act = mods[j]; j += 1
@@ -122,12 +122,12 @@ def run_fused(mods: Sequence[nn.Module], x: Tensor, residual: Optional[Tensor] =
         elif isinstance(m, FusedSequential):
             x = m(x)
             i += 1
-        elif isinstance(m, nn.BatchNorm2d) and x.is_cuda and x.shape[1] % 8 != 0:
+        elif K.is_batch_norm(m) and x.is_cuda and x.shape[1] % 8 != 0:
             # stand-alone BatchNorm on a width the fused pass cannot take (ReXNet-1.3x taps of DynamicUNet: 35, 61 ... channels;
             # behind a convolution the width is zero-padded instead): library call in the parameters' dtype
             x = m(x.to(m.weight.dtype if m.weight is not None else torch.float32)).to(x.dtype)
             i += 1
-        elif isinstance(m, nn.BatchNorm2d):
+        elif K.is_batch_norm(m):
             act = None
             j = i + 1
             if j < len(mods) and _is_act(mods[j]):

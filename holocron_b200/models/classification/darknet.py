@@ -47,7 +47,7 @@ class ResBlock(nn.Module):
         mods = list(self.conv)
         # the shortcut can be fused when the stack ends with [conv, BN, act] (no drop layer behind the activation)
         fusable = isinstance(mods[-1], nn.Module) and not isinstance(mods[-1], (DropBlock2d, nn.Dropout)) and \
-            any(isinstance(m, nn.BatchNorm2d) for m in mods[-3:])
+            any(K.is_batch_norm(m) for m in mods[-3:])
         if fusable and x.is_cuda:
             out = run_fused(mods, x, residual=x, res_after_act=True)
         else:

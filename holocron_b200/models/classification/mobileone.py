@@ -30,7 +30,7 @@ def _fused_branch_sum(branches: nn.ModuleList, x: Tensor, act: Optional[nn.Modul
     pairs: List[Tuple[Tensor, nn.BatchNorm2d]] = []
     xb = None
     for mod in branches:
-        if isinstance(mod, nn.BatchNorm2d):
+        if K.is_batch_norm(mod):
             xb = K.to_channels_last_bf16(x) if xb is None else xb
             pairs.append((xb, mod))
             continue
@@ -53,11 +53,11 @@ def _fused_branch_sum(branches: nn.ModuleList, x: Tensor, act: Optional[nn.Modul
 
 def _fusable(branches: nn.ModuleList, x: Tensor) -> bool:
     for mod in branches:
-        if isinstance(mod, nn.BatchNorm2d):
+        if K.is_batch_norm(mod):
             if mod.num_features % 8 != 0:
                 return False
         elif not (isinstance(mod, nn.Sequential) and len(mod) == 2 and isinstance(mod[0], nn.Conv2d)
-                  and isinstance(mod[1], nn.BatchNorm2d) and mod[1].num_features % 8 == 0
+                  and K.is_batch_norm(mod[1]) and mod[1].num_features % 8 == 0
                   and (_depthwise_ok(mod[0]) or _dense_ok(mod[0]))):
             return False
     return x.ndim == 4
@@ -97,7 +97,7 @@ class DepthConvBlock(_BranchSum):
         weight = torch.zeros_like(fused.weight.data)
         bias = torch.zeros_like(fused.bias.data)
         for mod in self:
-            if isinstance(mod, nn.BatchNorm2d):      # identity branch: a centre-tap filter
+            if K.is_batch_norm(mod):      # identity branch: a centre-tap filter
                 scale = mod.weight.data / torch.sqrt(mod.running_var + mod.eps)
                 bias += mod.bias.data - scale * mod.running_mean
                 weight[..., 1, 1] += scale.unsqueeze(1)
@@ -133,7 +133,7 @@ class PointConvBlock(_BranchSum):
         weight = torch.zeros_like(fused.weight.data)
         bias = torch.zeros_like(fused.bias.data)
         for mod in self:
-            if isinstance(mod, nn.BatchNorm2d):      # identity branch: a diagonal filter
+            if K.is_batch_norm(mod):      # identity branch: a diagonal filter
                 scale = mod.weight.data / torch.sqrt(mod.running_var + mod.eps)
                 bias += mod.bias.data - scale * mod.running_mean
                 idx = torch.arange(weight.shape[0], device=weight.device)

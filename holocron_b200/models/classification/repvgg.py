@@ -65,9 +65,9 @@ class RepBlock(nn.Module):
             return out if post is None else post(out)
         conv3, bn3 = cast(nn.Sequential, self.branches[0])
         conv1, bn1 = cast(nn.Sequential, self.branches[1])
-        if not (isinstance(bn3, nn.BatchNorm2d) and isinstance(bn1, nn.BatchNorm2d)):
-            raise NotImplementedError("the fused RepBlock needs nn.BatchNorm2d as norm_layer")
-        bns = [bn3, bn1] + ([cast(nn.BatchNorm2d, self.branches[2])] if len(self.branches) == 3 else [])
+        bns = [bn3, bn1] + ([self.branches[2]] if len(self.branches) == 3 else [])
+        if not all(K.is_batch_norm(b) for b in bns):
+            raise NotImplementedError("the fused RepBlock needs nn.BatchNorm2d or nn.SyncBatchNorm as norm_layer")
         if conv3.out_channels % 16 == 0 and all(b.eps == bn3.eps and b.momentum == bn3.momentum for b in bns) \
                 and bn3.momentum is not None:
             # whole block as one autograd node (input-gradient contributions chained through the conv epilogues)

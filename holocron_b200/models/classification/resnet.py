@@ -39,7 +39,7 @@ class _ResBlock(nn.Module):
         mods = list(self.conv)
         act = getattr(self, "activation", None)
         # fusable: the stack ends with [conv, BatchNorm] and the shortcut has the output's shape
-        if isinstance(mods[-1], nn.BatchNorm2d) and isinstance(mods[-2], nn.Conv2d):
+        if K.is_batch_norm(mods[-1]) and isinstance(mods[-2], nn.Conv2d):
             return run_fused(mods + ([act] if act is not None else []), x, residual=identity, res_after_act=False)
         out = self.conv(x)
         out = out + identity

@@ -89,8 +89,8 @@ class ReXBlock(nn.Module):
 
     def forward(self, x: Tensor, keep_padded: bool = False) -> Tensor:
         mods = list(self.conv)
-        if not all(isinstance(m, (nn.Conv2d, nn.BatchNorm2d, nn.SiLU, nn.ReLU6, SEBlock)) for m in mods):
-            raise NotImplementedError("fused ReXBlock expects the default BatchNorm2d / SiLU / ReLU6 layers")
+        if not all(isinstance(m, (nn.Conv2d, nn.SiLU, nn.ReLU6, SEBlock)) or K.is_batch_norm(m) for m in mods):
+            raise NotImplementedError("fused ReXBlock expects the default BatchNorm2d (or SyncBatchNorm) / SiLU / ReLU6 layers")
         xin = K.to_channels_last_bf16(x, K.round_up(x.shape[1], 16))
         i = 0
         y = xin
@@ -164,7 +164,7 @@ class ReXNet(nn.Sequential):
                 x = m(x, keep_padded=True)
                 i += 1
             elif isinstance(m, nn.Conv2d):
-                bn = mods[i + 1] if isinstance(mods[i + 1], nn.BatchNorm2d) else None
+                bn = mods[i + 1] if K.is_batch_norm(mods[i + 1]) else None
                 j = i + (2 if bn is not None else 1)
                 act = mods[j] if j < len(mods) and not isinstance(mods[j], (nn.Conv2d, ReXBlock)) else None
                 x = conv_bn_act(x, m, bn, act, keep_padded=True)

@@ -178,8 +178,9 @@ class UBlock(nn.Module):
         upfeat_ = self.upsample(upfeat)
         if downfeat.shape[-2:] != upfeat_.shape[-2:]:
             upfeat_ = F.interpolate(upfeat_, downfeat.shape[-2:], mode="nearest")
-        # skip features: BatchNorm alone (the activation follows the concatenation) - fused pass for nn.BatchNorm2d
-        left = run_fused([self.bn], downfeat) if isinstance(self.bn, nn.BatchNorm2d) else _in_dtype_of(self.bn, downfeat)
+        # skip features: BatchNorm alone (the activation follows the concatenation) - fused pass for nn.BatchNorm2d and
+        # nn.SyncBatchNorm
+        left = run_fused([self.bn], downfeat) if K.is_batch_norm(self.bn) else _in_dtype_of(self.bn, downfeat)
         if left.dtype != upfeat_.dtype and left.dtype == torch.float32:
             upfeat_ = upfeat_.float()          # fp32 skip features of a library encoder: keep their precision through the cat
         return self.block(torch.cat((left.to(upfeat_.dtype), upfeat_), dim=1))

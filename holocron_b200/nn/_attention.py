@@ -12,7 +12,7 @@ import torch
 from torch import Tensor, nn
 
 from .._lib import check, dtype_code, lib, ptr, require_cuda, stream_ptr
-from ._fused import BNBranch, _bn_batch_stats, attach_stats
+from ._fused import BNBranch, _bn_batch_stats, attach_stats, sync_group
 from ._pooling import _apply, _empty_cl, _nhwc, _pitch
 
 _VP3 = ctypes.c_void_p * 3
@@ -214,6 +214,10 @@ def triplet_attention(x: Tensor, branches: Sequence[Tuple[int, nn.Conv2d, nn.Bat
         b = dim % 4 - 1
         if bns[b] is not None:
             raise NotImplementedError(f"TripletAttention: two branches attend over dim {b + 1}")
+        if sync_group([bn], bn.training) is not None:
+            # the gate kernels keep each branch's statistics on the device between their launches: no all-reduce point
+            raise NotImplementedError("TripletAttention: a SyncBatchNorm that synchronises over its process group "
+                                      "(its statistics would silently stay per-GPU)")
         rows, cols = _plane_dims(b, c, h, w)
         if _uses_batch_stats(bn) and n * rows * cols == 1:   # F.batch_norm's check, before any launch
             raise ValueError(f"Expected more than 1 value per channel when training, got input size "

@@ -15,6 +15,7 @@ import weakref
 from typing import List, Optional, Sequence, Tuple
 
 import torch
+import torch.distributed as dist
 from torch import Tensor, nn
 
 from .._lib import DTYPE_CODE, ConvArgs, check, dtype_code, lib, ptr, require_cuda, stream_ptr
@@ -570,6 +571,38 @@ def conv2d_bias_act(x: Tensor, weight: Tensor, bias: Optional[Tensor], stride: i
 
 
 # ------------------------------------------------------------------------------------------------------
+BATCH_NORMS = (nn.BatchNorm2d, nn.SyncBatchNorm)
+
+
+def is_batch_norm(m: nn.Module) -> bool:
+    """Whether the fused BatchNorm pass takes ``m``: an ``nn.BatchNorm2d``, or the ``nn.SyncBatchNorm`` that
+    ``nn.SyncBatchNorm.convert_sync_batchnorm`` turns it into (not a subclass of it)."""
+    return isinstance(m, BATCH_NORMS)
+
+
+def sync_group(bns: Sequence[nn.Module], training: bool) -> Optional["dist.ProcessGroup"]:
+    """The process group whose ranks share the batch statistics of ``bns``, or None for per-GPU statistics.
+
+    ``nn.SyncBatchNorm``'s rule: synchronise only in training (batch statistics), with ``torch.distributed`` initialised
+    and more than one rank in the layer's group (``process_group``, default the world). Otherwise a converted layer runs
+    the plain BatchNorm path. The branches of one fused pass share one all-reduce, so they must agree on all of this."""
+    syncs = [b for b in bns if isinstance(b, nn.SyncBatchNorm)]
+    if not training or not syncs or not (dist.is_available() and dist.is_initialized()):
+        return None
+    group = syncs[0].process_group or dist.group.WORLD
+    if dist.get_world_size(group) < 2:
+        return None
+    if len(syncs) != len(bns) or any(b.process_group is not syncs[0].process_group for b in syncs):
+        raise NotImplementedError("one fused BatchNorm pass over branches that do not share one SyncBatchNorm process group")
+    return group
+
+
+def _all_reduce(t: Tensor, group) -> None:
+    """SUM all-reduce of ``t`` over ``group``, ordered on the current stream (captured into a CUDA graph like the
+    gradient bucket's)."""
+    dist.all_reduce(t, op=dist.ReduceOp.SUM, group=group)
+
+
 class BNBranch:
     """Non-tensor view of one BatchNorm2d's buffers/hyper-parameters handed to the fused function."""
     __slots__ = ("running_mean", "running_var", "eps", "momentum", "num_batches_tracked", "track_running_stats")
@@ -597,12 +630,17 @@ def _elem_bytes_info(kind: str, m: int, c: int, reads: int, writes: int) -> dict
     return dict(shape=(kind, m, c, reads, writes), launches=1, flops=0.0, bytes=2.0 * m * c * (reads + writes))
 
 
-def _bn_batch_stats(us: Sequence[Tensor], branches, g32, b32, stats: Tensor, c: int, c_log: int, m: int) -> None:
+def _bn_batch_stats(us: Sequence[Tensor], branches, g32, b32, stats: Tensor, c: int, c_log: int, m: int,
+                    group=None) -> Optional[Tensor]:
     """Training-mode statistics -> mean / rstd / scale / shift rows of ``stats`` (+ running-statistics update).
 
     Every input normally arrives with its (sum, sum of squares) partials attached by its producer (convolution epilogue,
-    previous block's forward pass); only tensors that come without them get a stand-alone statistics pass."""
-    if m == 1:   # what F.batch_norm raises in training: the variance of one value is undefined
+    previous block's forward pass); only tensors that come without them get a stand-alone statistics pass.
+
+    ``group`` (:func:`sync_group`): the branches' fp64 sums and row count are packed into one buffer, all-reduced over
+    the group (one collective for every branch) and finalised from the global values; the buffer is returned (its last
+    element, the global row count, is what the backward pass normalises by). Without a group: None."""
+    if m == 1 and group is None:   # what F.batch_norm raises in training: the variance of one value is undefined
         raise ValueError(f"Expected more than 1 value per channel when training, got input size {us[0].shape}")
     L = lib()
     nb = len(us)
@@ -623,12 +661,38 @@ def _bn_batch_stats(us: Sequence[Tensor], branches, g32, b32, stats: Tensor, c: 
     track = [b.track_running_stats for b in branches]
     if mom is None and any(track):
         raise NotImplementedError("cumulative moving average (momentum=None)")
-    check(L.hb_bn_finalize(_arr3(parts), _I3(*(slots + [0] * (3 - nb))), _arr3(g32), _arr3(b32),
-                           _arr3([b.running_mean if t else None for b, t in zip(branches, track)]),
-                           _arr3([b.running_var if t else None for b, t in zip(branches, track)]),
-                           _arr3([b.num_batches_tracked if t else None for b, t in zip(branches, track)]),
-                           ptr(stats[0]), ptr(stats[1]), ptr(stats[2]), ptr(stats[3]), nb, c, c_log, m, _c_float(eps),
-                           _c_float(0.0 if mom is None else mom), stream_ptr()), "hb_bn_finalize")
+    running = (_arr3([b.running_mean if t else None for b, t in zip(branches, track)]),
+               _arr3([b.running_var if t else None for b, t in zip(branches, track)]),
+               _arr3([b.num_batches_tracked if t else None for b, t in zip(branches, track)]))
+    outs = (ptr(stats[0]), ptr(stats[1]), ptr(stats[2]), ptr(stats[3]))
+    if group is None:
+        check(L.hb_bn_finalize(_arr3(parts), _I3(*(slots + [0] * (3 - nb))), _arr3(g32), _arr3(b32), *running, *outs, nb, c,
+                               c_log, m, _c_float(eps), _c_float(0.0 if mom is None else mom), stream_ptr()),
+              "hb_bn_finalize")
+        return None
+    sums = sync_sums_buffer(nb, c, stats.device)
+    check(L.hb_bn_partials_sums(_arr3(parts), _I3(*(slots + [0] * (3 - nb))), nb, c, c_log, m, ptr(sums), stream_ptr()),
+          "hb_bn_partials_sums")
+    _all_reduce(sums, group)
+    check(L.hb_bn_finalize_sums(ptr(sums), _arr3(g32), _arr3(b32), *running, *outs, nb, c, c_log, _c_float(eps),
+                                _c_float(0.0 if mom is None else mom), stream_ptr()), "hb_bn_finalize_sums")
+    return sums
+
+
+def sync_sums_buffer(nb: int, c: int, device) -> Tensor:
+    """fp64 buffer of one synchronised statistics all-reduce: [nb][c][2] (sum, sum of squares), then the row count."""
+    return torch.empty(nb * c * 2 + 1, device=device, dtype=torch.float64)
+
+
+def sync_count(sums: Tensor) -> Tensor:
+    """The row count element of a :func:`sync_sums_buffer` (after the all-reduce: the rows of every rank)."""
+    return sums[-1:]
+
+
+def sync_grad_sums(scratch: Tensor, nb: int, c: int) -> Tensor:
+    """The [1 + nb][c] (sum dz, sum dz*u_b) head of the backward scratch: what a synchronised backward all-reduces (the
+    per-block partials behind it stay local)."""
+    return scratch[:(1 + nb) * c]
 
 
 def _bn_forward_pass(us: Sequence[Tensor], stats: Tensor, res: Optional[Tensor], m: int, c: int, act: int, slope: float,
@@ -651,8 +715,16 @@ def _bn_forward_pass(us: Sequence[Tensor], stats: Tensor, res: Optional[Tensor],
 
 
 def _bn_backward_pass(dob: Tensor, us: Sequence[Tensor], stats: Tensor, res: Optional[Tensor], dus, dres, dgb, gacc, bacc,
-                      c_log: int, m: int, c: int, act: int, slope: float, training: bool, res_after: int) -> None:
-    """Two streaming passes (reduce, apply) + the C-sized finalisation between them (fixed-order, no atomics)."""
+                      c_log: int, m: int, c: int, act: int, slope: float, training: bool, res_after: int,
+                      sync=None) -> None:
+    """Two streaming passes (reduce, apply) + the C-sized finalisation between them (fixed-order, no atomics).
+
+    ``sync`` = (group, forward sums buffer) of a synchronised BatchNorm: the reduce pass' (sum dz, sum dz*u_b) are
+    all-reduced over the group before the apply pass, which normalises by the global row count. The BatchNorm parameter
+    gradients stay the local sums, as with ``nn.SyncBatchNorm``: the gradient all-reduce averages them over the ranks."""
+    if sync is not None:
+        _bn_backward_sync(dob, us, stats, res, dus, dres, dgb, gacc, bacc, c_log, m, c, act, slope, res_after, *sync)
+        return
     L = lib()
     nb = len(us)
     scratch = torch.empty(L.hb_bn_bwd_scratch_doubles(m, c, nb), device=dob.device, dtype=torch.float64)
@@ -671,23 +743,47 @@ def _bn_backward_pass(dob: Tensor, us: Sequence[Tensor], stats: Tensor, res: Opt
         stream_ptr())), "hb_bn_act_bwd_bf16")
 
 
+def _bn_backward_sync(dob: Tensor, us: Sequence[Tensor], stats: Tensor, res: Optional[Tensor], dus, dres, dgb, gacc, bacc,
+                      c_log: int, m: int, c: int, act: int, slope: float, res_after: int, group, fwd_sums: Tensor) -> None:
+    L = lib()
+    nb = len(us)
+    scratch = torch.empty(L.hb_bn_bwd_scratch_doubles(m, c, nb), device=dob.device, dtype=torch.float64)
+    up = [ptr(us[i]) if i < nb else ptr(None) for i in range(3)]
+    dup = [ptr(dus[i]) if i < nb else ptr(None) for i in range(3)]
+    nres = int(res is not None and not res_after)
+    nwr = sum(d is not None for d in dus) + (dres is not None)
+    info = _elem_bytes_info("bn_bwd", m, c, 1 + nb + nres, 0)
+    info["launches"] = 2
+    check(_timed("bn_bwd", info, lambda: L.hb_bn_act_bwd_reduce_bf16(
+        ptr(dob), up[0], up[1], up[2], nb, ptr(stats[2]), ptr(stats[3]), ptr(stats[0]), ptr(stats[1]), ptr(res), ptr(scratch),
+        ptr(dgb[0]) if dgb is not None else ptr(None), ptr(dgb[1]) if dgb is not None else ptr(None),
+        _arr3(gacc) if gacc is not None else None, _arr3(bacc) if bacc is not None else None, c_log, m, c, act,
+        _c_float(slope), res_after, stream_ptr())), "hb_bn_act_bwd_reduce_bf16")
+    _all_reduce(sync_grad_sums(scratch, nb, c), group)
+    info = _elem_bytes_info("bn_bwd", m, c, 1 + nb + nres, nwr)
+    check(_timed("bn_bwd", info, lambda: L.hb_bn_act_bwd_apply_bf16(
+        ptr(dob), up[0], up[1], up[2], nb, ptr(stats[2]), ptr(stats[3]), ptr(stats[0]), ptr(stats[1]), ptr(res), ptr(scratch),
+        ptr(sync_count(fwd_sums)), dup[0], dup[1], dup[2], ptr(dres), m, c, act, _c_float(slope), res_after, stream_ptr())),
+        "hb_bn_act_bwd_apply_bf16")
+
+
 def _bn_setup(us: Sequence[Tensor], branches, gammas: Sequence[Tensor], betas: Sequence[Tensor], training: bool, c: int,
-              c_log: int, m: int, dev) -> Tensor:
+              c_log: int, m: int, dev, group=None) -> Tuple[Tensor, Optional[Tensor]]:
     """[4, max(nb, 1), c] fp32 mean / rstd / scale / shift rows of the branches: batch statistics in training, the
-    running statistics otherwise. ``c_log``: the parameters' channel count (<= c, the activation's padded width)."""
+    running statistics otherwise. ``c_log``: the parameters' channel count (<= c, the activation's padded width).
+    Returns them with the all-reduced sums of a synchronised BatchNorm (``group``, :func:`_bn_batch_stats`) or None."""
     stats = torch.empty((4, max(len(branches), 1), c), device=dev, dtype=torch.float32)
     g32 = [g.detach().float() for g in gammas]
     b32 = [b.detach().float() for b in betas]
     if not branches:
-        return stats
+        return stats, None
     if training:
-        _bn_batch_stats(us, branches, g32, b32, stats, c, c_log, m)
-        return stats
+        return stats, _bn_batch_stats(us, branches, g32, b32, stats, c, c_log, m, group)
     for i, b in enumerate(branches):
         check(lib().hb_bn_eval_affine(ptr(g32[i]), ptr(b32[i]), ptr(b.running_mean), ptr(b.running_var), _c_float(b.eps), c,
                                       c_log, ptr(stats[2][i]), ptr(stats[3][i]), ptr(stats[0][i]), ptr(stats[1][i]),
                                       stream_ptr()), "hb_bn_eval_affine")
-    return stats
+    return stats, None
 
 
 def _bn_grad_targets(gammas: Sequence[Tensor], betas: Sequence[Tensor], c: int, dev):
@@ -705,7 +801,7 @@ class _BNActFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cfg, *tensors: Tensor) -> Tensor:
-        branches, act, slope, training, has_res, res_after, emit_stats = cfg
+        branches, act, slope, training, has_res, res_after, emit_stats, group = cfg
         nb = len(branches)
         us = [to_channels_last_bf16(t) for t in tensors[:nb]]
         gammas = tensors[nb:2 * nb]
@@ -717,10 +813,11 @@ class _BNActFn(torch.autograd.Function):
         m = n * h * w
         dev = us[0].device if nb else res.device
         c_log = gammas[0].numel() if nb else c   # parameters may be narrower than a zero-padded activation
-        stats = _bn_setup(us, branches, gammas, betas, training, c, c_log, m, dev)
+        stats, sums = _bn_setup(us, branches, gammas, betas, training, c, c_log, m, dev, group)
         out = _bn_forward_pass(us, stats, res, m, c, act, slope, int(res_after), (n, c, h, w), emit_stats)
         ctx.save_for_backward(stats, *us, *([res] if has_res else []), *gammas, *betas)
         ctx.cfg = (nb, act, slope, training, has_res, c_log, int(res_after))
+        ctx.sync = None if sums is None else (group, sums)
         return out
 
     @staticmethod
@@ -741,7 +838,8 @@ class _BNActFn(torch.autograd.Function):
         dus = [_empty_cl(n, c, h, w, dev) if need_u[i] else None for i in range(nb)]
         dres = _empty_cl(n, c, h, w, dev) if need_res else None
         gacc, bacc, dgb = _bn_grad_targets(gammas, betas, c, dev) if need_gb else (None, None, None)
-        _bn_backward_pass(dob, us, stats, res, dus, dres, dgb, gacc, bacc, c_log, m, c, act, slope, training, res_after)
+        _bn_backward_pass(dob, us, stats, res, dus, dres, dgb, gacc, bacc, c_log, m, c, act, slope, training, res_after,
+                          ctx.sync)
         grads: List[Optional[Tensor]] = [None]
         grads += dus
         grads += [dgb[0][i][:c_log] if dgb is not None else None for i in range(nb)]
@@ -756,7 +854,8 @@ def bn_act(us: Sequence[Tensor], bns: Sequence[nn.BatchNorm2d], act: int = ACT_N
            emit_stats: bool = False) -> Tensor:
     """act(sum_b BatchNorm_b(u_b) + residual) as one fused pass (training: the statistics come with the inputs from the
     kernels that produced them, see :func:`get_stats`); ``res_after_act`` moves the residual outside the activation:
-    act(sum_b ...) + residual. ``emit_stats``: the output carries its own statistics partials."""
+    act(sum_b ...) + residual. ``emit_stats``: the output carries its own statistics partials. ``bns`` may be
+    ``nn.SyncBatchNorm`` layers: their statistics are then shared over their process group (:func:`sync_group`)."""
     if not 1 <= len(us) <= 3 or len(us) != len(bns):
         raise ValueError("between 1 and 3 (input, BatchNorm2d) pairs are supported")
     require_cuda(*us)
@@ -764,7 +863,7 @@ def bn_act(us: Sequence[Tensor], bns: Sequence[nn.BatchNorm2d], act: int = ACT_N
         training = bns[0].training
     use_batch_stats = training or bns[0].running_mean is None
     cfg = ([BNBranch(b) for b in bns], int(act), float(slope), bool(use_batch_stats), residual is not None,
-           bool(res_after_act), bool(emit_stats))
+           bool(res_after_act), bool(emit_stats), sync_group(bns, training))
     args = list(us) + [b.weight for b in bns] + [b.bias for b in bns]
     if residual is not None:
         args.append(residual)
@@ -773,7 +872,7 @@ def bn_act(us: Sequence[Tensor], bns: Sequence[nn.BatchNorm2d], act: int = ACT_N
 
 def act_only(x: Tensor, act: int, slope: float = 0.0) -> Tensor:
     """Stand-alone activation through the fused pass (zero BN branches, x as the residual input)."""
-    cfg = ([], int(act), float(slope), False, True, False, False)
+    cfg = ([], int(act), float(slope), False, True, False, False, None)
     return _BNActFn.apply(cfg, x)
 
 
@@ -797,7 +896,7 @@ class _RepBlockFn(torch.autograd.Function):
 
     @staticmethod
     def forward(ctx, cfg, x: Tensor, w3: Tensor, w1: Tensor, *bn_params: Tensor) -> Tensor:
-        branches, act, slope, training, stride = cfg
+        branches, act, slope, training, stride, group = cfg
         nb = len(branches)
         gammas, betas = bn_params[:nb], bn_params[nb:]
         need_dx = ctx.needs_input_grad[1]
@@ -831,10 +930,11 @@ class _RepBlockFn(torch.autograd.Function):
         us = [y3, y1] + ([xb] if nb == 3 else [])
         n, c, h, w = y3.shape
         m = n * h * w
-        stats = _bn_setup(us, branches, gammas, betas, training, c, c, m, y3.device)
+        stats, sums = _bn_setup(us, branches, gammas, betas, training, c, c, m, y3.device, group)
         out = _bn_forward_pass(us, stats, None, m, c, act, slope, 0, (n, c, h, w), emit_stats=training)
         ctx.save_for_backward(stats, xb, y3, y1, w3, w1, *gammas, *betas)
         ctx.cfg = (nb, act, slope, training, stride, wd3, wd1, x.shape[1], stem)
+        ctx.sync = None if sums is None else (group, sums)
         return out
 
     @staticmethod
@@ -854,7 +954,7 @@ class _RepBlockFn(torch.autograd.Function):
         gacc, bacc, dgb = _bn_grad_targets(gammas, betas, c, dev)
         us = [y3, y1] + ([xb] if nb == 3 else [])
         _bn_backward_pass(dob, us, stats, None, [dy3, dy1] + ([dxid] if nb == 3 else []), None, dgb, gacc, bacc, c, m, c, act,
-                          slope, training, 0)
+                          slope, training, 0, ctx.sync)
         g_gamma = [None if dgb is None else dgb[0][i] for i in range(nb)]
         g_beta = [None if dgb is None else dgb[1][i] for i in range(nb)]
         dx = None
@@ -968,10 +1068,11 @@ def _stem_wgrad(col: Tensor, dyb: Tensor, weight: Tensor) -> Tensor:
 
 def repblock(x: Tensor, w3: Tensor, w1: Tensor, bns: Sequence[nn.BatchNorm2d], stride: int, act: int, slope: float,
              training: bool) -> Tensor:
-    """Fused train-form RepVGG block (see :class:`_RepBlockFn`). ``bns`` = [bn3, bn1] or [bn3, bn1, bn_identity]."""
+    """Fused train-form RepVGG block (see :class:`_RepBlockFn`). ``bns`` = [bn3, bn1] or [bn3, bn1, bn_identity], all
+    ``nn.BatchNorm2d`` or all ``nn.SyncBatchNorm`` (one statistics all-reduce for the three branches)."""
     require_cuda(x, w3, w1)
     use_batch_stats = training or bns[0].running_mean is None
-    cfg = ([BNBranch(b) for b in bns], int(act), float(slope), bool(use_batch_stats), int(stride))
+    cfg = ([BNBranch(b) for b in bns], int(act), float(slope), bool(use_batch_stats), int(stride), sync_group(bns, training))
     return _RepBlockFn.apply(cfg, x, w3, w1, *[b.weight for b in bns], *[b.bias for b in bns])
 
 

@@ -142,6 +142,17 @@ int hb_bn_finalize(const float* const* parts, const int* slots, const float* con
                    float* const* running_mean, float* const* running_var, long long* const* num_batches_tracked,
                    float* mean, float* rstd, float* scale, float* shift, int B, int C, int C_logical, int M, float eps,
                    float momentum, void* stream);
+/* Synchronised BatchNorm (nn.SyncBatchNorm), forward in two steps around a SUM all-reduce of `sums` over the ranks:
+ * hb_bn_partials_sums folds each branch's partial slots in hb_bn_finalize's fixed order into double sums[B][C][2]
+ * (sum, sum of squares; 0 on the padding channels) and writes the row count M as a double at sums[B*C*2] (B*C*2 + 1
+ * doubles). hb_bn_finalize_sums then writes what hb_bn_finalize writes, from the (all-reduced) sums and count: same
+ * arithmetic, the running variance unbiased over the summed count. Arguments as hb_bn_finalize. */
+int hb_bn_partials_sums(const float* const* parts, const int* slots, int B, int C, int C_logical, int M, double* sums,
+                        void* stream);
+int hb_bn_finalize_sums(const double* sums, const float* const* gamma, const float* const* beta,
+                        float* const* running_mean, float* const* running_var, long long* const* num_batches_tracked,
+                        float* mean, float* rstd, float* scale, float* shift, int B, int C, int C_logical, float eps,
+                        float momentum, void* stream);
 /* channels in [C_logical, C) are zero padding (the parameter arrays hold C_logical entries): scale = shift = 0 */
 int hb_bn_eval_affine(const float* gamma, const float* beta, const float* running_mean, const float* running_var,
                       float eps, int C, int C_logical, float* scale, float* shift, float* mean, float* rstd,
@@ -164,6 +175,19 @@ int hb_bn_act_bwd_bf16(const void* dout, const void* u0, const void* u1, const v
                        void* du0, void* du1, void* du2, void* dres, float* dgamma, float* dbeta,
                        float* const* gamma_grad_acc, float* const* beta_grad_acc, int C_logical, int M, int C, int act,
                        float slope, int train, int res_after, void* stream);
+/* hb_bn_act_bwd_bf16 (train = 1) in two steps around a SUM all-reduce of scratch[0 .. (1+B)*C) over the ranks of a
+ * synchronised BatchNorm. reduce: scratch[0][c] = sum dz, scratch[1+b][c] = sum dz*u_b over these M rows, and the LOCAL
+ * dgamma/dbeta written / added exactly as hb_bn_act_bwd_bf16 does. apply: du_b and dres from the (all-reduced) sums
+ * (scratch of the reduce step) over `count` rows (device double, e.g. hb_bn_partials_sums' count after its all-reduce). */
+int hb_bn_act_bwd_reduce_bf16(const void* dout, const void* u0, const void* u1, const void* u2, int B, const float* scale,
+                              const float* shift, const float* mean, const float* rstd, const void* residual,
+                              double* scratch, float* dgamma, float* dbeta, float* const* gamma_grad_acc,
+                              float* const* beta_grad_acc, int C_logical, int M, int C, int act, float slope, int res_after,
+                              void* stream);
+int hb_bn_act_bwd_apply_bf16(const void* dout, const void* u0, const void* u1, const void* u2, int B, const float* scale,
+                             const float* shift, const float* mean, const float* rstd, const void* residual,
+                             const double* sums, const double* count, void* du0, void* du1, void* du2, void* dres, int M,
+                             int C, int act, float slope, int res_after, void* stream);
 
 /* ---- depth-wise k x k convolution (NHWC bf16; weights fp32 [C,K,K]): FReLU's conv (activation.py:71-73) and the
  *      ReXNet depth-wise stage (holocron/models/classification/rexnet.py:112-125) -------------------------
