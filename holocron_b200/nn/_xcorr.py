@@ -29,26 +29,44 @@ def _single(v: Union[int, Tuple[int, int]], what: str) -> int:
     return int(v)
 
 
+def _out_size(h: int, w: int, kh: int, kw: int, stride: int, pad: int, dil: int) -> Tuple[int, int]:
+    """(Ho, Wo) of the sliding windows, refused with the errors of F.unfold, which the reference's forward calls."""
+    if stride <= 0:
+        raise RuntimeError(f"stride should be greater than zero, but got stride_height: {stride} stride_width: {stride}")
+    if dil <= 0:
+        raise RuntimeError(f"dilation should be greater than zero, but got dilation_height: {dil} dilation_width: {dil}")
+    if pad < 0:
+        raise RuntimeError(f"padding should be non-negative, but got pad_height: {pad} pad_width: {pad}")
+    span_h, span_w = h + 2 * pad - dil * (kh - 1) - 1, w + 2 * pad - dil * (kw - 1) - 1
+    if span_h < 0 or span_w < 0:
+        raise RuntimeError(f"Given input with spatial size ({h}, {w}), kernel_size=({kh}, {kw}), dilation=({dil}, {dil}), "
+                           f"padding=({pad}, {pad}), calculated shape of the array of sliding blocks as "
+                           f"({span_h // stride + 1}, {span_w // stride + 1}), but its components must be at least one.")
+    return span_h // stride + 1, span_w // stride + 1
+
+
 class _XcorrFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: Tensor, weight: Tensor, bias: Optional[Tensor], stride: int, pad: int, dil: int, mode: int,
                 normalize: bool, eps: float) -> Tensor:
-        require_cuda(x, weight)
         if x.ndim != 4 or weight.ndim != 4:
             raise ValueError("expected (N, C, H, W) input and (Cout, Cin, kh, kw) weight")
         n, cin, h, w = x.shape
         cout, cin_w, kh, kw = weight.shape
+        ho, wo = _out_size(h, w, kh, kw, stride, pad, dil)
+        require_cuda(x, weight)
         if cin_w != cin:
             # the reference ignores `groups`: a grouped weight makes its matmul fail with a shape error
             raise RuntimeError(f"weight expects {cin_w} input channels but the input has {cin} (groups are ignored)")
         x32 = x.detach().float().contiguous()
         w32 = weight.detach().float().contiguous()
         b32 = None if bias is None else bias.detach().float().contiguous()
-        ho = (h + 2 * pad - dil * (kh - 1) - 1) // stride + 1
-        wo = (w + 2 * pad - dil * (kw - 1) - 1) // stride + 1
         mean = torch.empty(n * ho * wo if normalize else 1, device=x.device, dtype=torch.float32)
         rstd = torch.empty_like(mean)
-        if mode == 0 and normalize and kh == kw and not os.environ.get("HB_NORMCONV_FP32"):
+        if n == 0:
+            # an empty batch has no windows (F.unfold gives an empty tensor); the kernels refuse an empty launch
+            out = torch.empty((0, cout, ho, wo), device=x.device, dtype=torch.float32)
+        elif mode == 0 and normalize and kh == kw and not os.environ.get("HB_NORMCONV_FP32"):
             out = _norm_conv_tensor_cores(x32, weight, b32, mean, rstd, stride, pad, dil, eps)
         else:
             out = torch.empty((n, cout, ho, wo), device=x.device, dtype=torch.float32)
@@ -74,13 +92,16 @@ class _XcorrFn(torch.autograd.Function):
                                    "reference (its in-place normalisation breaks autograd); only add2d without "
                                    "normalize_slices propagates to the input")
             dx = torch.empty_like(x32)
-            check(L.hb_add2d_dgrad(ptr(x32), ptr(w32), ptr(g), ptr(dx), n, cin, h, w, cout, kh, kw, stride, pad, dil,
-                                   stream_ptr()), "hb_add2d_dgrad")
+            if n:
+                check(L.hb_add2d_dgrad(ptr(x32), ptr(w32), ptr(g), ptr(dx), n, cin, h, w, cout, kh, kw, stride, pad, dil,
+                                       stream_ptr()), "hb_add2d_dgrad")
             dx = dx.to(xdt)
         if ctx.needs_input_grad[1]:
-            dw = torch.empty_like(w32)
-            check(L.hb_xcorr2d_wgrad(ptr(x32), ptr(w32), ptr(g), ptr(mean), ptr(rstd), ptr(dw), n, cin, h, w, cout, kh, kw,
-                                     stride, pad, dil, mode, int(normalize), _cf(eps), stream_ptr()), "hb_xcorr2d_wgrad")
+            dw = torch.empty_like(w32) if n else torch.zeros_like(w32)    # the launcher zeroes dw itself
+            if n:
+                check(L.hb_xcorr2d_wgrad(ptr(x32), ptr(w32), ptr(g), ptr(mean), ptr(rstd), ptr(dw), n, cin, h, w, cout, kh,
+                                         kw, stride, pad, dil, mode, int(normalize), _cf(eps), stream_ptr()),
+                      "hb_xcorr2d_wgrad")
             dw = dw.to(wdt)
         if has_bias and ctx.needs_input_grad[2]:
             db = g.sum((0, 2, 3))
