@@ -136,6 +136,7 @@ SIGNATURES = {
     "hb_lars_step": "ppii" + "ffff" + "ii" + "pp",
     "hb_ralars_step": "ppii" + "fffffff" + "ifi" + "pp",
     "hb_lookahead_sync": "ppi" + "f" + "p",
+    "hb_resample_batch": "p" + "i" * 8 + "p",
 }
 _CTYPE = {"p": ctypes.c_void_p, "i": ctypes.c_int, "z": ctypes.c_size_t, "f": ctypes.c_float, "q": ctypes.c_longlong}
 

@@ -1,0 +1,127 @@
+"""Host side of the batched resampling kernel (holocron_b200/csrc/resample.cu, ``hb_resample_batch``).
+
+``resample`` takes a batch of images, each with the inner size it is resized to and the signed offset of that inner box
+on a common canvas, validates what torchvision would refuse before anything is launched, writes one descriptor row per
+image into pinned host memory, uploads the table asynchronously (no host synchronisation) and launches one kernel that
+resizes every image and fills its canvas."""
+import math
+from typing import List, Optional, Sequence, Tuple
+
+import numpy as np
+import torch
+from torch import Tensor
+from torchvision.transforms.functional import InterpolationMode
+
+from .._lib import check, lib, require_cuda, stream_ptr
+
+# interpolation modes torchvision's tensor resize accepts, as the kernel's filter codes
+FILTERS = {InterpolationMode.NEAREST: 0, InterpolationMode.NEAREST_EXACT: 1, InterpolationMode.BILINEAR: 2,
+           InterpolationMode.BICUBIC: 3}
+PAD_MODES = {"constant": 0, "edge": 1, "reflect": 2, "symmetric": 3}
+DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2, torch.uint8: 3, torch.float64: 4}
+# Taps per axis that fit the kernel's shared-memory weight tables for every dtype: antialiased downscales up to about
+# 1/127 (bilinear) or 1/63 (bicubic).
+MAX_TAPS = 255
+_DESC_WORDS = 16
+_INT32_MAX = 2 ** 31 - 1
+
+
+def axis_taps(n_in: int, n_out: int, filter_code: int, antialias: bool, dtype: torch.dtype) -> int:
+    """The most taps a filter from n_in to n_out samples has along one axis, computed as the kernel computes its
+    support (in fp32, fp64 for fp64 images)."""
+    if filter_code < 2:
+        return 1
+    if not antialias:
+        return 2 if filter_code == 2 else 4
+    acc = np.float64 if dtype == torch.float64 else np.float32
+    scale = acc(n_in) / acc(n_out)
+    half = 1.0 if filter_code == 2 else 2.0
+    support = acc(half * float(scale)) if scale >= 1 else acc(half)
+    return int(math.ceil(support)) * 2 + 1
+
+
+def interpolation_code(interpolation) -> int:
+    """The kernel's filter for a torchvision interpolation, refusing what torchvision refuses for tensors."""
+    if not isinstance(interpolation, InterpolationMode):
+        raise TypeError("Argument interpolation should be a InterpolationMode or a corresponding Pillow integer constant")
+    if interpolation not in FILTERS:
+        raise NotImplementedError(f"interpolation {interpolation.value!r} is not supported for tensors "
+                                  f"(supported: {', '.join(m.value for m in FILTERS)})")
+    return FILTERS[interpolation]
+
+
+def _check_padding(pad_mode: str, pads: Tuple[int, int, int, int], h: int, w: int) -> None:
+    """pads = (left, top, right, bottom). torch's reflection pad refuses a padding >= the side it mirrors; torchvision's
+    symmetric pad indexes past the image for a padding > the side (IndexError on CPU tensors)."""
+    left, top, right, bottom = pads
+    if pad_mode == "reflect" and (max(left, right) >= w or max(top, bottom) >= h):
+        raise RuntimeError(f"Padding size should be less than the corresponding input dimension, but got: padding "
+                           f"({left}, {right}) at dimension 2 and ({top}, {bottom}) at dimension 1 of an image of "
+                           f"{h}x{w}")
+    if pad_mode == "symmetric" and (max(left, right) > w or max(top, bottom) > h):
+        raise IndexError(f"symmetric padding ({left}, {top}, {right}, {bottom}) exceeds the image size {h}x{w}")
+
+
+def descriptor_table(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]], canvas: Tuple[int, int],
+                     filter_code: int, antialias: bool, pad_mode: str) -> Tuple[np.ndarray, int, int]:
+    """(table, taps_y, taps_x): the int64 [N_total, 16] descriptor rows of hb_resample_batch, destination pointers left
+    at 0, and the most filter taps per axis. Raises what torchvision would raise for these placements."""
+    ref = sources[0]
+    C = ref.shape[-3]
+    Hc, Wc = canvas
+    rows: List[List[int]] = []
+    taps_y = taps_x = 1
+    for x, (h, w) in zip(sources, inner):
+        if x.dtype != ref.dtype or x.device != ref.device or x.ndim < 3 or x.shape[-3] != C:
+            raise ValueError("images of one call must share their dtype, device and channel count")
+        H, W = x.shape[-2:]
+        if h <= 0 or w <= 0 or H <= 0 or W <= 0:
+            raise RuntimeError(f"Input and output sizes should be greater than 0, but got input (H: {H}, W: {W}) "
+                               f"output (H: {h}, W: {w})")
+        dh, dw = Hc - h, Wc - w
+        top, left = dh // 2, dw // 2
+        _check_padding(pad_mode, (left, top, dw - left, dh - top), h, w)
+        sc, sh, sw = x.stride()[-3:]
+        if (W - 1) * sw > _INT32_MAX:
+            raise ValueError("image rows span more than 2**31 elements")
+        row = [x.data_ptr(), 0, sc, sh, sw, C, H, W, h, w, top, left, Hc, Wc, PAD_MODES[pad_mode], 0]
+        # leading dimensions of a source are images of their own
+        offsets = [0]
+        for n_k, s_k in zip(x.shape[:-3], x.stride()[:-3]):
+            offsets = [o + k * s_k for o in offsets for k in range(n_k)]
+        for o in offsets:
+            rows.append([row[0] + o * x.element_size()] + row[1:])
+        taps_y = max(taps_y, axis_taps(H, h, filter_code, antialias, x.dtype))
+        taps_x = max(taps_x, axis_taps(W, w, filter_code, antialias, x.dtype))
+    if max(taps_y, taps_x) > MAX_TAPS:
+        raise NotImplementedError(f"resampling needs {max(taps_y, taps_x)} filter taps per axis (at most {MAX_TAPS}: "
+                                  "downscale in two steps)")
+    return np.array(rows, dtype=np.int64), taps_y, taps_x
+
+
+def resample(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]], canvas: Tuple[int, int],
+             interpolation: InterpolationMode, antialias: bool, pad_mode: str = "constant",
+             out: Optional[Tensor] = None) -> Tensor:
+    """Resizes sources[i] ([..., C, H_i, W_i], CUDA, any strides) to inner[i] = (h_i, w_i) and centres it on a canvas
+    of ``canvas`` = (Hc, Wc) the way torchvision's ``pad`` places it (left / top padding = floor(delta / 2), negative
+    padding crops), filling the rest by ``pad_mode``. Returns ``out``, a contiguous tensor of shape
+    (N_total, C, Hc, Wc) holding one canvas per source image (leading dimensions of a source count as images)."""
+    if pad_mode not in PAD_MODES:
+        raise ValueError("Padding mode should be either constant, edge, reflect or symmetric")
+    filter_code = interpolation_code(interpolation)
+    antialias = bool(antialias) and filter_code >= 2
+    ref = sources[0]
+    require_cuda(*sources)
+    if ref.dtype not in DTYPES:
+        raise TypeError(f"unsupported dtype {ref.dtype}: expected one of {', '.join(map(str, DTYPES))}")
+    table, taps_y, taps_x = descriptor_table(sources, inner, canvas, filter_code, antialias, pad_mode)
+    n, C, (Hc, Wc) = table.shape[0], ref.shape[-3], canvas
+    if out is None:
+        out = torch.empty((n, C, Hc, Wc), dtype=ref.dtype, device=ref.device)
+    if out.shape != (n, C, Hc, Wc) or not out.is_contiguous() or out.dtype != ref.dtype or out.device != ref.device:
+        raise ValueError(f"out must be a contiguous {ref.dtype} tensor of shape {(n, C, Hc, Wc)} on {ref.device}")
+    table[:, 1] = out.data_ptr() + np.arange(n, dtype=np.int64) * (C * Hc * Wc * out.element_size())
+    descs = torch.from_numpy(table).pin_memory().to(ref.device, non_blocking=True)
+    check(lib().hb_resample_batch(descs.data_ptr(), n, Hc, Wc, filter_code, int(antialias), taps_y, taps_x,
+                                  DTYPES[ref.dtype], stream_ptr()), "hb_resample_batch")
+    return out

@@ -471,6 +471,20 @@ int hb_train_ctl_tick(void* ctl, void* stream);
 int hb_grad_clip_partials_max(void);
 int hb_grad_clip_norm(float* grads, long long n, float max_norm, double* scratch, void* ctl, void* stream);
 
+/* ---- transforms: holocron/transforms/interpolation.py:87-96 (Resize.forward: torchvision resize, then pad),
+ *      :144-156 (RandomZoomOut.forward: resize, then constant pad) - a batch of images in one launch -------------- */
+/* descs: device table of N rows of 16 int64 {src, dst, stride_c, stride_h, stride_w, C, H, W, h, w, top, left, Hc, Wc,
+ * pad_mode, 0}: pointers are addresses, strides count elements. Image n is read in place from the strided src [C][H][W], resampled
+ * to h x w, placed with its top-left corner at the signed offset (top, left) of the contiguous canvas dst [C][Hc][Wc]
+ * and the rest of the canvas filled by pad_mode (0 constant zero, 1 edge, 2 reflect: padding < side, 3 symmetric:
+ * padding <= side); box pixels outside the canvas are dropped. filter: 0 nearest, 1 nearest-exact, 2 bilinear,
+ * 3 bicubic (align_corners=False); antialias applies to 2 and 3. taps_y / taps_x: the most taps a row / column filter
+ * of the batch has (1, 2 or 4 without antialias, 2*ceil(support)+1 with it). canvas_h / canvas_w: the largest canvas
+ * of the batch. dtype: 0..2 as above, 3 = uint8, 4 = float64 (uint8 / fp16 / bf16 interpolate in fp32, float64 in
+ * fp64; uint8 results are clamped to [0, 255] and rounded half to even). */
+int hb_resample_batch(const void* descs, int N, int canvas_h, int canvas_w, int filter, int antialias, int taps_y,
+                      int taps_x, int dtype, void* stream);
+
 /* ---- bookkeeping (not part of the reference surface) ------------------------------------------------ */
 long long hb_launch_count(void);      /* kernels launched through this library since the last reset */
 void hb_launch_count_reset(void);
