@@ -10,6 +10,8 @@
 // recomputes the softmax and writes dlogits in one more pass.
 //   S == 1 : one warp per position, lanes stride over the K classes (coalesced rows)
 //   S  > 1 : one thread per position, consecutive threads = consecutive s (coalesced for every class k)
+#include <type_traits>
+
 #include "common.cuh"
 
 namespace {
@@ -20,25 +22,130 @@ constexpr int kThreads = 256;
 
 enum LossKind { FOCAL = 0, POLY = 1 };
 
+// The arguments of the class-axis kernels (focal / poly-1 with hard or soft targets, complement cross entropy).
 struct LossParams {
   const void* x;            // [N, K, S]
-  const long long* target;  // [N, S] hard targets (int64)         (hard)
-  const void* soft;         // [N, K, S] soft targets, same dtype  (soft)
+  const long long* target;  // [N, S] class indices (int64)          (hard targets, complement CE)
+  const void* soft;         // [N, K, S] soft targets, same dtype    (soft targets)
   const float* weight;      // [K] or null
-  float* loss_pos;          // [N*S] per-position loss
-  double* partials;         // [grid][2]: sum of valid losses, number of valid positions
+  float* loss_pos;          // forward: [N*S] per-position loss
+  double* partials;         // forward: [grid][2 or 3] per-block partial sums (see finalize_kernel)
+  const float* gout;        // backward: reduction none: [N*S]; else 1 element
+  const float* fwd_out;     // backward: {sum, count, mean} of the forward (count used for 'mean')
+  void* dx;                 // backward: [N, K, S]
   int N, K, S;
-  int ignore_index;         // honoured only when 0 <= ignore_index < K (reference quirk)
-  int kind;
-  float gamma, eps;
+  int ignore_index;         // class column: honoured only when 0 <= ignore_index < K (reference quirk)
+  int kind;                 // LossKind (hard targets)
+  int reduction;            // backward: 0 none, 1 mean, 2 sum
+  float gamma;              // focal exponent / complement-term weight
+  float eps;                // poly-1 epsilon
 };
 
-template <typename T, typename Acc>
-__device__ __forceinline__ float lse_thread(Acc x_at, int K) {
+// The gradient scale of one position's term: gout[pos] for 'none', gout[0] for 'sum' and gout[0] / den for 'mean', where
+// den is the forward's count *count for a term averaged over its counted positions, or the number of positions P when
+// count is null. `reduced` is the 'mean' / 'sum' value, the same for every position.
+struct GradScale {
+  const float* gout;
+  int reduction;
+  float reduced;
+  // `dropped`: a position left out of the count gets no share of a 'mean' / 'sum' gradient
+  __device__ __forceinline__ float at(long long pos, bool dropped = false) const {
+    return reduction == 0 ? gout[pos] : (dropped ? 0.f : reduced);
+  }
+};
+__device__ __forceinline__ GradScale grad_scale(const float* gout, int reduction, const float* count, long long P) {
+  const float reduced = reduction == 0 ? 0.f : (reduction == 1 ? gout[0] / (count ? *count : (float)P) : gout[0]);
+  return {gout, reduction, reduced};
+}
+
+// Block-wide sums of this thread's partials, stored as partials[NP * block + i] (NP = number of values), which
+// finalize_kernel folds in block order.
+template <class... D>
+__device__ __forceinline__ void store_partials(double* partials, double* red, D... v) {
+  constexpr int NP = sizeof...(D);
+  const double s[NP] = {block_sum<double>(v, red)...};
+  if (threadIdx.x == 0) {
+#pragma unroll
+    for (int i = 0; i < NP; ++i) partials[NP * blockIdx.x + i] = s[i];
+  }
+}
+
+// grid-stride iterations of the thread that starts at item i0 < stride: the soft-target kernels count their positions
+// from it after the loop, so the count needs no accumulator while the loop runs
+__device__ __forceinline__ double thread_iters(long long i0, long long total, long long stride) {
+  return i0 < total ? (double)((total - 1 - i0) / stride + 1) : 0.0;
+}
+
+// partials [n][NP] = {A, B, C} (NP = 3) or {A, B} (NP = 2, C = 0): A is the (weighted) sum of the per-position terms
+// counted by B; C a second term averaged over all P positions. out = {A + coef * C, B, A / B + coef * C / P} (with
+// C = 0: {A, B, A / B}), each summed in block order. One warp: lane u loads block i0 + u (32 blocks per round trip to L2)
+// and the sums take the blocks in order through shuffles.
+template <int NP>
+__global__ void finalize_kernel(const double* partials, int n, double P, float coef, float* out) {
+  const int lane = threadIdx.x & 31;
+  double s[3] = {0.0, 0.0, 0.0};
+  for (int i0 = 0; i0 < n; i0 += 32) {
+    double v[NP];
+#pragma unroll
+    for (int j = 0; j < NP; ++j) v[j] = i0 + lane < n ? partials[NP * (i0 + lane) + j] : 0.0;
+    const int m = n - i0 < 32 ? n - i0 : 32;
+    for (int u = 0; u < m; ++u) {
+#pragma unroll
+      for (int j = 0; j < NP; ++j) s[j] += __shfl_sync(0xffffffffu, v[j], u);
+    }
+  }
+  if (lane == 0) {
+    out[0] = (float)(s[0] + (double)coef * s[2]);
+    out[1] = (float)s[1];
+    out[2] = (float)(s[0] / s[1] + (double)coef * s[2] / P);
+  }
+}
+
+// k-loop shapes: one thread owns a position (S > 1) or a warp does, its lanes striding over the classes (S == 1)
+struct ThreadLanes {
+  static constexpr int kStep = 1;
+  int k0 = 0;
+  __device__ float max(float v) const { return v; }
+  __device__ float sum(float v) const { return v; }
+};
+struct WarpLanes {
+  static constexpr int kStep = 32;
+  int k0;
+  __device__ float max(float v) const { return warp_max(v); }
+  __device__ float sum(float v) const { return warp_sum(v); }
+};
+
+// Calls f(ln, xp, dp, st, pos) for each of this thread's positions: xp / dp point at the position's class 0 in x / dx and
+// st is the class stride. S == 1: a warp per position (WarpLanes over a contiguous row); S > 1: a thread per position.
+template <typename T, class F>
+__device__ __forceinline__ void for_each_position(const LossParams& p, F f) {
+  const T* x = (const T*)p.x;
+  T* dx = (T*)p.dx;
+  const long long P = (long long)p.N * p.S;
+  if (p.S == 1) {
+    const WarpLanes ln{threadIdx.x & 31};
+    const long long warps = (long long)gridDim.x * (kThreads / 32);
+    for (long long pos = (long long)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); pos < P; pos += warps)
+      f(ln, x + pos * p.K, dx + pos * p.K, 1LL, pos);
+  } else {
+    const ThreadLanes ln{};
+    const long long stride = (long long)gridDim.x * kThreads;
+    for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
+      const long long off = (pos / p.S) * p.K * p.S + pos % p.S;
+      f(ln, x + off, dx + off, (long long)p.S, pos);
+    }
+  }
+}
+
+// log sum_k exp(x_k) of one position, x_at(k) being class k
+template <class Ln, class X>
+__device__ __forceinline__ float lane_lse(const Ln& ln, X x_at, int K) {
   float mx = -INFINITY;
-  for (int k = 0; k < K; ++k) mx = fmaxf(mx, x_at(k));
+  for (int k = ln.k0; k < K; k += Ln::kStep) mx = fmaxf(mx, x_at(k));
+  mx = ln.max(mx);
   float s = 0.f;
-  for (int k = 0; k < K; ++k) s += expf(x_at(k) - mx);
+  for (int k = ln.k0; k < K; k += Ln::kStep) s += expf(x_at(k) - mx);
+  s = ln.sum(s);
   return mx + logf(s);
 }
 
@@ -70,141 +177,61 @@ __device__ __forceinline__ float hard_dloss(const LossParams& p, float logpt, fl
   return w * (-1.f - p.eps * pt);
 }
 
-// ---- hard targets, forward ------------------------------------------------------------------------
-template <typename T>
-__global__ void __launch_bounds__(kThreads) hard_fwd_kernel(LossParams p) {
-  __shared__ double red[32];
-  const T* x = (const T*)p.x;
-  const long long P = (long long)p.N * p.S;
-  double lsum = 0.0, lcnt = 0.0;
-  const bool ign = p.ignore_index >= 0 && p.ignore_index < p.K;
-  if (p.S == 1) {
-    const int lane = threadIdx.x & 31;
-    const long long warps = (long long)gridDim.x * (kThreads / 32);
-    for (long long pos = (long long)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); pos < P; pos += warps) {
-      const T* row = x + pos * p.K;
-      float mx = -INFINITY;
-      for (int k = lane; k < p.K; k += 32) mx = fmaxf(mx, to_f(row[k]));
-      mx = warp_max(mx);
-      float s = 0.f;
-      for (int k = lane; k < p.K; k += 32) s += expf(to_f(row[k]) - mx);
-      s = warp_sum(s);
-      if (lane == 0) {
-        const long long t = p.target[pos];
-        float l = NAN;
-        if (t >= 0 && t < p.K) {
-          const float logpt = to_f(row[t]) - (mx + logf(s));
-          l = hard_loss(p, logpt, p.weight ? p.weight[t] : 1.f);
-        }
-        p.loss_pos[pos] = l;
-        if (!(ign && t == p.ignore_index)) { lsum += l; lcnt += 1.0; }
-      }
-    }
-  } else {
-    const long long stride = (long long)gridDim.x * kThreads;
-    for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
-      const long long n = pos / p.S, s = pos % p.S;
-      const T* base = x + n * p.K * p.S + s;
-      auto x_at = [&](int k) { return to_f(base[(long long)k * p.S]); };
-      const float lse = lse_thread<T>(x_at, p.K);
-      const long long t = p.target[pos];
-      float l = NAN;
-      if (t >= 0 && t < p.K) l = hard_loss(p, x_at((int)t) - lse, p.weight ? p.weight[t] : 1.f);
+// ---- hard targets ---------------------------------------------------------------------------------
+template <typename T, bool kBackward, class Ln>
+__device__ __forceinline__ void hard_position(const LossParams& p, const Ln& ln, const T* xp, T* dp, long long st,
+                                              long long pos, double& lsum, double& lcnt) {
+  auto x_at = [&](int k) { return to_f(xp[k * st]); };
+  const float lse = lane_lse(ln, x_at, p.K);
+  const long long t = p.target[pos];
+  const bool inr = t >= 0 && t < p.K;
+  const bool skip = p.ignore_index >= 0 && p.ignore_index < p.K && t == p.ignore_index;
+  if (!kBackward) {
+    float l = NAN;
+    if (inr) l = hard_loss(p, x_at((int)t) - lse, p.weight ? p.weight[t] : 1.f);
+    if (ln.k0 == 0) {
       p.loss_pos[pos] = l;
-      if (!(ign && t == p.ignore_index)) { lsum += l; lcnt += 1.0; }
-    }
-  }
-  lsum = block_sum<double>(lsum, red);
-  lcnt = block_sum<double>(lcnt, red);
-  if (threadIdx.x == 0) { p.partials[2 * blockIdx.x] = lsum; p.partials[2 * blockIdx.x + 1] = lcnt; }
-}
-
-// out[0] = sum, out[1] = count, out[2] = mean  (fixed summation order)
-__global__ void finalize_kernel(const double* partials, int n, float* out) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    double s = 0.0, c = 0.0;
-    for (int i = 0; i < n; ++i) { s += partials[2 * i]; c += partials[2 * i + 1]; }
-    out[0] = (float)s;
-    out[1] = (float)c;
-    out[2] = (float)(s / c);
-  }
-}
-
-// ---- hard targets, backward -----------------------------------------------------------------------
-struct LossBwdParams {
-  LossParams f;
-  const float* gout;    // reduction none: [N*S]; else 1 element
-  const float* fwd_out; // {sum, count, mean} from the forward (count used for 'mean')
-  void* dx;             // [N, K, S]
-  int reduction;        // 0 none, 1 mean, 2 sum
-};
-
-template <typename T>
-__global__ void __launch_bounds__(kThreads) hard_bwd_kernel(LossBwdParams b) {
-  const LossParams& p = b.f;
-  const T* x = (const T*)p.x;
-  T* dx = (T*)b.dx;
-  const long long P = (long long)p.N * p.S;
-  const bool ign = p.ignore_index >= 0 && p.ignore_index < p.K;
-  const float gscale = b.reduction == 1 ? b.gout[0] / b.fwd_out[1] : (b.reduction == 2 ? b.gout[0] : 0.f);
-  if (p.S == 1) {
-    const int lane = threadIdx.x & 31;
-    const long long warps = (long long)gridDim.x * (kThreads / 32);
-    for (long long pos = (long long)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); pos < P; pos += warps) {
-      const T* row = x + pos * p.K;
-      float mx = -INFINITY;
-      for (int k = lane; k < p.K; k += 32) mx = fmaxf(mx, to_f(row[k]));
-      mx = warp_max(mx);
-      float s = 0.f;
-      for (int k = lane; k < p.K; k += 32) s += expf(to_f(row[k]) - mx);
-      s = warp_sum(s);
-      const float lse = mx + logf(s);
-      const long long t = p.target[pos];
-      float g = b.reduction == 0 ? b.gout[pos] : ((ign && t == p.ignore_index) ? 0.f : gscale);
-      float c = 0.f;
-      if (t >= 0 && t < p.K) c = g * hard_dloss(p, to_f(row[t]) - lse, p.weight ? p.weight[t] : 1.f);
-      for (int k = lane; k < p.K; k += 32) {
-        const float pk = expf(to_f(row[k]) - lse);
-        dx[pos * p.K + k] = from_f<T>(c * ((k == t ? 1.f : 0.f) - pk));
-      }
+      if (!skip) { lsum += l; lcnt += 1.0; }
     }
   } else {
-    const long long stride = (long long)gridDim.x * kThreads;
-    for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
-      const long long n = pos / p.S, s = pos % p.S;
-      const long long off = n * p.K * p.S + s;
-      auto x_at = [&](int k) { return to_f(x[off + (long long)k * p.S]); };
-      const float lse = lse_thread<T>(x_at, p.K);
-      const long long t = p.target[pos];
-      float g = b.reduction == 0 ? b.gout[pos] : ((ign && t == p.ignore_index) ? 0.f : gscale);
-      float c = 0.f;
-      if (t >= 0 && t < p.K) c = g * hard_dloss(p, x_at((int)t) - lse, p.weight ? p.weight[t] : 1.f);
-      for (int k = 0; k < p.K; ++k) {
-        const float pk = expf(x_at(k) - lse);
-        dx[off + (long long)k * p.S] = from_f<T>(c * ((k == t ? 1.f : 0.f) - pk));
-      }
+    float c = 0.f;
+    if (inr) c = grad_scale(p.gout, p.reduction, p.fwd_out + 1, 0).at(pos, skip) * hard_dloss(p, x_at((int)t) - lse, p.weight ? p.weight[t] : 1.f);
+    for (int k = ln.k0; k < p.K; k += Ln::kStep) {
+      const float pk = expf(x_at(k) - lse);
+      dp[k * st] = from_f<T>(c * ((k == t ? 1.f : 0.f) - pk));
     }
   }
+}
+
+template <typename T, bool kBackward>
+__global__ void __launch_bounds__(kThreads) hard_kernel(LossParams p) {
+  __shared__ double red[32];
+  double lsum = 0.0, lcnt = 0.0;
+  for_each_position<T>(p, [&](const auto& ln, const T* xp, T* dp, long long st, long long pos) {
+    hard_position<T, kBackward>(p, ln, xp, dp, st, pos, lsum, lcnt);
+  });
+  if (!kBackward) store_partials(p.partials, red, lsum, lcnt);
 }
 
 // ---- poly loss with soft targets ------------------------------------------------------------------
 // per position: L = sum_{k valid} w_k * (-z_k + eps * (1 - exp(z_k))),  z_k = log_softmax(x)_k * t_k
+// One thread per position at every S. The second partial counts the positions, so the finalize gives {sum, P, sum / P}.
 template <typename T, bool kBackward>
-__global__ void __launch_bounds__(kThreads) poly_soft_kernel(LossBwdParams b) {
+__global__ void __launch_bounds__(kThreads) poly_soft_kernel(LossParams p) {
   __shared__ double red[32];
-  const LossParams& p = b.f;
   const T* x = (const T*)p.x;
   const T* tg = (const T*)p.soft;
-  T* dx = (T*)b.dx;
+  T* dx = (T*)p.dx;
   const long long P = (long long)p.N * p.S;
   const bool ign = p.ignore_index >= 0 && p.ignore_index < p.K;
   double lsum = 0.0;
-  const long long stride = (long long)gridDim.x * kThreads;
-  for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
+  const ThreadLanes ln{};
+  const long long stride = (long long)gridDim.x * kThreads, pos0 = (long long)blockIdx.x * kThreads + threadIdx.x;
+  for (long long pos = pos0; pos < P; pos += stride) {
     const long long n = pos / p.S, s = pos % p.S;
     const long long off = n * p.K * p.S + s;
     auto x_at = [&](int k) { return to_f(x[off + (long long)k * p.S]); };
-    const float lse = lse_thread<T>(x_at, p.K);
+    const float lse = lane_lse(ln, x_at, p.K);
     if (!kBackward) {
       float l = 0.f;
       for (int k = 0; k < p.K; ++k) {
@@ -215,7 +242,7 @@ __global__ void __launch_bounds__(kThreads) poly_soft_kernel(LossBwdParams b) {
       p.loss_pos[pos] = l;
       lsum += l;
     } else {
-      const float g = b.reduction == 0 ? b.gout[pos] : (b.reduction == 1 ? b.gout[0] / (float)P : b.gout[0]);
+      const float g = grad_scale(p.gout, p.reduction, nullptr, P).at(pos);
       // dL/dx_j = c_j t_j - p_j * sum_k c_k t_k,   c_k = w_k * valid_k * (-1 - eps * exp(z_k))
       float tot = 0.f;
       for (int k = 0; k < p.K; ++k) {
@@ -235,20 +262,7 @@ __global__ void __launch_bounds__(kThreads) poly_soft_kernel(LossBwdParams b) {
       }
     }
   }
-  if (!kBackward) {
-    lsum = block_sum<double>(lsum, red);
-    if (threadIdx.x == 0) { p.partials[2 * blockIdx.x] = lsum; p.partials[2 * blockIdx.x + 1] = 0.0; }
-  }
-}
-
-__global__ void finalize_soft_kernel(const double* partials, int n, double P, float* out) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    double s = 0.0;
-    for (int i = 0; i < n; ++i) s += partials[2 * i];
-    out[0] = (float)s;
-    out[1] = (float)P;
-    out[2] = (float)(s / P);
-  }
+  if (!kBackward) store_partials(p.partials, red, lsum, thread_iters(pos0, P, stride));
 }
 
 int grid_for(long long work, int per_block) {
@@ -299,41 +313,74 @@ template <typename T> __device__ __forceinline__ void st8(T* p, const Vec8<T>& v
 // scalar kernels): 32-bit class stride (K * S < 2^31 checked by the launcher) so a class column is one IMAD.WIDE away, int
 // targets (one ISETP per logit instead of two), and MUFU.EX2 (exp_mufu) for the per-logit exponentials - arguments are <= 0,
 // where its error is ~2 ulp on the terms that matter; the per-position logf / expf / powf stay IEEE.
+
+// The front end of both register-column kernels: the KMAX class columns of the logits at xk (-inf beyond K) into r and,
+// with kSoft, of the soft targets at qk (0 beyond K) into q.
+template <typename T, int KMAX, bool kSoft>
+__device__ __forceinline__ void load_columns(Vec8<T> (&r)[KMAX], Vec8<T>* q, const T* xk, const T* qk, int K,
+                                             unsigned S) {
+  constexpr int V = Vec8<T>::N;
+  // classes k >= K hold -inf: the compute loops run unpredicated over KMAX (exp(-inf) = 0, never the max or the
+  // target); two dozen `k < K` predicates kept live across the body made ptxas shuffle them through P2R / R2P
+#pragma unroll
+  for (int k = 0; k < KMAX; ++k) {
+    if (k < K) {
+      r[k] = ld8(xk);
+      if constexpr (kSoft) q[k] = ld8(qk);
+    } else {
+#pragma unroll
+      for (int v = 0; v < V; ++v) {
+        r[k].v[v] = neg_inf<T>();
+        if constexpr (kSoft) q[k].v[v] = from_f<T>(0.f);
+      }
+    }
+    xk += S;
+    if constexpr (kSoft) qk += S;
+  }
+}
+
+// each position's max and sum of exp(x - max) over the columns; visit(k, v, x) sees every logit of the max pass
+template <typename T, int KMAX, class Visit>
+__device__ __forceinline__ void max_sumexp(const Vec8<T> (&r)[KMAX], float (&mx)[Vec8<T>::N], float (&sum)[Vec8<T>::N],
+                                           Visit visit) {
+  constexpr int V = Vec8<T>::N;
+#pragma unroll
+  for (int v = 0; v < V; ++v) { mx[v] = -INFINITY; sum[v] = 0.f; }
+#pragma unroll
+  for (int k = 0; k < KMAX; ++k) {
+#pragma unroll
+    for (int v = 0; v < V; ++v) {
+      const float f = to_f(r[k].v[v]);
+      mx[v] = fmaxf(mx[v], f);
+      visit(k, v, f);
+    }
+  }
+#pragma unroll
+  for (int k = 0; k < KMAX; ++k) {
+#pragma unroll
+    for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), mx[v]);
+  }
+}
+
 template <typename T, int KMAX, bool kBackward>
-__global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossBwdParams b) {
+__global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossParams p) {
   constexpr int V = Vec8<T>::N;
   __shared__ double red[32];
-  const LossParams& p = b.f;
   const T* x = (const T*)p.x;
-  T* dx = (T*)b.dx;
+  T* dx = (T*)p.dx;
   const int K = p.K;
   const unsigned S = (unsigned)p.S, SV = S / V;
   const long long PV = (long long)p.N * SV;
   const bool ign = p.ignore_index >= 0 && p.ignore_index < K;
-  float gscale = 0.f;
-  if (kBackward) gscale = b.reduction == 1 ? b.gout[0] / b.fwd_out[1] : (b.reduction == 2 ? b.gout[0] : 0.f);
+  GradScale gs{};
+  if (kBackward) gs = grad_scale(p.gout, p.reduction, p.fwd_out + 1, 0);
   double lsum = 0.0, lcnt = 0.0;
   const long long stride = (long long)gridDim.x * kThreads;
   for (long long pv = (long long)blockIdx.x * kThreads + threadIdx.x; pv < PV; pv += stride) {
     const long long n = pv / SV;
     const unsigned s0 = (unsigned)(pv - n * SV) * V;
-    const T* xp = x + n * K * S + s0;
-    // classes k >= K hold -inf: the compute loops below run unpredicated over KMAX (exp(-inf) = 0, never the max or the
-    // target); two dozen `k < K` predicates kept live across the body made ptxas shuffle them through P2R / R2P
     Vec8<T> r[KMAX];
-    {
-      const T* pk = xp;
-#pragma unroll
-      for (int k = 0; k < KMAX; ++k) {
-        if (k < K) {
-          r[k] = ld8(pk);
-        } else {
-#pragma unroll
-          for (int v = 0; v < V; ++v) r[k].v[v] = neg_inf<T>();
-        }
-        pk += S;
-      }
-    }
+    load_columns<T, KMAX, false>(r, nullptr, x + n * K * S + s0, nullptr, K, S);
     int t[V];       // class index, -1 when outside [0, K)
     bool skip[V];   // ignored position
 #pragma unroll
@@ -344,21 +391,8 @@ __global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossBwdParams b) {
     }
     float mx[V], sum[V], xt[V];
 #pragma unroll
-    for (int v = 0; v < V; ++v) { mx[v] = -INFINITY; sum[v] = 0.f; xt[v] = 0.f; }
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-#pragma unroll
-      for (int v = 0; v < V; ++v) {
-        const float f = to_f(r[k].v[v]);
-        mx[v] = fmaxf(mx[v], f);
-        xt[v] = t[v] == k ? f : xt[v];
-      }
-    }
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-#pragma unroll
-      for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), mx[v]);
-    }
+    for (int v = 0; v < V; ++v) xt[v] = 0.f;
+    max_sumexp<T, KMAX>(r, mx, sum, [&](int k, int v, float f) { xt[v] = t[v] == k ? f : xt[v]; });
     if (!kBackward) {
 #pragma unroll
       for (int v = 0; v < V; ++v) {
@@ -372,7 +406,7 @@ __global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossBwdParams b) {
 #pragma unroll
       for (int v = 0; v < V; ++v) {
         lse[v] = mx[v] + logf(sum[v]);
-        const float g = b.reduction == 0 ? b.gout[n * S + s0 + v] : (skip[v] ? 0.f : gscale);
+        const float g = gs.at(n * S + s0 + v, skip[v]);
         c[v] = 0.f;
         if (t[v] >= 0) c[v] = g * hard_dloss(p, xt[v] - lse[v], p.weight ? p.weight[t[v]] : 1.f);
       }
@@ -390,62 +424,31 @@ __global__ void __launch_bounds__(kThreads) hard_vec_kernel(LossBwdParams b) {
       }
     }
   }
-  if (!kBackward) {
-    lsum = block_sum<double>(lsum, red);
-    lcnt = block_sum<double>(lcnt, red);
-    if (threadIdx.x == 0) { p.partials[2 * blockIdx.x] = lsum; p.partials[2 * blockIdx.x + 1] = lcnt; }
-  }
+  if (!kBackward) store_partials(p.partials, red, lsum, lcnt);
 }
 
 // soft-target poly loss, same layout: logits AND soft targets in registers
 template <typename T, int KMAX, bool kBackward>
-__global__ void __launch_bounds__(kThreads) poly_soft_vec_kernel(LossBwdParams b) {
+__global__ void __launch_bounds__(kThreads) poly_soft_vec_kernel(LossParams p) {
   constexpr int V = Vec8<T>::N;
   __shared__ double red[32];
-  const LossParams& p = b.f;
   const T* x = (const T*)p.x;
   const T* tg = (const T*)p.soft;
-  T* dx = (T*)b.dx;
+  T* dx = (T*)p.dx;
   const int K = p.K;
   const unsigned S = (unsigned)p.S, SV = S / V;
   const long long PV = (long long)p.N * SV;
   const bool ign = p.ignore_index >= 0 && p.ignore_index < K;
   double lsum = 0.0;
-  const long long stride = (long long)gridDim.x * kThreads;
-  for (long long pv = (long long)blockIdx.x * kThreads + threadIdx.x; pv < PV; pv += stride) {
+  const long long stride = (long long)gridDim.x * kThreads, pv0 = (long long)blockIdx.x * kThreads + threadIdx.x;
+  for (long long pv = pv0; pv < PV; pv += stride) {
     const long long n = pv / SV;
     const unsigned s0 = (unsigned)(pv - n * SV) * V;
     const long long off = n * K * S + s0;
-    Vec8<T> r[KMAX], q[KMAX];   // k >= K: logits -inf, soft targets 0
-    {
-      const T* pk = x + off;
-      const T* qk = tg + off;
-#pragma unroll
-      for (int k = 0; k < KMAX; ++k) {
-        if (k < K) {
-          r[k] = ld8(pk);
-          q[k] = ld8(qk);
-        } else {
-#pragma unroll
-          for (int v = 0; v < V; ++v) { r[k].v[v] = neg_inf<T>(); q[k].v[v] = from_f<T>(0.f); }
-        }
-        pk += S;
-        qk += S;
-      }
-    }
+    Vec8<T> r[KMAX], q[KMAX];
+    load_columns<T, KMAX, true>(r, q, x + off, tg + off, K, S);
     float mx[V], sum[V], lse[V];
-#pragma unroll
-    for (int v = 0; v < V; ++v) { mx[v] = -INFINITY; sum[v] = 0.f; }
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-#pragma unroll
-      for (int v = 0; v < V; ++v) mx[v] = fmaxf(mx[v], to_f(r[k].v[v]));
-    }
-#pragma unroll
-    for (int k = 0; k < KMAX; ++k) {
-#pragma unroll
-      for (int v = 0; v < V; ++v) sum[v] += exp_shift(to_f(r[k].v[v]), mx[v]);
-    }
+    max_sumexp<T, KMAX>(r, mx, sum, [](int, int, float) {});
 #pragma unroll
     for (int v = 0; v < V; ++v) lse[v] = mx[v] + logf(sum[v]);
     float acc[V];   // forward: the loss; backward: sum_k c_k t_k
@@ -469,9 +472,7 @@ __global__ void __launch_bounds__(kThreads) poly_soft_vec_kernel(LossBwdParams b
     } else {
       float g[V];
 #pragma unroll
-      for (int v = 0; v < V; ++v)
-        g[v] = b.reduction == 0 ? b.gout[n * S + s0 + v]
-                                : (b.reduction == 1 ? b.gout[0] / (float)((long long)p.N * S) : b.gout[0]);
+      for (int v = 0; v < V; ++v) g[v] = grad_scale(p.gout, p.reduction, nullptr, (long long)p.N * S).at(n * S + s0 + v);
 #pragma unroll
       for (int k = 0; k < KMAX; ++k)
         if (k < K) {
@@ -492,48 +493,76 @@ __global__ void __launch_bounds__(kThreads) poly_soft_vec_kernel(LossBwdParams b
         }
     }
   }
-  if (!kBackward) {
-    lsum = block_sum<double>(lsum, red);
-    if (threadIdx.x == 0) { p.partials[2 * blockIdx.x] = lsum; p.partials[2 * blockIdx.x + 1] = 0.0; }
-  }
+  if (!kBackward) store_partials(p.partials, red, lsum, V * thread_iters(pv0, PV, stride));
 }
 
 template <typename T>
-bool vec_eligible(const LossBwdParams& b) {
+bool vec_eligible(const LossParams& p) {
   constexpr int V = Vec8<T>::N;
-  const LossParams& p = b.f;
   auto al8 = [](const void* q) { return q == nullptr || (reinterpret_cast<uintptr_t>(q) & 7) == 0; };
-  return p.S > 1 && p.S % V == 0 && p.K <= 32 && (long long)p.K * p.S < 0x7fffffffLL && al8(p.x) && al8(p.soft) && al8(b.dx);
+  return p.S > 1 && p.S % V == 0 && p.K <= 32 && (long long)p.K * p.S < 0x7fffffffLL && al8(p.x) && al8(p.soft) && al8(p.dx);
 }
 
-// launches the smallest KMAX instantiation that holds K; returns the grid size, 0 if not eligible
-#define HB_KMAX_DISPATCH(KERNEL, T, BWD, b, grid, st)                                   \
-  do {                                                                                  \
-    switch (((b).f.K + 3) / 4) {                                                        \
-      case 0: case 1: KERNEL<T, 4, BWD><<<grid, kThreads, 0, st>>>(b); break;           \
-      case 2: KERNEL<T, 8, BWD><<<grid, kThreads, 0, st>>>(b); break;                   \
-      case 3: KERNEL<T, 12, BWD><<<grid, kThreads, 0, st>>>(b); break;                  \
-      case 4: KERNEL<T, 16, BWD><<<grid, kThreads, 0, st>>>(b); break;                  \
-      case 5: KERNEL<T, 20, BWD><<<grid, kThreads, 0, st>>>(b); break;                  \
-      case 6: KERNEL<T, 24, BWD><<<grid, kThreads, 0, st>>>(b); break;                  \
-      case 7: KERNEL<T, 28, BWD><<<grid, kThreads, 0, st>>>(b); break;                  \
-      default: KERNEL<T, 32, BWD><<<grid, kThreads, 0, st>>>(b); break;                 \
-    }                                                                                   \
-  } while (0)
+// ---- host dispatch ---------------------------------------------------------------------------------
+template <typename T> struct Type { using type = T; };
 
-template <typename T, bool kBackward>
-int launch_hard_vec(const LossBwdParams& b, cudaStream_t st) {
-  if (!vec_eligible<T>(b)) return 0;
-  const int grid = grid_for((long long)b.f.N * b.f.S / Vec8<T>::N, kThreads);
-  HB_KMAX_DISPATCH(hard_vec_kernel, T, kBackward, b, grid, st);
-  return grid;
+// f(Type<T>{}) for the dtype code; cudaErrorInvalidValue for an unknown code
+template <class F>
+int dispatch_dtype(int dtype, F f) {
+  switch (dtype) {
+    case HB_DTYPE_F32: return f(Type<float>{});
+    case HB_DTYPE_BF16: return f(Type<__nv_bfloat16>{});
+    case HB_DTYPE_F16: return f(Type<__half>{});
+    default: return (int)cudaErrorInvalidValue;
+  }
 }
-template <typename T, bool kBackward>
-int launch_soft_vec(const LossBwdParams& b, cudaStream_t st) {
-  if (!vec_eligible<T>(b)) return 0;
-  const int grid = grid_for((long long)b.f.N * b.f.S / Vec8<T>::N, kThreads);
-  HB_KMAX_DISPATCH(poly_soft_vec_kernel, T, kBackward, b, grid, st);
-  return grid;
+
+// f(std::integral_constant<int, KMAX>{}) for the smallest register-column instantiation that holds K (K <= 32)
+template <class F>
+void dispatch_kmax(int K, F f) {
+  switch ((K + 3) / 4) {
+    case 0: case 1: f(std::integral_constant<int, 4>{}); break;
+    case 2: f(std::integral_constant<int, 8>{}); break;
+    case 3: f(std::integral_constant<int, 12>{}); break;
+    case 4: f(std::integral_constant<int, 16>{}); break;
+    case 5: f(std::integral_constant<int, 20>{}); break;
+    case 6: f(std::integral_constant<int, 24>{}); break;
+    case 7: f(std::integral_constant<int, 28>{}); break;
+    default: f(std::integral_constant<int, 32>{}); break;
+  }
+}
+
+// The focal / poly-1 entry points: the register-column kernel when it applies, else the scalar kernel (hard targets: a
+// warp per position at S == 1; soft targets: a thread per position); the forward then folds the partials into fwd_out.
+template <bool kSoft, bool kBackward>
+int class_loss(const LossParams& p, float* fwd_out, int dtype, void* stream) {
+  const long long P = (long long)p.N * p.S;
+  if (P == 0) return 0;
+  cudaStream_t st = (cudaStream_t)stream;
+  int grid = 0;
+  const int rc = dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    if (vec_eligible<T>(p)) {
+      grid = grid_for(P / Vec8<T>::N, kThreads);
+      dispatch_kmax(p.K, [&](auto kmax) {
+        constexpr int KMAX = decltype(kmax)::value;
+        if constexpr (kSoft) poly_soft_vec_kernel<T, KMAX, kBackward><<<grid, kThreads, 0, st>>>(p);
+        else hard_vec_kernel<T, KMAX, kBackward><<<grid, kThreads, 0, st>>>(p);
+      });
+    } else if constexpr (kSoft) {
+      grid = grid_for(P, kThreads);
+      poly_soft_kernel<T, kBackward><<<grid, kThreads, 0, st>>>(p);
+    } else {
+      grid = grid_for(P, p.S == 1 ? kThreads / 32 : kThreads);
+      hard_kernel<T, kBackward><<<grid, kThreads, 0, st>>>(p);
+    }
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
+  if (rc != 0 || kBackward) return rc;
+  finalize_kernel<2><<<1, 32, 0, st>>>(p.partials, grid, (double)P, 0.f, fwd_out);
+  HB_LAUNCH_CHECK();
+  return 0;
 }
 
 // ---- dice -----------------------------------------------------------------------------------------
@@ -653,34 +682,6 @@ int dice_blocks_per_class(long long per_class, int K) {
   return gx < 1 ? 1 : gx;
 }
 
-// ---- losses with three partial sums: complement CE and the mutual channel loss ----------------------
-// partials[3 * block + {0, 1, 2}] = {sum of w_y * ce over the non-ignored positions, sum of their w_y, sum of the second
-// term}; out = {A + coef * C, B, A / B + coef * C / P}: torch's weighted-mean cross entropy plus coef times the plain mean.
-__global__ void finalize3_kernel(const double* partials, int n, double P, float coef, float* out) {
-  if (threadIdx.x == 0 && blockIdx.x == 0) {
-    double a = 0.0, b = 0.0, c = 0.0;
-    for (int i = 0; i < n; ++i) { a += partials[3 * i]; b += partials[3 * i + 1]; c += partials[3 * i + 2]; }
-    out[0] = (float)(a + (double)coef * c);
-    out[1] = (float)b;
-    out[2] = (float)(a / b + (double)coef * c / P);
-  }
-}
-
-__device__ __forceinline__ void store3(double* partials, double a, double b, double c, double* red) {
-  a = block_sum<double>(a, red);
-  b = block_sum<double>(b, red);
-  c = block_sum<double>(c, red);
-  if (threadIdx.x == 0) { partials[3 * blockIdx.x] = a; partials[3 * blockIdx.x + 1] = b; partials[3 * blockIdx.x + 2] = c; }
-}
-
-// {d loss / d (w_y ce), d loss / d (second term)} of one position for the reduction (mean: the first over sum w_y)
-__device__ __forceinline__ void grad_scales(const float* gout, const float* fwd_out, int reduction, long long pos,
-                                            long long P, float& gce, float& g2) {
-  if (reduction == 0) { gce = g2 = gout[pos]; return; }
-  gce = g2 = gout[0];
-  if (reduction == 1) { gce /= fwd_out[1]; g2 /= (float)P; }
-}
-
 // ---- complement cross entropy ---------------------------------------------------------------------
 // per position (target y, A = the classes k != y outside the ignored column):
 //   L = w_y * ce * [y != ignore_index] + gamma * C,   ce = lse - x_y,
@@ -688,35 +689,9 @@ __device__ __forceinline__ void grad_scales(const float* gout, const float* fwd_
 // (q is the softmax over the non-target classes - the reference's p_k / (1 - p_y) without the cancellation of 1 - p_y).
 //   dC/dx_y = 0,   dC/dx_j = -1/(K-1) * q_j * ([j in A] w_j (1 + log q_j) - sum_{k in A} w_k q_k (1 + log q_k))
 // The CE part follows torch: any ignore_index value drops the row. The complement term drops the ignored column only.
-struct CceParams {
-  const void* x;            // [N, K, S]
-  const long long* target;  // [N, S]
-  const float* weight;      // [K] or null
-  float* loss_pos;          // [N*S]
-  double* partials;         // [grid][3]
-  const float* gout;        // backward: [N*S] (none) or 1 element
-  const float* fwd_out;     // backward: {sum, sum w_y, mean} of the forward
-  void* dx;
-  int N, K, S, ignore_index, reduction;
-  float gamma;
-};
-
-// k-loop shapes: one thread owns a position (S > 1) or a warp does, its lanes striding over the classes (S == 1)
-struct ThreadLanes {
-  static constexpr int kStep = 1;
-  int k0 = 0;
-  __device__ float max(float v) const { return v; }
-  __device__ float sum(float v) const { return v; }
-};
-struct WarpLanes {
-  static constexpr int kStep = 32;
-  int k0;
-  __device__ float max(float v) const { return warp_max(v); }
-  __device__ float sum(float v) const { return warp_sum(v); }
-};
-
+// partials[3 * block + {0, 1, 2}] = {sum of w_y * ce over the non-ignored positions, sum of their w_y, sum of C}.
 template <typename T, bool kBackward, class Ln>
-__device__ __forceinline__ void cce_position(const CceParams& p, const Ln& ln, const T* xp, T* dp, long long st,
+__device__ __forceinline__ void cce_position(const LossParams& p, const Ln& ln, const T* xp, T* dp, long long st,
                                              long long pos, double& sa, double& sb, double& sc) {
   const int K = p.K;
   auto x_at = [&](int k) { return to_f(xp[k * st]); };
@@ -765,8 +740,9 @@ __device__ __forceinline__ void cce_position(const CceParams& p, const Ln& ln, c
       sa += wce; sb += wv; sc += c;
     }
   } else {
-    float gce, gc;
-    grad_scales(p.gout, p.fwd_out, p.reduction, pos, (long long)p.N * p.S, gce, gc);
+    const long long P = (long long)p.N * p.S;
+    const float gce = grad_scale(p.gout, p.reduction, p.fwd_out + 1, P).at(pos);
+    const float gc = grad_scale(p.gout, p.reduction, nullptr, P).at(pos);
     const float cw = (inr && tl != p.ignore_index) ? gce * w_at(t) : 0.f;
     const float cc = (comp && inr) ? -p.gamma * gc * inv : 0.f;
     for (int k = ln.k0; k < K; k += Ln::kStep) {
@@ -782,26 +758,13 @@ __device__ __forceinline__ void cce_position(const CceParams& p, const Ln& ln, c
 }
 
 template <typename T, bool kBackward>
-__global__ void __launch_bounds__(kThreads) cce_kernel(CceParams p) {
+__global__ void __launch_bounds__(kThreads) cce_kernel(LossParams p) {
   __shared__ double red[32];
-  const T* x = (const T*)p.x;
-  T* dx = (T*)p.dx;
-  const long long P = (long long)p.N * p.S;
   double sa = 0.0, sb = 0.0, sc = 0.0;
-  if (p.S == 1) {
-    const WarpLanes ln{threadIdx.x & 31};
-    const long long warps = (long long)gridDim.x * (kThreads / 32);
-    for (long long pos = (long long)blockIdx.x * (kThreads / 32) + (threadIdx.x >> 5); pos < P; pos += warps)
-      cce_position<T, kBackward>(p, ln, x + pos * p.K, dx + pos * p.K, 1, pos, sa, sb, sc);
-  } else {
-    const ThreadLanes ln{};
-    const long long stride = (long long)gridDim.x * kThreads;
-    for (long long pos = (long long)blockIdx.x * kThreads + threadIdx.x; pos < P; pos += stride) {
-      const long long off = (pos / p.S) * p.K * p.S + pos % p.S;
-      cce_position<T, kBackward>(p, ln, x + off, dx + off, p.S, pos, sa, sb, sc);
-    }
-  }
-  if (!kBackward) store3(p.partials, sa, sb, sc, red);
+  for_each_position<T>(p, [&](const auto& ln, const T* xp, T* dp, long long st, long long pos) {
+    cce_position<T, kBackward>(p, ln, xp, dp, st, pos, sa, sb, sc);
+  });
+  if (!kBackward) store_partials(p.partials, red, sa, sb, sc);
 }
 
 // ---- mutual channel loss --------------------------------------------------------------------------
@@ -916,7 +879,7 @@ __global__ void __launch_bounds__(kThreads) mcl_fwd_kernel(McParams p) {
     p.lse_d[pos] = lse;
     sa += wce; sb += wv; sc += div;
   }
-  store3(p.partials, sa, sb, sc, red);
+  store_partials(p.partials, red, sa, sb, sc);
 }
 
 // pass C: one block per (sample, class); per row of the class R = sum_s G_s p_s with G_s = -(alpha/cnum) g_s at the
@@ -932,8 +895,7 @@ __global__ void __launch_bounds__(kThreads) mcl_rdot_kernel(McParams p) {
   const float* lse_c = p.row_lse + (long long)n * C + c * p.xi;
   for (int j = 0; j < p.xi; ++j) acc[j * blockDim.x + threadIdx.x] = 0.f;
   for (long long s = threadIdx.x; s < p.S; s += blockDim.x) {
-    float gce, g;
-    grad_scales(p.gout, p.fwd_out, p.reduction, n * p.S + s, P, gce, g);
+    const float g = grad_scale(p.gout, p.reduction, nullptr, P).at(n * p.S + s);
     float pv = 0.f;
     int jv = 0;
     for (int j = 0; j < p.xi; ++j) {
@@ -964,10 +926,10 @@ __global__ void __launch_bounds__(kThreads) mcl_bwd_kernel(McParams p) {
     const float* lse_n = p.row_lse + n * C;
     const float* rdot_n = p.rdot + n * C;
     const long long tl = p.target[pos];
-    float gce, gdiv;
-    grad_scales(p.gout, p.fwd_out, p.reduction, pos, P, gce, gdiv);
+    const float gdiv = grad_scale(p.gout, p.reduction, nullptr, P).at(pos);
     const bool ce_on = tl != p.ignore_index && tl >= 0 && tl < p.cnum;
-    gce = ce_on ? gce * (p.weight ? p.weight[tl] : 1.f) : 0.f;
+    const float gce = ce_on ? grad_scale(p.gout, p.reduction, p.fwd_out + 1, P).at(pos) * (p.weight ? p.weight[tl] : 1.f)
+                            : 0.f;
     const float lse = p.lse_d[pos];
     for (int c = 0; c < p.cnum; ++c) {
       const long long oc = off + (long long)c * p.xi * p.S;
@@ -1013,30 +975,7 @@ int hb_cls_loss_hard_fwd(const void* x, const long long* target, const float* we
   LossParams p{};
   p.x = x; p.target = target; p.weight = weight; p.loss_pos = loss_pos; p.partials = partials;
   p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.kind = kind; p.gamma = gamma; p.eps = eps;
-  const long long P = (long long)N * S;
-  if (P == 0) return 0;
-  int grid = 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  LossBwdParams vb{};
-  vb.f = p;
-  switch (dtype) {
-    case HB_DTYPE_F32: grid = launch_hard_vec<float, false>(vb, st); break;
-    case HB_DTYPE_BF16: grid = launch_hard_vec<__nv_bfloat16, false>(vb, st); break;
-    case HB_DTYPE_F16: grid = launch_hard_vec<__half, false>(vb, st); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  if (grid == 0) {
-    grid = grid_for(P, S == 1 ? kThreads / 32 : kThreads);
-    switch (dtype) {
-      case HB_DTYPE_F32: hard_fwd_kernel<float><<<grid, kThreads, 0, st>>>(p); break;
-      case HB_DTYPE_BF16: hard_fwd_kernel<__nv_bfloat16><<<grid, kThreads, 0, st>>>(p); break;
-      default: hard_fwd_kernel<__half><<<grid, kThreads, 0, st>>>(p); break;
-    }
-  }
-  HB_LAUNCH_CHECK();
-  finalize_kernel<<<1, 32, 0, st>>>(partials, grid, fwd_out);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return class_loss<false, false>(p, fwd_out, dtype, stream);
 }
 
 // reduction: 0 none (gout[N*S]), 1 mean, 2 sum (gout[1]). dx has the dtype/shape of x.
@@ -1044,89 +983,29 @@ int hb_cls_loss_hard_bwd(const void* x, const long long* target, const float* we
                          const float* fwd_out, void* dx, int N, int K, int S, int ignore_index, int kind, float gamma,
                          float eps, int reduction, int dtype, void* stream) {
   if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
-  LossBwdParams b{};
-  b.f.x = x; b.f.target = target; b.f.weight = weight;
-  b.f.N = N; b.f.K = K; b.f.S = S; b.f.ignore_index = ignore_index; b.f.kind = kind; b.f.gamma = gamma; b.f.eps = eps;
-  b.gout = gout; b.fwd_out = fwd_out; b.dx = dx; b.reduction = reduction;
-  const long long P = (long long)N * S;
-  if (P == 0) return 0;
-  int grid = 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case HB_DTYPE_F32: grid = launch_hard_vec<float, true>(b, st); break;
-    case HB_DTYPE_BF16: grid = launch_hard_vec<__nv_bfloat16, true>(b, st); break;
-    case HB_DTYPE_F16: grid = launch_hard_vec<__half, true>(b, st); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  if (grid == 0) {
-    grid = grid_for(P, S == 1 ? kThreads / 32 : kThreads);
-    switch (dtype) {
-      case HB_DTYPE_F32: hard_bwd_kernel<float><<<grid, kThreads, 0, st>>>(b); break;
-      case HB_DTYPE_BF16: hard_bwd_kernel<__nv_bfloat16><<<grid, kThreads, 0, st>>>(b); break;
-      default: hard_bwd_kernel<__half><<<grid, kThreads, 0, st>>>(b); break;
-    }
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  LossParams p{};
+  p.x = x; p.target = target; p.weight = weight; p.gout = gout; p.fwd_out = fwd_out; p.dx = dx;
+  p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.kind = kind; p.reduction = reduction; p.gamma = gamma;
+  p.eps = eps;
+  return class_loss<false, true>(p, nullptr, dtype, stream);
 }
 
 int hb_poly_soft_fwd(const void* x, const void* soft, const float* weight, float* loss_pos, double* partials,
                      float* fwd_out, int N, int K, int S, int ignore_index, float eps, int dtype, void* stream) {
   if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
-  LossBwdParams b{};
-  b.f.x = x; b.f.soft = soft; b.f.weight = weight; b.f.loss_pos = loss_pos; b.f.partials = partials;
-  b.f.N = N; b.f.K = K; b.f.S = S; b.f.ignore_index = ignore_index; b.f.kind = POLY; b.f.eps = eps;
-  const long long P = (long long)N * S;
-  if (P == 0) return 0;
-  int grid = 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case HB_DTYPE_F32: grid = launch_soft_vec<float, false>(b, st); break;
-    case HB_DTYPE_BF16: grid = launch_soft_vec<__nv_bfloat16, false>(b, st); break;
-    case HB_DTYPE_F16: grid = launch_soft_vec<__half, false>(b, st); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  if (grid == 0) {
-    grid = grid_for(P, kThreads);
-    switch (dtype) {
-      case HB_DTYPE_F32: poly_soft_kernel<float, false><<<grid, kThreads, 0, st>>>(b); break;
-      case HB_DTYPE_BF16: poly_soft_kernel<__nv_bfloat16, false><<<grid, kThreads, 0, st>>>(b); break;
-      default: poly_soft_kernel<__half, false><<<grid, kThreads, 0, st>>>(b); break;
-    }
-  }
-  HB_LAUNCH_CHECK();
-  finalize_soft_kernel<<<1, 32, 0, st>>>(partials, grid, (double)P, fwd_out);
-  HB_LAUNCH_CHECK();
-  return 0;
+  LossParams p{};
+  p.x = x; p.soft = soft; p.weight = weight; p.loss_pos = loss_pos; p.partials = partials;
+  p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.kind = POLY; p.eps = eps;
+  return class_loss<true, false>(p, fwd_out, dtype, stream);
 }
 
 int hb_poly_soft_bwd(const void* x, const void* soft, const float* weight, const float* gout, void* dx, int N, int K,
                      int S, int ignore_index, float eps, int reduction, int dtype, void* stream) {
   if (bad_nks(N, K, S)) return (int)cudaErrorInvalidValue;
-  LossBwdParams b{};
-  b.f.x = x; b.f.soft = soft; b.f.weight = weight;
-  b.f.N = N; b.f.K = K; b.f.S = S; b.f.ignore_index = ignore_index; b.f.kind = POLY; b.f.eps = eps;
-  b.gout = gout; b.dx = dx; b.reduction = reduction;
-  const long long P = (long long)N * S;
-  if (P == 0) return 0;
-  int grid = 0;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case HB_DTYPE_F32: grid = launch_soft_vec<float, true>(b, st); break;
-    case HB_DTYPE_BF16: grid = launch_soft_vec<__nv_bfloat16, true>(b, st); break;
-    case HB_DTYPE_F16: grid = launch_soft_vec<__half, true>(b, st); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  if (grid == 0) {
-    grid = grid_for(P, kThreads);
-    switch (dtype) {
-      case HB_DTYPE_F32: poly_soft_kernel<float, true><<<grid, kThreads, 0, st>>>(b); break;
-      case HB_DTYPE_BF16: poly_soft_kernel<__nv_bfloat16, true><<<grid, kThreads, 0, st>>>(b); break;
-      default: poly_soft_kernel<__half, true><<<grid, kThreads, 0, st>>>(b); break;
-    }
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  LossParams p{};
+  p.x = x; p.soft = soft; p.weight = weight; p.gout = gout; p.dx = dx;
+  p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.kind = POLY; p.reduction = reduction; p.eps = eps;
+  return class_loss<true, true>(p, nullptr, dtype, stream);
 }
 
 // scratch: double[hb_dice_scratch_doubles(K)] (per-block partials + the K folded pairs); out: float[1]; coef: float[2K]
@@ -1140,22 +1019,15 @@ int hb_dice_fwd(const void* x, const void* target, const float* weight, double* 
   double* part = scratch;
   double* sums = scratch + 2 * (size_t)gx * K;
   dim3 grid(gx, K);
-  switch (dtype) {
-#define HB_DICE_SUMS(T)                                                                                         \
-  {                                                                                                             \
-    const int vec = S % Vec16<T>::N == 0 && aligned16(x) && aligned16(target);                                 \
-    dice_sums_kernel<T><<<grid, kThreads, 0, st>>>((const T*)x, (const T*)target, N, K, S, gamma, part, vec); \
-  }
-    case HB_DTYPE_F32: HB_DICE_SUMS(float) break;
-    case HB_DTYPE_BF16: HB_DICE_SUMS(__nv_bfloat16) break;
-    case HB_DTYPE_F16: HB_DICE_SUMS(__half) break;
-#undef HB_DICE_SUMS
-    default: return (int)cudaErrorInvalidValue;
-  }
-  HB_LAUNCH_CHECK();
-  dice_finalize_kernel<<<1, kThreads, 0, st>>>(part, gx, sums, weight, K, gamma, eps, out, coef);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    const int vec = S % Vec16<T>::N == 0 && aligned16(x) && aligned16(target);
+    dice_sums_kernel<T><<<grid, kThreads, 0, st>>>((const T*)x, (const T*)target, N, K, S, gamma, part, vec);
+    HB_LAUNCH_CHECK();
+    dice_finalize_kernel<<<1, kThreads, 0, st>>>(part, gx, sums, weight, K, gamma, eps, out, coef);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_dice_bwd(const void* target, const float* coef, const float* gout, void* dx, int N, int K, long long S, int dtype,
@@ -1164,65 +1036,51 @@ int hb_dice_bwd(const void* target, const float* coef, const float* gout, void* 
   const long long total = (long long)N * K * S;
   if (total == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-#define HB_DICE_BWD(T)                                                                                     \
-  {                                                                                                        \
-    const int vec = S % Vec16<T>::N == 0 && aligned16(target) && aligned16(dx);                           \
-    const int grid = grid_for(total, kThreads * (vec ? Vec16<T>::N * 2 : 4));                             \
-    dice_bwd_kernel<T><<<grid, kThreads, 0, st>>>((const T*)target, coef, gout, (T*)dx, N, K, S, vec);    \
-  }
-    case HB_DTYPE_F32: HB_DICE_BWD(float) break;
-    case HB_DTYPE_BF16: HB_DICE_BWD(__nv_bfloat16) break;
-    case HB_DTYPE_F16: HB_DICE_BWD(__half) break;
-#undef HB_DICE_BWD
-    default: return (int)cudaErrorInvalidValue;
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    const int vec = S % Vec16<T>::N == 0 && aligned16(target) && aligned16(dx);
+    const int grid = grid_for(total, kThreads * (vec ? Vec16<T>::N * 2 : 4));
+    dice_bwd_kernel<T><<<grid, kThreads, 0, st>>>((const T*)target, coef, gout, (T*)dx, N, K, S, vec);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
-
-#define HB_LOSS_DTYPE_SWITCH(dtype, LAUNCH)              \
-  switch (dtype) {                                       \
-    case HB_DTYPE_F32: LAUNCH(float); break;             \
-    case HB_DTYPE_BF16: LAUNCH(__nv_bfloat16); break;    \
-    case HB_DTYPE_F16: LAUNCH(__half); break;            \
-    default: return (int)cudaErrorInvalidValue;          \
-  }
 
 int hb_cce_fwd(const void* x, const long long* target, const float* weight, float* loss_pos, double* partials,
                float* fwd_out, int N, int K, int S, int ignore_index, float gamma, int dtype, void* stream) {
   if (bad_nks(N, K, S) || (gamma != 0.f && K < 2)) return (int)cudaErrorInvalidValue;  // C divides by K - 1
-  CceParams p{};
+  LossParams p{};
   p.x = x; p.target = target; p.weight = weight; p.loss_pos = loss_pos; p.partials = partials;
   p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.gamma = gamma;
   const long long P = (long long)N * S;
   if (P == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(P, S == 1 ? kThreads / 32 : kThreads);
-#define HB_CCE_FWD(T) cce_kernel<T, false><<<grid, kThreads, 0, st>>>(p)
-  HB_LOSS_DTYPE_SWITCH(dtype, HB_CCE_FWD)
-#undef HB_CCE_FWD
-  HB_LAUNCH_CHECK();
-  finalize3_kernel<<<1, 32, 0, st>>>(partials, grid, (double)P, gamma, fwd_out);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    cce_kernel<T, false><<<grid, kThreads, 0, st>>>(p);
+    HB_LAUNCH_CHECK();
+    finalize_kernel<3><<<1, 32, 0, st>>>(partials, grid, (double)P, gamma, fwd_out);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_cce_bwd(const void* x, const long long* target, const float* weight, const float* gout, const float* fwd_out,
                void* dx, int N, int K, int S, int ignore_index, float gamma, int reduction, int dtype, void* stream) {
   if (bad_nks(N, K, S) || (gamma != 0.f && K < 2)) return (int)cudaErrorInvalidValue;  // C divides by K - 1
-  CceParams p{};
+  LossParams p{};
   p.x = x; p.target = target; p.weight = weight; p.gout = gout; p.fwd_out = fwd_out; p.dx = dx;
   p.N = N; p.K = K; p.S = S; p.ignore_index = ignore_index; p.reduction = reduction; p.gamma = gamma;
   const long long P = (long long)N * S;
   if (P == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(P, S == 1 ? kThreads / 32 : kThreads);
-#define HB_CCE_BWD(T) cce_kernel<T, true><<<grid, kThreads, 0, st>>>(p)
-  HB_LOSS_DTYPE_SWITCH(dtype, HB_CCE_BWD)
-#undef HB_CCE_BWD
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    cce_kernel<typename decltype(type)::type, true><<<grid, kThreads, 0, st>>>(p);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_mcl_fwd(const void* x, const long long* target, const float* weight, const unsigned char* mask, float* row_lse,
@@ -1237,19 +1095,17 @@ int hb_mcl_fwd(const void* x, const long long* target, const float* weight, cons
   if (P == 0 || rows == 0) return 0;
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(P, kThreads);
-#define HB_MCL_FWD(T)                                                                                      \
-  {                                                                                                        \
-    const int vec = S % Vec16<T>::N == 0 && aligned16(x);                                                  \
-    mcl_row_lse_kernel<T><<<(unsigned)rows, kThreads, 0, st>>>((const T*)x, S, vec, row_lse);              \
-    HB_LAUNCH_CHECK();                                                                                     \
-    mcl_fwd_kernel<T><<<grid, kThreads, 0, st>>>(p);                                                       \
-  }
-  HB_LOSS_DTYPE_SWITCH(dtype, HB_MCL_FWD)
-#undef HB_MCL_FWD
-  HB_LAUNCH_CHECK();
-  finalize3_kernel<<<1, 32, 0, st>>>(partials, grid, (double)P, -alpha, fwd_out);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    const int vec = S % Vec16<T>::N == 0 && aligned16(x);
+    mcl_row_lse_kernel<T><<<(unsigned)rows, kThreads, 0, st>>>((const T*)x, S, vec, row_lse);
+    HB_LAUNCH_CHECK();
+    mcl_fwd_kernel<T><<<grid, kThreads, 0, st>>>(p);
+    HB_LAUNCH_CHECK();
+    finalize_kernel<3><<<1, 32, 0, st>>>(partials, grid, (double)P, -alpha, fwd_out);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_mcl_bwd(const void* x, const long long* target, const float* weight, const unsigned char* mask,
@@ -1266,18 +1122,14 @@ int hb_mcl_bwd(const void* x, const long long* target, const float* weight, cons
   cudaStream_t st = (cudaStream_t)stream;
   const int grid = grid_for(P, kThreads);
   const size_t smem = (size_t)xi * rt * sizeof(float);
-#define HB_MCL_BWD(T)                                                                                      \
-  {                                                                                                        \
-    mcl_rdot_kernel<T><<<(unsigned)groups, rt, smem, st>>>(p);                                             \
-    HB_LAUNCH_CHECK();                                                                                     \
-    mcl_bwd_kernel<T><<<grid, kThreads, 0, st>>>(p);                                                       \
-  }
-  HB_LOSS_DTYPE_SWITCH(dtype, HB_MCL_BWD)
-#undef HB_MCL_BWD
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    mcl_rdot_kernel<T><<<(unsigned)groups, rt, smem, st>>>(p);
+    HB_LAUNCH_CHECK();
+    mcl_bwd_kernel<T><<<grid, kThreads, 0, st>>>(p);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
-
-#undef HB_LOSS_DTYPE_SWITCH
 
 }  // extern "C"

@@ -27,6 +27,39 @@ def _weight(weight, x: Tensor) -> Optional[Tensor]:
     return weight.detach().to(device=x.device, dtype=torch.float32).contiguous()
 
 
+def _index_targets(target: Tensor, n: int, s: int) -> Tensor:
+    """Class-index targets as the flat int64 [N*S] vector the kernels read."""
+    tc = target.contiguous().view(-1)
+    if tc.dtype != torch.long:
+        tc = tc.long()
+    if tc.numel() != n * s:
+        raise ValueError("target shape does not match the input's (N, ...) dims")
+    return tc
+
+
+def _position_buffers(x: Tensor, n: int, s: int, num_partials: int):
+    """A forward's per-position loss, per-block partial sums (num_partials per block) and {sum, count, mean}."""
+    loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
+    partials = torch.empty(num_partials * lib().hb_loss_max_partials(), device=x.device, dtype=torch.float64)
+    fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
+    return loss_pos, partials, fwd_out
+
+
+def _reduced(x: Tensor, loss_pos: Tensor, fwd_out: Tensor, reduction: int, flat: bool = False) -> Tensor:
+    """mean, sum, or the per-position loss: flat [N*S], or shaped (N, ...) like x without its class axis."""
+    if reduction == 1:
+        return fwd_out[2].to(x.dtype)
+    if reduction == 2:
+        return fwd_out[0].to(x.dtype)
+    out = loss_pos.to(x.dtype)
+    return out if flat else out.view(x.shape[0], *x.shape[2:])
+
+
+def _grad(gout: Tensor) -> Tensor:
+    """The incoming gradient as the flat fp32 vector the backward kernels read."""
+    return gout.detach().float().contiguous().view(-1)
+
+
 class _HardLossFn(torch.autograd.Function):
     """kind 0: focal, 1: poly-1; hard (int64) targets."""
 
@@ -35,32 +68,21 @@ class _HardLossFn(torch.autograd.Function):
                 gamma: float, eps: float) -> Tensor:
         require_cuda(x, target)
         xc = x.contiguous()
-        tc = target.contiguous().view(-1)
-        if tc.dtype != torch.long:
-            tc = tc.long()
         n, k, s = _nks(xc)
-        if tc.numel() != n * s:
-            raise ValueError("target shape does not match the input's (N, ...) dims")
-        L = lib()
-        loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
-        partials = torch.empty(2 * L.hb_loss_max_partials(), device=x.device, dtype=torch.float64)
-        fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
-        check(L.hb_cls_loss_hard_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n, k, s,
-                                     int(ignore_index), kind, _cf(gamma), _cf(eps), dtype_code(xc), stream_ptr()),
-              "hb_cls_loss_hard_fwd")
+        tc = _index_targets(target, n, s)
+        loss_pos, partials, fwd_out = _position_buffers(x, n, s, 2)
+        check(lib().hb_cls_loss_hard_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n,
+                                         k, s, int(ignore_index), kind, _cf(gamma), _cf(eps), dtype_code(xc),
+                                         stream_ptr()), "hb_cls_loss_hard_fwd")
         ctx.save_for_backward(xc, tc, weight, fwd_out)
         ctx.cfg = (n, k, s, int(ignore_index), reduction, kind, gamma, eps)
-        if reduction == 1:
-            return fwd_out[2].to(x.dtype)
-        if reduction == 2:
-            return fwd_out[0].to(x.dtype)
-        return loss_pos.to(x.dtype)
+        return _reduced(x, loss_pos, fwd_out, reduction, flat=True)
 
     @staticmethod
     def backward(ctx, gout: Tensor):
         xc, tc, weight, fwd_out = ctx.saved_tensors
         n, k, s, ignore_index, reduction, kind, gamma, eps = ctx.cfg
-        g = gout.detach().float().contiguous().view(-1)
+        g = _grad(gout)
         dx = torch.empty_like(xc)
         check(lib().hb_cls_loss_hard_bwd(ptr(xc), ptr(tc), ptr(weight), ptr(g), ptr(fwd_out), ptr(dx), n, k, s,
                                          ignore_index, kind, _cf(gamma), _cf(eps), reduction, dtype_code(xc),
@@ -76,25 +98,18 @@ class _PolySoftFn(torch.autograd.Function):
         xc = x.contiguous()
         tc = target.to(xc.dtype).contiguous()
         n, k, s = _nks(xc)
-        L = lib()
-        loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
-        partials = torch.empty(2 * L.hb_loss_max_partials(), device=x.device, dtype=torch.float64)
-        fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
-        check(L.hb_poly_soft_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n, k, s,
-                                 int(ignore_index), _cf(eps), dtype_code(xc), stream_ptr()), "hb_poly_soft_fwd")
+        loss_pos, partials, fwd_out = _position_buffers(x, n, s, 2)
+        check(lib().hb_poly_soft_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n, k,
+                                     s, int(ignore_index), _cf(eps), dtype_code(xc), stream_ptr()), "hb_poly_soft_fwd")
         ctx.save_for_backward(xc, tc, weight)
         ctx.cfg = (n, k, s, int(ignore_index), reduction, eps)
-        if reduction == 1:
-            return fwd_out[2].to(x.dtype)
-        if reduction == 2:
-            return fwd_out[0].to(x.dtype)
-        return loss_pos.to(x.dtype).view(x.shape[0], *x.shape[2:])
+        return _reduced(x, loss_pos, fwd_out, reduction)
 
     @staticmethod
     def backward(ctx, gout: Tensor):
         xc, tc, weight = ctx.saved_tensors
         n, k, s, ignore_index, reduction, eps = ctx.cfg
-        g = gout.detach().float().contiguous().view(-1)
+        g = _grad(gout)
         dx = torch.empty_like(xc)
         check(lib().hb_poly_soft_bwd(ptr(xc), ptr(tc), ptr(weight), ptr(g), ptr(dx), n, k, s, ignore_index, _cf(eps),
                                      reduction, dtype_code(xc), stream_ptr()), "hb_poly_soft_bwd")
@@ -107,29 +122,20 @@ class _ComplementCEFn(torch.autograd.Function):
                 gamma: float) -> Tensor:
         require_cuda(x, target)
         xc = x.contiguous()
-        tc = target.contiguous().view(-1)
         n, k, s = _nks(xc)
-        if tc.numel() != n * s:
-            raise ValueError("target shape does not match the input's (N, ...) dims")
-        L = lib()
-        loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
-        partials = torch.empty(3 * L.hb_loss_max_partials(), device=x.device, dtype=torch.float64)
-        fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
-        check(L.hb_cce_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n, k, s,
-                           int(ignore_index), _cf(gamma), dtype_code(xc), stream_ptr()), "hb_cce_fwd")
+        tc = _index_targets(target, n, s)
+        loss_pos, partials, fwd_out = _position_buffers(x, n, s, 3)
+        check(lib().hb_cce_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(loss_pos), ptr(partials), ptr(fwd_out), n, k, s,
+                               int(ignore_index), _cf(gamma), dtype_code(xc), stream_ptr()), "hb_cce_fwd")
         ctx.save_for_backward(xc, tc, weight, fwd_out)
         ctx.cfg = (n, k, s, int(ignore_index), reduction, gamma)
-        if reduction == 1:
-            return fwd_out[2].to(x.dtype)
-        if reduction == 2:
-            return fwd_out[0].to(x.dtype)
-        return loss_pos.to(x.dtype).view(x.shape[0], *x.shape[2:])
+        return _reduced(x, loss_pos, fwd_out, reduction)
 
     @staticmethod
     def backward(ctx, gout: Tensor):
         xc, tc, weight, fwd_out = ctx.saved_tensors
         n, k, s, ignore_index, reduction, gamma = ctx.cfg
-        g = gout.detach().float().contiguous().view(-1)
+        g = _grad(gout)
         dx = torch.empty_like(xc)
         check(lib().hb_cce_bwd(ptr(xc), ptr(tc), ptr(weight), ptr(g), ptr(fwd_out), ptr(dx), n, k, s, ignore_index,
                                _cf(gamma), reduction, dtype_code(xc), stream_ptr()), "hb_cce_bwd")
@@ -142,33 +148,24 @@ class _MutualChannelFn(torch.autograd.Function):
                 reduction: int, xi: int, alpha: float) -> Tensor:
         require_cuda(x, target)
         xc = x.contiguous()
-        tc = target.contiguous().view(-1)
         n, c, s = _nks(xc)
         cnum = c // xi
-        if tc.numel() != n * s:
-            raise ValueError("target shape does not match the input's (N, ...) dims")
-        L = lib()
+        tc = _index_targets(target, n, s)
         row_lse = torch.empty(n * c, device=x.device, dtype=torch.float32)
-        loss_pos = torch.empty(n * s, device=x.device, dtype=torch.float32)
         lse_d = torch.empty(n * s, device=x.device, dtype=torch.float32)
-        partials = torch.empty(3 * L.hb_loss_max_partials(), device=x.device, dtype=torch.float64)
-        fwd_out = torch.empty(3, device=x.device, dtype=torch.float32)
-        check(L.hb_mcl_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(mask), ptr(row_lse), ptr(loss_pos), ptr(lse_d),
-                           ptr(partials), ptr(fwd_out), n, cnum, xi, s, int(ignore_index), _cf(alpha), dtype_code(xc),
-                           stream_ptr()), "hb_mcl_fwd")
+        loss_pos, partials, fwd_out = _position_buffers(x, n, s, 3)
+        check(lib().hb_mcl_fwd(ptr(xc), ptr(tc), ptr(weight), ptr(mask), ptr(row_lse), ptr(loss_pos), ptr(lse_d),
+                               ptr(partials), ptr(fwd_out), n, cnum, xi, s, int(ignore_index), _cf(alpha),
+                               dtype_code(xc), stream_ptr()), "hb_mcl_fwd")
         ctx.save_for_backward(xc, tc, weight, mask, row_lse, lse_d, fwd_out)
         ctx.cfg = (n, cnum, xi, s, int(ignore_index), reduction, alpha)
-        if reduction == 1:
-            return fwd_out[2].to(x.dtype)
-        if reduction == 2:
-            return fwd_out[0].to(x.dtype)
-        return loss_pos.to(x.dtype).view(x.shape[0], *x.shape[2:])
+        return _reduced(x, loss_pos, fwd_out, reduction)
 
     @staticmethod
     def backward(ctx, gout: Tensor):
         xc, tc, weight, mask, row_lse, lse_d, fwd_out = ctx.saved_tensors
         n, cnum, xi, s, ignore_index, reduction, alpha = ctx.cfg
-        g = gout.detach().float().contiguous().view(-1)
+        g = _grad(gout)
         rdot = torch.empty_like(row_lse)
         dx = torch.empty_like(xc)
         check(lib().hb_mcl_bwd(ptr(xc), ptr(tc), ptr(weight), ptr(mask), ptr(row_lse), ptr(lse_d), ptr(g), ptr(fwd_out),
@@ -234,7 +231,7 @@ class _DiceFn(torch.autograd.Function):
     def backward(ctx, gout: Tensor):
         tc, coef = ctx.saved_tensors
         n, k, s = ctx.cfg
-        g = gout.detach().float().contiguous().view(-1)
+        g = _grad(gout)
         dx = torch.empty_like(tc)
         check(lib().hb_dice_bwd(ptr(tc), ptr(coef), ptr(g), ptr(dx), n, k, s, dtype_code(tc), stream_ptr()), "hb_dice_bwd")
         return dx, None, None, None, None

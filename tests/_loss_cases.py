@@ -1,8 +1,8 @@
 """The loss kernel cases and a Python mirror of the dispatch and grid geometry of csrc/losses.cu (no GPU).
 
 ``route`` names, for each entry point a case calls, the kernel instantiation launched and its grid: the launcher
-conditions of ``hb_cls_loss_hard_*``, ``hb_poly_soft_*``, ``hb_dice_*``, ``hb_cce_*`` and ``hb_mcl_*``, and
-``vec_eligible``, ``HB_KMAX_DISPATCH``, ``grid_for``, ``dice_blocks_per_class`` and ``mcl_rdot_threads``. A kernel's
+conditions of ``hb_cls_loss_hard_*``, ``hb_poly_soft_*`` (``class_loss``), ``hb_dice_*``, ``hb_cce_*`` and ``hb_mcl_*``,
+and ``vec_eligible``, ``dispatch_kmax``, ``grid_for``, ``dice_blocks_per_class`` and ``mcl_rdot_threads``. A kernel's
 branch on ``S == 1`` (one warp or one thread per position) and on its ``vec`` flag is part of the name after a ``/``.
 Every kernel except the row / group / finalize kernels is grid-stride: a thread starting at item ``i0 < stride`` runs
 ``ceil((total - i0) / stride)`` iterations, at least ``total // stride`` and at most ``ceil(total / stride)``. The SM
@@ -27,13 +27,13 @@ def _instantiations() -> Tuple[str, ...]:
         T = TYPES[dt][0]
         for kern in ("hard_vec_kernel", "poly_soft_vec_kernel"):
             out += [f"{kern}<{T},{km},{str(bwd).lower()}>" for km in KMAXES for bwd in (False, True)]
-        out += [f"hard_{d}_kernel<{T}>/{b}" for d in ("fwd", "bwd") for b in ("warp", "thread")]
+        out += [f"hard_kernel<{T},{str(bwd).lower()}>/{b}" for bwd in (False, True) for b in ("warp", "thread")]
         out += [f"poly_soft_kernel<{T},{str(bwd).lower()}>" for bwd in (False, True)]
         out += [f"dice_{d}_kernel<{T}>/{v}" for d in ("sums", "bwd") for v in ("vec", "scalar")]
         out += [f"cce_kernel<{T},{str(bwd).lower()}>/{b}" for bwd in (False, True) for b in ("warp", "thread")]
         out += [f"mcl_row_lse_kernel<{T}>/{v}" for v in ("vec", "scalar")]
         out += [f"mcl_{k}_kernel<{T}>" for k in ("fwd", "rdot", "bwd")]
-    return tuple(out) + ("finalize_kernel", "finalize_soft_kernel", "finalize3_kernel", "dice_finalize_kernel")
+    return tuple(out) + ("finalize_kernel<2>", "finalize_kernel<3>", "dice_finalize_kernel")
 
 
 # every kernel instantiation in losses.cu, one entry per side of a kernel's S == 1 / vec branch
@@ -153,11 +153,11 @@ def route(cs: Case, sms: int) -> Dict[str, Launch]:
                 gx = grid_for(p // v, THREADS, sms)
                 out[d] = Launch(f"{kern}<{T},{kmax(cs.k)},{str(bwd).lower()}>", p // v, gx * THREADS, gx)
             elif cs.family == "hard":
-                out[d] = _lanes(cs, f"hard_{d}_kernel<{T}>", sms)
+                out[d] = _lanes(cs, f"hard_kernel<{T},{str(bwd).lower()}>", sms)
             else:
                 gx = grid_for(p, THREADS, sms)
                 out[d] = Launch(f"poly_soft_kernel<{T},{str(bwd).lower()}>", p, gx * THREADS, gx)
-        out["finalize"] = Launch("finalize_kernel" if cs.family == "hard" else "finalize_soft_kernel", 0, 1, 1, 32)
+        out["finalize"] = Launch("finalize_kernel<2>", 0, 1, 1, 32)
         return out
     if cs.family == "dice":
         vec, v = dice_vec(cs), vec16_width(cs.dtype)
@@ -172,13 +172,13 @@ def route(cs: Case, sms: int) -> Dict[str, Launch]:
                 "bwd": Launch(f"dice_bwd_kernel<{T}>/{tag}", btotal, bgrid * THREADS, bgrid)}
     if cs.family == "cce":
         return {"fwd": _lanes(cs, f"cce_kernel<{T},false>", sms), "bwd": _lanes(cs, f"cce_kernel<{T},true>", sms),
-                "finalize": Launch("finalize3_kernel", 0, 1, 1, 32)}
+                "finalize": Launch("finalize_kernel<3>", 0, 1, 1, 32)}
     if cs.family == "mcl":
         vec = cs.s % vec16_width(cs.dtype) == 0 and _aligned(cs, 16)
         gx = grid_for(p, THREADS, sms)
         return {"row_lse": Launch(f"mcl_row_lse_kernel<{T}>/{'vec' if vec else 'scalar'}", 0, 1, cs.n * cs.k),
                 "fwd": Launch(f"mcl_fwd_kernel<{T}>", p, gx * THREADS, gx),
-                "finalize": Launch("finalize3_kernel", 0, 1, 1, 32),
+                "finalize": Launch("finalize_kernel<3>", 0, 1, 1, 32),
                 "rdot": Launch(f"mcl_rdot_kernel<{T}>", 0, 1, cs.n * cs.cnum, mcl_rdot_threads(cs.xi)),
                 "bwd": Launch(f"mcl_bwd_kernel<{T}>", p, gx * THREADS, gx)}
     raise ValueError(cs.family)

@@ -2,12 +2,14 @@
 per-element bounds of tests/_loss_oracle.py, without a GPU.
 
 The routing mirror must send the cases through every kernel instantiation of csrc/losses.cu at the SM counts of both
-H100 variants, and the cases tagged ``wrap`` must give every thread of every grid-stride launch a second iteration. The
+H100 variants, its list of instantiations must be the set of kernels the compiler built from losses.cu, and the cases tagged ``wrap`` must give every thread of every grid-stride launch a second iteration. The
 entry points must refuse malformed shapes with cudaErrorInvalidValue before they launch or query a device: they are
 called with null pointers in a child process that sees no CUDA device. And the bounds must not be vacuous: each planted
 fault, applied to the fp64 reference, must break the bound of at least one element of every case it applies to."""
 import json
 import os
+import re
+import shutil
 import subprocess
 import sys
 from pathlib import Path
@@ -47,7 +49,31 @@ def test_wrap_cases_wrap(sms):
                 assert launch.min_iters >= 2, D.describe(cs, sms)
     paths = {D.route(cs, sms)["fwd"].kernel.split("<")[0] + D.route(cs, sms)["fwd"].kernel.split(">")[-1]
              for cs in wraps if cs.family == "hard"}
-    assert paths == {"hard_vec_kernel", "hard_fwd_kernel/thread", "hard_fwd_kernel/warp"}
+    assert paths == {"hard_vec_kernel", "hard_kernel/thread", "hard_kernel/warp"}
+
+
+def test_mirror_lists_the_compiled_kernels():
+    """The mirror's instantiations, without their /warp /thread /vec /scalar branch names, are exactly the entry functions
+    in the -Xptxas -v output that holocron_b200/csrc/build.py keeps in csrc/build/losses.log."""
+    log = ROOT / "holocron_b200" / "csrc" / "build" / "losses.log"
+    if not log.exists():
+        pytest.skip(f"{log.name} absent: build the library first (python -m holocron_b200.csrc.build)")
+    mangled = re.findall(r"Compiling entry function '(\w+)'", log.read_text())
+    assert mangled, f"{log.name} holds no ptxas -v output"
+    tool = shutil.which("cu++filt") or shutil.which("c++filt")
+    if tool is None:
+        pytest.skip("no demangler (cu++filt or c++filt) on PATH")
+    lines = subprocess.run([tool], input="\n".join(mangled), capture_output=True, text=True, check=True).stdout.split("\n")
+    compiled = []
+    for line in lines[:len(mangled)]:
+        # c++filt: "void (anonymous namespace)::k<float, 4, false>(...)"; cu++filt: "void <unnamed>::k<float, (int)4, (bool)0>(...)"
+        name = re.sub(r"\(anonymous namespace\)::|<unnamed>::|\(int\)", "", line).removeprefix("void ")
+        name = name.replace("(bool)0", "false").replace("(bool)1", "true")
+        compiled.append(name.split("(")[0].replace(" ", ""))
+    assert len(set(compiled)) == len(compiled), compiled
+    mirror = {k.split("/")[0] for k in D.INSTANTIATIONS}
+    assert set(compiled) == mirror, (f"compiled, not in the mirror: {sorted(set(compiled) - mirror)}; "
+                                     f"in the mirror, not compiled: {sorted(mirror - set(compiled))}")
 
 
 def test_case_geometry():
