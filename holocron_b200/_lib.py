@@ -137,6 +137,8 @@ SIGNATURES = {
     "hb_ralars_step": "ppii" + "fffffff" + "ifi" + "pp",
     "hb_lookahead_sync": "ppi" + "f" + "p",
     "hb_resample_batch": "p" + "i" * 8 + "p",
+    "hb_detect_scratch_bytes": "piii",
+    "hb_detect": "piii" + "p" * 6,
 }
 _CTYPE = {"p": ctypes.c_void_p, "i": ctypes.c_int, "z": ctypes.c_size_t, "f": ctypes.c_float, "q": ctypes.c_longlong}
 

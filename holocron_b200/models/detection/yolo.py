@@ -30,6 +30,7 @@ from ...ops.boxes import box_iou
 from .._blocks import FusedSequential
 from ..classification.darknet import DarknetBodyV1
 from ..utils import conv_sequence
+from ._postprocess import Segment, detect_padded, kernel_takes, to_detections
 
 __all__ = ["YOLOv1", "yolov1"]
 
@@ -124,7 +125,18 @@ class _YOLO(nn.Module):
 
     def post_process(self, b_coords: Tensor, b_o: Tensor, b_scores: Tensor, grid_shape: Tuple[int, int],
                      rpn_nms_thresh: float = 0.7, box_score_thresh: float = 0.05) -> List[Dict[str, Tensor]]:
-        """Objectness >= 0.5, class confidence x objectness >= ``box_score_thresh``, NMS (reference yolo.py:160-233)."""
+        """Objectness >= 0.5, class confidence x objectness >= ``box_score_thresh``, NMS (reference yolo.py:160-233).
+        CUDA inputs go through the batched kernels of ``csrc/detect.cu`` when they reproduce the loop exactly (see
+        :func:`~._postprocess.kernel_takes`): one launch chain for the batch and one device-to-host copy. Other inputs
+        take the reference's per-image loop."""
+        if b_o.is_cuda:
+            seg = self._segment(b_coords, b_o, b_scores, grid_shape, rpn_nms_thresh, box_score_thresh)
+            if kernel_takes(seg[0], b_o, b_scores):
+                padded = detect_padded([seg])
+                if b_o.dtype == torch.float32:
+                    return to_detections(*padded)
+                # an image without any candidate past objectness gets empty tensors of b_o's dtype in the reference
+                return to_detections(*padded, no_candidate=~(b_o >= 0.5).any(dim=1), empty_dtype=b_o.dtype)
         pred_xyxy = self.to_isoboxes(b_coords.reshape(-1, *grid_shape, self.num_anchors, 4), grid_shape,
                                      clamp=True).reshape(b_o.shape[0], -1, 4)
         detections = []
@@ -143,6 +155,27 @@ class _YOLO(nn.Module):
                 coords, scores, labels = coords[kept_idxs], scores[kept_idxs], labels[kept_idxs]
             detections.append({"boxes": coords, "scores": scores, "labels": labels})
         return detections
+
+    def _segment(self, b_coords: Tensor, b_o: Tensor, b_scores: Tensor, grid_shape: Tuple[int, int],
+                 rpn_nms_thresh: float, box_score_thresh: float) -> Segment:
+        """post_process's inputs as one kernel segment: unclamped xyxy boxes [B, M, 4] (the kernel clamps them),
+        objectness and class scores widened to fp32 (exact; the reference forms their product in fp32)."""
+        pred_xyxy = self.to_isoboxes(b_coords.reshape(-1, *grid_shape, self.num_anchors, 4), grid_shape,
+                                     clamp=False).reshape(b_o.shape[0], -1, 4)
+        return pred_xyxy, b_o.float(), b_scores.float(), box_score_thresh, rpn_nms_thresh
+
+    def detect_padded(self, x: Tensor) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """The detections of the eval forward as padded device tensors, with no host synchronisation at all (an eval
+        forward that can be captured in a CUDA graph): ``boxes [B, cap, 4]``, ``scores [B, cap]``, ``labels [B, cap]``
+        (int64) and ``counts [B]`` (int32), cap = H * W * num_anchors. Image b's detections are the first
+        ``counts[b]`` rows, equal to ``forward(x)[b]`` in the model's current mode (call it in eval mode)."""
+        if isinstance(x, (list, tuple)):
+            x = torch.stack(x, dim=0)
+        b_coords, b_o, b_scores = self._format_outputs(self._forward(x))
+        n, grid = b_coords.shape[0], (b_coords.shape[1], b_coords.shape[2])
+        b_scores = b_scores.expand(*b_o.shape, self.num_classes).reshape(n, -1, self.num_classes)
+        return detect_padded([self._segment(b_coords.reshape(n, -1, 4), b_o.reshape(n, -1), b_scores, grid,
+                                            self.rpn_nms_thresh, self.box_score_thresh)])
 
 
 class YOLOv1(_YOLO):

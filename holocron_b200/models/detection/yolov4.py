@@ -20,6 +20,7 @@ from ...ops.boxes import box_iou, ciou_loss
 from .._blocks import FusedSequential
 from ..classification.darknet import DarknetBodyV4
 from ..utils import conv_sequence
+from ._postprocess import Segment, detect_padded, kernel_takes, to_detections
 
 __all__ = ["Neck", "PAN", "YOLOv4", "YoloLayer", "Yolov4Head", "yolov4"]
 
@@ -119,6 +120,18 @@ class YoloLayer(nn.Module):
     @staticmethod
     def post_process(boxes: Tensor, b_o: Tensor, b_scores: Tensor, rpn_nms_thresh: float = 0.7,
                      box_score_thresh: float = 0.05) -> List[Dict[str, Tensor]]:
+        """Reference yolov4.py:303-335. CUDA inputs go through the batched kernels of ``csrc/detect.cu`` when they
+        reproduce the loop exactly (see :func:`~._postprocess.kernel_takes`): one launch chain for the batch and one
+        device-to-host copy (the per-image counts). Other inputs take the reference's per-image loop."""
+        if b_o.is_cuda and kernel_takes(boxes, b_o, b_scores):
+            return to_detections(*detect_padded([YoloLayer._segment(boxes, b_o, b_scores, rpn_nms_thresh,
+                                                                    box_score_thresh)]))
+        return YoloLayer._post_process_per_image(boxes, b_o, b_scores, rpn_nms_thresh, box_score_thresh)
+
+    @staticmethod
+    def _post_process_per_image(boxes: Tensor, b_o: Tensor, b_scores: Tensor, rpn_nms_thresh: float,
+                                box_score_thresh: float) -> List[Dict[str, Tensor]]:
+        """The reference's loop over images (boolean-mask gathers, one torchvision nms per image)."""
         b_o = torch.sigmoid(b_o)
         b_scores = torch.sigmoid(b_scores)
         boxes = boxes.clamp(0, 1)
@@ -138,6 +151,14 @@ class YoloLayer(nn.Module):
                 labels = torch.zeros(0, dtype=torch.long, device=b_o.device)
             detections.append({"boxes": coords, "scores": scores, "labels": labels})
         return detections
+
+    @staticmethod
+    def _segment(boxes: Tensor, b_o: Tensor, b_scores: Tensor, rpn_nms_thresh: float, box_score_thresh: float) -> Segment:
+        """post_process's inputs as one kernel segment: the (B, H, W, A) candidates flattened in the order of the
+        reference's boolean masks, objectness and class probabilities through the same sigmoid, then widened to fp32."""
+        n = b_o.shape[0]
+        return (boxes.reshape(n, -1, 4), torch.sigmoid(b_o).float().reshape(n, -1),
+                torch.sigmoid(b_scores).float().reshape(n, -1, b_scores.shape[-1]), box_score_thresh, rpn_nms_thresh)
 
     def _assignment(self, b: int, h: int, w: int, na: int, target: List[Dict[str, Tensor]], dev):
         """Per ground-truth box: image index, cell, best-shape anchor, linear index of its (image, cell, anchor) slot and
@@ -235,7 +256,11 @@ class YoloLayer(nn.Module):
 
 
 class Yolov4Head(nn.Module):
-    """Three detection heads with their down-sampling bridges (reference yolov4.py:445-640)."""
+    """Three detection heads with their down-sampling bridges (reference yolov4.py:445-640).
+
+    In eval mode on CUDA, ``forward`` decodes the three scales with each YoloLayer's ``_format_outputs`` and thresholds
+    and post-processes them in one kernel chain; it does not call ``yolo1`` / ``yolo2`` / ``yolo3`` as modules, so
+    forward hooks registered on the YoloLayers do not fire on that path (they do in training and on CPU)."""
 
     def __init__(self, num_classes: int = 80, anchors: Optional[Tensor] = None, act_layer=None, norm_layer=None,
                  drop_layer=None, conv_layer=None) -> None:
@@ -269,11 +294,27 @@ class Yolov4Head(nn.Module):
             head[-1].weight.data.zero_()
             head[-1].bias.data.zero_()
 
-    def forward(self, feats: List[Tensor], target: Optional[List[Dict[str, Tensor]]] = None):
+    def _heads(self, feats: List[Tensor]) -> Tuple[Tensor, Tensor, Tensor]:
         o1 = self.head1(feats[0])
         h2 = self.head2_1(torch.cat([self.pre_head2(feats[0]), feats[1]], dim=1))
         o2 = self.head2_2(h2)
         o3 = self.head3(torch.cat([self.pre_head3(h2), feats[2]], dim=1))
+        return o1, o2, o3
+
+    def _detect(self, outs: Tuple[Tensor, Tensor, Tensor]) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """The three scales as three segments of ONE kernel chain: suppressed per scale with each layer's thresholds,
+        concatenated per image in scale order on the device."""
+        return detect_padded([layer._segment(*layer._format_outputs(o), layer.rpn_nms_thresh, layer.box_score_thresh)
+                              for layer, o in zip((self.yolo1, self.yolo2, self.yolo3), outs)])
+
+    def detect_padded(self, feats: List[Tensor]) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """See :meth:`YOLOv4.detect_padded`."""
+        return self._detect(self._heads(feats))
+
+    def forward(self, feats: List[Tensor], target: Optional[List[Dict[str, Tensor]]] = None):
+        o1, o2, o3 = self._heads(feats)
+        if not self.training and o1.is_cuda:     # one read-back for the batch, not one per scale
+            return to_detections(*self._detect((o1, o2, o3)))
         y1, y2, y3 = self.yolo1(o1, target), self.yolo2(o2, target), self.yolo3(o3, target)
         if not self.training:
             return [{k: torch.cat((d1[k], d2[k], d3[k]), dim=0) for k in ("boxes", "scores", "labels")}
@@ -310,6 +351,15 @@ class YOLOv4(nn.Module):
         out = self.backbone(x)
         x20, x13, x6 = self.neck(out)
         return self.head((x20, x13, x6), target)
+
+    def detect_padded(self, x: Tensor) -> Tuple[Tensor, Tensor, Tensor, Tensor]:
+        """The detections of the eval forward as padded device tensors, with no host synchronisation at all (an eval
+        forward that can be captured in a CUDA graph): ``boxes [B, cap, 4]``, ``scores [B, cap]``, ``labels [B, cap]``
+        (int64) and ``counts [B]`` (int32), cap = the candidates of the three scales. Image b's detections are the first
+        ``counts[b]`` rows, equal to ``forward(x)[b]`` in the model's current mode (call it in eval mode)."""
+        if not isinstance(x, torch.Tensor):
+            x = torch.stack(x, dim=0)
+        return self.head.detect_padded(list(self.neck(self.backbone(x))))
 
 
 def yolov4(pretrained: bool = False, progress: bool = True, pretrained_backbone: bool = False, **kwargs: Any) -> YOLOv4:

@@ -485,6 +485,28 @@ int hb_grad_clip_norm(float* grads, long long n, float max_norm, double* scratch
 int hb_resample_batch(const void* descs, int N, int canvas_h, int canvas_w, int filter, int antialias, int taps_y,
                       int taps_x, int dtype, void* stream);
 
+/* ---- YOLO inference post-processing (holocron/models/detection/yolo.py:159-233, yolov4.py:303-335) ------------------
+ * One segment = one set of decoded candidates per image: boxes fp32 [B, M, 4] xyxy (16-byte aligned), objectness fp32
+ * [B, M] and class scores fp32 [B, M, K], all contiguous, with its own thresholds (YOLOv1/v2: one segment; YOLOv4: one
+ * per scale, suppressed independently and concatenated in segment order). Per image and segment: candidates with
+ * objectness >= 0.5 and score = (first) max over classes * objectness >= score_thresh, boxes clamped to [0, 1], sorted
+ * by score (descending, equal scores in candidate order), then non-maximum suppression at IoU > iou_thresh with
+ * torchvision's arithmetic. Outputs, padded to cap = sum of M: out_boxes fp32 [B, cap, 4], out_scores fp32 [B, cap],
+ * out_labels int64 [B, cap] (kept detections first, zeros after), counts int32 [B]. No host synchronisation, no atomics.
+ * scratch: hb_detect_scratch_bytes(...) bytes, 256-byte aligned (0 = invalid table: nseg outside 1..4, B < 0, K < 1,
+ * M outside 0..2^20, more than 65535 (image, segment) pairs or a cap over 2^31 - 1). */
+typedef struct hb_detect_seg {
+  const float* boxes;
+  const float* obj;
+  const float* cls;
+  int M;
+  float score_thresh;
+  float iou_thresh;
+} hb_detect_seg;
+size_t hb_detect_scratch_bytes(const hb_detect_seg* segs, int nseg, int B, int K);
+int hb_detect(const hb_detect_seg* segs, int nseg, int B, int K, void* scratch, float* out_boxes, float* out_scores,
+              long long* out_labels, int* counts, void* stream);
+
 /* ---- bookkeeping (not part of the reference surface) ------------------------------------------------ */
 long long hb_launch_count(void);      /* kernels launched through this library since the last reset */
 void hb_launch_count_reset(void);
