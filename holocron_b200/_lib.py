@@ -137,6 +137,7 @@ SIGNATURES = {
     "hb_ralars_step": "ppii" + "fffffff" + "ifi" + "pp",
     "hb_lookahead_sync": "ppi" + "f" + "p",
     "hb_resample_batch": "p" + "i" * 8 + "p",
+    "hb_erase_batch": "pp" + "i" * 4 + "p",
     "hb_detect_scratch_bytes": "piii",
     "hb_detect": "piii" + "p" * 6,
 }

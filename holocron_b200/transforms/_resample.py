@@ -3,7 +3,9 @@
 ``resample`` takes a batch of images, each with the inner size it is resized to and the signed offset of that inner box
 on a common canvas, validates what torchvision would refuse before anything is launched, writes one descriptor row per
 image into pinned host memory, uploads the table asynchronously (no host synchronisation) and launches one kernel that
-resizes every image and fills its canvas."""
+resizes every image and fills its canvas. An image may be cropped to a box first (its row then points at the box's
+top-left pixel and has the box's size) and mirrored left-right (its row points at the last column with a negated column
+stride): the kernel reads both as any other strided source."""
 import math
 from typing import List, Optional, Sequence, Tuple
 
@@ -63,28 +65,43 @@ def _check_padding(pad_mode: str, pads: Tuple[int, int, int, int], h: int, w: in
 
 
 def descriptor_table(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]], canvas: Tuple[int, int],
-                     filter_code: int, antialias: bool, pad_mode: str) -> Tuple[np.ndarray, int, int]:
+                     filter_code: int, antialias: bool, pad_mode: str,
+                     boxes: Optional[Sequence[Tuple[int, int, int, int]]] = None,
+                     flips: Optional[Sequence[bool]] = None) -> Tuple[np.ndarray, int, int]:
     """(table, taps_y, taps_x): the int64 [N_total, 16] descriptor rows of hb_resample_batch, destination pointers left
-    at 0, and the most filter taps per axis. Raises what torchvision would raise for these placements."""
+    at 0, and the most filter taps per axis. Raises what torchvision would raise for these placements.
+
+    ``boxes[i] = (top, left, height, width)`` crops source i to that box (inside the image) before it is resized;
+    ``flips[i]`` mirrors it left-right."""
     ref = sources[0]
     C = ref.shape[-3]
     Hc, Wc = canvas
     rows: List[List[int]] = []
     taps_y = taps_x = 1
-    for x, (h, w) in zip(sources, inner):
+    for k, (x, (h, w)) in enumerate(zip(sources, inner)):
         if x.dtype != ref.dtype or x.device != ref.device or x.ndim < 3 or x.shape[-3] != C:
             raise ValueError("images of one call must share their dtype, device and channel count")
         H, W = x.shape[-2:]
+        sc, sh, sw = x.stride()[-3:]
+        base = x.data_ptr()
+        if boxes is not None:
+            bi, bj, bh, bw = boxes[k]
+            if bi < 0 or bj < 0 or bi + bh > H or bj + bw > W:
+                raise ValueError(f"crop box {tuple(boxes[k])} is not inside the {H}x{W} image")
+            base += (bi * sh + bj * sw) * x.element_size()
+            H, W = bh, bw
+        if flips is not None and flips[k]:
+            base += (W - 1) * sw * x.element_size()
+            sw = -sw
         if h <= 0 or w <= 0 or H <= 0 or W <= 0:
             raise RuntimeError(f"Input and output sizes should be greater than 0, but got input (H: {H}, W: {W}) "
                                f"output (H: {h}, W: {w})")
         dh, dw = Hc - h, Wc - w
         top, left = dh // 2, dw // 2
         _check_padding(pad_mode, (left, top, dw - left, dh - top), h, w)
-        sc, sh, sw = x.stride()[-3:]
-        if (W - 1) * sw > _INT32_MAX:
+        if (W - 1) * abs(sw) > _INT32_MAX:
             raise ValueError("image rows span more than 2**31 elements")
-        row = [x.data_ptr(), 0, sc, sh, sw, C, H, W, h, w, top, left, Hc, Wc, PAD_MODES[pad_mode], 0]
+        row = [base, 0, sc, sh, sw, C, H, W, h, w, top, left, Hc, Wc, PAD_MODES[pad_mode], 0]
         # leading dimensions of a source are images of their own
         offsets = [0]
         for n_k, s_k in zip(x.shape[:-3], x.stride()[:-3]):
@@ -101,11 +118,13 @@ def descriptor_table(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]]
 
 def resample(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]], canvas: Tuple[int, int],
              interpolation: InterpolationMode, antialias: bool, pad_mode: str = "constant",
-             out: Optional[Tensor] = None) -> Tensor:
+             out: Optional[Tensor] = None, boxes: Optional[Sequence[Tuple[int, int, int, int]]] = None,
+             flips: Optional[Sequence[bool]] = None) -> Tensor:
     """Resizes sources[i] ([..., C, H_i, W_i], CUDA, any strides) to inner[i] = (h_i, w_i) and centres it on a canvas
     of ``canvas`` = (Hc, Wc) the way torchvision's ``pad`` places it (left / top padding = floor(delta / 2), negative
     padding crops), filling the rest by ``pad_mode``. Returns ``out``, a contiguous tensor of shape
-    (N_total, C, Hc, Wc) holding one canvas per source image (leading dimensions of a source count as images)."""
+    (N_total, C, Hc, Wc) holding one canvas per source image (leading dimensions of a source count as images).
+    ``boxes`` and ``flips`` (one entry per source) crop and mirror the sources first (``descriptor_table``)."""
     if pad_mode not in PAD_MODES:
         raise ValueError("Padding mode should be either constant, edge, reflect or symmetric")
     filter_code = interpolation_code(interpolation)
@@ -114,7 +133,7 @@ def resample(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]], canvas
     require_cuda(*sources)
     if ref.dtype not in DTYPES:
         raise TypeError(f"unsupported dtype {ref.dtype}: expected one of {', '.join(map(str, DTYPES))}")
-    table, taps_y, taps_x = descriptor_table(sources, inner, canvas, filter_code, antialias, pad_mode)
+    table, taps_y, taps_x = descriptor_table(sources, inner, canvas, filter_code, antialias, pad_mode, boxes, flips)
     n, C, (Hc, Wc) = table.shape[0], ref.shape[-3], canvas
     if out is None:
         out = torch.empty((n, C, Hc, Wc), dtype=ref.dtype, device=ref.device)

@@ -1,0 +1,142 @@
+"""``RandomResizedCrop``, ``RandomHorizontalFlip`` and ``RandomErasing`` of torchvision, the random transforms of the
+reference's classification training recipe (references/classification/train.py:101-107), on one CUDA launch per call.
+
+Each subclasses the torchvision class of the same name: constructor, validation, attributes and ``repr`` are
+torchvision's, and the random draws are torchvision's own ``get_params`` (and ``torch.rand(1) < p``), called in
+torchvision's order on the default CPU generator. Only ``forward`` differs, in what it takes:
+
+- one tensor: what the torchvision class does to that tensor (one draw, leading dimensions carried along);
+- a list or tuple of ``(C, H_i, W_i)`` CUDA tensors: one draw set per image, in list order, so a seeded list call draws
+  exactly what calling the torchvision module image by image draws, and one launch for the whole list, which returns
+  the stacked ``(N, C, h, w)`` result. ``RandomResizedCrop`` returns canvases of ``size``; ``RandomHorizontalFlip`` and
+  ``RandomErasing`` take images of one shape and raise ``ValueError`` otherwise, before any draw. Sources are read in
+  place whatever their strides: pass a stacked batch as ``batch.unbind(0)``;
+- ``RandomErasing(inplace=True)`` writes only the rectangles, into the given tensors, and returns the input as given.
+
+A chain of batched calls does not draw what a per-image ``T.Compose`` of the same transforms draws: the chain makes
+every image's crop draws, then every image's flip draw, and so on, where ``Compose`` goes image by image. Each single
+call is draw-for-draw with its torchvision class.
+
+Outputs are torchvision's on CUDA tensors: crops are resampled by the kernel of ``Resize`` (torchvision's filters with
+torch's CUDA arithmetic), flips are exact copies, and erased pixels hold the fp32 values cast to the image dtype as
+torch's copy casts them. Deviations: PIL images and CPU tensors raise ``HolocronB200Error``; dtypes other than uint8,
+fp16, bf16, fp32 and fp64 raise ``TypeError``; a crop needing more than 255 filter taps per axis (antialiased
+downscales beyond about 1/127 bilinear, 1/63 bicubic) raises ``NotImplementedError``.
+"""
+from typing import List, Optional, Tuple
+
+import torch
+from torch import Tensor
+from torchvision.transforms import transforms as T
+from torchvision.transforms.functional import InterpolationMode
+
+from ._erase import Rect, erase
+from ._resample import resample
+from .interpolation import Images, _batch, _finish, _resize_options
+
+__all__ = ["RandomErasing", "RandomHorizontalFlip", "RandomResizedCrop"]
+
+
+def _one_shape(images: Images, items: List[Tensor]) -> None:
+    if isinstance(images, (list, tuple)) and any(x.shape != items[0].shape for x in items):
+        raise ValueError(f"{type(images).__name__} of images of different shapes: this transform stacks images of one "
+                         "shape (RandomResizedCrop resizes them to one)")
+
+
+def _planes(items: List[Tensor]) -> List[Tensor]:
+    return [x if x.ndim >= 3 else x.unsqueeze(0) for x in items]
+
+
+class RandomResizedCrop(T.RandomResizedCrop):
+    """torchvision's ``RandomResizedCrop`` on a batched CUDA resampling kernel: a random box of each image, resized to
+    ``size``.
+
+    >>> import torch
+    >>> from holocron_b200.transforms import RandomResizedCrop
+    >>> tf = RandomResizedCrop(176, scale=(0.3, 1.0))
+    >>> out = tf([torch.randint(0, 256, (3, 300, 400), dtype=torch.uint8, device="cuda"),
+    ...           torch.randint(0, 256, (3, 500, 350), dtype=torch.uint8, device="cuda")])
+    """
+
+    def forward(self, img: Images) -> Tensor:
+        items = _batch(img, three_d=False)
+        boxes = [self.get_params(x, self.scale, self.ratio) for x in items]
+        size = (int(self.size[0]), int(self.size[1]))
+        interpolation, antialias = _resize_options(self.interpolation, None, self.antialias)
+        if isinstance(img, Tensor):
+            if tuple(boxes[0][2:]) == size:
+                # torchvision's resize hands back the crop itself when it already has the target size
+                i, j, h, w = boxes[0]
+                return img[..., i:i + h, j:j + w]
+            if img.ndim == 2:  # torchvision's resize refuses what torch's interpolate refuses
+                raise ValueError("Input and output must have the same number of spatial dimensions, but got input "
+                                 f"with spatial dimensions of {[img.shape[-1]]} and output size of {list(size)}.")
+        out = resample(_planes(items), [size] * len(items), size, interpolation, antialias, boxes=boxes)
+        return _finish(img, out, size)
+
+
+class RandomHorizontalFlip(T.RandomHorizontalFlip):
+    """torchvision's ``RandomHorizontalFlip`` on a batched CUDA kernel: each image is mirrored left-right with
+    probability ``p``.
+
+    >>> import torch
+    >>> from holocron_b200.transforms import RandomHorizontalFlip
+    >>> batch = torch.rand(8, 3, 176, 176, device="cuda")
+    >>> out = RandomHorizontalFlip()(batch.unbind(0))
+    """
+
+    def forward(self, img: Images) -> Images:
+        items = _batch(img, three_d=False)
+        _one_shape(img, items)
+        flips = [bool(torch.rand(1) < self.p) for _ in items]
+        if isinstance(img, Tensor) and not flips[0]:
+            return img
+        size = (int(items[0].shape[-2]), int(items[0].shape[-1]))
+        # a nearest resample at the image's own size is an exact copy; a flip reads the columns backwards
+        out = resample(_planes(items), [size] * len(items), size, InterpolationMode.NEAREST, False, flips=flips)
+        return _finish(img, out, size)
+
+
+class RandomErasing(T.RandomErasing):
+    """torchvision's ``RandomErasing`` on a batched CUDA kernel: with probability ``p``, a random rectangle of each
+    image is filled with ``value`` (one number, one per channel, or ``"random"``: per-pixel standard normal draws, made
+    on the host by torchvision's ``get_params``).
+
+    >>> import torch
+    >>> from holocron_b200.transforms import RandomErasing
+    >>> batch = torch.rand(8, 3, 176, 176, device="cuda")
+    >>> out = RandomErasing(p=1.0, scale=(0.02, 0.2), value="random")(batch.unbind(0))
+    """
+
+    def _draw(self, x: Tensor) -> Tuple[bool, Optional[Rect]]:
+        """torchvision's forward up to ``F.erase`` for one image: whether it erases, and the rectangle and values, None
+        when get_params found no rectangle in its 10 attempts (torchvision then assigns the image to itself)."""
+        if not torch.rand(1) < self.p:
+            return False, None
+        if isinstance(self.value, (int, float)):
+            value = [float(self.value)]
+        elif isinstance(self.value, str):
+            value = None
+        elif isinstance(self.value, (list, tuple)):
+            value = [float(v) for v in self.value]
+        else:
+            value = self.value
+        if value is not None and len(value) not in (1, x.shape[-3]):
+            raise ValueError("If value is a sequence, it should have either a single value or "
+                             f"{x.shape[-3]} (number of input channels)")
+        i, j, h, w, v = self.get_params(x, scale=self.scale, ratio=self.ratio, value=value)
+        return True, (None if v is x else (i, j, h, w, v))
+
+    def forward(self, img: Images) -> Images:
+        items = _batch(img, three_d=False)
+        _one_shape(img, items)
+        draws = [self._draw(x) for x in items]
+        if isinstance(img, Tensor):
+            chosen, rect = draws[0]
+            # torchvision hands back the input unless it erases a copy
+            if not chosen or (rect is None and self.inplace):
+                return img
+        out = erase(_planes(items), [rect for _, rect in draws], self.inplace)
+        if self.inplace:
+            return img
+        return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))

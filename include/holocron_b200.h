@@ -484,6 +484,22 @@ int hb_grad_clip_norm(float* grads, long long n, float max_norm, double* scratch
  * fp64; uint8 results are clamped to [0, 255] and rounded half to even). */
 int hb_resample_batch(const void* descs, int N, int canvas_h, int canvas_w, int filter, int antialias, int taps_y,
                       int taps_x, int dtype, void* stream);
+/* Crop boxes and horizontal flips (torchvision RandomResizedCrop, RandomHorizontalFlip) are hb_resample_batch rows: a
+ * crop (i, j, h, w) points src at pixel (i, j) with H, W = h, w; a flip points src at the last column and negates
+ * stride_w (resampled at its own size with the nearest filter, an exact copy). */
+
+/* ---- random erasing: torchvision.transforms.RandomErasing (get_params: rectangle and values drawn on the host;
+ *      forward: F.erase, img[..., i:i+h, j:j+w] = v on a clone or in place), as the reference's classification recipe
+ *      applies it (references/classification/train.py:101-107) - a batch of images in one launch ----------------- */
+/* descs: device table of N rows of 16 int64 {src, dst, stride_c, stride_h, stride_w, C, H, W, top, left, h, w, fill,
+ * voff, 0, 0}: pointers are addresses, strides count elements. dst != src: dst is a contiguous [C][H][W] copy of the
+ * strided src with the rectangle rows [top, top+h) x columns [left, left+w) filled; dst == src: only the rectangle is
+ * written, in place through the source strides. fill: 0 none (nothing erased), 1 one value per channel at
+ * values[voff + c], 2 one value per pixel at values[voff + (c*h + y)*w + x]. values: fp32, cast as torch's copy casts
+ * (fp16 / bf16 round to nearest even, uint8 = (uint8_t)(int64_t)v, fp64 exact). rows: the most row segments an image
+ * writes (C*H when copying, C*h in place); row_len: the longest segment (W when copying, w in place). dtype: as for
+ * hb_resample_batch. */
+int hb_erase_batch(const void* descs, const float* values, int N, int rows, int row_len, int dtype, void* stream);
 
 /* ---- YOLO inference post-processing (holocron/models/detection/yolo.py:159-233, yolov4.py:303-335) ------------------
  * One segment = one set of decoded candidates per image: boxes fp32 [B, M, 4] xyxy (16-byte aligned), objectness fp32
