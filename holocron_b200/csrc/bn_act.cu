@@ -677,17 +677,6 @@ __global__ void __launch_bounds__(kFinCh * kFinLanes) bn_bwd_finalize_kernel(Bwd
   }
 }
 
-// persistent grid: `per_sm` blocks per SM, grid-stride over rows
-inline dim3 make_grid(const SlabGeo& g, int M, int z, int per_sm = 4, int min_rows = 4) {
-  long long row_blocks = ((long long)M + g.rows_t - 1) / g.rows_t;
-  long long cap = (HB_NUM_SMS * per_sm) / g.slabs;
-  if (cap < 1) cap = 1;
-  long long want = (row_blocks + min_rows - 1) / min_rows;   // at least ~min_rows rows per lane when there is enough work
-  if (want < 1) want = 1;
-  if (want > cap) want = cap;
-  return dim3((unsigned)want, (unsigned)g.slabs, (unsigned)z);
-}
-
 inline int env_int(const char* name, int dflt) {
   const char* v = getenv(name);
   return v ? atoi(v) : dflt;
@@ -781,7 +770,7 @@ inline int launch_bwd_reduce(const BwdParams& p, float* dgamma, float* dbeta, fl
   const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_reduce_kernel<decltype(nb)::value>>(smem); });
   if (!occ) return (int)cudaErrorInvalidValue;
   if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_reduce_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_red);
-  const dim3 grid = make_grid(g, p.M, 1, (use_occ && occ < cap_red) ? occ : cap_red);
+  const dim3 grid = g.grid(p.M, (use_occ && occ < cap_red) ? occ : cap_red);
   kernel<<<grid, kThreads, smem, st>>>(p, g);
   HB_LAUNCH_CHECK();
   BwdFinalizeParams f{};
@@ -807,7 +796,7 @@ inline int launch_bwd_apply(const BwdParams& p, cudaStream_t st) {
   const auto [kernel, occ] = with_nb(B, [&](auto nb) { return instance<bn_act_bwd_apply_kernel<decltype(nb)::value>>(smem); });
   if (!occ) return (int)cudaErrorInvalidValue;
   if (occ_debug) fprintf(stderr, "[hb] bn_act_bwd_apply_kernel<%d> smem %zu: %d resident blocks/SM (cap %d)\n", B, smem, occ, cap_app);
-  const dim3 grid = make_grid(g, p.M, 1, (use_occ && occ < cap_app) ? occ : cap_app);
+  const dim3 grid = g.grid(p.M, (use_occ && occ < cap_app) ? occ : cap_app);
   kernel<<<grid, kThreads, smem, st>>>(p, g);
   HB_LAUNCH_CHECK();
   return 0;
@@ -822,7 +811,7 @@ int hb_bn_stats_partials_bf16(const void* u, int M, int C, float* parts, int* sl
   if (C % 8 != 0 || !slots) return (int)cudaErrorInvalidValue;
   const SlabGeo g = SlabGeo::make(C);
   static const int min_rows = env_int("HB_BN_STATS_ROWS", 16);
-  const dim3 grid = make_grid(g, M, 1, 4, min_rows);
+  const dim3 grid = g.grid(M, 4, min_rows);
   *slots = (int)grid.x;
   bn_stats_partials_kernel<<<grid, kThreads, 0, (cudaStream_t)stream>>>((const __nv_bfloat16*)u, M, C, g, parts);
   HB_LAUNCH_CHECK();
@@ -908,7 +897,7 @@ int hb_bn_act_fwd_bf16(const void* u0, const void* u1, const void* u2, int B, co
   const int fixed = (B + (residual != nullptr) >= 3) ? 3 : 4;
   // <= 4 blocks per SM: the caller's out_stats buffer has 4 x SMs slots (bn_stat_slots)
   const int per_sm = per_sm_env > 0 ? (per_sm_env < 4 ? per_sm_env : 4) : (use_occ ? (occ < 4 ? occ : 4) : fixed);
-  const dim3 grid = make_grid(g, M, 1, per_sm);
+  const dim3 grid = g.grid(M, per_sm);
   if (out_stat_slots) *out_stat_slots = (int)grid.x;
   kernel<<<grid, kThreads, smem, st>>>(p, g);
   HB_LAUNCH_CHECK();
@@ -921,7 +910,7 @@ int hb_bn_act_fwd_bf16(const void* u0, const void* u1, const void* u2, int B, co
 // (entries may be NULL) to fp32 [C_logical] gradient buffers that dgamma_b / dbeta_b are ADDED to.
 size_t hb_bn_bwd_scratch_doubles(int M, int C, int B) {
   const SlabGeo g = SlabGeo::make(C);
-  const dim3 grid = make_grid(g, M, 1, 3);   // upper bound of the reduction pass' row blocks (cap <= 3 per SM)
+  const dim3 grid = g.grid(M, 3);   // upper bound of the reduction pass' row blocks (cap <= 3 per SM)
   return (size_t)(1 + B) * C * (1 + (size_t)grid.x);
 }
 

@@ -5,15 +5,24 @@
 // blocks (reference holocron/models/classification/rexnet.py:112-125: dw 3x3, stride 1|2, no bias).
 #include <cstdlib>
 #include "common.cuh"
+#include "slab.cuh"
 
 namespace {
 
 using namespace hb;
 
-constexpr int kThreads = 256;
+constexpr int kThreads = kSlabThreads;
 
 // neighbouring threads re-read the same taps: the L1-allocating load
 __device__ __forceinline__ void load8(const __nv_bfloat16* p, float* f) { unpack8(ld16(p), f); }
+
+// the vector at p when ok, else zeros (p is then not read)
+__device__ __forceinline__ Vec16<__nv_bfloat16> ld16_or_zero(const __nv_bfloat16* p, bool ok) {
+  Vec16<__nv_bfloat16> v;
+  if (ok) v = ld16(p);
+  else v.raw = make_uint4(0, 0, 0, 0);
+  return v;
+}
 
 struct DwParams {
   int N, H, W, C, Ho, Wo, K, stride, pad;
@@ -85,29 +94,45 @@ __global__ void __launch_bounds__(kThreads) dw_bwd_data_kernel(const __nv_bfloat
   }
 }
 
-// ---- 3x3 specialisations: fixed channel group per thread (block = channel groups x pixel lanes, as in the BN
-// kernels), the block's slab of the filter sits in shared memory (float4 reads). The generic kernels above
+// ---- 3x3 specialisations: fixed channel group per thread (block = channel groups x pixel lanes, the SlabGeo of
+// slab.cuh), the block's slab of the filter sits in shared memory (float4 reads). The generic kernels above
 // re-read 72 scalar weights per output vector and recompute the channel group of every element: instruction-bound,
-// far from the HBM time on the ReXNet expansions.
+// far from the HBM time on the ReXNet expansions. The slab kernels read the geometry as a __grid_constant__ parameter:
+// passed as a plain by-value struct, ptxas spills dw3x3_kernel<false, 0>, which has no register to spare at 3 blocks/SM.
+
+// The block's channel slab of the 3x3 filter w [C][9], tap-major: ws[k][ch] = w[slab channel ch][k], or tap 8 - k with
+// kFlip; 0 past the last channel. Ends on a barrier, which every thread of the block has to reach.
+template <bool kFlip>
+__device__ __forceinline__ void stage_filter(float (&ws)[9][256], const float* __restrict__ w, const SlabGeo& g) {
+  const int nch = g.cg_t * 8;
+  for (int i = threadIdx.x; i < 9 * nch; i += kThreads) {
+    const int k = i / nch, ch = i % nch;
+    const int c = blockIdx.y * nch + ch;
+    ws[k][ch] = c < g.cg_total * 8 ? w[c * 9 + (kFlip ? 8 - k : k)] : 0.f;
+  }
+  __syncthreads();
+}
+
+// the 8 staged filter values of tap k for channel group tx of the slab
+__device__ __forceinline__ void tap8(const float (&ws)[9][256], int k, int tx, float* wk) {
+  const float4 a = *reinterpret_cast<const float4*>(&ws[k][tx * 8]);
+  const float4 b = *reinterpret_cast<const float4*>(&ws[k][tx * 8 + 4]);
+  wk[0] = a.x; wk[1] = a.y; wk[2] = a.z; wk[3] = a.w;
+  wk[4] = b.x; wk[5] = b.y; wk[6] = b.z; wk[7] = b.w;
+}
+
 // kStride: 1 or 2 known at compile time (the backward index arithmetic divides by the stride: a runtime divisor costs
 // ~40 instructions per tap, which makes the data-gradient pass instruction bound); 0 = runtime stride.
 template <bool kBackward, int kStride>
 __global__ void __launch_bounds__(kThreads, 3) dw3x3_kernel(const __nv_bfloat16* __restrict__ src, const float* __restrict__ w,
                                                          const float* __restrict__ bias, __nv_bfloat16* __restrict__ dst,
-                                                         DwParams p, int cg_t, int rows_t) {
+                                                         DwParams p, const __grid_constant__ SlabGeo g) {
   // forward:  src = x [N,H,W,C],   dst = y  [N,Ho,Wo,C]: y[ho,wo]  = b + sum_{r,s} x[ho*st+r-pad, wo*st+s-pad] * w[r,s]
   // backward: src = dy [N,Ho,Wo,C], dst = dx [N,H,W,C]:  dx[hi,wi] = sum_{r,s} dy[(hi+pad-r)/st, (wi+pad-s)/st] * w[r,s]
-  __shared__ __align__(16) float ws[9][256];   // the block's channel slab of the filter, tap-major
-  const int cv = p.C / 8;
-  const int tx = threadIdx.x % cg_t, ty = threadIdx.x / cg_t;
-  const int cg = blockIdx.y * cg_t + tx;
-  for (int i = threadIdx.x; i < 9 * cg_t * 8; i += kThreads) {
-    const int k = i / (cg_t * 8), ch = i % (cg_t * 8);
-    const int c = blockIdx.y * cg_t * 8 + ch;
-    ws[k][ch] = c < p.C ? w[c * 9 + k] : 0.f;
-  }
-  __syncthreads();
-  if (ty >= rows_t || cg >= cv) return;
+  __shared__ __align__(16) float ws[9][256];
+  const auto [tx, ty, cg, active] = g.thread();
+  stage_filter<false>(ws, w, g);
+  if (!active) return;
   float b[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) b[j] = (!kBackward && bias) ? bias[cg * 8 + j] : 0.f;
@@ -115,8 +140,8 @@ __global__ void __launch_bounds__(kThreads, 3) dw3x3_kernel(const __nv_bfloat16*
   const int OH = kBackward ? p.H : p.Ho, OW = kBackward ? p.W : p.Wo;   // grid walked by this kernel
   const int IH = kBackward ? p.Ho : p.H, IW = kBackward ? p.Wo : p.W;   // grid of src
   const long long M = (long long)p.N * OH * OW;
-  const long long stride_m = (long long)gridDim.x * rows_t;
-  for (long long m = (long long)blockIdx.x * rows_t + ty; m < M; m += stride_m) {
+  const long long stride_m = (long long)gridDim.x * g.rows_t;
+  for (long long m = (long long)blockIdx.x * g.rows_t + ty; m < M; m += stride_m) {
     // 32-bit index arithmetic (the launcher checks M < 2^31): 64-bit runtime divisions cost ~100 instructions each
     const unsigned mu = (unsigned)m;
     const unsigned t1 = mu / (unsigned)OW;
@@ -151,9 +176,8 @@ __global__ void __launch_bounds__(kThreads, 3) dw3x3_kernel(const __nv_bfloat16*
 #pragma unroll
     for (int k = 0; k < 9; ++k) {
       if (ok[k]) {
-        const float4 w0 = *reinterpret_cast<const float4*>(&ws[k][tx * 8]);
-        const float4 w1 = *reinterpret_cast<const float4*>(&ws[k][tx * 8 + 4]);
-        const float wk[8] = {w0.x, w0.y, w0.z, w0.w, w1.x, w1.y, w1.z, w1.w};
+        float wk[8];
+        tap8(ws, k, tx, wk);
 #pragma unroll
         for (int j = 0; j < 8; ++j) acc[j] = fmaf(__bfloat162float(v[k].v[j]), wk[j], acc[j]);
       }
@@ -173,26 +197,19 @@ __global__ void __launch_bounds__(kThreads, 3) dw3x3_kernel(const __nv_bfloat16*
 template <int kStride, bool kFlip>
 __global__ void __launch_bounds__(kThreads, 2) dw3x3_quad_kernel(const __nv_bfloat16* __restrict__ src, const float* __restrict__ w,
                                                               const float* __restrict__ bias, __nv_bfloat16* __restrict__ dst,
-                                                              int N, int IH, int IW, int OH, int OW, int C, int pad, int cg_t,
-                                                              int rows_t) {
-  __shared__ __align__(16) float ws[9][256];   // the block's channel slab of the filter, tap-major (flipped for kFlip)
-  const int cv = C / 8;
-  const int tx = threadIdx.x % cg_t, ty = threadIdx.x / cg_t;
-  const int cg = blockIdx.y * cg_t + tx;
-  for (int i = threadIdx.x; i < 9 * cg_t * 8; i += kThreads) {
-    const int k = i / (cg_t * 8), ch = i % (cg_t * 8);
-    const int c = blockIdx.y * cg_t * 8 + ch;
-    ws[k][ch] = c < C ? w[c * 9 + (kFlip ? 8 - k : k)] : 0.f;
-  }
-  __syncthreads();
-  if (ty >= rows_t || cg >= cv) return;
+                                                              int N, int IH, int IW, int OH, int OW, int C, int pad,
+                                                              const __grid_constant__ SlabGeo g) {
+  __shared__ __align__(16) float ws[9][256];
+  const auto [tx, ty, cg, active] = g.thread();
+  stage_filter<kFlip>(ws, w, g);
+  if (!active) return;
   float b[8];
 #pragma unroll
   for (int j = 0; j < 8; ++j) b[j] = (!kFlip && bias) ? bias[cg * 8 + j] : 0.f;
   constexpr int kIn = 3 * kStride + 3;          // input columns feeding 4 outputs: (4 - 1) * S + 3
   const int qw = (OW + 3) >> 2;                 // quads per output row
   const unsigned total = (unsigned)N * OH * qw;
-  for (unsigned q = blockIdx.x * rows_t + ty; q < total; q += gridDim.x * rows_t) {
+  for (unsigned q = blockIdx.x * g.rows_t + ty; q < total; q += gridDim.x * g.rows_t) {
     const unsigned t1 = q / (unsigned)qw;
     const int ow0 = (int)(q - t1 * (unsigned)qw) * 4;
     const unsigned n = t1 / (unsigned)OH;
@@ -213,17 +230,11 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_quad_kernel(const __nv_bflo
 #pragma unroll
       for (int c = 0; c < kIn; ++c) {           // all loads of the row in flight before the first use
         const int iw = iw0 + c;
-        if (iw >= 0 && iw < IW) v[c] = ld16(row + (size_t)iw * C);
-        else v[c].raw = make_uint4(0, 0, 0, 0);
+        v[c] = ld16_or_zero(row + (size_t)iw * C, iw >= 0 && iw < IW);
       }
       float wk[3][8];
 #pragma unroll
-      for (int s2 = 0; s2 < 3; ++s2) {
-        const float4 w0 = *reinterpret_cast<const float4*>(&ws[r * 3 + s2][tx * 8]);
-        const float4 w1 = *reinterpret_cast<const float4*>(&ws[r * 3 + s2][tx * 8 + 4]);
-        wk[s2][0] = w0.x; wk[s2][1] = w0.y; wk[s2][2] = w0.z; wk[s2][3] = w0.w;
-        wk[s2][4] = w1.x; wk[s2][5] = w1.y; wk[s2][6] = w1.z; wk[s2][7] = w1.w;
-      }
+      for (int s2 = 0; s2 < 3; ++s2) tap8(ws, r * 3 + s2, tx, wk[s2]);
 #pragma unroll
       for (int c = 0; c < kIn; ++c) {
         float f[8];
@@ -254,22 +265,15 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_quad_kernel(const __nv_bflo
 // 3 - 6 vector loads per 4 outputs; the one-output kernel issues 9 predicated loads per output.
 __global__ void __launch_bounds__(kThreads, 2) dw3x3_dgrad_s2_quad_kernel(const __nv_bfloat16* __restrict__ dy,
                                                                         const float* __restrict__ w, __nv_bfloat16* __restrict__ dx,
-                                                                        int N, int H, int W, int Ho, int Wo, int C, int cg_t,
-                                                                        int rows_t) {
+                                                                        int N, int H, int W, int Ho, int Wo, int C,
+                                                                        const __grid_constant__ SlabGeo g) {
   __shared__ __align__(16) float ws[9][256];
-  const int cv = C / 8;
-  const int tx = threadIdx.x % cg_t, ty = threadIdx.x / cg_t;
-  const int cg = blockIdx.y * cg_t + tx;
-  for (int i = threadIdx.x; i < 9 * cg_t * 8; i += kThreads) {
-    const int k = i / (cg_t * 8), ch = i % (cg_t * 8);
-    const int c = blockIdx.y * cg_t * 8 + ch;
-    ws[k][ch] = c < C ? w[c * 9 + k] : 0.f;
-  }
-  __syncthreads();
-  if (ty >= rows_t || cg >= cv) return;
+  const auto [tx, ty, cg, active] = g.thread();
+  stage_filter<false>(ws, w, g);
+  if (!active) return;
   const int qw = (W + 3) >> 2;
   const unsigned total = (unsigned)N * H * qw;
-  for (unsigned q = blockIdx.x * rows_t + ty; q < total; q += gridDim.x * rows_t) {
+  for (unsigned q = blockIdx.x * g.rows_t + ty; q < total; q += gridDim.x * g.rows_t) {
     const unsigned t1 = q / (unsigned)qw;
     const int w0 = (int)(q - t1 * (unsigned)qw) * 4;
     const unsigned n = t1 / (unsigned)H;
@@ -287,18 +291,10 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_dgrad_s2_quad_kernel(const 
       const __nv_bfloat16* row = dn + (size_t)oh * Wo * C;
       Vec16<__nv_bfloat16> v[3];
 #pragma unroll
-      for (int i = 0; i < 3; ++i) {
-        if (c0 + i < Wo) v[i] = ld16(row + (size_t)(c0 + i) * C);
-        else v[i].raw = make_uint4(0, 0, 0, 0);
-      }
+      for (int i = 0; i < 3; ++i) v[i] = ld16_or_zero(row + (size_t)(c0 + i) * C, c0 + i < Wo);
       float wk[3][8];
 #pragma unroll
-      for (int s2 = 0; s2 < 3; ++s2) {
-        const float4 a = *reinterpret_cast<const float4*>(&ws[r * 3 + s2][tx * 8]);
-        const float4 b = *reinterpret_cast<const float4*>(&ws[r * 3 + s2][tx * 8 + 4]);
-        wk[s2][0] = a.x; wk[s2][1] = a.y; wk[s2][2] = a.z; wk[s2][3] = a.w;
-        wk[s2][4] = b.x; wk[s2][5] = b.y; wk[s2][6] = b.z; wk[s2][7] = b.w;
-      }
+      for (int s2 = 0; s2 < 3; ++s2) tap8(ws, r * 3 + s2, tx, wk[s2]);
       float f[3][8];
 #pragma unroll
       for (int i = 0; i < 3; ++i)
@@ -319,45 +315,16 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_dgrad_s2_quad_kernel(const 
   }
 }
 
-inline dim3 dw_quad_grid(long long quads, int cv, int& cg_t, int& rows_t, int per_sm) {
-  const int nslab = (cv + 31) / 32;
-  cg_t = (cv + nslab - 1) / nslab;
-  rows_t = kThreads / cg_t;
-  const int slabs = (cv + cg_t - 1) / cg_t;
-  long long gx = (quads + rows_t * 2 - 1) / (rows_t * 2);
-  long long cap = (HB_NUM_SMS * per_sm) / slabs;
-  if (cap < 1) cap = 1;
-  if (gx > cap) gx = cap;
-  if (gx < 1) gx = 1;
-  return dim3((unsigned)gx, (unsigned)slabs);
-}
-
-inline dim3 dw_grid(long long M, int cv, int& cg_t, int& rows_t, int per_sm) {
-  const int nslab = (cv + 31) / 32;
-  cg_t = (cv + nslab - 1) / nslab;      // balanced channel slabs (see bn_act.cu)
-  rows_t = kThreads / cg_t;
-  const int slabs = (cv + cg_t - 1) / cg_t;
-  long long gx = (M + rows_t * 4 - 1) / (rows_t * 4);
-  long long cap = (HB_NUM_SMS * per_sm) / slabs;
-  if (cap < 1) cap = 1;
-  if (gx > cap) gx = cap;
-  if (gx < 1) gx = 1;
-  return dim3((unsigned)gx, (unsigned)slabs);
-}
-
 // dw[c,r,s] = sum_{n,ho,wo} dy * x_shifted ; db[c] = sum dy.  part: double [gridDim.x][C][KK+1] per-block partial sums (last
 // column = bias grad), folded in a fixed order by dw_weight_finalize_kernel: deterministic (the first version added doubles
-// atomically). Block geometry as in the BN kernels: tx = channel group within a 32-group slab, ty = pixel lane
+// atomically). tx = channel group within the slab, ty = pixel lane (SlabGeo::thread)
 template <int KS>
 __global__ void __launch_bounds__(kThreads, KS == 3 ? 2 : 1) dw_bwd_weight_kernel(const __nv_bfloat16* __restrict__ x,
                                                                  const __nv_bfloat16* __restrict__ dy, double* part,
-                                                                 DwParams p, int cg_t, int rows_t) {
+                                                                 DwParams p, const __grid_constant__ SlabGeo g) {
   constexpr int KK = KS * KS;
   __shared__ float red[kThreads * 8];
-  const int cv = p.C / 8;
-  const int tx = threadIdx.x % cg_t, ty = threadIdx.x / cg_t;
-  const int cg = blockIdx.y * cg_t + tx;
-  const bool active = ty < rows_t && cg < cv;
+  const auto [tx, ty, cg, active] = g.thread();
   float acc[KK + 1][8];
 #pragma unroll
   for (int k = 0; k <= KK; ++k)
@@ -365,19 +332,19 @@ __global__ void __launch_bounds__(kThreads, KS == 3 ? 2 : 1) dw_bwd_weight_kerne
     for (int j = 0; j < 8; ++j) acc[k][j] = 0.f;
   if (active) {
     const long long M = (long long)p.N * p.Ho * p.Wo;
-    const long long stride_m = (long long)gridDim.x * rows_t;
-    for (long long m = (long long)blockIdx.x * rows_t + ty; m < M; m += stride_m) {
+    const long long stride_m = (long long)gridDim.x * g.rows_t;
+    for (long long m = (long long)blockIdx.x * g.rows_t + ty; m < M; m += stride_m) {
       const unsigned mu = (unsigned)m;            // M < 2^31 checked by the launcher
       const unsigned t1 = mu / (unsigned)p.Wo;
       const int wo = (int)(mu - t1 * (unsigned)p.Wo);
       const int n = (int)(t1 / (unsigned)p.Ho);
       const int ho = (int)(t1 - (unsigned)n * (unsigned)p.Ho);
-      float g[8];
+      float gy[8];
       if constexpr (KS == 3) {
         // loads are issued one filter row (3 taps) ahead of their use: 80 accumulators leave no room for all 9 vectors
         Vec16<__nv_bfloat16> gv = ld16(dy + m * p.C + cg * 8);
 #pragma unroll
-        for (int j = 0; j < 8; ++j) { g[j] = __bfloat162float(gv.v[j]); acc[KK][j] += g[j]; }
+        for (int j = 0; j < 8; ++j) { gy[j] = __bfloat162float(gv.v[j]); acc[KK][j] += gy[j]; }
 #pragma unroll
         for (int r = 0; r < 3; ++r) {
           const int hi = ho * p.stride + r - p.pad;
@@ -394,15 +361,15 @@ __global__ void __launch_bounds__(kThreads, KS == 3 ? 2 : 1) dw_bwd_weight_kerne
           for (int s = 0; s < 3; ++s) {
             if (ok[s]) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) acc[r * 3 + s][j] = fmaf(g[j], __bfloat162float(xv3[s].v[j]), acc[r * 3 + s][j]);
+              for (int j = 0; j < 8; ++j) acc[r * 3 + s][j] = fmaf(gy[j], __bfloat162float(xv3[s].v[j]), acc[r * 3 + s][j]);
             }
           }
         }
         continue;
       }
-      load8(dy + m * p.C + cg * 8, g);
+      load8(dy + m * p.C + cg * 8, gy);
 #pragma unroll
-      for (int j = 0; j < 8; ++j) acc[KK][j] += g[j];
+      for (int j = 0; j < 8; ++j) acc[KK][j] += gy[j];
 #pragma unroll
       for (int r = 0; r < KS; ++r) {
         const int hi = ho * p.stride + r - p.pad;
@@ -414,43 +381,37 @@ __global__ void __launch_bounds__(kThreads, KS == 3 ? 2 : 1) dw_bwd_weight_kerne
           float xv[8];
           load8(x + (((long long)n * p.H + hi) * p.W + wi) * p.C + cg * 8, xv);
 #pragma unroll
-          for (int j = 0; j < 8; ++j) acc[r * KS + s][j] = fmaf(g[j], xv[j], acc[r * KS + s][j]);
+          for (int j = 0; j < 8; ++j) acc[r * KS + s][j] = fmaf(gy[j], xv[j], acc[r * KS + s][j]);
         }
       }
     }
   }
-  const int nch = cg_t * 8;
 #pragma unroll
   for (int k = 0; k <= KK; ++k) {
     __syncthreads();
 #pragma unroll
     for (int j = 0; j < 8; ++j) red[threadIdx.x * 8 + j] = acc[k][j];
     __syncthreads();
-    for (int ch = threadIdx.x; ch < nch; ch += kThreads) {
-      const int ctx = ch / 8, j = ch % 8;
-      const int gcg = blockIdx.y * cg_t + ctx;
-      if (gcg >= cv) continue;
-      double a = 0.0;
-      for (int r = 0; r < rows_t; ++r) a += (double)red[(r * cg_t + ctx) * 8 + j];
-      part[((size_t)blockIdx.x * p.C + gcg * 8 + j) * (KK + 1) + k] = a;
-    }
+    fold_row_lanes<double, 1>(g, red, [&](int c, const double (&a)[1]) {
+      part[((size_t)blockIdx.x * p.C + c) * (KK + 1) + k] = a[0];
+    });
   }
 }
 
 // 3x3 weight gradient, stride 1 / 2: a thread owns ONE filter row r and FOUR consecutive output pixels of a row. It loads the 4
 // dy vectors and the 3*S + 3 input vectors of input row oh*S + r - pad (all in flight before the first use) and keeps 3 taps x 8
 // channels (+ the bias column on r == 0) of accumulators: 32 instead of 80, so two blocks per SM fit without serialising the
-// loads filter row by filter row, and 7.5 / 11.25 vector loads per output pixel instead of 10. ty = lane * 3 + r.
+// loads filter row by filter row, and 7.5 / 11.25 vector loads per output pixel instead of 10. ty = lane * 3 + r: the block
+// walks rows_t / 3 quads per step.
 template <int kStride>
 __global__ void __launch_bounds__(kThreads, 2) dw3x3_wgrad_quad_kernel(const __nv_bfloat16* __restrict__ x,
                                                                     const __nv_bfloat16* __restrict__ dy, double* part,
-                                                                    DwParams p, int cg_t, int lanes) {
+                                                                    DwParams p, const __grid_constant__ SlabGeo g) {
   __shared__ float red[kThreads * 8];
-  const int cv = p.C / 8;
-  const int tx = threadIdx.x % cg_t, ty = threadIdx.x / cg_t;
-  const int r = ty % 3, lane = ty / 3;
-  const int cg = blockIdx.y * cg_t + tx;
-  const bool active = lane < lanes && cg < cv;
+  const int tx = threadIdx.x % g.cg_t, ty = threadIdx.x / g.cg_t;
+  const int r = ty % 3, lane = ty / 3, lanes = g.rows_t / 3;
+  const int cg = blockIdx.y * g.cg_t + tx;
+  const bool active = lane < lanes && cg < g.cg_total;
   float acc[4][8];
 #pragma unroll
   for (int k = 0; k < 4; ++k)
@@ -472,30 +433,26 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_wgrad_quad_kernel(const __n
       const __nv_bfloat16* dyp = dy + (((size_t)n * p.Ho + oh) * p.Wo + ow0) * C + cg * 8;
       Vec16<__nv_bfloat16> gv[4], xv[kIn];
 #pragma unroll
-      for (int o = 0; o < 4; ++o) {
-        if (ow0 + o < p.Wo) gv[o] = ld16(dyp + (size_t)o * C);
-        else gv[o].raw = make_uint4(0, 0, 0, 0);
-      }
+      for (int o = 0; o < 4; ++o) gv[o] = ld16_or_zero(dyp + (size_t)o * C, ow0 + o < p.Wo);
       if (hok) {
         const __nv_bfloat16* row = x + (((size_t)n * p.H + ih) * p.W) * C + cg * 8;
         const int iw0 = ow0 * kStride - p.pad;
 #pragma unroll
         for (int c = 0; c < kIn; ++c) {
           const int iw = iw0 + c;
-          if (iw >= 0 && iw < p.W) xv[c] = ld16(row + (size_t)iw * C);
-          else xv[c].raw = make_uint4(0, 0, 0, 0);
+          xv[c] = ld16_or_zero(row + (size_t)iw * C, iw >= 0 && iw < p.W);
         }
       }
-      float g[4][8];
+      float gy[4][8];
 #pragma unroll
       for (int o = 0; o < 4; ++o)
 #pragma unroll
-        for (int j = 0; j < 8; ++j) g[o][j] = __bfloat162float(gv[o].v[j]);
+        for (int j = 0; j < 8; ++j) gy[o][j] = __bfloat162float(gv[o].v[j]);
       if (r == 0) {
 #pragma unroll
         for (int o = 0; o < 4; ++o)
 #pragma unroll
-          for (int j = 0; j < 8; ++j) acc[3][j] += g[o][j];
+          for (int j = 0; j < 8; ++j) acc[3][j] += gy[o][j];
       }
       if (hok) {
 #pragma unroll
@@ -508,14 +465,14 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_wgrad_quad_kernel(const __n
             const int s2 = c - o * kStride;   // compile-time after unrolling
             if (s2 >= 0 && s2 < 3) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) acc[s2][j] = fmaf(g[o][j], f[j], acc[s2][j]);
+              for (int j = 0; j < 8; ++j) acc[s2][j] = fmaf(gy[o][j], f[j], acc[s2][j]);
             }
           }
         }
       }
     }
   }
-  const int nch = cg_t * 8;
+  const int nch = g.cg_t * 8;
 #pragma unroll
   for (int k = 0; k < 4; ++k) {
     __syncthreads();
@@ -526,10 +483,10 @@ __global__ void __launch_bounds__(kThreads, 2) dw3x3_wgrad_quad_kernel(const __n
     for (int idx = threadIdx.x; idx < nch * nr; idx += kThreads) {
       const int rr = idx / nch, ch = idx - rr * nch;
       const int ctx = ch / 8, j = ch % 8;
-      const int gcg = blockIdx.y * cg_t + ctx;
-      if (gcg >= cv) continue;
+      const int gcg = blockIdx.y * g.cg_t + ctx;
+      if (gcg >= g.cg_total) continue;
       double a = 0.0;
-      for (int l = 0; l < lanes; ++l) a += (double)red[(((l * 3 + rr) * cg_t) + ctx) * 8 + j];
+      for (int l = 0; l < lanes; ++l) a += (double)red[(((l * 3 + rr) * g.cg_t) + ctx) * 8 + j];
       part[((size_t)blockIdx.x * p.C + gcg * 8 + j) * 10 + (k < 3 ? rr * 3 + k : 9)] = a;
     }
   }
@@ -564,15 +521,23 @@ __global__ void __launch_bounds__(256) dw_weight_finalize_kernel(const double* p
   else if (db) db[c] = (float)a;
 }
 
-// channel-slab geometry of the weight-gradient kernels and the number of row blocks (<= 2 blocks per SM over all slabs)
-inline void dw_wgrad_geo(int C, int& cg_t, int& rows_t, int& slabs, int& gx_max) {
-  const int cv = C / 8;
-  const int nslab = (cv + 31) / 32;
-  cg_t = (cv + nslab - 1) / nslab;
-  rows_t = kThreads / cg_t;
-  slabs = (cv + cg_t - 1) / cg_t;
-  gx_max = (HB_NUM_SMS * 2) / slabs;
-  if (gx_max < 1) gx_max = 1;
+// row blocks per SM of the weight-gradient kernels; hb_dwconv_wgrad_scratch_doubles sizes their partial sums for it
+constexpr int kWgradPerSm = 2;
+
+// HB_DISABLE_DW_QUAD set: the 3x3 launchers take the one-output kernels (dw3x3_kernel, dw_bwd_weight_kernel<3>) where they
+// would take the four-output ones. Read once per process.
+inline bool quad_kernels_on() {
+  static const bool on = getenv("HB_DISABLE_DW_QUAD") == nullptr;
+  return on;
+}
+
+// dw3x3_kernel with the stride as a template argument when it is 1 or 2
+template <bool kBackward>
+void launch_dw3x3(dim3 grid, cudaStream_t st, const __nv_bfloat16* src, const float* w, const float* bias,
+                  __nv_bfloat16* dst, const DwParams& p, const SlabGeo& g) {
+  const auto kernel = p.stride == 1 ? dw3x3_kernel<kBackward, 1> : p.stride == 2 ? dw3x3_kernel<kBackward, 2>
+                                                                                  : dw3x3_kernel<kBackward, 0>;
+  kernel<<<grid, kThreads, 0, st>>>(src, w, bias, dst, p, g);
 }
 
 // 0 when the geometry is supported (fills p), otherwise cudaErrorInvalidValue, before any launch or device query:
@@ -596,30 +561,22 @@ int hb_dwconv_fwd_bf16(const void* x, const float* w, const float* bias, void* y
                        int stride, int pad, void* stream) {
   DwParams p;
   if (int rc = make_params(p, N, H, W, C, K, stride, pad)) return rc;
-  const long long total = (long long)N * p.Ho * p.Wo * (C / 8);
-  if (K == 3 && (long long)N * p.Ho * p.Wo < 0x7fffffffLL) {
-    int cg_t, rows_t;
-    const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
-    __nv_bfloat16* yb = (__nv_bfloat16*)y;
-    cudaStream_t st = (cudaStream_t)stream;
-    static const bool quad_on = getenv("HB_DISABLE_DW_QUAD") == nullptr;
-    if (quad_on && (stride == 1 || stride == 2) && p.Wo >= 4) {
+  const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
+  __nv_bfloat16* yb = (__nv_bfloat16*)y;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long M = (long long)N * p.Ho * p.Wo;
+  if (K == 3 && M < 0x7fffffffLL) {
+    const SlabGeo g = SlabGeo::make(C);
+    if (quad_kernels_on() && (stride == 1 || stride == 2) && p.Wo >= 4) {
       const long long quads = (long long)N * p.Ho * ((p.Wo + 3) / 4);
-      const dim3 qgrid = dw_quad_grid(quads, C / 8, cg_t, rows_t, 2);
-      if (stride == 1) dw3x3_quad_kernel<1, false><<<qgrid, kThreads, 0, st>>>(xb, w, bias, yb, N, H, W, p.Ho, p.Wo, C, pad, cg_t, rows_t);
-      else dw3x3_quad_kernel<2, false><<<qgrid, kThreads, 0, st>>>(xb, w, bias, yb, N, H, W, p.Ho, p.Wo, C, pad, cg_t, rows_t);
-      HB_LAUNCH_CHECK();
-      return 0;
+      const auto kernel = stride == 1 ? dw3x3_quad_kernel<1, false> : dw3x3_quad_kernel<2, false>;
+      kernel<<<g.grid(quads, 2, 2), kThreads, 0, st>>>(xb, w, bias, yb, N, H, W, p.Ho, p.Wo, C, pad, g);
+    } else {
+      launch_dw3x3<false>(g.grid(M, 3, 4), st, xb, w, bias, yb, p, g);
     }
-    const dim3 grid = dw_grid((long long)N * p.Ho * p.Wo, C / 8, cg_t, rows_t, 3);
-    if (stride == 1) dw3x3_kernel<false, 1><<<grid, kThreads, 0, st>>>(xb, w, bias, yb, p, cg_t, rows_t);
-    else if (stride == 2) dw3x3_kernel<false, 2><<<grid, kThreads, 0, st>>>(xb, w, bias, yb, p, cg_t, rows_t);
-    else dw3x3_kernel<false, 0><<<grid, kThreads, 0, st>>>(xb, w, bias, yb, p, cg_t, rows_t);
-    HB_LAUNCH_CHECK();
-    return 0;
+  } else {
+    dw_fwd_kernel<<<stream_grid((size_t)(M * (C / 8)), kThreads, 16), kThreads, 0, st>>>(xb, w, bias, yb, p);
   }
-  dw_fwd_kernel<<<stream_grid((size_t)total, kThreads, 16), kThreads, 0, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)x, w, bias, (__nv_bfloat16*)y, p);
   HB_LAUNCH_CHECK();
   return 0;
 }
@@ -628,37 +585,25 @@ int hb_dwconv_bwd_data_bf16(const void* dy, const float* w, void* dx, int N, int
                             int pad, void* stream) {
   DwParams p;
   if (int rc = make_params(p, N, H, W, C, K, stride, pad)) return rc;
-  const long long total = (long long)N * H * W * (C / 8);
-  if (K == 3 && (long long)N * H * W < 0x7fffffffLL) {
-    int cg_t, rows_t;
-    const __nv_bfloat16* dyb = (const __nv_bfloat16*)dy;
-    __nv_bfloat16* dxb = (__nv_bfloat16*)dx;
-    cudaStream_t st = (cudaStream_t)stream;
-    static const bool quad_on = getenv("HB_DISABLE_DW_QUAD") == nullptr;
-    if (quad_on && stride == 1 && W >= 4 && pad <= 2) {
+  const __nv_bfloat16* dyb = (const __nv_bfloat16*)dy;
+  __nv_bfloat16* dxb = (__nv_bfloat16*)dx;
+  cudaStream_t st = (cudaStream_t)stream;
+  const long long M = (long long)N * H * W;
+  if (K == 3 && M < 0x7fffffffLL) {
+    const SlabGeo g = SlabGeo::make(C);
+    const long long quads = (long long)N * H * ((W + 3) / 4);
+    if (quad_kernels_on() && stride == 1 && W >= 4 && pad <= 2) {
       // stride 1: the data gradient is the correlation of dy [N,Ho,Wo,C] with the flipped filter, padding 2 - pad
-      const long long quads = (long long)N * H * ((W + 3) / 4);
-      const dim3 qgrid = dw_quad_grid(quads, C / 8, cg_t, rows_t, 2);
-      dw3x3_quad_kernel<1, true><<<qgrid, kThreads, 0, st>>>(dyb, w, nullptr, dxb, N, p.Ho, p.Wo, H, W, C, 2 - pad, cg_t, rows_t);
-      HB_LAUNCH_CHECK();
-      return 0;
+      dw3x3_quad_kernel<1, true><<<g.grid(quads, 2, 2), kThreads, 0, st>>>(dyb, w, nullptr, dxb, N, p.Ho, p.Wo, H, W, C,
+                                                                           2 - pad, g);
+    } else if (quad_kernels_on() && stride == 2 && pad == 1 && W >= 4) {
+      dw3x3_dgrad_s2_quad_kernel<<<g.grid(quads, 2, 2), kThreads, 0, st>>>(dyb, w, dxb, N, H, W, p.Ho, p.Wo, C, g);
+    } else {
+      launch_dw3x3<true>(g.grid(M, 3, 4), st, dyb, w, nullptr, dxb, p, g);
     }
-    if (quad_on && stride == 2 && pad == 1 && W >= 4) {
-      const long long quads = (long long)N * H * ((W + 3) / 4);
-      const dim3 qgrid = dw_quad_grid(quads, C / 8, cg_t, rows_t, 2);
-      dw3x3_dgrad_s2_quad_kernel<<<qgrid, kThreads, 0, st>>>(dyb, w, dxb, N, H, W, p.Ho, p.Wo, C, cg_t, rows_t);
-      HB_LAUNCH_CHECK();
-      return 0;
-    }
-    const dim3 grid = dw_grid((long long)N * H * W, C / 8, cg_t, rows_t, 3);
-    if (stride == 1) dw3x3_kernel<true, 1><<<grid, kThreads, 0, st>>>(dyb, w, nullptr, dxb, p, cg_t, rows_t);
-    else if (stride == 2) dw3x3_kernel<true, 2><<<grid, kThreads, 0, st>>>(dyb, w, nullptr, dxb, p, cg_t, rows_t);
-    else dw3x3_kernel<true, 0><<<grid, kThreads, 0, st>>>(dyb, w, nullptr, dxb, p, cg_t, rows_t);
-    HB_LAUNCH_CHECK();
-    return 0;
+  } else {
+    dw_bwd_data_kernel<<<stream_grid((size_t)(M * (C / 8)), kThreads, 16), kThreads, 0, st>>>(dyb, w, dxb, p);
   }
-  dw_bwd_data_kernel<<<stream_grid((size_t)total, kThreads, 16), kThreads, 0, (cudaStream_t)stream>>>(
-      (const __nv_bfloat16*)dy, w, (__nv_bfloat16*)dx, p);
   HB_LAUNCH_CHECK();
   return 0;
 }
@@ -667,9 +612,7 @@ int hb_dwconv_bwd_data_bf16(const void* dy, const float* w, void* dx, int N, int
 // the shapes it refuses (K outside {1, 3, 5, 7})
 size_t hb_dwconv_wgrad_scratch_doubles(int C, int K) {
   if (C <= 0 || C % 8 != 0 || (K != 1 && K != 3 && K != 5 && K != 7)) return 0;
-  int cg_t, rows_t, slabs, gx_max;
-  dw_wgrad_geo(C, cg_t, rows_t, slabs, gx_max);
-  return (size_t)gx_max * C * (K * K + 1);
+  return (size_t)SlabGeo::make(C).max_blocks(kWgradPerSm) * C * (K * K + 1);
 }
 
 // dw fp32 [C,K,K], db fp32 [C] (or NULL); scratch: double[hb_dwconv_wgrad_scratch_doubles(C, K)]. K in {1, 3, 5, 7}.
@@ -678,40 +621,27 @@ int hb_dwconv_bwd_weight_bf16(const void* x, const void* dy, float* dw, float* d
   DwParams p;
   if (int rc = make_params(p, N, H, W, C, K, stride, pad)) return rc;
   if (K != 1 && K != 3 && K != 5 && K != 7) return (int)cudaErrorInvalidValue;
-  cudaStream_t st = (cudaStream_t)stream;
-  const int KK = K * K;
-  int cg_t, rows_t, slabs, gx_max;
-  dw_wgrad_geo(C, cg_t, rows_t, slabs, gx_max);
   const long long M = (long long)N * p.Ho * p.Wo;
   if (M >= 0x7fffffffLL) return (int)cudaErrorInvalidValue;
   const __nv_bfloat16* xb = (const __nv_bfloat16*)x;
   const __nv_bfloat16* dyb = (const __nv_bfloat16*)dy;
-  static const bool quad_on = getenv("HB_DISABLE_DW_QUAD") == nullptr;
-  long long gx;
-  if (quad_on && K == 3 && (stride == 1 || stride == 2) && rows_t >= 3) {
-    const int lanes = rows_t / 3;
+  cudaStream_t st = (cudaStream_t)stream;
+  const int KK = K * K;
+  const SlabGeo g = SlabGeo::make(C);
+  dim3 grid;
+  if (quad_kernels_on() && K == 3 && (stride == 1 || stride == 2) && g.rows_t >= 3) {
     const long long quads = (long long)N * p.Ho * ((p.Wo + 3) / 4);
-    gx = (quads + lanes * 2 - 1) / (lanes * 2);
-    if (gx > gx_max) gx = gx_max;
-    if (gx < 1) gx = 1;
-    const dim3 grid((unsigned)gx, (unsigned)slabs);
-    if (stride == 1) dw3x3_wgrad_quad_kernel<1><<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, cg_t, lanes);
-    else dw3x3_wgrad_quad_kernel<2><<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, cg_t, lanes);
+    grid = g.grid(quads, kWgradPerSm, 2, g.rows_t / 3);   // one quad per three row lanes
+    const auto kernel = stride == 1 ? dw3x3_wgrad_quad_kernel<1> : dw3x3_wgrad_quad_kernel<2>;
+    kernel<<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, g);
   } else {
-    gx = (M + rows_t * 8 - 1) / (rows_t * 8);
-    if (gx > gx_max) gx = gx_max;
-    if (gx < 1) gx = 1;
-    const dim3 grid((unsigned)gx, (unsigned)slabs);
-    switch (K) {
-      case 1: dw_bwd_weight_kernel<1><<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, cg_t, rows_t); break;
-      case 3: dw_bwd_weight_kernel<3><<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, cg_t, rows_t); break;
-      case 5: dw_bwd_weight_kernel<5><<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, cg_t, rows_t); break;
-      case 7: dw_bwd_weight_kernel<7><<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, cg_t, rows_t); break;
-      default: return (int)cudaErrorInvalidValue;
-    }
+    grid = g.grid(M, kWgradPerSm, 8);
+    const auto kernel = K == 1 ? dw_bwd_weight_kernel<1> : K == 3 ? dw_bwd_weight_kernel<3>
+                      : K == 5 ? dw_bwd_weight_kernel<5> : dw_bwd_weight_kernel<7>;
+    kernel<<<grid, kThreads, 0, st>>>(xb, dyb, scratch, p, g);
   }
   HB_LAUNCH_CHECK();
-  dw_weight_finalize_kernel<<<(C * (KK + 1) + 7) / 8, dim3(8, 32), 0, st>>>(scratch, (int)gx, dw, db, C, KK);
+  dw_weight_finalize_kernel<<<(C * (KK + 1) + 7) / 8, dim3(8, 32), 0, st>>>(scratch, (int)grid.x, dw, db, C, KK);
   HB_LAUNCH_CHECK();
   return 0;
 }

@@ -1,5 +1,5 @@
-// Channel-slab geometry of the NHWC bf16 row-streaming kernels (bn_act.cu, se_gate.cu) and the fixed-order fold of their
-// per-block channel sums.
+// Channel-slab geometry of the NHWC bf16 row-streaming kernels (bn_act.cu, se_gate.cu, dwconv.cu), their persistent
+// grids and the fixed-order fold of their per-block channel sums.
 // A block of kSlabThreads threads covers one slab of cg_t 8-channel groups x rows_t row lanes: thread (tx, ty) owns the 8
 // consecutive channels (one 128-bit bf16 vector) of group tx on the rows of lane ty, so its per-channel values stay in
 // registers while it walks the rows.
@@ -26,6 +26,22 @@ struct SlabGeo {
     g.slabs = (g.cg_total + g.cg_t - 1) / g.cg_t;
     return g;
   }
+  // most row blocks (grid.x) when the grid holds per_sm blocks per SM over all slabs
+  __host__ int max_blocks(int per_sm) const {
+    const int cap = (HB_NUM_SMS * per_sm) / slabs;
+    return cap < 1 ? 1 : cap;
+  }
+  // persistent grid (row blocks x slabs), grid-stride over `items` with `lanes` items per block and step: at least
+  // ~min_rows items per lane when there is enough work, at most max_blocks(per_sm) row blocks
+  __host__ dim3 grid(long long items, int per_sm, int min_rows, int lanes) const {
+    const long long row_blocks = (items + lanes - 1) / lanes, cap = max_blocks(per_sm);
+    long long want = (row_blocks + min_rows - 1) / min_rows;
+    if (want < 1) want = 1;
+    if (want > cap) want = cap;
+    return dim3((unsigned)want, (unsigned)slabs);
+  }
+  // one item per row lane
+  __host__ dim3 grid(long long items, int per_sm, int min_rows = 4) const { return grid(items, per_sm, min_rows, rows_t); }
   // this thread's channel group tx inside the slab, row lane ty, global channel group cg, and whether it streams rows (a
   // spare lane or a group past the last one streams nothing but still has to reach the block's barriers)
   struct Thread {

@@ -11,12 +11,13 @@ most (R + 2) * 2^-24 * sum|values|. Statistics therefore satisfy, per channel,
     |mean - mu| <= 2^-23 |mu| + (R+2) 2^-24 mean|u|
     |var - v|   <= (R+2) 2^-24 (mean u^2 + 2 |mu| mean|u|)
 and every bf16 output lies within one ulp at the fp64 reference plus the fp32 error of what was rounded."""
-from typing import NamedTuple, Optional, Sequence
+from typing import Optional, Sequence
 
 import torch
 import torch.nn.functional as F
 
 from _bounds import ulp
+from _slab import geometry, grid_rows  # noqa: F401  (re-exported: the geometry the BatchNorm tests run on)
 
 ACT_NONE, ACT_RELU, ACT_RELU6, ACT_SILU, ACT_LEAKY, ACT_MISH, ACT_HARDMISH, ACT_FRELU = range(8)
 EPS32 = 2.0 ** -24          # unit roundoff of fp32
@@ -75,33 +76,11 @@ def batch_stats(u: torch.Tensor):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
-# geometry (SlabGeo::make of slab.cuh, make_grid and RowRing of bn_act.cu)
+# geometry (tests/_slab.py mirrors SlabGeo of slab.cuh; RowRing of bn_act.cu)
 # ---------------------------------------------------------------------------------------------------------------------
-class Geo(NamedTuple):
-    cg_total: int   # 8-channel groups
-    slabs: int      # channel slabs (grid.y)
-    cg_t: int       # groups per slab
-    rows_t: int     # row lanes per block
-
-
-def geometry(c: int) -> Geo:
-    cg_total = c // 8
-    slabs = -(-cg_total // 32)
-    cg_t = -(-cg_total // slabs)
-    return Geo(cg_total, slabs, cg_t, 256 // cg_t)
-
-
 def ring_depth(tensors: int) -> int:
     """Rows in flight per thread with ``tensors`` streamed inputs; a ring has depth + 1 slots."""
     return 7 if tensors <= 2 else 3
-
-
-def grid_rows(c: int, m: int, sms: int, per_sm: int, min_rows: int = 4) -> int:
-    """grid.x (row blocks) of make_grid."""
-    g = geometry(c)
-    row_blocks = -(-m // g.rows_t)
-    cap = max((sms * per_sm) // g.slabs, 1)
-    return max(min(-(-row_blocks // min_rows), cap), 1)
 
 
 def rows_per_lane(c: int, m: int, grid_x: int) -> int:

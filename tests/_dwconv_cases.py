@@ -2,12 +2,14 @@
 
 ``route`` names the kernel each direction of a case takes and the grid it gets, the way ``narrow_n_tiles`` /
 ``fprop_slots`` mirror conv_fprop.cu: the launcher conditions of ``hb_dwconv_fwd_bf16``, ``hb_dwconv_bwd_data_bf16``
-and ``hb_dwconv_bwd_weight_bf16``, and ``dw_quad_grid``, ``dw_grid``, ``dw_wgrad_geo`` and ``stream_grid``. Every
-kernel is grid-stride: a thread starting at item ``i0 < S`` (S = grid x items per block) runs
+and ``hb_dwconv_bwd_weight_bf16``, their ``SlabGeo::grid`` arguments (the slab geometry itself is mirrored in
+tests/_slab.py) and ``stream_grid``. Every kernel is grid-stride: a thread starting at item ``i0 < S`` (S = grid x items per block) runs
 ``ceil((total - i0) / S)`` iterations, at least ``total // S`` and at most ``ceil(total / S)``. The SM count sizes the
 grids, so the mirror takes it as an argument (H100 SXM: 132, H100 PCIe: 114)."""
 from dataclasses import dataclass
-from typing import Dict, List, Optional, Tuple
+from typing import Dict, List, Optional
+
+import _slab as S
 
 THREADS = 256
 INT_MAX = 0x7FFFFFFF
@@ -92,43 +94,15 @@ def _cdiv(a: int, b: int) -> int:
     return -(-a // b)
 
 
-def slab_geo(c: int) -> Tuple[int, int, int]:
-    """(cg_t, rows_t, slabs): balanced channel slabs of at most 32 groups of 8 channels, the rest of the 256 threads as
-    pixel lanes."""
-    cv = c // 8
-    nslab = _cdiv(cv, 32)
-    cg_t = _cdiv(cv, nslab)
-    return cg_t, THREADS // cg_t, _cdiv(cv, cg_t)
-
-
-def _capped(need: int, sms: int, per_sm: int, slabs: int) -> int:
-    cap = max((sms * per_sm) // slabs, 1)
-    return max(min(need, cap), 1)
-
-
-def dw_quad_grid(quads: int, c: int, sms: int, per_sm: int = 2) -> Tuple[int, int]:
-    """(gx, rows_t) of dw_quad_grid."""
-    _, rows_t, slabs = slab_geo(c)
-    return _capped(_cdiv(quads, rows_t * 2), sms, per_sm, slabs), rows_t
-
-
-def dw_grid(m: int, c: int, sms: int, per_sm: int = 3) -> Tuple[int, int]:
-    """(gx, rows_t) of dw_grid."""
-    _, rows_t, slabs = slab_geo(c)
-    return _capped(_cdiv(m, rows_t * 4), sms, per_sm, slabs), rows_t
-
-
 def stream_grid(work: int, per_block: int, sms: int, max_waves: int = 8) -> int:
     return max(min(_cdiv(work, per_block), sms * max_waves), 1)
 
 
-def wgrad_gx_max(c: int, sms: int) -> int:
-    """gx_max of dw_wgrad_geo: at most 2 row blocks per SM over all channel slabs."""
-    return max((sms * 2) // slab_geo(c)[2], 1)
+WGRAD_PER_SM = 2           # kWgradPerSm: row blocks per SM of the weight-gradient kernels
 
 
 def scratch_doubles(c: int, k: int, sms: int) -> int:
-    return wgrad_gx_max(c, sms) * c * (k * k + 1)
+    return S.max_blocks(c, sms, WGRAD_PER_SM) * c * (k * k + 1)
 
 
 @dataclass(frozen=True)
@@ -154,12 +128,13 @@ class WgradLaunch(Launch):
 
 def route_fwd(cs: Case, sms: int, quad: bool = True) -> Launch:
     n, c, ho, wo, s = cs.n, cs.c, cs.ho, cs.wo, cs.stride
+    rows_t = S.geometry(c).rows_t
     if cs.k == 3 and n * ho * wo < INT_MAX:
         if quad and s in (1, 2) and wo >= 4:
             quads = n * ho * _cdiv(wo, 4)
-            gx, rows_t = dw_quad_grid(quads, c, sms)
+            gx = S.grid_rows(c, quads, sms, 2, 2)
             return Launch(f"dw3x3_quad_kernel<{s},false>", quads, gx * rows_t, gx)
-        gx, rows_t = dw_grid(n * ho * wo, c, sms)
+        gx = S.grid_rows(c, n * ho * wo, sms, 3, 4)
         return Launch(f"dw3x3_kernel<false,{s if s in (1, 2) else 0}>", n * ho * wo, gx * rows_t, gx)
     total = n * ho * wo * (c // 8)
     grid = stream_grid(total, THREADS, sms, 16)
@@ -168,15 +143,16 @@ def route_fwd(cs: Case, sms: int, quad: bool = True) -> Launch:
 
 def route_dgrad(cs: Case, sms: int, quad: bool = True) -> Launch:
     n, c, h, w, s, pad = cs.n, cs.c, cs.h, cs.w, cs.stride, cs.pad
+    rows_t = S.geometry(c).rows_t
     if cs.k == 3 and n * h * w < INT_MAX:
         quads = n * h * _cdiv(w, 4)
         if quad and s == 1 and w >= 4 and pad <= 2:
-            gx, rows_t = dw_quad_grid(quads, c, sms)
+            gx = S.grid_rows(c, quads, sms, 2, 2)
             return Launch("dw3x3_quad_kernel<1,true>", quads, gx * rows_t, gx)
         if quad and s == 2 and pad == 1 and w >= 4:
-            gx, rows_t = dw_quad_grid(quads, c, sms)
+            gx = S.grid_rows(c, quads, sms, 2, 2)
             return Launch("dw3x3_dgrad_s2_quad_kernel", quads, gx * rows_t, gx)
-        gx, rows_t = dw_grid(n * h * w, c, sms)
+        gx = S.grid_rows(c, n * h * w, sms, 3, 4)
         return Launch(f"dw3x3_kernel<true,{s if s in (1, 2) else 0}>", n * h * w, gx * rows_t, gx)
     total = n * h * w * (c // 8)
     grid = stream_grid(total, THREADS, sms, 16)
@@ -186,16 +162,15 @@ def route_dgrad(cs: Case, sms: int, quad: bool = True) -> Launch:
 def route_wgrad(cs: Case, sms: int, quad: bool = True) -> WgradLaunch:
     """The weight-gradient kernel; ``gx`` is also the row count dw_weight_finalize_kernel folds."""
     n, c, ho, wo, s = cs.n, cs.c, cs.ho, cs.wo, cs.stride
-    _, rows_t, _ = slab_geo(c)
-    gx_max = wgrad_gx_max(c, sms)
+    rows_t = S.geometry(c).rows_t
     if quad and cs.k == 3 and s in (1, 2) and rows_t >= 3:
         lanes = rows_t // 3
         quads = n * ho * _cdiv(wo, 4)
-        gx = max(min(_cdiv(quads, lanes * 2), gx_max), 1)
+        gx = S.grid_rows(c, quads, sms, WGRAD_PER_SM, 2, lanes)
         # four outputs per quad feed each accumulator (three taps x 8 channels, and the bias column on r == 0)
         return WgradLaunch(f"dw3x3_wgrad_quad_kernel<{s}>", quads, gx * lanes, gx, 4 * _cdiv(quads, gx * lanes))
     m = n * ho * wo
-    gx = max(min(_cdiv(m, rows_t * 8), gx_max), 1)
+    gx = S.grid_rows(c, m, sms, WGRAD_PER_SM, 8)
     return WgradLaunch(f"dw_bwd_weight_kernel<{cs.k}>", m, gx * rows_t, gx, _cdiv(m, gx * rows_t))
 
 
