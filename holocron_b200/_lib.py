@@ -138,6 +138,7 @@ SIGNATURES = {
     "hb_lookahead_sync": "ppi" + "f" + "p",
     "hb_resample_batch": "p" + "i" * 8 + "p",
     "hb_erase_batch": "pp" + "i" * 4 + "p",
+    "hb_autoaugment_batch": "pppp" + "i" * 5 + "p",
     "hb_detect_scratch_bytes": "piii",
     "hb_detect": "piii" + "p" * 6,
 }

@@ -1,5 +1,6 @@
-"""``RandomResizedCrop``, ``RandomHorizontalFlip`` and ``RandomErasing`` of torchvision, the random transforms of the
-reference's classification training recipe (references/classification/train.py:101-107), on one CUDA launch per call.
+"""``RandomResizedCrop``, ``RandomHorizontalFlip``, ``TrivialAugmentWide`` and ``RandomErasing`` of torchvision, the
+random transforms of the reference's classification training recipe (references/classification/train.py:101-107), on
+one CUDA launch per call (two for a ``TrivialAugmentWide`` batch where an image drew a histogram op).
 
 Each subclasses the torchvision class of the same name: constructor, validation, attributes and ``repr`` are
 torchvision's, and the random draws are torchvision's own ``get_params`` (and ``torch.rand(1) < p``), called in
@@ -27,14 +28,15 @@ from typing import List, Optional, Tuple
 
 import torch
 from torch import Tensor
-from torchvision.transforms import transforms as T
+from torchvision.transforms import autoaugment, transforms as T
 from torchvision.transforms.functional import InterpolationMode
 
+from ._autoaugment import apply_ops, check_images, check_options
 from ._erase import Rect, erase
 from ._resample import resample
 from .interpolation import Images, _batch, _finish, _resize_options
 
-__all__ = ["RandomErasing", "RandomHorizontalFlip", "RandomResizedCrop"]
+__all__ = ["RandomErasing", "RandomHorizontalFlip", "RandomResizedCrop", "TrivialAugmentWide"]
 
 
 def _one_shape(images: Images, items: List[Tensor]) -> None:
@@ -139,4 +141,49 @@ class RandomErasing(T.RandomErasing):
         out = erase(_planes(items), [rect for _, rect in draws], self.inplace)
         if self.inplace:
             return img
+        return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))
+
+
+class TrivialAugmentWide(autoaugment.TrivialAugmentWide):
+    """torchvision's ``TrivialAugmentWide`` on batched CUDA kernels: each image gets one of fourteen ops, drawn at
+    random with a random magnitude and sign, all images of a call in at most two launches.
+
+    The draws are torchvision's (``torch.randint`` for the op, then for the magnitude bin when the op has several, then
+    for the sign when the op is signed), one set per image in list order, on the default CPU generator; the magnitude
+    table is built once per call. The output is torchvision's tensor path on CUDA, bit for bit for the per-channel value
+    ops, Color and Sharpness. The affine ops (ShearX/Y, TranslateX/Y, Rotate) match it except where a sampling
+    coordinate lies within fp32 rounding of a nearest-neighbour tie, or a bilinear value within it of a rounding tie:
+    torch forms its sampling grid with a cuBLAS product whose summation order is not fixed. Images over 65,793 pixels
+    may also take a Contrast value one lower or higher, where torch's own fp32 sum of the grayscale is inexact.
+
+    Deviations: torchvision's PIL path (the one the reference recipe runs, on PIL images) gives different pixels; PIL
+    images and CPU tensors raise ``HolocronB200Error``; dtypes other than uint8 raise ``TypeError`` whatever op is
+    drawn; fill values outside [0, 255] raise ``ValueError``. A single tensor given the Identity op is handed back
+    itself, as torchvision hands it back.
+
+    >>> import torch
+    >>> from torchvision.transforms import InterpolationMode
+    >>> from holocron_b200.transforms import TrivialAugmentWide
+    >>> batch = torch.randint(0, 256, (8, 3, 176, 176), dtype=torch.uint8, device="cuda")
+    >>> out = TrivialAugmentWide(interpolation=InterpolationMode.BILINEAR)(batch.unbind(0))
+    """
+
+    def forward(self, img: Images) -> Tensor:
+        items = _batch(img, three_d=False)
+        _one_shape(img, items)
+        check_options(self.interpolation, self.fill, check_images(items))
+        op_meta = self._augmentation_space(self.num_magnitude_bins)
+        names = list(op_meta.keys())
+        ops = []
+        for _ in items:  # torchvision's forward, draw for draw
+            op_name = names[int(torch.randint(len(op_meta), (1,)).item())]
+            magnitudes, signed = op_meta[op_name]
+            magnitude = (float(magnitudes[torch.randint(len(magnitudes), (1,), dtype=torch.long)].item())
+                         if magnitudes.ndim > 0 else 0.0)
+            if signed and torch.randint(2, (1,)):
+                magnitude *= -1.0
+            ops.append((op_name, magnitude))
+        if isinstance(img, Tensor) and ops[0][0] == "Identity":
+            return img
+        out = apply_ops(items, ops, self.interpolation, self.fill)
         return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))

@@ -501,6 +501,22 @@ int hb_resample_batch(const void* descs, int N, int canvas_h, int canvas_w, int 
  * hb_resample_batch. */
 int hb_erase_batch(const void* descs, const float* values, int N, int rows, int row_len, int dtype, void* stream);
 
+/* ---- TrivialAugmentWide: torchvision.transforms.TrivialAugmentWide.forward (op, magnitude and sign drawn on the
+ *      host) and the torchvision.transforms.autoaugment._apply_op it calls on a uint8 tensor, as the reference's
+ *      classification recipe applies it (references/classification/train.py:103) - a batch in at most two launches -- */
+/* descs: device table of N rows of 16 int64 {src, dst, stride_c, stride_h, stride_w, C, H, W, op, stat, mask, fill,
+ * bilinear, 0, 0, 0}: pointers are addresses, strides count elements (bytes). Image n is read in place from the
+ * strided uint8 src [C][H][W] (C 1 or 3; every row of one call has the same C, H and W) and written to the contiguous
+ * dst [C][H][W]. op: 0 Identity, 1 ShearX, 2 ShearY, 3 TranslateX, 4 TranslateY, 5 Rotate, 6 Brightness, 7 Color,
+ * 8 Contrast, 9 Sharpness, 10 Posterize, 11 Solarize, 12 AutoContrast, 13 Equalize. stat: the image's index k in
+ * stat_images for ops 8, 12 and 13, else -1. mask: the Posterize mask. fill: 1 when the affine ops fill out-of-image
+ * pixels with params[n][9 + c], 0 for zeros. bilinear: 1 bilinear, 0 nearest. params: fp32 [N][16] {r, 1 - r,
+ * solarize threshold, the 6 inverse affine matrix coefficients, 3 fill values, 0...}, r = 1 + magnitude formed in
+ * double. stat_images: int64 [n_stat] image indices, in the order of their stat index. scratch: int32 [3 * n_stat]
+ * [slices][256] histogram partials (not read when n_stat = 0). Arithmetic: torchvision's CUDA tensor path, in fp32. */
+int hb_autoaugment_batch(const void* descs, const float* params, const long long* stat_images, int* scratch, int N,
+                         int n_stat, int H, int W, int slices, void* stream);
+
 /* ---- YOLO inference post-processing (holocron/models/detection/yolo.py:159-233, yolov4.py:303-335) ------------------
  * One segment = one set of decoded candidates per image: boxes fp32 [B, M, 4] xyxy (16-byte aligned), objectness fp32
  * [B, M] and class scores fp32 [B, M, K], all contiguous, with its own thresholds (YOLOv1/v2: one segment; YOLOv4: one
