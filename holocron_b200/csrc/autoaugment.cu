@@ -25,14 +25,13 @@
 // histogram slices, summed in slice order, where the op needs statistics) and apply it with 16-byte loads and stores
 // where rows are contiguous and aligned; Color reads the three channels of a pixel; Sharpness reads its 3x3 stencil
 // through L1; the affine ops gather 1 or 4 taps per channel from fp32 coordinates computed once per pixel.
-#include "common.cuh"
+#include "pixel.cuh"
 
 using namespace hb;
 
 namespace {
 
 constexpr int kThreads = 256;
-constexpr int kChunk = 16;
 
 // op codes: the order of TrivialAugmentWide._augmentation_space
 enum Op {
@@ -48,39 +47,8 @@ struct AugDesc {
   long long src, dst, sc, sh, sw, C, H, W, op, stat, mask, fill, bilinear, reserved0, reserved1, reserved2;
 };
 
-__device__ __forceinline__ uint8_t trunc_u8(float v) { return (uint8_t)__float2int_rz(clamp_nan(v, 0.f, 255.f)); }
-
-__device__ __forceinline__ uint8_t blend(float r, float q, uint8_t v, float b) {
-  return trunc_u8(__fadd_rn(__fmul_rn(r, (float)v), __fmul_rn(q, b)));
-}
-
-__device__ __forceinline__ uint8_t gray(uint8_t r, uint8_t g, uint8_t b) {
-  return (uint8_t)__float2int_rz(
-      __fadd_rn(__fadd_rn(__fmul_rn(0.2989f, (float)r), __fmul_rn(0.587f, (float)g)), __fmul_rn(0.114f, (float)b)));
-}
-
 __device__ __forceinline__ bool needs_stats(int op) {
   return op == kContrast || op == kAutoContrast || op == kEqualize;
-}
-
-__device__ __forceinline__ Vec16<uint8_t> load_chunk(const uint8_t* p, long long sw, int len) {
-  Vec16<uint8_t> v;
-  if (len == kChunk && sw == 1 && aligned16(p)) return ld16(p);
-  v.raw = make_uint4(0, 0, 0, 0);
-#pragma unroll
-  for (int j = 0; j < kChunk; ++j)
-    if (j < len) v.v[j] = p[j * sw];
-  return v;
-}
-
-__device__ __forceinline__ void store_chunk(uint8_t* p, const Vec16<uint8_t>& v, int len) {
-  if (len == kChunk && aligned16(p)) {
-    st16(p, v);
-    return;
-  }
-#pragma unroll
-  for (int j = 0; j < kChunk; ++j)
-    if (j < len) p[j] = v.v[j];
 }
 
 __global__ void __launch_bounds__(kThreads) histogram_kernel(const AugDesc* __restrict__ descs,

@@ -1,6 +1,9 @@
 """``RandomResizedCrop``, ``RandomHorizontalFlip``, ``TrivialAugmentWide`` and ``RandomErasing`` of torchvision, the
-random transforms of the reference's classification training recipe (references/classification/train.py:101-107), on
-one CUDA launch per call (two for a ``TrivialAugmentWide`` batch where an image drew a histogram op).
+random transforms of the reference's classification training recipe (references/classification/train.py:101-107), and
+``ColorJitter``, the photometric augmentation of its segmentation and detection recipes
+(references/segmentation/train.py:133-140, references/detection/train.py:116-125), on one CUDA launch per call (two for
+a ``TrivialAugmentWide`` batch where an image drew a histogram op, and for a ``ColorJitter`` batch where an image has a
+contrast factor).
 
 Each subclasses the torchvision class of the same name: constructor, validation, attributes and ``repr`` are
 torchvision's, and the random draws are torchvision's own ``get_params`` (and ``torch.rand(1) < p``), called in
@@ -9,9 +12,9 @@ torchvision's order on the default CPU generator. Only ``forward`` differs, in w
 - one tensor: what the torchvision class does to that tensor (one draw, leading dimensions carried along);
 - a list or tuple of ``(C, H_i, W_i)`` CUDA tensors: one draw set per image, in list order, so a seeded list call draws
   exactly what calling the torchvision module image by image draws, and one launch for the whole list, which returns
-  the stacked ``(N, C, h, w)`` result. ``RandomResizedCrop`` returns canvases of ``size``; ``RandomHorizontalFlip`` and
-  ``RandomErasing`` take images of one shape and raise ``ValueError`` otherwise, before any draw. Sources are read in
-  place whatever their strides: pass a stacked batch as ``batch.unbind(0)``;
+  the stacked ``(N, C, h, w)`` result. ``RandomResizedCrop`` returns canvases of ``size``; the other transforms take
+  images of one shape and raise ``ValueError`` otherwise, before any draw. Sources are read in place whatever their
+  strides: pass a stacked batch as ``batch.unbind(0)``;
 - ``RandomErasing(inplace=True)`` writes only the rectangles, into the given tensors, and returns the input as given.
 
 A chain of batched calls does not draw what a per-image ``T.Compose`` of the same transforms draws: the chain makes
@@ -20,9 +23,11 @@ call is draw-for-draw with its torchvision class.
 
 Outputs are torchvision's on CUDA tensors: crops are resampled by the kernel of ``Resize`` (torchvision's filters with
 torch's CUDA arithmetic), flips are exact copies, and erased pixels hold the fp32 values cast to the image dtype as
-torch's copy casts them. Deviations: PIL images and CPU tensors raise ``HolocronB200Error``; dtypes other than uint8,
-fp16, bf16, fp32 and fp64 raise ``TypeError``; a crop needing more than 255 filter taps per axis (antialiased
-downscales beyond about 1/127 bilinear, 1/63 bicubic) raises ``NotImplementedError``.
+torch's copy casts them; ``TrivialAugmentWide`` and ``ColorJitter`` follow torchvision's fp32 arithmetic operation by
+operation (their docstrings state where they may differ). Deviations: PIL images and CPU tensors raise
+``HolocronB200Error``; dtypes other than uint8, fp16, bf16, fp32 and fp64 raise ``TypeError`` (other than uint8 for
+``TrivialAugmentWide``, other than uint8 and fp32 for ``ColorJitter``); a crop needing more than 255 filter taps per
+axis (antialiased downscales beyond about 1/127 bilinear, 1/63 bicubic) raises ``NotImplementedError``.
 """
 from typing import List, Optional, Tuple
 
@@ -32,11 +37,12 @@ from torchvision.transforms import autoaugment, transforms as T
 from torchvision.transforms.functional import InterpolationMode
 
 from ._autoaugment import apply_ops, check_images, check_options
+from ._color import check_images as check_color_images, jitter
 from ._erase import Rect, erase
 from ._resample import resample
 from .interpolation import Images, _batch, _finish, _resize_options
 
-__all__ = ["RandomErasing", "RandomHorizontalFlip", "RandomResizedCrop", "TrivialAugmentWide"]
+__all__ = ["ColorJitter", "RandomErasing", "RandomHorizontalFlip", "RandomResizedCrop", "TrivialAugmentWide"]
 
 
 def _one_shape(images: Images, items: List[Tensor]) -> None:
@@ -186,4 +192,41 @@ class TrivialAugmentWide(autoaugment.TrivialAugmentWide):
         if isinstance(img, Tensor) and ops[0][0] == "Identity":
             return img
         out = apply_ops(items, ops, self.interpolation, self.fill)
+        return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))
+
+
+class ColorJitter(T.ColorJitter):
+    """torchvision's ``ColorJitter`` on batched CUDA kernels: brightness, contrast, saturation and hue of each image,
+    in a random order with random factors, all images of a call in at most two launches.
+
+    The draws are torchvision's ``get_params`` (``torch.randperm(4)``, then one ``uniform_`` per factor that is not
+    ``None``), one call per image of a list in list order, one for a single tensor and all its leading indices (each
+    leading index still takes its own contrast mean). The output is torchvision's tensor path on CUDA: bit for bit on
+    uint8 images, except that on images over 65,793 pixels a contrast value, and what the later ops make of it, may
+    differ where torch's own fp32 sum of the grayscale is inexact; on fp32 images bit for bit for brightness,
+    saturation and hue, and within the rounding of torch's fp32 sum for contrast and the ops after it (the mean here
+    is an fp64 sum in a fixed order).
+
+    Deviations: PIL images and CPU tensors raise ``HolocronB200Error``; dtypes other than uint8 and fp32 raise
+    ``TypeError``, and so do channel counts other than 1 and 3 even when every factor is ``None``. A single tensor is
+    handed back itself where torchvision hands it back: every factor ``None``, or one channel and only saturation and
+    hue set.
+
+    >>> import torch
+    >>> from holocron_b200.transforms import ColorJitter
+    >>> batch = torch.randint(0, 256, (8, 3, 256, 256), dtype=torch.uint8, device="cuda")
+    >>> out = ColorJitter(brightness=0.3, contrast=0.3, saturation=0.1, hue=0.02)(batch.unbind(0))
+    """
+
+    def forward(self, img: Images) -> Tensor:
+        items = _batch(img, three_d=False)
+        _one_shape(img, items)
+        C = check_color_images(items)
+        draws = [self.get_params(self.brightness, self.contrast, self.saturation, self.hue) for _ in items]
+        if isinstance(img, Tensor):
+            _, b, c, s, h = draws[0]
+            # torchvision hands back the input when no op changes it
+            if b is None and c is None and (C == 1 or (s is None and h is None)):
+                return img
+        out = jitter(items, draws)
         return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))

@@ -517,6 +517,24 @@ int hb_erase_batch(const void* descs, const float* values, int N, int rows, int 
 int hb_autoaugment_batch(const void* descs, const float* params, const long long* stat_images, int* scratch, int N,
                          int n_stat, int H, int W, int slices, void* stream);
 
+/* ---- ColorJitter: torchvision.transforms.ColorJitter.forward (order and factors drawn on the host by get_params) on a
+ *      uint8 or fp32 tensor, as the reference's segmentation and detection recipes apply it
+ *      (references/segmentation/train.py:133-140, references/detection/train.py:116-125) - a batch in at most two
+ *      launches -------------------------------------------------------------------------------------------------- */
+/* descs: device table of N rows of 16 int64 {src, dst, stride_c, stride_h, stride_w, C, H, W, n_ops, op0, op1, op2,
+ * op3, contrast_at, stat, 0}: pointers are addresses, strides count elements. Image n is read in place from the
+ * strided src [C][H][W] (C 1 or 3; every row of one call has the same C, H and W) and written to the contiguous dst
+ * [C][H][W]. op0..op(n_ops - 1): the ops in the order applied, 0 brightness, 1 contrast, 2 saturation, 3 hue (n_ops 0:
+ * a copy); saturation and hue leave a one-channel image unchanged. contrast_at: the index of contrast among them (the
+ * ops its mean sees come before it), or -1. stat: the image's index k in stat_images when it has a contrast op, else
+ * -1. params: fp32 [N][8] {brightness r, 1 - r, contrast r, 1 - r, saturation r, 1 - r, hue factor, mean factor},
+ * 1 - r formed in double; the contrast mean is the fp32 sum of the grayscale times the mean factor (torch's: f32(n) /
+ * f32(n*H*W) for an image that is one of n leading indices of a tensor). stat_images: int64 [n_stat] image indices, in the order of their stat index. scratch: [n_stat][slices]
+ * partial grayscale sums, int64 for uint8 and fp64 for fp32 (not read when n_stat = 0). dtype: 3 = uint8, 0 = fp32.
+ * Arithmetic: torchvision's CUDA tensor path, in fp32. */
+int hb_color_jitter_batch(const void* descs, const float* params, const long long* stat_images, void* scratch, int N,
+                          int n_stat, int H, int W, int slices, int dtype, void* stream);
+
 /* ---- YOLO inference post-processing (holocron/models/detection/yolo.py:159-233, yolov4.py:303-335) ------------------
  * One segment = one set of decoded candidates per image: boxes fp32 [B, M, 4] xyxy (16-byte aligned), objectness fp32
  * [B, M] and class scores fp32 [B, M, K], all contiguous, with its own thresholds (YOLOv1/v2: one segment; YOLOv4: one
