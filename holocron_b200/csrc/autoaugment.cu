@@ -58,17 +58,14 @@ __global__ void __launch_bounds__(kThreads) histogram_kernel(const AugDesc* __re
   const int s = blockIdx.x % slices, row = blockIdx.x / slices;
   const int k = row / 3, c = row - 3 * k;
   const AugDesc& d = descs[stat_images[k]];
-  const int C = (int)d.C, W = (int)d.W;
+  const int C = (int)d.C;
   const bool to_gray = d.op == kContrast && C == 3;
   if (to_gray ? c > 0 : c >= C) return;
   hist[threadIdx.x] = 0;
   __syncthreads();
-  const long long HW = d.H * d.W, per = (HW + slices - 1) / slices;
-  const long long p0 = s * per, p1 = min(HW, p0 + per);
-  const uint8_t* src = reinterpret_cast<const uint8_t*>(d.src);
-  for (long long p = p0 + threadIdx.x; p < p1; p += kThreads) {
-    const long long y = p / W, x = p - y * W;
-    const uint8_t* px = src + y * d.sh + x * d.sw;
+  const Slice sl = pixel_slice(d, s, slices);
+  for (long long p = sl.p0 + threadIdx.x; p < sl.p1; p += kThreads) {
+    const uint8_t* px = pixel_at<uint8_t>(d, p);
     const uint8_t v = to_gray ? gray(px[0], px[d.sc], px[2 * d.sc]) : px[c * d.sc];
     atomicAdd(&hist[v], 1);
   }
@@ -92,15 +89,7 @@ __device__ void build_luts(const AugDesc& d, const float* P, const int* __restri
   }
   __syncthreads();
   if (op == kContrast) {
-    __shared__ long long part[kThreads / 32];
-    long long v = (long long)t * cnt[0][t];
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    if ((t & 31) == 0) part[t >> 5] = v;
-    __syncthreads();
-    long long sum = 0;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) sum += part[w];
+    const long long sum = ordered_block_sum<kThreads>((long long)t * cnt[0][t]);
     // torch's CUDA mean: the fp32 sum times the fp32 factor 1 / numel
     const float mean = __fmul_rn((float)sum, __fdiv_rn(1.f, (float)(d.H * d.W)));
     const uint8_t out = blend(r, q, (uint8_t)t, mean);
@@ -173,7 +162,7 @@ __global__ void __launch_bounds__(kThreads) apply_kernel(const AugDesc* __restri
                                                          int rows_per_tile, int tiles) {
   __shared__ uint8_t lut[3][256];
   __shared__ int cnt[3][256];
-  const int n = blockIdx.x / tiles, tile = blockIdx.x - n * tiles;
+  const int n = blockIdx.x / tiles;
   const AugDesc& d = descs[n];
   const float* P = params + 16LL * n;
   const int C = (int)d.C, H = (int)d.H, W = (int)d.W;
@@ -190,8 +179,7 @@ __global__ void __launch_bounds__(kThreads) apply_kernel(const AugDesc* __restri
   uint8_t* dst = reinterpret_cast<uint8_t*>(d.dst);
   const long long sc = d.sc, sh = d.sh, sw = d.sw;
   const float r = P[kR], q = P[kQ];
-  const int y0 = tile * rows_per_tile, nrows = min(H - y0, rows_per_tile);
-  const int cpr = (W + kChunk - 1) / kChunk;
+  const RowTile tile(n, tiles, rows_per_tile, H, W);
   // geometric ops: theta^T / [w/2, h/2] as _gen_affine_grid forms it
   const float hw = 0.5f * (float)W, hh = 0.5f * (float)H;
   const float ax = __fdiv_rn(P[kMatrix], hw), bx = __fdiv_rn(P[kMatrix + 1], hw), cx = __fdiv_rn(P[kMatrix + 2], hw);
@@ -199,8 +187,8 @@ __global__ void __launch_bounds__(kThreads) apply_kernel(const AugDesc* __restri
               cy = __fdiv_rn(P[kMatrix + 5], hh);
   const bool has_fill = d.fill != 0, bilinear = d.bilinear != 0;
 
-  for (int item = threadIdx.x; item < nrows * cpr; item += kThreads) {
-    const int y = y0 + item / cpr, x0 = (item % cpr) * kChunk, len = min(kChunk, W - x0);
+  for (int item = threadIdx.x; item < tile.items(); item += kThreads) {
+    const auto [y, x0, len] = Chunk(tile, item, W);
     const uint8_t* srow = src + y * sh + x0 * sw;
     uint8_t* drow = dst + ((long long)y * W + x0);
     const long long plane = (long long)H * W;
@@ -318,10 +306,8 @@ extern "C" int hb_autoaugment_batch(const void* descs, const float* params, cons
     histogram_kernel<<<(unsigned)blocks, kThreads, 0, s>>>(d, stat_images, scratch, slices);
     HB_LAUNCH_CHECK();
   }
-  const int cpr = (W + kChunk - 1) / kChunk;
-  const int rows_per_tile = cpr >= kThreads ? 1 : kThreads / cpr;
-  const int tiles = (H + rows_per_tile - 1) / rows_per_tile;
-  if ((long long)N * tiles > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  int rows_per_tile, tiles;
+  if (!row_tiles<kThreads>(N, H, W, rows_per_tile, tiles)) return (int)cudaErrorInvalidValue;
   apply_kernel<<<(unsigned)(N * tiles), kThreads, 0, s>>>(d, params, scratch, slices, rows_per_tile, tiles);
   HB_LAUNCH_CHECK();
   return 0;

@@ -180,36 +180,23 @@ __device__ __forceinline__ void stats_body(const JitterDesc* __restrict__ descs,
                                            const long long* __restrict__ stat_images, void* scratch, int slices) {
   constexpr bool kU8 = sizeof(T) == 1;
   using Acc = typename std::conditional<kU8, long long, double>::type;
-  __shared__ Acc part[kThreads / 32];
   const int s = blockIdx.x % slices, k = blockIdx.x / slices;
   const long long n = stat_images[k];
   const JitterDesc& d = descs[n];
   const Chain ch = load_chain(d, params + kParams * n);
-  const long long HW = d.H * d.W, per = (HW + slices - 1) / slices;
-  const long long p0 = s * per, p1 = min(HW, p0 + per);
-  const T* src = reinterpret_cast<const T*>(d.src);
-  const long long W = d.W, sc = d.sc, sh = d.sh, sw = d.sw;
+  const Slice sl = pixel_slice(d, s, slices);
+  const long long sc = d.sc;
   Acc acc = 0;
-  for (long long p = p0 + threadIdx.x; p < p1; p += kThreads) {
-    const long long y = p / W, x = p - y * W;
-    const T* px = src + y * sh + x * sw;
+  for (long long p = sl.p0 + threadIdx.x; p < sl.p1; p += kThreads) {
+    const T* px = pixel_at<T>(d, p);
     float r[1] = {(float)px[0]}, g[1] = {r[0]}, b[1] = {r[0]};
     if (ch.rgb) g[0] = (float)px[sc], b[0] = (float)px[2 * sc];
     run_ops<kU8, 1>(ch, 0, ch.at, 0.f, r, g, b);
     const float l = ch.rgb ? gray_px<kU8>(r[0], g[0], b[0]) : r[0];
     acc += kU8 ? (Acc)(int)l : (Acc)l;
   }
-  // fixed order: a butterfly per warp, then the warps in order
-#pragma unroll
-  for (int o = 16; o > 0; o >>= 1) acc += __shfl_xor_sync(0xffffffffu, acc, o);
-  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = acc;
-  __syncthreads();
-  if (threadIdx.x == 0) {
-    Acc sum = 0;
-#pragma unroll
-    for (int w = 0; w < kThreads / 32; ++w) sum += part[w];
-    static_cast<Acc*>(scratch)[(long long)k * slices + s] = sum;
-  }
+  const Acc sum = ordered_block_sum<kThreads>(acc);
+  if (threadIdx.x == 0) static_cast<Acc*>(scratch)[(long long)k * slices + s] = sum;
 }
 
 __global__ void __launch_bounds__(kThreads) jitter_stats_kernel(const JitterDesc* __restrict__ descs,
@@ -225,7 +212,7 @@ __device__ __forceinline__ void apply_body(const JitterDesc* __restrict__ descs,
                                            const void* scratch, int slices, int rows_per_tile, int tiles) {
   constexpr bool kU8 = sizeof(T) == 1;
   constexpr int kVec = Vec16<T>::N;  // pixels per 16-byte vector: a chunk is kChunk / kVec vectors per channel
-  const int n = blockIdx.x / tiles, tile = blockIdx.x - n * tiles;
+  const int n = blockIdx.x / tiles;
   const JitterDesc& d = descs[n];
   const Chain ch = load_chain(d, params + (long long)kParams * n);
   const int C = (int)d.C, H = (int)d.H, W = (int)d.W;
@@ -248,10 +235,9 @@ __device__ __forceinline__ void apply_body(const JitterDesc* __restrict__ descs,
   const T* src = reinterpret_cast<const T*>(d.src);
   T* dst = reinterpret_cast<T*>(d.dst);
   const long long sc = d.sc, sh = d.sh, sw = d.sw, plane = (long long)H * W;
-  const int y0 = tile * rows_per_tile, nrows = min(H - y0, rows_per_tile);
-  const int cpr = (W + kChunk - 1) / kChunk;
-  for (int item = threadIdx.x; item < nrows * cpr; item += kThreads) {
-    const int y = y0 + item / cpr, x0 = (item % cpr) * kChunk, len = min(kChunk, W - x0);
+  const RowTile tile(n, tiles, rows_per_tile, H, W);
+  for (int item = threadIdx.x; item < tile.items(); item += kThreads) {
+    const auto [y, x0, len] = Chunk(tile, item, W);
     const T* srow = src + y * sh + x0 * sw;
     T* drow = dst + ((long long)y * W + x0);
 #pragma unroll 1
@@ -286,21 +272,20 @@ __global__ void __launch_bounds__(kThreads) jitter_apply_kernel(const JitterDesc
 extern "C" int hb_color_jitter_batch(const void* descs, const float* params, const long long* stat_images,
                                      void* scratch, int N, int n_stat, int H, int W, int slices, int dtype,
                                      void* stream) {
-  if (N <= 0 || n_stat < 0 || n_stat > N || H <= 0 || W <= 0 || slices <= 0 || (dtype != 0 && dtype != 3))
+  if (N <= 0 || n_stat < 0 || n_stat > N || H <= 0 || W <= 0 || slices <= 0 ||
+      (dtype != HB_DTYPE_F32 && dtype != HB_DTYPE_U8))
     return (int)cudaErrorInvalidValue;
   const auto* d = static_cast<const JitterDesc*>(descs);
   auto s = static_cast<cudaStream_t>(stream);
-  const int is_u8 = dtype == 3;
+  const int is_u8 = dtype == HB_DTYPE_U8;
   if (n_stat > 0) {
     const long long blocks = (long long)n_stat * slices;
     if (blocks > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
     jitter_stats_kernel<<<(unsigned)blocks, kThreads, 0, s>>>(d, params, stat_images, scratch, slices, is_u8);
     HB_LAUNCH_CHECK();
   }
-  const int cpr = (W + kChunk - 1) / kChunk;
-  const int rows_per_tile = cpr >= kThreads ? 1 : kThreads / cpr;
-  const int tiles = (H + rows_per_tile - 1) / rows_per_tile;
-  if ((long long)N * tiles > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  int rows_per_tile, tiles;
+  if (!row_tiles<kThreads>(N, H, W, rows_per_tile, tiles)) return (int)cudaErrorInvalidValue;
   jitter_apply_kernel<<<(unsigned)(N * tiles), kThreads, 0, s>>>(d, params, scratch, slices, rows_per_tile, tiles,
                                                                   is_u8);
   HB_LAUNCH_CHECK();

@@ -9,6 +9,8 @@
 #define HB_DTYPE_F32 0
 #define HB_DTYPE_BF16 1
 #define HB_DTYPE_F16 2
+#define HB_DTYPE_U8 3
+#define HB_DTYPE_F64 4
 
 
 #define HB_NUM_SMS (hb::num_sms())

@@ -142,8 +142,8 @@ extern "C" int hb_erase_batch(const void* descs, const float* values, int N, int
     case HB_DTYPE_F32: return launch<float>(d, values, N, rows, row_len, s);
     case HB_DTYPE_BF16: return launch<__nv_bfloat16>(d, values, N, rows, row_len, s);
     case HB_DTYPE_F16: return launch<__half>(d, values, N, rows, row_len, s);
-    case 3: return launch<uint8_t>(d, values, N, rows, row_len, s);
-    case 4: return launch<double>(d, values, N, rows, row_len, s);
+    case HB_DTYPE_U8: return launch<uint8_t>(d, values, N, rows, row_len, s);
+    case HB_DTYPE_F64: return launch<double>(d, values, N, rows, row_len, s);
     default: return (int)cudaErrorInvalidValue;
   }
 }

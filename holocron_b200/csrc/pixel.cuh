@@ -1,6 +1,7 @@
 // Per-pixel arithmetic of torchvision's colour ops on CUDA tensors (_functional_tensor.py), shared by the batched
-// TrivialAugmentWide (autoaugment.cu) and ColorJitter (color_jitter.cu) kernels, and the 16-pixel row chunks they read
-// and write. Every product and sum is rounded on its own (no FMA contraction), as torch runs them as separate kernels.
+// TrivialAugmentWide (autoaugment.cu) and ColorJitter (color_jitter.cu) kernels, the 16-pixel row chunks they read
+// and write, and the geometry and reductions of their two launches. Every product and sum is rounded on its own (no
+// FMA contraction), as torch runs them as separate kernels.
 #pragma once
 #include "common.cuh"
 
@@ -74,5 +75,72 @@ __device__ __forceinline__ void store_chunk(float* p, const Vec16<float>& v, int
   for (int j = 0; j < Vec16<float>::N; ++j)
     if (j < len) p[j] = v.v[j];
 }
+
+// ---- the two launches of a batch ------------------------------------------------------------------------------------
+// A descriptor row (Desc) starts with src, dst, sc, sh, sw, C, H, W: addresses, strides in elements.
+
+// Statistics launch: slice s of `slices` cuts an image's H*W pixels, in row-major order, into runs of
+// ceil(H*W / slices) pixels; it is [p0, p1), empty past the end.
+struct Slice {
+  long long p0, p1;
+};
+
+template <typename Desc> __device__ __forceinline__ Slice pixel_slice(const Desc& d, int s, int slices) {
+  const long long HW = d.H * d.W, per = (HW + slices - 1) / slices;
+  const long long p0 = s * per;
+  return {p0, min(HW, p0 + per)};
+}
+
+// the address of row-major pixel p of the image's first channel
+template <typename T, typename Desc> __device__ __forceinline__ const T* pixel_at(const Desc& d, long long p) {
+  const int W = (int)d.W;
+  const long long y = p / W, x = p - y * W;
+  return reinterpret_cast<const T*>(d.src) + y * d.sh + x * d.sw;
+}
+
+// A sum over the CTA in a fixed order, so that floating-point sums repeat bit for bit: a butterfly within each warp,
+// then the warp sums in warp order. Every thread gets the result.
+template <int kThreads, typename Acc> __device__ __forceinline__ Acc ordered_block_sum(Acc v) {
+  __shared__ Acc part[kThreads / 32];
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  if ((threadIdx.x & 31) == 0) part[threadIdx.x >> 5] = v;
+  __syncthreads();
+  Acc sum = 0;
+#pragma unroll
+  for (int w = 0; w < kThreads / 32; ++w) sum += part[w];
+  return sum;
+}
+
+// Apply launch: CTA n * tiles + t holds tile t of image n, `rows_per_tile` rows of it (one when a row has kThreads
+// chunks or more), and a thread takes one kChunk-pixel chunk of a row at a time. False when the grid of N images
+// would pass 2^31 - 1 CTAs.
+template <int kThreads> inline bool row_tiles(int N, int H, int W, int& rows_per_tile, int& tiles) {
+  const int cpr = (W + kChunk - 1) / kChunk;
+  rows_per_tile = cpr >= kThreads ? 1 : kThreads / cpr;
+  tiles = (H + rows_per_tile - 1) / rows_per_tile;
+  return (long long)N * tiles <= 0x7fffffffLL;
+}
+
+// The tile of this CTA in image n = blockIdx.x / tiles: rows [y0, y0 + rows), cpr chunks per row.
+struct RowTile {
+  int y0, rows, cpr;
+
+  __device__ __forceinline__ RowTile(int n, int tiles, int rows_per_tile, int H, int W) {
+    const int tile = blockIdx.x - n * tiles;
+    y0 = tile * rows_per_tile;
+    rows = min(H - y0, rows_per_tile);
+    cpr = (W + kChunk - 1) / kChunk;
+  }
+  __device__ __forceinline__ int items() const { return rows * cpr; }
+};
+
+// item i of a tile: row y, first column x0 and len pixels
+struct Chunk {
+  int y, x0, len;
+
+  __device__ __forceinline__ Chunk(const RowTile& t, int i, int W)
+      : y(t.y0 + i / t.cpr), x0((i % t.cpr) * kChunk), len(min(kChunk, W - x0)) {}
+};
 
 }  // namespace hb

@@ -16,6 +16,7 @@ from torchvision.transforms.functional import (InterpolationMode, _get_inverse_a
                                                _interpolation_modes_from_int)
 
 from .._lib import check, lib, require_cuda, stream_ptr
+from ._table import DESC_WORDS, INT32_MAX, batch_out, check_batch, check_images, planes, slices_for, upload
 
 # op codes of the kernel: the order of torchvision's TrivialAugmentWide._augmentation_space
 OPS = ("Identity", "ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Brightness", "Color", "Contrast",
@@ -23,28 +24,11 @@ OPS = ("Identity", "ShearX", "ShearY", "TranslateX", "TranslateY", "Rotate", "Br
 CODE = {name: i for i, name in enumerate(OPS)}
 STAT_OPS = ("Contrast", "AutoContrast", "Equalize")
 _BLEND_OPS = ("Brightness", "Color", "Contrast", "Sharpness")
-_DESC_WORDS = 16
 _PARAM_WORDS = 16
 R, Q, THRESHOLD, MATRIX, FILL = 0, 1, 2, 3, 9
-# pixels one histogram CTA counts, and the most slices an (image, channel) is cut into
-_SLICE_PIXELS = 4096
-_MAX_SLICES = 64
-_INT32_MAX = 2 ** 31 - 1
+SUPPORTED = (torch.uint8,)
 
 Op = Tuple[str, float]
-
-
-def check_images(items: Sequence[Tensor]) -> int:
-    """The channel count of a batch of images, refusing what the kernels do not take."""
-    ref = items[0]
-    if ref.dtype != torch.uint8:
-        raise TypeError(f"Only torch.uint8 image tensors are supported, but found {ref.dtype}")
-    if ref.ndim < 3:
-        raise TypeError(f"Input image tensor should have at least 3 dimensions, but found {ref.ndim}")
-    C = int(ref.shape[-3])
-    if C not in (1, 3):
-        raise TypeError(f"Input image tensor permitted channel values are [1, 3], but found {C}")
-    return C
 
 
 def check_options(interpolation, fill, C: int) -> Tuple[bool, Optional[List[float]]]:
@@ -102,35 +86,25 @@ def op_params(op: str, magnitude: float, H: int, W: int) -> Tuple[int, np.ndarra
     return mask, params
 
 
-def slices_for(H: int, W: int) -> int:
-    """How many CTAs count the histogram of one (image, channel): enough that a large image is not one serial walk."""
-    return max(1, min(_MAX_SLICES, -(-H * W // _SLICE_PIXELS)))
-
-
 def op_table(sources: Sequence[Tensor], ops: Sequence[Op], bilinear: bool, fill: Optional[List[float]],
              out: Tensor) -> Tuple[np.ndarray, np.ndarray, List[int]]:
     """(table, params, stat_images): the int64 [N_total, 16] rows and fp32 [N_total, 16] parameters of
     hb_autoaugment_batch, and the images whose op needs a histogram. Leading dimensions of a source are images of their
     own, given that source's op; destinations are consecutive images of the contiguous ``out``."""
-    ref = sources[0]
-    C, H, W = (int(s) for s in ref.shape[-3:])
-    if C * H * W > _INT32_MAX:
+    check_batch(sources, one_shape=True)
+    C, H, W = (int(s) for s in sources[0].shape[-3:])
+    if C * H * W > INT32_MAX:
         raise ValueError("images of more than 2**31 - 1 elements")
     rows: List[List[int]] = []
     params: List[np.ndarray] = []
     stat_images: List[int] = []
     fill_flag = int(fill is not None)
     for x, (op, magnitude) in zip(sources, ops):
-        if x.dtype != ref.dtype or x.device != ref.device or x.ndim < 3 or x.shape[-3:] != ref.shape[-3:]:
-            raise ValueError("images of one call must share their shape, dtype and device")
         mask, p = op_params(op, magnitude, H, W)
         if fill is not None:
             p[FILL:FILL + C] = fill
         sc, sh, sw = x.stride()[-3:]
-        offsets = [0]
-        for n_k, s_k in zip(x.shape[:-3], x.stride()[:-3]):
-            offsets = [o + k * s_k for o in offsets for k in range(n_k)]
-        for o in offsets:
+        for o in planes(x):
             stat = -1
             if op in STAT_OPS:
                 stat = len(stat_images)
@@ -139,7 +113,7 @@ def op_table(sources: Sequence[Tensor], ops: Sequence[Op], bilinear: bool, fill:
             rows.append([x.data_ptr() + o, dst, sc, sh, sw, C, H, W, CODE[op], stat, mask, fill_flag, int(bilinear),
                          0, 0, 0])
             params.append(p)
-    return (np.array(rows, dtype=np.int64).reshape(-1, _DESC_WORDS),
+    return (np.array(rows, dtype=np.int64).reshape(-1, DESC_WORDS),
             np.stack(params).astype(np.float32).reshape(-1, _PARAM_WORDS), stat_images)
 
 
@@ -151,27 +125,15 @@ def apply_ops(sources: Sequence[Tensor], ops: Sequence[Op], interpolation, fill,
     if len(sources) != len(ops):
         raise ValueError(f"{len(sources)} images and {len(ops)} ops")
     require_cuda(*sources)
-    C = check_images(sources)
+    C = check_images(sources, SUPPORTED)
     bilinear, fill = check_options(interpolation, fill, C)
     ref = sources[0]
-    shape = (sum(math.prod(x.shape[:-3]) for x in sources), *ref.shape[-3:])
-    if out is None:
-        out = torch.empty(shape, dtype=ref.dtype, device=ref.device)
-    if out.shape != shape or not out.is_contiguous() or out.dtype != ref.dtype or out.device != ref.device:
-        raise ValueError(f"out must be a contiguous {ref.dtype} tensor of shape {shape} on {ref.device}")
+    out = batch_out(sources, out, ref.shape[-3:])
     table, params, stat_images = op_table(sources, ops, bilinear, fill, out)
     H, W = int(ref.shape[-2]), int(ref.shape[-1])
     slices = slices_for(H, W)
     scratch = torch.empty(max(1, 3 * len(stat_images) * slices * 256), dtype=torch.int32, device=ref.device)
-    stats = np.array(stat_images, dtype=np.int64)
-    table_bytes, params_bytes = table.nbytes, params.nbytes
-    buf = torch.empty(table_bytes + params_bytes + stats.nbytes, dtype=torch.uint8, pin_memory=True)
-    buf.numpy()[:table_bytes] = table.view(np.uint8).reshape(-1)
-    buf.numpy()[table_bytes:table_bytes + params_bytes] = params.view(np.uint8).reshape(-1)
-    buf.numpy()[table_bytes + params_bytes:] = stats.view(np.uint8)
-    dev = buf.to(ref.device, non_blocking=True)
-    base = dev.data_ptr()
-    check(lib().hb_autoaugment_batch(base, base + table_bytes, base + table_bytes + params_bytes, scratch.data_ptr(),
-                                     table.shape[0], len(stat_images), H, W, slices, stream_ptr()),
-          "hb_autoaugment_batch")
+    _dev, (descs, params_at, stats_at) = upload(ref.device, table, params, np.array(stat_images, dtype=np.int64))
+    check(lib().hb_autoaugment_batch(descs, params_at, stats_at, scratch.data_ptr(), table.shape[0], len(stat_images),
+                                     H, W, slices, stream_ptr()), "hb_autoaugment_batch")
     return out

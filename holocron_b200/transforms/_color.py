@@ -14,33 +14,17 @@ import torch
 from torch import Tensor
 
 from .._lib import check, lib, require_cuda, stream_ptr
-from ._autoaugment import slices_for
-from ._resample import DTYPES
+from ._table import DESC_WORDS, DTYPES, INT32_MAX, batch_out, check_batch, check_images, planes, slices_for, upload
 
 # op codes of the kernel: torchvision's fn_idx values
 OPS = ("brightness", "contrast", "saturation", "hue")
 CONTRAST, HUE = 1, 3
 MEAN = 7  # the parameter slot of the contrast mean's factor
 SUPPORTED = (torch.uint8, torch.float32)
-_DESC_WORDS = 16
 _PARAM_WORDS = 8
-_INT32_MAX = 2 ** 31 - 1
 
 # (fn_idx, brightness, contrast, saturation, hue), as ColorJitter.get_params returns it
 Draw = Tuple[Sequence[int], Optional[float], Optional[float], Optional[float], Optional[float]]
-
-
-def check_images(items: Sequence[Tensor]) -> int:
-    """The channel count of a batch of images, refusing what the kernels do not take."""
-    ref = items[0]
-    if ref.dtype not in SUPPORTED:
-        raise TypeError(f"Only torch.uint8 and torch.float32 image tensors are supported, but found {ref.dtype}")
-    if ref.ndim < 3:
-        raise TypeError(f"Input image tensor should have at least 3 dimensions, but found {ref.ndim}")
-    C = int(ref.shape[-3])
-    if C not in (1, 3):
-        raise TypeError(f"Input image tensor permitted channel values are [1, 3], but found {C}")
-    return C
 
 
 def chain(draw: Draw) -> Tuple[List[int], int, np.ndarray]:
@@ -70,25 +54,20 @@ def jitter_table(sources: Sequence[Tensor], draws: Sequence[Draw],
     """(table, params, stat_images): the int64 [N_total, 16] rows and fp32 [N_total, 8] parameters of
     hb_color_jitter_batch, and the images with a contrast op. Leading dimensions of a source are images of their own,
     given that source's draw; destinations are consecutive images of the contiguous ``out``."""
-    ref = sources[0]
-    C, H, W = (int(s) for s in ref.shape[-3:])
-    if C * H * W > _INT32_MAX:
+    check_batch(sources, one_shape=True)
+    C, H, W = (int(s) for s in sources[0].shape[-3:])
+    if C * H * W > INT32_MAX:
         raise ValueError("images of more than 2**31 - 1 elements")
-    item = ref.element_size()
+    item = sources[0].element_size()
     rows: List[List[int]] = []
     params: List[np.ndarray] = []
     stat_images: List[int] = []
     for x, draw in zip(sources, draws):
-        if x.dtype != ref.dtype or x.device != ref.device or x.ndim < 3 or x.shape[-3:] != ref.shape[-3:]:
-            raise ValueError("images of one call must share their shape, dtype and device")
         ops, at, p = chain(draw)
         p[MEAN] = mean_factor(math.prod(x.shape[:-3]), H, W)
         codes = ops + [-1] * (4 - len(ops))
         sc, sh, sw = x.stride()[-3:]
-        offsets = [0]
-        for n_k, s_k in zip(x.shape[:-3], x.stride()[:-3]):
-            offsets = [o + k * s_k for o in offsets for k in range(n_k)]
-        for o in offsets:
+        for o in planes(x):
             stat = -1
             if at >= 0:
                 stat = len(stat_images)
@@ -96,7 +75,7 @@ def jitter_table(sources: Sequence[Tensor], draws: Sequence[Draw],
             dst = out.data_ptr() + len(rows) * C * H * W * item
             rows.append([x.data_ptr() + o * item, dst, sc, sh, sw, C, H, W, len(ops), *codes, at, stat, 0])
             params.append(p)
-    return (np.array(rows, dtype=np.int64).reshape(-1, _DESC_WORDS),
+    return (np.array(rows, dtype=np.int64).reshape(-1, DESC_WORDS),
             np.stack(params).astype(np.float32).reshape(-1, _PARAM_WORDS), stat_images)
 
 
@@ -107,27 +86,15 @@ def jitter(sources: Sequence[Tensor], draws: Sequence[Draw], out: Optional[Tenso
     if len(sources) != len(draws):
         raise ValueError(f"{len(sources)} images and {len(draws)} draws")
     require_cuda(*sources)
-    check_images(sources)
+    check_images(sources, SUPPORTED)
     ref = sources[0]
-    shape = (sum(math.prod(x.shape[:-3]) for x in sources), *ref.shape[-3:])
-    if out is None:
-        out = torch.empty(shape, dtype=ref.dtype, device=ref.device)
-    if out.shape != shape or not out.is_contiguous() or out.dtype != ref.dtype or out.device != ref.device:
-        raise ValueError(f"out must be a contiguous {ref.dtype} tensor of shape {shape} on {ref.device}")
+    out = batch_out(sources, out, ref.shape[-3:])
     table, params, stat_images = jitter_table(sources, draws, out)
     H, W = int(ref.shape[-2]), int(ref.shape[-1])
     slices = slices_for(H, W)
     # one int64 (uint8 images) or fp64 (fp32 images) partial sum per (image with contrast, slice)
     scratch = torch.empty(max(1, len(stat_images) * slices), dtype=torch.int64, device=ref.device)
-    stats = np.array(stat_images, dtype=np.int64)
-    table_bytes, params_bytes = table.nbytes, params.nbytes
-    buf = torch.empty(table_bytes + params_bytes + stats.nbytes, dtype=torch.uint8, pin_memory=True)
-    buf.numpy()[:table_bytes] = table.view(np.uint8).reshape(-1)
-    buf.numpy()[table_bytes:table_bytes + params_bytes] = params.view(np.uint8).reshape(-1)
-    buf.numpy()[table_bytes + params_bytes:] = stats.view(np.uint8)
-    dev = buf.to(ref.device, non_blocking=True)
-    base = dev.data_ptr()
-    check(lib().hb_color_jitter_batch(base, base + table_bytes, base + table_bytes + params_bytes, scratch.data_ptr(),
-                                      table.shape[0], len(stat_images), H, W, slices, DTYPES[ref.dtype],
-                                      stream_ptr()), "hb_color_jitter_batch")
+    _dev, (descs, params_at, stats_at) = upload(ref.device, table, params, np.array(stat_images, dtype=np.int64))
+    check(lib().hb_color_jitter_batch(descs, params_at, stats_at, scratch.data_ptr(), table.shape[0], len(stat_images),
+                                      H, W, slices, DTYPES[ref.dtype], stream_ptr()), "hb_color_jitter_batch")
     return out

@@ -7,17 +7,14 @@ that copies every image with its rectangle filled, or fills the rectangles in pl
 from typing import List, Optional, Sequence, Tuple
 
 import numpy as np
-import torch
 from torch import Tensor
 
 from .._lib import check, lib, require_cuda, stream_ptr
-from ._resample import DTYPES
+from ._table import DESC_WORDS, INT32_MAX, batch_out, check_batch, dtype_code, planes, upload
 
 # (top, left, height, width, values): values broadcast to the rectangle's [C, h, w], as torchvision assigns them
 Rect = Tuple[int, int, int, int, Tensor]
 FILL_NONE, FILL_CHANNEL, FILL_PIXEL = 0, 1, 2
-_DESC_WORDS = 16
-_INT32_MAX = 2 ** 31 - 1
 
 
 def _fill(v: Tensor, C: int, h: int, w: int) -> Tuple[int, Tensor]:
@@ -36,10 +33,10 @@ def erase_table(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inpl
     """(table, values, rows, row_len): the int64 [N_total, 16] rows of hb_erase_batch, the fp32 value tensors in the
     order of their offsets, and the grid extent (the most row segments an image writes, the longest segment).
     Destinations are the sources themselves in place, else consecutive images of the contiguous ``out``."""
+    check_batch(sources, one_shape=True)
     ref = sources[0]
-    shape = tuple(ref.shape[-3:])
-    C, H, W = shape
-    if C * H * W > _INT32_MAX:
+    C, H, W = ref.shape[-3:]
+    if C * H * W > INT32_MAX:
         raise ValueError("images of more than 2**31 - 1 elements")
     rows: List[List[int]] = []
     values: List[Tensor] = []
@@ -48,8 +45,6 @@ def erase_table(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inpl
     row_len = W if not inplace else 0
     es = ref.element_size()
     for x, rect in zip(sources, rects):
-        if x.dtype != ref.dtype or x.device != ref.device or x.ndim < 3 or tuple(x.shape[-3:]) != shape:
-            raise ValueError("images of one call must share their shape, dtype and device")
         fill, (i, j, h, w), off = FILL_NONE, (0, 0, 0, 0), 0
         if rect is not None:
             i, j, h, w, v = rect
@@ -62,17 +57,14 @@ def erase_table(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inpl
             if inplace:
                 most_rows, row_len = max(most_rows, C * h), max(row_len, w)
         sc, sh, sw = x.stride()[-3:]
-        if (W - 1) * abs(sw) > _INT32_MAX:
+        if (W - 1) * abs(sw) > INT32_MAX:
             raise ValueError("image rows span more than 2**31 elements")
-        # leading dimensions of a source are images of their own, erased alike
-        offsets = [0]
-        for n_k, s_k in zip(x.shape[:-3], x.stride()[:-3]):
-            offsets = [o + k * s_k for o in offsets for k in range(n_k)]
-        for o in offsets:
+        # leading dimensions of a source are erased alike
+        for o in planes(x):
             src = x.data_ptr() + o * es
             dst = src if inplace else out.data_ptr() + len(rows) * C * H * W * es
             rows.append([src, dst, sc, sh, sw, C, H, W, i, j, h, w, fill, off, 0, 0])
-    return np.array(rows, dtype=np.int64).reshape(-1, _DESC_WORDS), values, most_rows, row_len
+    return np.array(rows, dtype=np.int64).reshape(-1, DESC_WORDS), values, most_rows, row_len
 
 
 def erase(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inplace: bool,
@@ -82,22 +74,10 @@ def erase(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inplace: b
     of the erased images (leading dimensions of a source count as images)."""
     ref = sources[0]
     require_cuda(*sources)
-    if ref.dtype not in DTYPES:
-        raise TypeError(f"unsupported dtype {ref.dtype}: expected one of {', '.join(map(str, DTYPES))}")
+    dtype = dtype_code(ref)
     if not inplace:
-        shape = (sum(x[..., 0, 0, 0].numel() for x in sources), *ref.shape[-3:])
-        if out is None:
-            out = torch.empty(shape, dtype=ref.dtype, device=ref.device)
-        if out.shape != shape or not out.is_contiguous() or out.dtype != ref.dtype or out.device != ref.device:
-            raise ValueError(f"out must be a contiguous {ref.dtype} tensor of shape {shape} on {ref.device}")
+        out = batch_out(sources, out, ref.shape[-3:])
     table, values, rows, row_len = erase_table(sources, rects, inplace, out)
-    table_bytes = table.nbytes
-    nvals = sum(v.numel() for v in values)
-    buf = torch.empty(table_bytes + 4 * nvals, dtype=torch.uint8, pin_memory=True)
-    buf[:table_bytes].view(torch.int64).copy_(torch.from_numpy(table).view(-1))
-    if values:
-        torch.cat(values, out=buf[table_bytes:].view(torch.float32))
-    dev = buf.to(ref.device, non_blocking=True)
-    check(lib().hb_erase_batch(dev.data_ptr(), dev.data_ptr() + table_bytes, table.shape[0], rows, row_len,
-                               DTYPES[ref.dtype], stream_ptr()), "hb_erase_batch")
+    _dev, (descs, vals) = upload(ref.device, table, values)
+    check(lib().hb_erase_batch(descs, vals, table.shape[0], rows, row_len, dtype, stream_ptr()), "hb_erase_batch")
     return out

@@ -15,17 +15,15 @@ from torch import Tensor
 from torchvision.transforms.functional import InterpolationMode
 
 from .._lib import check, lib, require_cuda, stream_ptr
+from ._table import INT32_MAX, batch_out, check_batch, dtype_code, planes, upload
 
 # interpolation modes torchvision's tensor resize accepts, as the kernel's filter codes
 FILTERS = {InterpolationMode.NEAREST: 0, InterpolationMode.NEAREST_EXACT: 1, InterpolationMode.BILINEAR: 2,
            InterpolationMode.BICUBIC: 3}
 PAD_MODES = {"constant": 0, "edge": 1, "reflect": 2, "symmetric": 3}
-DTYPES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2, torch.uint8: 3, torch.float64: 4}
 # Taps per axis that fit the kernel's shared-memory weight tables for every dtype: antialiased downscales up to about
 # 1/127 (bilinear) or 1/63 (bicubic).
 MAX_TAPS = 255
-_DESC_WORDS = 16
-_INT32_MAX = 2 ** 31 - 1
 
 
 def axis_taps(n_in: int, n_out: int, filter_code: int, antialias: bool, dtype: torch.dtype) -> int:
@@ -73,14 +71,12 @@ def descriptor_table(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]]
 
     ``boxes[i] = (top, left, height, width)`` crops source i to that box (inside the image) before it is resized;
     ``flips[i]`` mirrors it left-right."""
-    ref = sources[0]
-    C = ref.shape[-3]
+    check_batch(sources, one_shape=False)
+    C = sources[0].shape[-3]
     Hc, Wc = canvas
     rows: List[List[int]] = []
     taps_y = taps_x = 1
     for k, (x, (h, w)) in enumerate(zip(sources, inner)):
-        if x.dtype != ref.dtype or x.device != ref.device or x.ndim < 3 or x.shape[-3] != C:
-            raise ValueError("images of one call must share their dtype, device and channel count")
         H, W = x.shape[-2:]
         sc, sh, sw = x.stride()[-3:]
         base = x.data_ptr()
@@ -99,14 +95,10 @@ def descriptor_table(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]]
         dh, dw = Hc - h, Wc - w
         top, left = dh // 2, dw // 2
         _check_padding(pad_mode, (left, top, dw - left, dh - top), h, w)
-        if (W - 1) * abs(sw) > _INT32_MAX:
+        if (W - 1) * abs(sw) > INT32_MAX:
             raise ValueError("image rows span more than 2**31 elements")
         row = [base, 0, sc, sh, sw, C, H, W, h, w, top, left, Hc, Wc, PAD_MODES[pad_mode], 0]
-        # leading dimensions of a source are images of their own
-        offsets = [0]
-        for n_k, s_k in zip(x.shape[:-3], x.stride()[:-3]):
-            offsets = [o + k * s_k for o in offsets for k in range(n_k)]
-        for o in offsets:
+        for o in planes(x):
             rows.append([row[0] + o * x.element_size()] + row[1:])
         taps_y = max(taps_y, axis_taps(H, h, filter_code, antialias, x.dtype))
         taps_x = max(taps_x, axis_taps(W, w, filter_code, antialias, x.dtype))
@@ -131,16 +123,12 @@ def resample(sources: Sequence[Tensor], inner: Sequence[Tuple[int, int]], canvas
     antialias = bool(antialias) and filter_code >= 2
     ref = sources[0]
     require_cuda(*sources)
-    if ref.dtype not in DTYPES:
-        raise TypeError(f"unsupported dtype {ref.dtype}: expected one of {', '.join(map(str, DTYPES))}")
+    dtype = dtype_code(ref)
     table, taps_y, taps_x = descriptor_table(sources, inner, canvas, filter_code, antialias, pad_mode, boxes, flips)
     n, C, (Hc, Wc) = table.shape[0], ref.shape[-3], canvas
-    if out is None:
-        out = torch.empty((n, C, Hc, Wc), dtype=ref.dtype, device=ref.device)
-    if out.shape != (n, C, Hc, Wc) or not out.is_contiguous() or out.dtype != ref.dtype or out.device != ref.device:
-        raise ValueError(f"out must be a contiguous {ref.dtype} tensor of shape {(n, C, Hc, Wc)} on {ref.device}")
+    out = batch_out(sources, out, (C, Hc, Wc))
     table[:, 1] = out.data_ptr() + np.arange(n, dtype=np.int64) * (C * Hc * Wc * out.element_size())
-    descs = torch.from_numpy(table).pin_memory().to(ref.device, non_blocking=True)
-    check(lib().hb_resample_batch(descs.data_ptr(), n, Hc, Wc, filter_code, int(antialias), taps_y, taps_x,
-                                  DTYPES[ref.dtype], stream_ptr()), "hb_resample_batch")
+    _dev, (descs,) = upload(ref.device, table)
+    check(lib().hb_resample_batch(descs, n, Hc, Wc, filter_code, int(antialias), taps_y, taps_x, dtype, stream_ptr()),
+          "hb_resample_batch")
     return out

@@ -36,11 +36,13 @@ from torch import Tensor
 from torchvision.transforms import autoaugment, transforms as T
 from torchvision.transforms.functional import InterpolationMode
 
-from ._autoaugment import apply_ops, check_images, check_options
-from ._color import check_images as check_color_images, jitter
+from . import _autoaugment, _color
+from ._autoaugment import apply_ops, check_options
+from ._color import jitter
 from ._erase import Rect, erase
 from ._resample import resample
-from .interpolation import Images, _batch, _finish, _resize_options
+from ._table import check_images
+from .interpolation import Images, _batch, _finish, _planes, _resize_options
 
 __all__ = ["ColorJitter", "RandomErasing", "RandomHorizontalFlip", "RandomResizedCrop", "TrivialAugmentWide"]
 
@@ -51,8 +53,8 @@ def _one_shape(images: Images, items: List[Tensor]) -> None:
                          "shape (RandomResizedCrop resizes them to one)")
 
 
-def _planes(items: List[Tensor]) -> List[Tensor]:
-    return [x if x.ndim >= 3 else x.unsqueeze(0) for x in items]
+def _hw(items: List[Tensor]) -> Tuple[int, int]:
+    return int(items[0].shape[-2]), int(items[0].shape[-1])
 
 
 class RandomResizedCrop(T.RandomResizedCrop):
@@ -99,7 +101,7 @@ class RandomHorizontalFlip(T.RandomHorizontalFlip):
         flips = [bool(torch.rand(1) < self.p) for _ in items]
         if isinstance(img, Tensor) and not flips[0]:
             return img
-        size = (int(items[0].shape[-2]), int(items[0].shape[-1]))
+        size = _hw(items)
         # a nearest resample at the image's own size is an exact copy; a flip reads the columns backwards
         out = resample(_planes(items), [size] * len(items), size, InterpolationMode.NEAREST, False, flips=flips)
         return _finish(img, out, size)
@@ -147,7 +149,7 @@ class RandomErasing(T.RandomErasing):
         out = erase(_planes(items), [rect for _, rect in draws], self.inplace)
         if self.inplace:
             return img
-        return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))
+        return _finish(img, out, _hw(items))
 
 
 class TrivialAugmentWide(autoaugment.TrivialAugmentWide):
@@ -177,7 +179,7 @@ class TrivialAugmentWide(autoaugment.TrivialAugmentWide):
     def forward(self, img: Images) -> Tensor:
         items = _batch(img, three_d=False)
         _one_shape(img, items)
-        check_options(self.interpolation, self.fill, check_images(items))
+        check_options(self.interpolation, self.fill, check_images(items, _autoaugment.SUPPORTED))
         op_meta = self._augmentation_space(self.num_magnitude_bins)
         names = list(op_meta.keys())
         ops = []
@@ -192,7 +194,7 @@ class TrivialAugmentWide(autoaugment.TrivialAugmentWide):
         if isinstance(img, Tensor) and ops[0][0] == "Identity":
             return img
         out = apply_ops(items, ops, self.interpolation, self.fill)
-        return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))
+        return _finish(img, out, _hw(items))
 
 
 class ColorJitter(T.ColorJitter):
@@ -221,7 +223,7 @@ class ColorJitter(T.ColorJitter):
     def forward(self, img: Images) -> Tensor:
         items = _batch(img, three_d=False)
         _one_shape(img, items)
-        C = check_color_images(items)
+        C = check_images(items, _color.SUPPORTED)
         draws = [self.get_params(self.brightness, self.contrast, self.saturation, self.hue) for _ in items]
         if isinstance(img, Tensor):
             _, b, c, s, h = draws[0]
@@ -229,4 +231,4 @@ class ColorJitter(T.ColorJitter):
             if b is None and c is None and (C == 1 or (s is None and h is None)):
                 return img
         out = jitter(items, draws)
-        return _finish(img, out, (int(items[0].shape[-2]), int(items[0].shape[-1])))
+        return _finish(img, out, _hw(items))

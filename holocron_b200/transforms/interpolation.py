@@ -73,6 +73,11 @@ def _batch(images: Images, three_d: bool = True) -> List[Tensor]:
     return items
 
 
+def _planes(items: List[Tensor]) -> List[Tensor]:
+    """The images of a call as [..., C, H, W] sources: a (H, W) tensor is one channel."""
+    return [x if x.ndim >= 3 else x.unsqueeze(0) for x in items]
+
+
 def _finish(images: Images, out: Tensor, size: Tuple[int, int]) -> Tensor:
     """The stacked canvases of a list, or the one canvas of a tensor in that tensor's leading shape."""
     if isinstance(images, (list, tuple)):
@@ -82,8 +87,7 @@ def _finish(images: Images, out: Tensor, size: Tuple[int, int]) -> Tensor:
 
 def _place(images: Images, items: List[Tensor], inner: List[Tuple[int, int]], size, interpolation, antialias,
            pad_mode: str) -> Tensor:
-    sources = [x if x.ndim >= 3 else x.unsqueeze(0) for x in items]
-    out = resample(sources, inner, (size[0], size[1]), interpolation, antialias, pad_mode)
+    out = resample(_planes(items), inner, (size[0], size[1]), interpolation, antialias, pad_mode)
     return _finish(images, out, (size[0], size[1]))
 
 

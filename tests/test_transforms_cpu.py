@@ -14,7 +14,7 @@ from PIL import Image
 import _transforms_oracle as O
 from holocron_b200 import HolocronB200Error, _lib
 from holocron_b200 import transforms as T
-from holocron_b200.transforms import _resample
+from holocron_b200.transforms import _resample, _table
 from holocron_b200.transforms.interpolation import ResizeMethod
 
 ROOT = Path(__file__).resolve().parents[1]
@@ -144,6 +144,14 @@ def test_header_entry_and_binding():
     assert decl is not None
     assert _lib.SIGNATURES["hb_resample_batch"] == "p" + "i" * 8 + "p"
     assert len(decl.group(2).split(",")) == 10
+
+
+def test_dtype_codes_match_the_kernels():
+    text = (ROOT / "holocron_b200" / "csrc" / "common.cuh").read_text()
+    codes = {name: int(v) for name, v in re.findall(r"#define HB_DTYPE_(\w+) (\d+)", text)}
+    names = {torch.float32: "F32", torch.bfloat16: "BF16", torch.float16: "F16", torch.uint8: "U8",
+             torch.float64: "F64"}
+    assert codes == {names[dt]: code for dt, code in _table.DTYPES.items()}
 
 
 def test_pil_and_cpu_tensors_refused():
