@@ -18,10 +18,9 @@
 //   3. apply: one read of x and one write of y.
 // The backward pass mirrors it: the same pool traversal over x and dy gives sum(dy * x) per plane element, small kernels
 // run the sigmoid, BatchNorm and convolution backward (fixed-order partials for dgamma, dbeta and dW, the plane
-// gradients in gather form), and one pass writes dx. Max indices follow torch's max(dim).indices (zpool.cuh). Nothing
+// gradients in gather form), and one pass writes dx. Max indices follow torch's max(dim).indices (nhwc.cuh). Nothing
 // uses atomics or synchronises with the host: every run gives the same bits and the sequence is graph-capturable.
-#include "common.cuh"
-#include "zpool.cuh"
+#include "nhwc.cuh"
 
 namespace {
 
@@ -36,9 +35,6 @@ constexpr int kTaps = 2 * 7 * 7;
 constexpr int kBranches = 3;
 
 __device__ __forceinline__ float sigmoid_f(float s) { return 1.f / (1.f + expf(-s)); }
-
-bool bad_dtype(int dtype) { return dtype != HB_DTYPE_F32 && dtype != HB_DTYPE_BF16; }
-int vec_width(int dtype) { return dtype == HB_DTYPE_F32 ? 4 : 8; }
 
 // ------------------------------------------------------------------------------------------------ SAM
 // A group of gl lanes per pixel row; lane l holds vectors l, l + gl, ...
@@ -60,7 +56,7 @@ __global__ void __launch_bounds__(kThreads) sam_fwd_kernel(const T* __restrict__
         if (v * V + l < C) s = fmaf(w[v * V + l], to_f(xv.v[l]), s);
     }
   }
-  for (int off = 1; off < gl; off <<= 1) s += __shfl_xor_sync(0xffffffffu, s, off);   // every lane: the same bits
+  s = group_sum(s, gl);
   if (!live) return;
   const float g = sigmoid_f(s + b[0]);
   if (lane == 0) gate[r] = g;
@@ -108,7 +104,7 @@ __global__ void __launch_bounds__(kThreads) sam_bwd_kernel(const T* __restrict__
           if (v * V + l < C) dg = fmaf(to_f(gv[k].v[l]), to_f(xv[k].v[l]), dg);
       }
     }
-    for (int off = 1; off < gl; off <<= 1) dg += __shfl_xor_sync(0xffffffffu, dg, off);
+    dg = group_sum(dg, gl);
     if (!live) continue;
     const float g = gate[r];
     const float ds = dg * (g * (1.f - g));
@@ -144,17 +140,22 @@ __global__ void __launch_bounds__(kThreads) sam_bwd_kernel(const T* __restrict__
   }
 }
 
-// out[c] = sum over rows of part[row][c], in row order (fp64)
+// column c of part [rows][cols] summed in row order (fp64)
+__device__ __forceinline__ float ordered_column_sum(const float* __restrict__ part, int rows, int cols, int c) {
+  double t = 0.0;
+  for (int r = 0; r < rows; ++r) t += (double)part[(size_t)r * cols + c];
+  return (float)t;
+}
+
+// out[c] = sum over rows of part[row][c]
 __global__ void __launch_bounds__(kThreads) column_sum_kernel(const float* __restrict__ part, int rows, int cols,
                                                               int out_cols, float* __restrict__ out) {
   const int c = blockIdx.x * kThreads + threadIdx.x;
   if (c >= out_cols) return;
-  double t = 0.0;
-  for (int r = 0; r < rows; ++r) t += (double)part[(size_t)r * cols + c];
-  out[c] = (float)t;
+  out[c] = ordered_column_sum(part, rows, cols, c);
 }
 
-int sam_groups(int dtype, int Cp) { return pow2_at_least(Cp / vec_width(dtype), 32); }
+int sam_groups(int dtype, int Cp) { return lane_group(Cp / vec_width(dtype)); }
 
 int sam_blocks(long long R, int gl) {
   const long long need = (R + kThreads / gl - 1) / (kThreads / gl);
@@ -162,8 +163,7 @@ int sam_blocks(long long R, int gl) {
 }
 
 bool bad_sam(long long R, int C, int Cp, int dtype) {
-  if (bad_dtype(dtype) || R <= 0 || C <= 0 || Cp < C || Cp % vec_width(dtype) != 0) return true;
-  return Cp / vec_width(dtype) > 32 * kMaxLaneVecs;
+  return bad_rows(C, Cp, dtype) || R <= 0 || Cp / vec_width(dtype) > 32 * kMaxLaneVecs;
 }
 
 // ------------------------------------------------------------------------------------------------ triplet: pool
@@ -233,18 +233,9 @@ __global__ void __launch_bounds__(kThreads) tri_pool_kernel(const T* __restrict_
         }
       }
     }
-    // C reduction of pixel (h, w): xor butterfly over the gl lanes of the row (groups are warp-aligned)
-    for (int off = 1; off < p.gl; off <<= 1) {
-      csum += __shfl_xor_sync(0xffffffffu, csum, off);
-      if (!kBwd) {
-        const float om = __shfl_xor_sync(0xffffffffu, cmax, off);
-        const int oi = __shfl_xor_sync(0xffffffffu, cidx, off);
-        if (better(om, oi, cmax, cidx)) {
-          cmax = om;
-          cidx = oi;
-        }
-      }
-    }
+    // C reduction of pixel (h, w) over the gl lanes of the row
+    if (kBwd) csum = group_sum(csum, p.gl);
+    else group_max_sum(cmax, cidx, csum, p.gl);
     if (want_c && live && lane == 0) {
       const size_t pix = ((size_t)n * p.H + h) * p.W + w;
       if (kBwd) {
@@ -522,9 +513,7 @@ __global__ void __launch_bounds__(128) tri_wgrad_reduce_kernel(Planes q, PtrArr 
   const Plane pl = plane_of(q, blockIdx.x);
   const int t = threadIdx.x;
   if (t >= kTaps) return;
-  double a = 0.0;
-  for (int k = 0; k < pl.blocks; ++k) a += (double)pl.part[(size_t)k * kTaps + t];
-  ptr_of(dw, blockIdx.x)[t] = (float)a;
+  ptr_of(dw, blockIdx.x)[t] = ordered_column_sum(pl.part, pl.blocks, kTaps, t);
 }
 
 // ------------------------------------------------------------------------------------------------ triplet: x passes
@@ -621,15 +610,14 @@ __global__ void __launch_bounds__(kThreads) tri_dx_kernel(const T* __restrict__ 
 
 // rows per CTA of the pool pass: the lane groups of a CTA, bounded by the shared per-row state
 int tri_row_block(int H, int Cp, int dtype) {
-  const int gl = pow2_at_least(Cp / vec_width(dtype), 32);
-  int hb = kThreads / gl;
+  int hb = kThreads / lane_group(Cp / vec_width(dtype));
   if (hb * Cp > kSlab) hb = kSlab / Cp;
   return hb < H ? hb : H;
 }
 
 bool bad_triplet(int N, int H, int W, int C, int Cp, int dtype) {
-  return bad_dtype(dtype) || N <= 0 || H <= 0 || W <= 0 || C <= 0 || Cp < C || Cp % vec_width(dtype) != 0 ||
-         Cp > kSlab || (long long)N * H * W * Cp >= (1LL << 40) || N > 65535;
+  return bad_rows(C, Cp, dtype) || N <= 0 || H <= 0 || W <= 0 || Cp > kSlab || (long long)N * H * W * Cp >= (1LL << 40) ||
+         N > 65535;
 }
 
 template <typename T>
@@ -654,7 +642,7 @@ int make_pool(PoolParams& p, int N, int H, int W, int C, int Cp, int dtype) {
   if (bad_triplet(N, H, W, C, Cp, dtype)) return (int)cudaErrorInvalidValue;
   p = PoolParams{};
   p.N = N; p.H = H; p.W = W; p.C = C; p.Cp = Cp;
-  p.gl = pow2_at_least(Cp / vec_width(dtype), 32);
+  p.gl = lane_group(Cp / vec_width(dtype));
   p.HB = tri_row_block(H, Cp, dtype);
   p.nHB = (H + p.HB - 1) / p.HB;
   return 0;
@@ -705,11 +693,12 @@ int hb_sam_fwd(const void* x, const float* w, const float* b, void* y, float* ga
   if (bad_sam(R, C, Cp, dtype)) return (int)cudaErrorInvalidValue;
   const int gl = sam_groups(dtype, Cp);
   const unsigned grid = (unsigned)(((long long)R * gl + kThreads - 1) / kThreads);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == HB_DTYPE_F32) sam_fwd_kernel<float><<<grid, kThreads, 0, st>>>((const float*)x, w, b, (float*)y, gate, R, C, Cp, gl);
-  else sam_fwd_kernel<bf16><<<grid, kThreads, 0, st>>>((const bf16*)x, w, b, (bf16*)y, gate, R, C, Cp, gl);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    sam_fwd_kernel<T><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const T*)x, w, b, (T*)y, gate, R, C, Cp, gl);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_sam_bwd(const void* x, const void* dy, const float* w, const float* gate, void* dx, float* part, float* dwdb,
@@ -718,13 +707,13 @@ int hb_sam_bwd(const void* x, const void* dy, const float* w, const float* gate,
   const int gl = sam_groups(dtype, Cp);
   const int blocks = sam_blocks(R, gl);
   cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == HB_DTYPE_F32)
-    sam_bwd_kernel<float><<<blocks, kThreads, 0, st>>>((const float*)x, (const float*)dy, w, gate, (float*)dx, part, R,
-                                                       C, Cp, gl);
-  else
-    sam_bwd_kernel<bf16><<<blocks, kThreads, 0, st>>>((const bf16*)x, (const bf16*)dy, w, gate, (bf16*)dx, part, R, C,
-                                                      Cp, gl);
-  HB_LAUNCH_CHECK();
+  if (int rc = with_dtype(dtype, [&](auto t) {
+        using T = decltype(t);
+        sam_bwd_kernel<T><<<blocks, kThreads, 0, st>>>((const T*)x, (const T*)dy, w, gate, (T*)dx, part, R, C, Cp, gl);
+        HB_LAUNCH_CHECK();
+        return 0;
+      }))
+    return rc;
   // dwdb[0..C) = dw, dwdb[C] = db: the dw columns, then the db column moved next to them
   column_sum_kernel<<<(C + kThreads - 1) / kThreads, kThreads, 0, st>>>(part, blocks, Cp + 1, C, dwdb);
   HB_LAUNCH_CHECK();
@@ -746,9 +735,9 @@ int hb_triplet_pool_fwd(const void* x, float* pc, int* ic, float* pw, int* iw, f
     return (int)cudaErrorInvalidValue;
   p.pc = pc; p.ic = ic; p.pw = pw; p.iw = iw;
   if (ph) { p.hp_max = hp_max; p.hp_sum = hp_sum; p.hp_idx = hp_idx; }
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_pool<float>(false, x, nullptr, p, ph, ih, st)
-                               : launch_pool<bf16>(false, x, nullptr, p, ph, ih, st);
+  return with_dtype(dtype, [&](auto t) {
+    return launch_pool<decltype(t)>(false, x, nullptr, p, ph, ih, (cudaStream_t)stream);
+  });
 }
 
 int hb_triplet_pool_bwd(const void* x, const void* dy, float* dgc, float* dgw, float* hp_sum, float* dgh, int N, int H,
@@ -758,9 +747,9 @@ int hb_triplet_pool_bwd(const void* x, const void* dy, float* dgc, float* dgw, f
   if ((dgh && !hp_sum) || (!dgc && !dgw && !dgh)) return (int)cudaErrorInvalidValue;
   p.pc = dgc; p.pw = dgw;
   if (dgh) p.hp_sum = hp_sum;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_pool<float>(true, x, dy, p, dgh, nullptr, st)
-                               : launch_pool<bf16>(true, x, dy, p, dgh, nullptr, st);
+  return with_dtype(dtype, [&](auto t) {
+    return launch_pool<decltype(t)>(true, x, dy, p, dgh, nullptr, (cudaStream_t)stream);
+  });
 }
 
 int hb_triplet_conv_fwd(const float* const* plane, const float* const* weight, float* const* z, float* const* parts,
@@ -846,11 +835,12 @@ int hb_triplet_apply(const void* x, void* y, const float* gc, const float* gh, c
   p.nb = (float)((gc != nullptr) + (gh != nullptr) + (gw != nullptr));
   const size_t total = (size_t)N * H * W * (Cp / vec_width(dtype));
   const int grid = stream_grid(total, kThreads, 16);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == HB_DTYPE_F32) tri_apply_kernel<float><<<grid, kThreads, 0, st>>>((const float*)x, (float*)y, p);
-  else tri_apply_kernel<bf16><<<grid, kThreads, 0, st>>>((const bf16*)x, (bf16*)y, p);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    tri_apply_kernel<T><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const T*)x, (T*)y, p);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_triplet_dx(const void* dy, void* dx, const float* gc, const float* gh, const float* gw, const float* dpc,
@@ -867,11 +857,12 @@ int hb_triplet_dx(const void* dy, void* dx, const float* gc, const float* gh, co
   p.nb = (float)((gc != nullptr) + (gh != nullptr) + (gw != nullptr));
   const size_t total = (size_t)N * H * W * (Cp / vec_width(dtype));
   const int grid = stream_grid(total, kThreads, 16);
-  cudaStream_t st = (cudaStream_t)stream;
-  if (dtype == HB_DTYPE_F32) tri_dx_kernel<float><<<grid, kThreads, 0, st>>>((const float*)dy, (float*)dx, p);
-  else tri_dx_kernel<bf16><<<grid, kThreads, 0, st>>>((const bf16*)dy, (bf16*)dx, p);
-  HB_LAUNCH_CHECK();
-  return 0;
+  return with_dtype(dtype, [&](auto t) {
+    using T = decltype(t);
+    tri_dx_kernel<T><<<grid, kThreads, 0, (cudaStream_t)stream>>>((const T*)dy, (T*)dx, p);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 }  // extern "C"

@@ -8,7 +8,9 @@
 // are written as zeros. "Uniform" vectors (C/G % 8 == 0, the RedNet case) have all 8 channels in one group, so a pixel's
 // K^2 weights of that group are loaded once into registers; "mixed" vectors (e.g. C = 12, G = 6) look the group up per
 // channel. Nothing here synchronises with the host; reductions run in a fixed order (no atomics).
-#include "common.cuh"
+#include <type_traits>
+
+#include "nhwc.cuh"
 
 namespace {
 
@@ -22,11 +24,6 @@ constexpr size_t kSmemMax = 112 * 1024;      // halo tile budget: two CTAs per S
 struct InvParams {
   int N, H, W, C, Cp, Ho, Wo, Kp, G, stride, pad, dil;
 };
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(valid ? 16 : 0));
-}
 
 // Tile geometry shared by the host launchers and the kernels: nv channel vectors per pixel, th x kTileW output pixels,
 // and the input box (halo included) those pixels read.
@@ -54,26 +51,6 @@ Tile make_tile(const InvParams& p, int K, int nv) {
   return t;
 }
 
-// Copies the CTA's input box [in_h][in_w][nv vectors] into shared memory (cp.async, zero-filled outside the image and
-// past the last channel vector).
-__device__ __forceinline__ void stage_x(uint4* xs, const bf16* __restrict__ x, const InvParams& p, int n, int oy0, int ox0,
-                                        int vbase, int nv, int in_h, int in_w) {
-  const int iy0 = oy0 * p.stride - p.pad, ix0 = ox0 * p.stride - p.pad;
-  const int cv = p.Cp / 8;
-  const int total = in_h * in_w * nv;
-  for (int e = threadIdx.x; e < total; e += blockDim.x) {
-    const int v = e % nv, q = e / nv;
-    const int yy = q / in_w, xx = q - yy * in_w;
-    const int hi = iy0 + yy, wi = ix0 + xx;
-    const bool ok = hi >= 0 && hi < p.H && wi >= 0 && wi < p.W && vbase + v < cv;
-    const bf16* src = ok ? x + (((size_t)n * p.H + hi) * p.W + wi) * p.Cp + (vbase + v) * 8 : x;
-    cp_async16(xs + e, src, ok);
-  }
-  asm volatile("cp.async.commit_group;\n" ::);
-  asm volatile("cp.async.wait_group 0;\n" ::);
-  __syncthreads();
-}
-
 // Forward. kSmem = false (only when a dilated halo box exceeds kSmemMax) reads the taps from global memory instead.
 template <int K, bool kUniform, bool kSmem>
 __global__ void __launch_bounds__(kThreads) inv_fwd_kernel(const bf16* __restrict__ x, const bf16* __restrict__ ker,
@@ -83,7 +60,9 @@ __global__ void __launch_bounds__(kThreads) inv_fwd_kernel(const bf16* __restric
   const int n = blockIdx.z;
   const int oy0 = (blockIdx.x / tl.tiles_w) * tl.th, ox0 = (blockIdx.x % tl.tiles_w) * kTileW;
   const int vbase = blockIdx.y * tl.nv;
-  if (kSmem) stage_x(xs, x, p, n, oy0, ox0, vbase, tl.nv, tl.in_h, tl.in_w);
+  if (kSmem)
+    stage_box(xs, x, (size_t)n * p.H * p.W, p.H, p.W, p.Cp, oy0 * p.stride - p.pad, ox0 * p.stride - p.pad, tl.in_h,
+              tl.in_w, tl.nv, vbase);
   const int v = threadIdx.x % tl.nv, pix = threadIdx.x / tl.nv;
   const int ty = pix / kTileW, tx = pix % kTileW;
   const int oy = oy0 + ty, ox = ox0 + tx, cvec = vbase + v;
@@ -210,7 +189,8 @@ __global__ void __launch_bounds__(kThreads) inv_bwd_kernel_kernel(const bf16* __
   const int n = blockIdx.z;
   const int oy0 = (blockIdx.x / tl.tiles_w) * tl.th, ox0 = (blockIdx.x % tl.tiles_w) * kTileW;
   const int vbase = blockIdx.y * tl.nv;
-  stage_x(xs, x, p, n, oy0, ox0, vbase, tl.nv, tl.in_h, tl.in_w);
+  stage_box(xs, x, (size_t)n * p.H * p.W, p.H, p.W, p.Cp, oy0 * p.stride - p.pad, ox0 * p.stride - p.pad, tl.in_h,
+            tl.in_w, tl.nv, vbase);
   const int v = threadIdx.x % tl.nv, pix = threadIdx.x / tl.nv;
   const int ty = pix / kTileW, tx = pix % kTileW;
   const int oy = oy0 + ty, ox = ox0 + tx, cvec = vbase + v;
@@ -286,20 +266,13 @@ __global__ void __launch_bounds__(kThreads) inv_bwd_kernel_generic_kernel(const 
 // every 8-channel vector lies inside one group and no vector is padding
 bool uniform_vectors(const InvParams& p) { return (p.C / p.G) % 8 == 0 && p.Cp == p.C; }
 
-// opts a kernel into more than the default 48 KiB of dynamic shared memory (a host-side attribute, no synchronisation)
-template <typename Kern>
-cudaError_t allow_smem(Kern kern, size_t bytes) {
-  if (bytes <= 48 * 1024) return cudaSuccess;
-  return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kSmemMax);
-}
-
 template <int K, bool kUniform>
 int launch_fwd(const bf16* x, const bf16* ker, bf16* y, const InvParams& p, cudaStream_t st) {
   const int cv = p.Cp / 8;
   const Tile tl = make_tile(p, K, cv >= 4 ? 4 : (cv >= 2 ? 2 : 1));
   const dim3 grid((unsigned)(tl.tiles_w * tl.tiles_h), (unsigned)tl.slabs, (unsigned)p.N);
   if (tl.smem <= kSmemMax) {
-    if (cudaError_t e = allow_smem(inv_fwd_kernel<K, kUniform, true>, tl.smem)) return (int)e;
+    if (cudaError_t e = allow_smem(inv_fwd_kernel<K, kUniform, true>, tl.smem, kSmemMax)) return (int)e;
     inv_fwd_kernel<K, kUniform, true><<<grid, tl.threads(), tl.smem, st>>>(x, ker, y, p, tl);
   } else {
     inv_fwd_kernel<K, kUniform, false><<<grid, tl.threads(), 0, st>>>(x, ker, y, p, tl);
@@ -317,7 +290,7 @@ int launch_bwd_kernel(const bf16* x, const bf16* dy, bf16* dker, const InvParams
     if (nv < vg) nv = vg;
     const Tile tl = make_tile(p, K, nv);
     if (tl.smem <= kSmemMax) {
-      if (cudaError_t e = allow_smem(inv_bwd_kernel_kernel<K>, tl.smem)) return (int)e;
+      if (cudaError_t e = allow_smem(inv_bwd_kernel_kernel<K>, tl.smem, kSmemMax)) return (int)e;
       const dim3 grid((unsigned)(tl.tiles_w * tl.tiles_h), (unsigned)tl.slabs, (unsigned)p.N);
       inv_bwd_kernel_kernel<K><<<grid, tl.threads(), tl.smem, st>>>(x, dy, dker, p, tl, vg);
       HB_LAUNCH_CHECK();
@@ -345,6 +318,16 @@ int make_params(InvParams& p, int N, int H, int W, int C, int Cp, int Kp, int K,
   return 0;
 }
 
+// f(std::integral_constant<int, K>{}) for the K make_params accepts
+template <typename F> int with_k(int K, F&& f) {
+  switch (K) {
+    case 1: return f(std::integral_constant<int, 1>{});
+    case 3: return f(std::integral_constant<int, 3>{});
+    case 5: return f(std::integral_constant<int, 5>{});
+    default: return f(std::integral_constant<int, 7>{});
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -358,12 +341,10 @@ int hb_involution_fwd_bf16(const void* x, const void* ker, void* y, int N, int H
   bf16* yb = (bf16*)y;
   cudaStream_t st = (cudaStream_t)stream;
   const bool u = uniform_vectors(p);
-  switch (K) {
-    case 1: return u ? launch_fwd<1, true>(xb, kb, yb, p, st) : launch_fwd<1, false>(xb, kb, yb, p, st);
-    case 3: return u ? launch_fwd<3, true>(xb, kb, yb, p, st) : launch_fwd<3, false>(xb, kb, yb, p, st);
-    case 5: return u ? launch_fwd<5, true>(xb, kb, yb, p, st) : launch_fwd<5, false>(xb, kb, yb, p, st);
-    default: return u ? launch_fwd<7, true>(xb, kb, yb, p, st) : launch_fwd<7, false>(xb, kb, yb, p, st);
-  }
+  return with_k(K, [&](auto k) {
+    constexpr int KK = decltype(k)::value;
+    return u ? launch_fwd<KK, true>(xb, kb, yb, p, st) : launch_fwd<KK, false>(xb, kb, yb, p, st);
+  });
 }
 
 int hb_involution_bwd_data_bf16(const void* dy, const void* ker, void* dx, int N, int H, int W, int C, int Cp, int Kp,
@@ -376,41 +357,22 @@ int hb_involution_bwd_data_bf16(const void* dy, const void* ker, void* dx, int N
   cudaStream_t st = (cudaStream_t)stream;
   const dim3 grid(stream_grid((size_t)N * H * W * (Cp / 8), kThreads, 16));
   const bool u = uniform_vectors(p);
-  switch (K) {
-    case 1:
-      if (u) inv_bwd_data_kernel<1, true><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      else inv_bwd_data_kernel<1, false><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      break;
-    case 3:
-      if (u) inv_bwd_data_kernel<3, true><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      else inv_bwd_data_kernel<3, false><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      break;
-    case 5:
-      if (u) inv_bwd_data_kernel<5, true><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      else inv_bwd_data_kernel<5, false><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      break;
-    default:
-      if (u) inv_bwd_data_kernel<7, true><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-      else inv_bwd_data_kernel<7, false><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  return with_k(K, [&](auto k) {
+    constexpr int KK = decltype(k)::value;
+    if (u) inv_bwd_data_kernel<KK, true><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
+    else inv_bwd_data_kernel<KK, false><<<grid, kThreads, 0, st>>>(dyb, kb, dxb, p);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_involution_bwd_kernel_bf16(const void* x, const void* dy, void* dker, int N, int H, int W, int C, int Cp, int Kp,
                                   int K, int G, int stride, int pad, int dil, void* stream) {
   InvParams p;
   if (int rc = make_params(p, N, H, W, C, Cp, Kp, K, G, stride, pad, dil)) return rc;
-  const bf16* xb = (const bf16*)x;
-  const bf16* dyb = (const bf16*)dy;
-  bf16* kb = (bf16*)dker;
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (K) {
-    case 1: return launch_bwd_kernel<1>(xb, dyb, kb, p, st);
-    case 3: return launch_bwd_kernel<3>(xb, dyb, kb, p, st);
-    case 5: return launch_bwd_kernel<5>(xb, dyb, kb, p, st);
-    default: return launch_bwd_kernel<7>(xb, dyb, kb, p, st);
-  }
+  return with_k(K, [&](auto k) {
+    return launch_bwd_kernel<decltype(k)::value>((const bf16*)x, (const bf16*)dy, (bf16*)dker, p, (cudaStream_t)stream);
+  });
 }
 
 }  // extern "C"

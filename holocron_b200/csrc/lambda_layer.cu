@@ -15,7 +15,9 @@
 // up to 8 (the transient per-position gradient of lp, sum_h q * dy); dvpos [B,HW,dv*u] fp32 (global share of dv).
 #include <math.h>
 
-#include "common.cuh"
+#include <type_traits>
+
+#include "nhwc.cuh"
 
 namespace {
 
@@ -31,11 +33,6 @@ struct LamParams {
 };
 
 __device__ __forceinline__ float bf(bf16 x) { return __bfloat162float(x); }
-
-__device__ __forceinline__ void cp_async16(void* smem, const void* gmem, bool valid) {
-  const unsigned s = (unsigned)__cvta_generic_to_shared(smem);
-  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;\n" ::"r"(s), "l"(gmem), "r"(valid ? 16 : 0));
-}
 
 // (max, sum of exp(x - max)) pairs: combine b into a
 __device__ __forceinline__ void lse_combine(float& ma, float& sa, float mb, float sb) {
@@ -118,22 +115,12 @@ __global__ void __launch_bounds__(kThreads) lam_content_kernel(const bf16* __res
 }
 
 // Copies the halo box [(kTile + r - 1)^2 pixels][U vectors] of v channels [v0*U, v0*U + 8U) around an output tile into
-// shared memory (cp.async, zero outside the image and past the last channel vector).
+// shared memory.
 template <int U>
 __device__ __forceinline__ void stage_v(uint4* vs, const bf16* __restrict__ v, const LamParams& p, int b, int ty0, int tx0,
                                         int v0) {
   const int pad = p.r / 2, box = kTile + p.r - 1;
-  const int total = box * box * U, cv = p.Cvp / 8, vec0 = v0 * U / 8;
-  for (int e = threadIdx.x; e < total; e += blockDim.x) {
-    const int uv = e % U, pix = e / U;
-    const int gy = ty0 - pad + pix / box, gx = tx0 - pad + pix % box;
-    const bool ok = gy >= 0 && gy < p.H && gx >= 0 && gx < p.W && vec0 + uv < cv;
-    const bf16* src = ok ? v + ((size_t)b * p.HW + gy * p.W + gx) * p.Cvp + (size_t)(vec0 + uv) * 8 : v;
-    cp_async16(vs + e, src, ok);
-  }
-  asm volatile("cp.async.commit_group;\n" ::);
-  asm volatile("cp.async.wait_group 0;\n" ::);
-  __syncthreads();
+  stage_box(vs, v, (size_t)b * p.HW, p.H, p.W, p.Cvp, ty0 - pad, tx0 - pad, box, box, U, v0 * U / 8);
 }
 
 // Output: a CTA covers an 8 x 8 tile of one sample, thread = (position, head), dv in chunks of 8. Content term from lc,
@@ -595,12 +582,6 @@ int make_params(LamParams& p, int B, int H, int W, int dk, int u, int heads, int
   return 0;
 }
 
-template <typename Kern>
-cudaError_t allow_smem(Kern kern, size_t bytes) {
-  if (bytes <= 48 * 1024) return cudaSuccess;
-  return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes);
-}
-
 struct HaloGrid {
   dim3 grid, block;
   size_t smem;
@@ -617,29 +598,34 @@ HaloGrid halo_grid(const LamParams& p, int U) {
   return g;
 }
 
+template <int V> using Int = std::integral_constant<int, V>;
+
+// f(Int<dk>{}) and f(Int<u>{}) for the dk and u make_params accepts
+template <typename F> int with_dk(int dk, F&& f) {
+  switch (dk) {
+    case 8: return f(Int<8>{});
+    case 16: return f(Int<16>{});
+    default: return f(Int<32>{});
+  }
+}
+
+template <typename F> int with_u(int u, F&& f) {
+  switch (u) {
+    case 1: return f(Int<1>{});
+    case 2: return f(Int<2>{});
+    case 3: return f(Int<3>{});
+    default: return f(Int<4>{});
+  }
+}
+
 // Dispatch of the (DK, U, local) instantiations; the global variant does not read v in these kernels and takes U = 1.
 template <template <int, int, bool> class Launch, typename... Args>
 int dispatch(const LamParams& p, Args... args) {
-  if (p.r == 0) {
-    switch (p.dk) {
-      case 8: return Launch<8, 1, false>::run(p, args...);
-      case 16: return Launch<16, 1, false>::run(p, args...);
-      default: return Launch<32, 1, false>::run(p, args...);
-    }
-  }
-#define HB_LAM_U(DKV)                                     \
-  switch (p.u) {                                          \
-    case 1: return Launch<DKV, 1, true>::run(p, args...); \
-    case 2: return Launch<DKV, 2, true>::run(p, args...); \
-    case 3: return Launch<DKV, 3, true>::run(p, args...); \
-    default: return Launch<DKV, 4, true>::run(p, args...); \
-  }
-  switch (p.dk) {
-    case 8: HB_LAM_U(8)
-    case 16: HB_LAM_U(16)
-    default: HB_LAM_U(32)
-  }
-#undef HB_LAM_U
+  return with_dk(p.dk, [&](auto dk) {
+    constexpr int DK = decltype(dk)::value;
+    if (p.r == 0) return Launch<DK, 1, false>::run(p, args...);
+    return with_u(p.u, [&](auto u) { return Launch<DK, decltype(u)::value, true>::run(p, args...); });
+  });
 }
 
 template <int DK, int U, bool kLocal>
@@ -647,7 +633,7 @@ struct OutLaunch {
   static int run(const LamParams& p, const bf16* q, const bf16* v, const float* Rt, const float* lc, const float* lp,
                  bf16* y, cudaStream_t st) {
     const HaloGrid g = halo_grid(p, U);
-    if (cudaError_t e = allow_smem(lam_out_kernel<DK, U, kLocal>, g.smem)) return (int)e;
+    if (cudaError_t e = allow_smem(lam_out_kernel<DK, U, kLocal>, g.smem, g.smem)) return (int)e;
     lam_out_kernel<DK, U, kLocal><<<g.grid, g.block, g.smem, st>>>(q, v, Rt, lc, lp, y, p, g.tiles_w);
     HB_LAUNCH_CHECK();
     return 0;
@@ -659,7 +645,7 @@ struct DqLaunch {
   static int run(const LamParams& p, const bf16* dy, const bf16* v, const float* Rt, const float* lc, const float* lp,
                  bf16* dq, cudaStream_t st) {
     const HaloGrid g = halo_grid(p, U);
-    if (cudaError_t e = allow_smem(lam_dq_kernel<DK, U, kLocal>, g.smem)) return (int)e;
+    if (cudaError_t e = allow_smem(lam_dq_kernel<DK, U, kLocal>, g.smem, g.smem)) return (int)e;
     lam_dq_kernel<DK, U, kLocal><<<g.grid, g.block, g.smem, st>>>(dy, v, Rt, lc, lp, dq, p, g.tiles_w);
     HB_LAUNCH_CHECK();
     return 0;
@@ -677,18 +663,6 @@ struct DvLaunch {
     return 0;
   }
 };
-
-// the global variant runs the U = 1 instantiations of the output and dq kernels; dv keeps the real U
-template <int DK, bool kLocal>
-int dv_by_u(const LamParams& p, const bf16* kt, const float* stats, const float* dlc, const bf16* dlp, const float* Rt,
-            const float* dvpos, bf16* dv, cudaStream_t st) {
-  switch (p.u) {
-    case 1: return DvLaunch<DK, 1, kLocal>::run(p, kt, stats, dlc, dlp, Rt, dvpos, dv, st);
-    case 2: return DvLaunch<DK, 2, kLocal>::run(p, kt, stats, dlc, dlp, Rt, dvpos, dv, st);
-    case 3: return DvLaunch<DK, 3, kLocal>::run(p, kt, stats, dlc, dlp, Rt, dvpos, dv, st);
-    default: return DvLaunch<DK, 4, kLocal>::run(p, kt, stats, dlc, dlp, Rt, dvpos, dv, st);
-  }
-}
 
 }  // namespace
 
@@ -745,18 +719,14 @@ int hb_lambda_bwd_v_bf16(const void* k, const float* stats, const float* dlc, co
   const bf16* kb = (const bf16*)k;
   const bf16* gb = (const bf16*)dlp;
   bf16* o = (bf16*)dv_out;
-  if (r > 0) {
-    switch (dk) {
-      case 8: return dv_by_u<8, true>(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
-      case 16: return dv_by_u<16, true>(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
-      default: return dv_by_u<32, true>(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
-    }
-  }
-  switch (dk) {
-    case 8: return dv_by_u<8, false>(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
-    case 16: return dv_by_u<16, false>(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
-    default: return dv_by_u<32, false>(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
-  }
+  // unlike the output and dq kernels, the global variant of dv runs with the layer's u
+  return with_dk(dk, [&](auto d) {
+    return with_u(u, [&](auto uu) {
+      constexpr int DK = decltype(d)::value, U = decltype(uu)::value;
+      return r > 0 ? DvLaunch<DK, U, true>::run(p, kb, stats, dlc, gb, Rt, dvpos, o, st)
+                   : DvLaunch<DK, U, false>::run(p, kb, stats, dlc, gb, Rt, dvpos, o, st);
+    });
+  });
 }
 
 // scratch: B * dk * u * r * r floats (the per-sample partials)
@@ -764,7 +734,7 @@ int hb_lambda_bwd_r_bf16(const void* dlp, const void* v, float* scratch, float* 
   HB_LAM_PARAMS
   if (r == 0) return (int)cudaErrorInvalidValue;
   const size_t smem = dr_smem_bytes(p);
-  if (cudaError_t e = allow_smem(lam_dr_partial_kernel, smem)) return (int)e;
+  if (cudaError_t e = allow_smem(lam_dr_partial_kernel, smem, smem)) return (int)e;
   lam_dr_partial_kernel<<<dim3((unsigned)r, (unsigned)B), kThreads, smem, st>>>((const bf16*)dlp, (const bf16*)v, scratch, p);
   HB_LAUNCH_CHECK();
   const int per = dk * u * r * r;

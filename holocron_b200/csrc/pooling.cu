@@ -15,8 +15,7 @@
 // writes dx once: dmax at the saved index plus dmean / L everywhere. The order is "NaN first, then larger, then lower
 // index", so ties and NaNs route the gradient as torch's max(dim).indices does. Partial results are combined in a
 // fixed order (no atomics): every run gives the same bits. Nothing here synchronises with the host.
-#include "common.cuh"
-#include "zpool.cuh"
+#include "nhwc.cuh"
 
 namespace {
 
@@ -262,16 +261,7 @@ __global__ void __launch_bounds__(kThreads) last_fwd_kernel(const T* __restrict_
       }
     }
   }
-  // the groups of a warp are aligned, so xor partners stay within the group; every lane runs the shuffles
-  for (int off = 1; off < g; off <<= 1) {
-    const float om = __shfl_xor_sync(0xffffffffu, mx, off);
-    const int oi = __shfl_xor_sync(0xffffffffu, ix, off);
-    sm += __shfl_xor_sync(0xffffffffu, sm, off);
-    if (better(om, oi, mx, ix)) {
-      mx = om;
-      ix = oi;
-    }
-  }
+  group_max_sum(mx, ix, sm, g);
   if (!live || lane != 0) return;
   y[(size_t)r * 2] = same_bits<T>(mx);
   y[(size_t)r * 2 + 1] = from_f<T>(sm / (float)C);
@@ -297,14 +287,9 @@ __global__ void __launch_bounds__(kThreads) last_bwd_kernel(const T* __restrict_
   }
 }
 
-bool bad_dtype(int dtype) { return dtype != HB_DTYPE_F32 && dtype != HB_DTYPE_BF16; }
-
-int vec_width(int dtype) { return dtype == HB_DTYPE_F32 ? 4 : 8; }
-
 // 0 when the shape is supported (fills p), otherwise cudaErrorInvalidValue
 int make_blur(BlurParams& p, const float* taps, int N, int H, int W, int C, int Cp, int K, int stride, int dtype) {
-  if (bad_dtype(dtype) || N <= 0 || H <= 0 || W <= 0 || C <= 0 || Cp < C || Cp % vec_width(dtype) != 0 || K < 2 ||
-      K > kMaxTaps || stride < 1 || taps == nullptr)
+  if (bad_rows(C, Cp, dtype) || N <= 0 || H <= 0 || W <= 0 || K < 2 || K > kMaxTaps || stride < 1 || taps == nullptr)
     return (int)cudaErrorInvalidValue;
   p.N = N; p.H = H; p.W = W; p.C = C; p.Cp = Cp; p.K = K; p.stride = stride;
   p.pad = ((stride - 1) + (K - 1)) / 2;
@@ -342,10 +327,8 @@ int launch_blur(bool fwd, const void* in, void* out, const BlurParams& p, cudaSt
 }
 
 int make_mid(MidParams& p, int A, int L, int M, int C, int Cp, int with_mean, int dtype) {
-  const int V = vec_width(dtype);
-  if (bad_dtype(dtype) || A <= 0 || L <= 0 || M <= 0 || C <= 0 || Cp < C || Cp % V != 0 || M % Cp != 0)
-    return (int)cudaErrorInvalidValue;
-  if ((M / V + 31) / 32 > 65535) return (int)cudaErrorInvalidValue;   // grid.y slabs of nv <= 32 vectors
+  if (bad_rows(C, Cp, dtype) || A <= 0 || L <= 0 || M <= 0 || M % Cp != 0) return (int)cudaErrorInvalidValue;
+  if ((M / vec_width(dtype) + 31) / 32 > 65535) return (int)cudaErrorInvalidValue;   // grid.y slabs of nv <= 32 vectors
   p = MidParams{A, L, M, C, Cp, with_mean ? 1 : 0};
   return 0;
 }
@@ -378,7 +361,7 @@ template <typename T>
 int launch_last(bool fwd, const void* in, void* out, int* idx, int R, int C, int Cp, cudaStream_t st) {
   constexpr int V = Vec16<T>::N;
   if (fwd) {
-    const int g = pow2_at_least((C + V - 1) / V, 32);
+    const int g = lane_group((C + V - 1) / V);
     const unsigned grid = (unsigned)(((long long)R * g + kThreads - 1) / kThreads);
     last_fwd_kernel<T><<<grid, kThreads, 0, st>>>((const T*)in, (T*)out, idx, R, C, Cp, g);
   } else {
@@ -393,9 +376,7 @@ int launch_last(bool fwd, const void* in, void* out, int* idx, int R, int C, int
   return 0;
 }
 
-bool bad_last(int R, int C, int Cp, int dtype) {
-  return bad_dtype(dtype) || R <= 0 || C <= 0 || Cp < C || Cp % vec_width(dtype) != 0;
-}
+bool bad_last(int R, int C, int Cp, int dtype) { return bad_rows(C, Cp, dtype) || R <= 0; }
 
 }  // namespace
 
@@ -405,46 +386,42 @@ int hb_blurpool_fwd(const void* x, void* y, const float* taps, int N, int H, int
                     int dtype, void* stream) {
   BlurParams p;
   if (int rc = make_blur(p, taps, N, H, W, C, Cp, K, stride, dtype)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_blur<float>(true, x, y, p, st) : launch_blur<bf16>(true, x, y, p, st);
+  return with_dtype(dtype, [&](auto t) { return launch_blur<decltype(t)>(true, x, y, p, (cudaStream_t)stream); });
 }
 
 int hb_blurpool_bwd(const void* dy, void* dx, const float* taps, int N, int H, int W, int C, int Cp, int K, int stride,
                     int dtype, void* stream) {
   BlurParams p;
   if (int rc = make_blur(p, taps, N, H, W, C, Cp, K, stride, dtype)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_blur<float>(false, dy, dx, p, st) : launch_blur<bf16>(false, dy, dx, p, st);
+  return with_dtype(dtype, [&](auto t) { return launch_blur<decltype(t)>(false, dy, dx, p, (cudaStream_t)stream); });
 }
 
 int hb_pool_mid_fwd(const void* x, void* y, int* idx, int A, int L, int M, int C, int Cp, int with_mean, int dtype,
                     void* stream) {
   MidParams p;
   if (int rc = make_mid(p, A, L, M, C, Cp, with_mean, dtype)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_mid_fwd<float>(x, y, idx, p, st) : launch_mid_fwd<bf16>(x, y, idx, p, st);
+  return with_dtype(dtype, [&](auto t) { return launch_mid_fwd<decltype(t)>(x, y, idx, p, (cudaStream_t)stream); });
 }
 
 int hb_pool_mid_bwd(const void* dy, const int* idx, void* dx, int A, int L, int M, int C, int Cp, int with_mean,
                     int dtype, void* stream) {
   MidParams p;
   if (int rc = make_mid(p, A, L, M, C, Cp, with_mean, dtype)) return rc;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_mid_bwd<float>(dy, idx, dx, p, st) : launch_mid_bwd<bf16>(dy, idx, dx, p, st);
+  return with_dtype(dtype, [&](auto t) { return launch_mid_bwd<decltype(t)>(dy, idx, dx, p, (cudaStream_t)stream); });
 }
 
 int hb_pool_last_fwd(const void* x, void* y, int* idx, int R, int C, int Cp, int dtype, void* stream) {
   if (bad_last(R, C, Cp, dtype)) return (int)cudaErrorInvalidValue;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_last<float>(true, x, y, idx, R, C, Cp, st)
-                               : launch_last<bf16>(true, x, y, idx, R, C, Cp, st);
+  return with_dtype(dtype, [&](auto t) {
+    return launch_last<decltype(t)>(true, x, y, idx, R, C, Cp, (cudaStream_t)stream);
+  });
 }
 
 int hb_pool_last_bwd(const void* dy, const int* idx, void* dx, int R, int C, int Cp, int dtype, void* stream) {
   if (bad_last(R, C, Cp, dtype)) return (int)cudaErrorInvalidValue;
-  cudaStream_t st = (cudaStream_t)stream;
-  return dtype == HB_DTYPE_F32 ? launch_last<float>(false, dy, dx, (int*)idx, R, C, Cp, st)
-                               : launch_last<bf16>(false, dy, dx, (int*)idx, R, C, Cp, st);
+  return with_dtype(dtype, [&](auto t) {
+    return launch_last<decltype(t)>(false, dy, dx, (int*)idx, R, C, Cp, (cudaStream_t)stream);
+  });
 }
 
 }  // extern "C"

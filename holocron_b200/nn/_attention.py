@@ -12,8 +12,8 @@ import torch
 from torch import Tensor, nn
 
 from .._lib import check, dtype_code, lib, ptr, require_cuda, stream_ptr
-from ._fused import BNBranch, _bn_batch_stats, attach_stats, sync_group
-from ._pooling import _apply, _empty_cl, _nhwc, _pitch
+from ._fused import BNBranch, _bn_batch_stats, _empty_cl, attach_stats, sync_group
+from ._nhwc import compute_dtype, crop, nhwc, pitch, require_4d, run_native
 
 _VP3 = ctypes.c_void_p * 3
 _I3 = ctypes.c_int * 3
@@ -30,9 +30,9 @@ def _f32(t: Tensor) -> Tensor:
     return t.detach().reshape(-1).float().contiguous()
 
 
-def _require_4d(name: str, x: Tensor) -> None:
-    if x.ndim != 4:
-        raise NotImplementedError(f"{name}: 4-D (N, C, H, W) inputs only, got shape {tuple(x.shape)}")
+def _enabled(en: Sequence[bool], make) -> List[Optional[Tensor]]:
+    """make(b) for each enabled branch b, None for the others."""
+    return [make(b) if en[b] else None for b in range(3)]
 
 
 # --------------------------------------------------------------------------------------------------------- SAM
@@ -42,10 +42,10 @@ class _SamFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: Tensor, weight: Tensor, bias: Tensor) -> Tensor:
         n, c, h, w = x.shape
-        cp = _pitch(c, x.dtype)
-        xc = _nhwc(x, cp)
+        cp = pitch(c, x.dtype)
+        xc = nhwc(x, cp)
         w32, b32 = _f32(weight), _f32(bias)
-        y = _empty_cl(n, cp, h, w, xc)
+        y = _empty_cl(n, cp, h, w, xc.device, xc.dtype)
         gate = torch.empty(n * h * w, dtype=torch.float32, device=x.device)
         check(lib().hb_sam_fwd(ptr(xc), ptr(w32), ptr(b32), ptr(y), ptr(gate), n * h * w, c, cp, dtype_code(xc),
                                stream_ptr()), "hb_sam_fwd")
@@ -64,23 +64,23 @@ class _SamFn(torch.autograd.Function):
         slots = L.hb_sam_bwd_slots(n * h * w, c, cp, dt)
         part = torch.empty((max(slots, 1), cp + 1), dtype=torch.float32, device=xc.device)
         dwdb = torch.empty(c + 1, dtype=torch.float32, device=xc.device)
-        dx = _empty_cl(n, cp, h, w, xc)
+        dx = _empty_cl(n, cp, h, w, xc.device, xc.dtype)
         check(L.hb_sam_bwd(ptr(xc), ptr(dyc), ptr(w32), ptr(gate), ptr(dx), ptr(part), ptr(dwdb), n * h * w, c, cp, dt,
                            stream_ptr()), "hb_sam_bwd")
-        return (dx if cp == c else dx[:, :c]), dwdb[:c].view(wshape).to(wdt), dwdb[c:].to(bdt)
+        return crop(dx, c), dwdb[:c].view(wshape).to(wdt), dwdb[c:].to(bdt)
 
 
 def sam(x: Tensor, weight: Tensor, bias: Tensor) -> Tensor:
     """SAM's forward (reference attention.py:29-30): x * sigmoid(conv2d(x, weight, bias)) with a [1, C, 1, 1] filter."""
-    _require_4d("SAM", x)
+    require_4d("SAM", x)
     if x.shape[1] != weight.shape[1]:
         raise RuntimeError(f"SAM: built for {weight.shape[1]} channels, got an input with {x.shape[1]}")
-    dt = x.dtype if x.dtype in (torch.float32, torch.bfloat16) else torch.float32
-    if _pitch(x.shape[1], dt) * dt.itemsize > 16 * SAM_MAX_VECTORS:
+    dt = compute_dtype(x.dtype)
+    if pitch(x.shape[1], dt) * dt.itemsize > 16 * SAM_MAX_VECTORS:
         raise NotImplementedError(f"SAM: at most {16 * SAM_MAX_VECTORS // dt.itemsize} channels in {dt}, got "
                                   f"{x.shape[1]}")
     require_cuda(x)
-    return _apply(_SamFn, x, weight, bias)
+    return run_native(_SamFn, x, weight, bias)
 
 
 # --------------------------------------------------------------------------------------------------------- triplet
@@ -103,16 +103,16 @@ class _TripletFn(torch.autograd.Function):
     @staticmethod
     def forward(ctx, x: Tensor, bns, *params) -> Tensor:
         n, c, h, w = x.shape
-        cp = _pitch(c, x.dtype)
+        cp = pitch(c, x.dtype)
         dev = x.device
-        xc = _nhwc(x, cp)
+        xc = nhwc(x, cp)
         L = lib()
         dt = dtype_code(xc)
         en = [bn is not None for bn in bns]
         dims = [_plane_dims(b, c, h, w) for b in range(3)]
         f32 = dict(dtype=torch.float32, device=dev)
-        planes = [torch.empty((n, 2) + dims[b], **f32) if en[b] else None for b in range(3)]
-        idx = [torch.empty((n,) + dims[b], dtype=torch.int32, device=dev) if en[b] else None for b in range(3)]
+        planes = _enabled(en, lambda b: torch.empty((n, 2) + dims[b], **f32))
+        idx = _enabled(en, lambda b: torch.empty((n,) + dims[b], dtype=torch.int32, device=dev))
         hp = [None, None, None]
         if en[1]:
             nhb = -(-h // L.hb_triplet_row_block(h, c, cp, dt))
@@ -124,13 +124,13 @@ class _TripletFn(torch.autograd.Function):
         rows = _I3(*[d[0] for d in dims])
         cols = _I3(*[d[1] for d in dims])
         blocks = [-(-(n * d[0] * d[1]) // _THREADS) for d in dims]
-        wts = [_f32(params[3 * b]) if en[b] else None for b in range(3)]
-        z = [torch.empty((n, 1) + dims[b], **f32) if en[b] else None for b in range(3)]
-        parts = [torch.empty((blocks[b], 1, 2), **f32) if en[b] else None for b in range(3)]
+        wts = _enabled(en, lambda b: _f32(params[3 * b]))
+        z = _enabled(en, lambda b: torch.empty((n, 1) + dims[b], **f32))
+        parts = _enabled(en, lambda b: torch.empty((blocks[b], 1, 2), **f32))
         slots = _I3()
         check(L.hb_triplet_conv_fwd(_vp3(planes), _vp3(wts), _vp3(z), _vp3(parts), slots, rows, cols, n,
                                     stream_ptr()), "hb_triplet_conv_fwd")
-        stats = [torch.empty((4, 1), **f32) if en[b] else None for b in range(3)]
+        stats = _enabled(en, lambda b: torch.empty((4, 1), **f32))
         train = None
         for b in range(3):
             if not en[b]:
@@ -146,9 +146,9 @@ class _TripletFn(torch.autograd.Function):
                                           ctypes.c_float(bn.eps), 1, 1, ptr(stats[b][2]), ptr(stats[b][3]),
                                           ptr(stats[b][0]), ptr(stats[b][1]), stream_ptr()), "hb_bn_eval_affine")
             train = _uses_batch_stats(bn)
-        gates = [torch.empty((n,) + dims[b], **f32) if en[b] else None for b in range(3)]
+        gates = _enabled(en, lambda b: torch.empty((n,) + dims[b], **f32))
         check(L.hb_triplet_gate(_vp3(z), _vp3(stats), _vp3(gates), rows, cols, n, stream_ptr()), "hb_triplet_gate")
-        y = _empty_cl(n, cp, h, w, xc)
+        y = _empty_cl(n, cp, h, w, dev, xc.dtype)
         check(L.hb_triplet_apply(ptr(xc), ptr(y), ptr(gates[0]), ptr(gates[1]), ptr(gates[2]), n, h, w, c, cp, dt,
                                  stream_ptr()), "hb_triplet_apply")
         ctx.save_for_backward(xc, *planes, *idx, *z, *gates, *stats, *wts)
@@ -170,25 +170,25 @@ class _TripletFn(torch.autograd.Function):
         cols = _I3(*[d[1] for d in dims])
         f32 = dict(dtype=torch.float32, device=dev)
         dyc = dy.contiguous(memory_format=torch.channels_last)
-        dg = [torch.empty((n,) + dims[b], **f32) if en[b] else None for b in range(3)]
+        dg = _enabled(en, lambda b: torch.empty((n,) + dims[b], **f32))
         hp_sum = None
         if en[1]:
             hp_sum = torch.empty((n, -(-h // L.hb_triplet_row_block(h, c, cp, dt)), w, c), **f32)
         check(L.hb_triplet_pool_bwd(ptr(xc), ptr(dyc), ptr(dg[0]), ptr(dg[2]), ptr(hp_sum), ptr(dg[1]), n, h, w, c,
                                     cp, dt, stream_ptr()), "hb_triplet_pool_bwd")
-        dz = [torch.empty((n,) + dims[b], **f32) if en[b] else None for b in range(3)]
-        bparts = [torch.empty((blocks[b], 2), **f32) if en[b] else None for b in range(3)]
-        dgamma = [torch.empty(1, **f32) if en[b] else None for b in range(3)]
-        dbeta = [torch.empty(1, **f32) if en[b] else None for b in range(3)]
+        dz = _enabled(en, lambda b: torch.empty((n,) + dims[b], **f32))
+        bparts = _enabled(en, lambda b: torch.empty((blocks[b], 2), **f32))
+        dgamma = _enabled(en, lambda b: torch.empty(1, **f32))
+        dbeta = _enabled(en, lambda b: torch.empty(1, **f32))
         check(L.hb_triplet_bn_bwd(_vp3(dg), _vp3(z), _vp3(gates), _vp3(stats), _vp3(dz), _vp3(bparts),
                                   _vp3(dgamma), _vp3(dbeta), rows, cols, n, ctypes.c_float(1.0 / sum(en)),
                                   int(train), stream_ptr()), "hb_triplet_bn_bwd")
-        dplane = [torch.empty((n, 2) + dims[b], **f32) if en[b] else None for b in range(3)]
-        wparts = [torch.empty((blocks[b], _TAPS), **f32) if en[b] else None for b in range(3)]
-        dw = [torch.empty(_TAPS, **f32) if en[b] else None for b in range(3)]
+        dplane = _enabled(en, lambda b: torch.empty((n, 2) + dims[b], **f32))
+        wparts = _enabled(en, lambda b: torch.empty((blocks[b], _TAPS), **f32))
+        dw = _enabled(en, lambda b: torch.empty(_TAPS, **f32))
         check(L.hb_triplet_conv_bwd(_vp3(planes), _vp3(wts), _vp3(dz), _vp3(dplane), _vp3(wparts), _vp3(dw), rows,
                                     cols, n, stream_ptr()), "hb_triplet_conv_bwd")
-        dx = _empty_cl(n, cp, h, w, xc)
+        dx = _empty_cl(n, cp, h, w, dev, xc.dtype)
         check(L.hb_triplet_dx(ptr(dyc), ptr(dx), ptr(gates[0]), ptr(gates[1]), ptr(gates[2]), ptr(dplane[0]),
                               ptr(dplane[1]), ptr(dplane[2]), ptr(idx[0]), ptr(idx[1]), ptr(idx[2]), n, h, w, c, cp,
                               dt, stream_ptr()), "hb_triplet_dx")
@@ -197,14 +197,14 @@ class _TripletFn(torch.autograd.Function):
             for k, g in enumerate((dw[b], dgamma[b], dbeta[b])):
                 i = 3 * b + k
                 grads.append(None if g is None or pdt[i] is None else g.view(pshape[i]).to(pdt[i]))
-        return (dx if cp == c else dx[:, :c]), None, *grads
+        return crop(dx, c), None, *grads
 
 
 def triplet_attention(x: Tensor, branches: Sequence[Tuple[int, nn.Conv2d, nn.BatchNorm2d]]) -> Tensor:
     """The mean over ``branches`` of x gated along each branch's dim (DimAttention.forward, attention.py:50-56, and
     TripletAttention.forward, :72-77). A branch is (dim, 7x7 conv, BatchNorm2d) with dim in 1..3 or its negative form;
     one launch sequence serves every branch."""
-    _require_4d("TripletAttention", x)
+    require_4d("TripletAttention", x)
     n, c, h, w = x.shape
     bns: List[Optional[nn.BatchNorm2d]] = [None, None, None]
     params: List[Optional[Tensor]] = [None] * 9
@@ -224,9 +224,9 @@ def triplet_attention(x: Tensor, branches: Sequence[Tuple[int, nn.Conv2d, nn.Bat
                              f"{torch.Size((n, 1, rows, cols))}")
         bns[b] = bn
         params[3 * b:3 * b + 3] = [conv.weight, bn.weight, bn.bias]
-    if _pitch(c, torch.bfloat16 if x.dtype == torch.bfloat16 else torch.float32) > 2048:
+    if pitch(c, compute_dtype(x.dtype)) > 2048:
         raise NotImplementedError(f"TripletAttention: at most 2048 channels, got {c}")
     if len({_uses_batch_stats(bn) for bn in bns if bn is not None}) > 1:
         raise NotImplementedError("TripletAttention: branches mixing training and evaluation BatchNorm modes")
     require_cuda(x)
-    return _apply(_TripletFn, x, tuple(bns), *params)
+    return run_native(_TripletFn, x, tuple(bns), *params)

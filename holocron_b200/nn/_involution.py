@@ -5,6 +5,7 @@ import torch
 
 from .._lib import check, lib, ptr, require_cuda, stream_ptr
 from . import _fused as K
+from ._nhwc import crop
 
 SUPPORTED_KERNEL_SIZES = (1, 3, 5, 7)
 
@@ -58,7 +59,7 @@ class _InvolutionFn(torch.autograd.Function):
                                            stream_ptr()), "hb_involution_fwd_bf16")
         ctx.save_for_backward(xb, kb)
         ctx.cfg = (c, k, stride, pad, dil, groups)
-        return y if cp == c else y[:, :c]
+        return crop(y, c)
 
     @staticmethod
     def backward(ctx, dy: Tensor):
@@ -73,7 +74,7 @@ class _InvolutionFn(torch.autograd.Function):
             dxp = K._empty_cl(n, cp, h, w, dyb.device)
             check(L.hb_involution_bwd_data_bf16(ptr(dyb), ptr(kb), ptr(dxp), n, h, w, c, cp, kp, k, groups, stride, pad,
                                                 dil, stream_ptr()), "hb_involution_bwd_data_bf16")
-            dx = dxp if cp == c else dxp[:, :c]
+            dx = crop(dxp, c)
         if ctx.needs_input_grad[1]:
             dker = K._empty_cl(n, kp, ho, wo, dyb.device)
             check(L.hb_involution_bwd_kernel_bf16(ptr(xb), ptr(dyb), ptr(dker), n, h, w, c, cp, kp, k, groups, stride,

@@ -3,8 +3,7 @@ depth-wise conv2d, holocron/nn/modules/downsample.py:106-151) without the padded
 ``GlobalMaxPool2d`` (:80-99) and ``z_pool`` (holocron/nn/functional.py:139-147) with their backward passes writing the
 input gradient once, without a zero-filled scatter target or a ``torch.cat``.
 
-bf16 and fp32 tensors run natively (fp32 is not rounded through bf16: that would create ties and move the gradient of
-the max); other float dtypes are computed in fp32 and cast back. 4-D outputs are channels_last."""
+bf16 and fp32 tensors run natively, other float dtypes in fp32 (``_nhwc``). 4-D outputs are channels_last."""
 import ctypes
 from typing import Tuple
 
@@ -12,6 +11,8 @@ import torch
 from torch import Tensor
 
 from .._lib import check, dtype_code, lib, ptr, require_cuda, stream_ptr
+from ._fused import _empty_cl
+from ._nhwc import crop, nhwc, pitch as _pitch, require_4d, run_native
 
 MAX_BLUR_KERNEL = 7
 Z_POOL_DIMS = (1, 2, 3, -1, -2, -3)
@@ -54,33 +55,6 @@ def blur_taps(coeffs: Tensor, dtype: torch.dtype):
     return (ctypes.c_float * len(taps))(*taps)
 
 
-def _compute_dtype(x: Tensor) -> torch.dtype:
-    if not x.is_floating_point():
-        raise RuntimeError(f"pooling: floating-point input expected, got {x.dtype}")
-    return x.dtype if x.dtype in (torch.float32, torch.bfloat16) else torch.float32
-
-
-def _pitch(c: int, dtype: torch.dtype) -> int:
-    """Channels per NHWC row: C rounded up to one 16-byte vector."""
-    v = 16 // torch.tensor([], dtype=dtype).element_size()
-    return (c + v - 1) // v * v
-
-
-def _empty_cl(n: int, c: int, h: int, w: int, like: Tensor) -> Tensor:
-    return torch.empty((n, c, h, w), dtype=like.dtype, device=like.device, memory_format=torch.channels_last)
-
-
-def _nhwc(x: Tensor, cp: int) -> Tensor:
-    """x as channels_last with a row pitch of ``cp`` channels. The padding channels are left uninitialised: the kernels
-    never read them into a result."""
-    n, c, h, w = x.shape
-    if cp == c:
-        return x.contiguous(memory_format=torch.channels_last)
-    out = _empty_cl(n, cp, h, w, x)
-    out[:, :c] = x
-    return out
-
-
 class _BlurPoolFn(torch.autograd.Function):
     """x [N, C, H, W] -> y [N, Cp, Ho, Wo] channels_last (the caller drops the padding channels)."""
 
@@ -90,8 +64,8 @@ class _BlurPoolFn(torch.autograd.Function):
         cp = _pitch(c, x.dtype)
         pad = blur_padding(k, stride)
         ho, wo = (h + 2 * pad - k) // stride + 1, (w + 2 * pad - k) // stride + 1
-        xc = _nhwc(x, cp)
-        y = _empty_cl(n, cp, ho, wo, xc)
+        xc = nhwc(x, cp)
+        y = _empty_cl(n, cp, ho, wo, xc.device, xc.dtype)
         check(lib().hb_blurpool_fwd(ptr(xc), ptr(y), ctypes.cast(taps, ctypes.c_void_p), n, h, w, c, cp, k, stride,
                                     dtype_code(xc), stream_ptr()), "hb_blurpool_fwd")
         ctx.cfg = (taps, k, stride, c, h, w)
@@ -102,10 +76,10 @@ class _BlurPoolFn(torch.autograd.Function):
         taps, k, stride, c, h, w = ctx.cfg
         n, cp = dy.shape[:2]
         dyc = dy.contiguous(memory_format=torch.channels_last)
-        dx = _empty_cl(n, cp, h, w, dyc)
+        dx = _empty_cl(n, cp, h, w, dyc.device, dyc.dtype)
         check(lib().hb_blurpool_bwd(ptr(dyc), ptr(dx), ctypes.cast(taps, ctypes.c_void_p), n, h, w, c, cp, k, stride,
                                     dtype_code(dyc), stream_ptr()), "hb_blurpool_bwd")
-        return (dx if cp == c else dx[:, :c]), None, None, None
+        return crop(dx, c), None, None, None
 
 
 # Reduction modes: "hw" reduces H*W (global max pooling), 1 / 2 / 3 reduce that dim into (max, mean) (z_pool).
@@ -126,16 +100,16 @@ class _ReduceFn(torch.autograd.Function):
     def forward(ctx, x: Tensor, mode) -> Tensor:
         n, c, h, w = x.shape
         cp = _pitch(c, x.dtype)
-        xc = _nhwc(x, cp)
+        xc = nhwc(x, cp)
         L = lib()
         if mode == 1:
-            y = _empty_cl(n, 2, h, w, xc)
+            y = _empty_cl(n, 2, h, w, xc.device, xc.dtype)
             idx = torch.empty(n * h * w, dtype=torch.int32, device=x.device)
             check(L.hb_pool_last_fwd(ptr(xc), ptr(y), ptr(idx), n * h * w, c, cp, dtype_code(xc), stream_ptr()),
                   "hb_pool_last_fwd")
         else:
             a, l, m, shape = _mid_view(mode, n, cp, h, w)
-            y = _empty_cl(*shape, xc)
+            y = _empty_cl(*shape, xc.device, xc.dtype)
             idx = torch.empty(a * m, dtype=torch.int32, device=x.device)
             check(L.hb_pool_mid_fwd(ptr(xc), ptr(y), ptr(idx), a, l, m, c, cp, int(mode != "hw"), dtype_code(xc),
                                     stream_ptr()), "hb_pool_mid_fwd")
@@ -149,7 +123,7 @@ class _ReduceFn(torch.autograd.Function):
         mode, c, cp, h, w = ctx.cfg
         n = dy.shape[0]
         dyc = dy.contiguous(memory_format=torch.channels_last)
-        dx = _empty_cl(n, cp, h, w, dyc)
+        dx = _empty_cl(n, cp, h, w, dyc.device, dyc.dtype)
         L = lib()
         if mode == 1:
             check(L.hb_pool_last_bwd(ptr(dyc), ptr(idx), ptr(dx), n * h * w, c, cp, dtype_code(dyc), stream_ptr()),
@@ -158,32 +132,21 @@ class _ReduceFn(torch.autograd.Function):
             a, l, m, _ = _mid_view(mode, n, cp, h, w)
             check(L.hb_pool_mid_bwd(ptr(dyc), ptr(idx), ptr(dx), a, l, m, c, cp, int(mode != "hw"), dtype_code(dyc),
                                     stream_ptr()), "hb_pool_mid_bwd")
-        return (dx if cp == c else dx[:, :c]), None
-
-
-def _apply(fn, x: Tensor, *args, crop: bool = True) -> Tensor:
-    """Runs ``fn`` in the compute dtype of ``x``, drops the padding channels and casts back to the input dtype."""
-    dt = _compute_dtype(x)
-    y = fn.apply(x if x.dtype == dt else x.to(dt), *args)
-    c = x.shape[1]
-    if crop and y.shape[1] != c:
-        y = y[:, :c]
-    return y if y.dtype == x.dtype else y.to(x.dtype)
+        return crop(dx, c), None
 
 
 def blur_pool2d(x: Tensor, coeffs: Tensor, channels: int, kernel_size: int, stride: int) -> Tensor:
     """BlurPool2d's forward (reference downsample.py:148-151): the reflection-padded depth-wise binomial filter."""
     check_blurpool(channels, tuple(x.shape), kernel_size, stride)
     require_cuda(x)
-    return _apply(_BlurPoolFn, x, blur_taps(coeffs, x.dtype), int(kernel_size), int(stride))
+    return run_native(_BlurPoolFn, x, blur_taps(coeffs, x.dtype), int(kernel_size), int(stride))
 
 
 def global_max_pool2d(x: Tensor) -> Tensor:
     """(N, C, H, W) -> (N, C, 1, 1): the max over space; its gradient goes to the element max(dim).indices names."""
-    if x.ndim != 4:
-        raise NotImplementedError(f"GlobalMaxPool2d: 4-D (N, C, H, W) inputs only, got shape {tuple(x.shape)}")
+    require_4d("GlobalMaxPool2d", x)
     require_cuda(x)
-    return _apply(_ReduceFn, x, "hw")
+    return run_native(_ReduceFn, x, "hw")
 
 
 def z_pool(x: Tensor, dim: int) -> Tensor:
@@ -194,4 +157,4 @@ def z_pool(x: Tensor, dim: int) -> Tensor:
                                   f"and dim {dim}")
     require_cuda(x)
     dim = dim % 4
-    return _apply(_ReduceFn, x, dim, crop=dim != 1)
+    return run_native(_ReduceFn, x, dim, crop_channels=dim != 1)

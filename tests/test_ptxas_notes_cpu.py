@@ -2,14 +2,17 @@
 holocron_b200/csrc/build.py keeps in csrc/build/<unit>.log, when it has to serialise wgmma instructions
 (C7511: not enough registers for the pipeline; C7520: a warpgroup arrive it inserted on a divergent path) or to insert
 warpgroup arrives around accumulator accesses (C7519). Any of these puts every MMA of the kernel behind the previous
-one. Spills are checked as well: they would put the accumulators in local memory."""
+one. Spills are checked as well: they would put the accumulators in local memory. The pooling, attention, involution and
+lambda units hold no wgmma; their register-heavy kernels (SAM backward, the lambda output and dq kernels at their
+launch-bound cap) are checked for spills."""
 import re
 from pathlib import Path
 
 import pytest
 
 BUILD = Path(__file__).resolve().parents[1] / "holocron_b200" / "csrc" / "build"
-UNITS = ["conv_fprop", "conv_rows", "conv_wgrad", "conv_wgrad_rows"]
+UNITS = ["conv_fprop", "conv_rows", "conv_wgrad", "conv_wgrad_rows", "attention", "pooling", "involution",
+         "lambda_layer"]
 SERIALISED = re.compile(r"\((C7511|C7519|C7520)\)")
 SPILLS = re.compile(r"(\d+) bytes spill stores, (\d+) bytes spill loads")
 
