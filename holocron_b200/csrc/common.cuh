@@ -139,4 +139,29 @@ __host__ inline int stream_grid(size_t work_items, int per_block, int max_waves 
   return (int)(need < cap ? need : cap);
 }
 
+// Output extent of a window of k taps (dilation dil) sliding with `stride` over `in` pixels padded by `pad` on both
+// sides. False unless in, k, stride, dil >= 1, pad >= 0, the dilated window fits the padded input and the extent fits
+// an int. The span is computed in 64 bits and tested before the division, which truncates towards zero: on its own,
+// (in + 2 * pad - dil * (k - 1) - 1) / stride + 1 gives 1 for a window up to stride - 1 pixels too large.
+inline bool window_out(int in, int k, int stride, int pad, int dil, int& out) {
+  if (in < 1 || k < 1 || stride < 1 || dil < 1 || pad < 0) return false;
+  const long long span = (long long)in + 2LL * pad - (long long)dil * (k - 1) - 1;
+  if (span < 0 || span / stride >= 0x7fffffffLL) return false;
+  out = (int)(span / stride + 1);
+  return true;
+}
+
+template <typename T> struct Type { using type = T; };
+
+// f(Type<T>{}) for the dtype code; cudaErrorInvalidValue for an unknown code
+template <class F>
+int dispatch_dtype(int dtype, F f) {
+  switch (dtype) {
+    case HB_DTYPE_F32: return f(Type<float>{});
+    case HB_DTYPE_BF16: return f(Type<__nv_bfloat16>{});
+    case HB_DTYPE_F16: return f(Type<__half>{});
+    default: return (int)cudaErrorInvalidValue;
+  }
+}
+
 }  // namespace hb

@@ -10,102 +10,66 @@ namespace {
 
 using namespace hb;
 
-// w: [Cout][R][S][Cin] fp32.  wf: [CoutF][R][S][CinP] bf16 (zero padded).  wd: [CinD][R][S][CoutP] bf16 with
-// wd[ci][r][s][co] = w[co][R-1-r][S-1-s][ci] (rows ci >= Cin and columns co >= Cout are zero).
-__global__ void pack_weights_kernel(const float* __restrict__ w, __nv_bfloat16* __restrict__ wf,
-                                    __nv_bfloat16* __restrict__ wd, int Cout, int Cin, int R, int S, int CinP, int CinD,
-                                    int CoutP, int CoutF) {
-  const size_t nf = (size_t)CoutF * R * S * CinP;
-  const size_t nd = wd ? (size_t)CinD * R * S * CoutP : 0;
-  const size_t stride = (size_t)gridDim.x * blockDim.x;
-  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < nf + nd; i += stride) {
-    if (i < nf) {
-      const int ci = i % CinP;
-      size_t t = i / CinP;
-      const int s = t % S; t /= S;
-      const int r = t % R;
-      const int co = t / R;
-      const float v = (ci < Cin && co < Cout) ? w[(((size_t)co * R + r) * S + s) * Cin + ci] : 0.f;
-      wf[i] = __float2bfloat16_rn(v);
-    } else {
-      const size_t k = i - nf;
-      const int co = k % CoutP;
-      size_t t = k / CoutP;
-      const int s = t % S; t /= S;
-      const int r = t % R;
-      const int ci = t / R;
-      const float v = (co < Cout && ci < Cin) ? w[(((size_t)co * R + (R - 1 - r)) * S + (S - 1 - s)) * Cin + ci] : 0.f;
-      wd[k] = __float2bfloat16_rn(v);
-    }
+// One filter to pack. w: [Cout][R][S][Cin] fp32.  wf: [CoutF][R][S][CinP] bf16 (zero padded).  wd (may be null):
+// [CinD][R][S][CoutP] bf16 with wd[ci][r][s][co] = w[co][R-1-r][S-1-s][ci] (rows ci >= Cin and columns co >= Cout are zero).
+struct PackMeta {
+  const float* w;
+  __nv_bfloat16* wf;
+  __nv_bfloat16* wd;
+  int Cout, Cin, R, S, CinP, CinD, CoutP, CoutF;
+
+  __host__ __device__ size_t nf() const { return (size_t)CoutF * R * S * CinP; }
+  __host__ __device__ size_t total() const { return nf() + (wd ? (size_t)CinD * R * S * CoutP : 0); }
+};
+constexpr int kPackChunk = 4096;
+
+// Element i of the packed pair: wf[i] for i < nf, else wd[i - nf]. The divisions and the w offset run in the index type
+// I (unsigned when the pair has fewer than 2^31 elements); the filter coordinates fit an int.
+template <typename I>
+__device__ __forceinline__ void pack_element(const PackMeta& m, I i, I nf) {
+  const int R = m.R, S = m.S, Cin = m.Cin, Cout = m.Cout;
+  if (i < nf) {
+    const int ci = i % (I)m.CinP;
+    I t = i / (I)m.CinP;
+    const int s = t % S; t /= S;
+    const int r = t % R;
+    const int co = t / R;
+    const float v = (ci < Cin && co < Cout) ? m.w[(((I)co * R + r) * S + s) * Cin + ci] : 0.f;
+    m.wf[i] = __float2bfloat16_rn(v);
+  } else {
+    const I k = i - nf;
+    const int co = k % (I)m.CoutP;
+    I t = k / (I)m.CoutP;
+    const int s = t % S; t /= S;
+    const int r = t % R;
+    const int ci = t / R;
+    const float v = (co < Cout && ci < Cin) ? m.w[(((I)co * R + (R - 1 - r)) * S + (S - 1 - s)) * Cin + ci] : 0.f;
+    m.wd[k] = __float2bfloat16_rn(v);
   }
+}
+
+__global__ void pack_weights_kernel(const __grid_constant__ PackMeta m) {
+  const size_t nf = m.nf(), total = m.total();
+  const size_t stride = (size_t)gridDim.x * blockDim.x;
+  for (size_t i = (size_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += stride) pack_element<size_t>(m, i, nf);
 }
 
 // Multi-tensor variant: one launch packs every filter of a network (table row = one filter, chunk = 4096 output
 // elements of one filter), instead of one launch per layer and step.
-struct PackMeta {
-  const float* w;
-  __nv_bfloat16* wf;
-  __nv_bfloat16* wd;   // may be null
-  int Cout, Cin, R, S, CinP, CinD, CoutP, CoutF;
-};
-constexpr int kPackChunk = 4096;
-
 __global__ void __launch_bounds__(256) pack_weights_multi_kernel(const PackMeta* __restrict__ metas,
                                                                  const int2* __restrict__ chunks) {
   const int2 ck = chunks[blockIdx.x];
   const PackMeta m = metas[ck.x];
-  const size_t nf = (size_t)m.CoutF * m.R * m.S * m.CinP;
-  const size_t nd = m.wd ? (size_t)m.CinD * m.R * m.S * m.CoutP : 0;
+  const size_t nf = m.nf(), total = m.total();
   const size_t base = (size_t)ck.y * kPackChunk;
-  const size_t end = min(base + (size_t)kPackChunk, nf + nd);
-  if (nf + nd < 0x7fffffffu) {
+  const size_t end = min(base + (size_t)kPackChunk, total);
+  if (total < 0x7fffffffu) {
     // every filter of a real network: 32-bit index arithmetic (the four runtime div/mod pairs per element dominated this kernel
     // when done on size_t: ALU bound, not memory bound, for RepVGG-A0's 18 M packed elements)
-    const unsigned nf32 = (unsigned)nf, end32 = (unsigned)end;
-    const unsigned R = m.R, S = m.S, CinP = m.CinP, CoutP = m.CoutP, Cin = m.Cin, Cout = m.Cout;
-    for (unsigned i = (unsigned)base + threadIdx.x; i < end32; i += 256) {
-      if (i < nf32) {
-        const unsigned ci = i % CinP;
-        unsigned t = i / CinP;
-        const unsigned s = t % S; t /= S;
-        const unsigned r = t % R;
-        const unsigned co = t / R;
-        const float v = (ci < Cin && co < Cout) ? m.w[((co * R + r) * S + s) * Cin + ci] : 0.f;
-        m.wf[i] = __float2bfloat16_rn(v);
-      } else {
-        const unsigned k = i - nf32;
-        const unsigned co = k % CoutP;
-        unsigned t = k / CoutP;
-        const unsigned s = t % S; t /= S;
-        const unsigned r = t % R;
-        const unsigned ci = t / R;
-        const float v = (co < Cout && ci < Cin) ? m.w[((co * R + (R - 1 - r)) * S + (S - 1 - s)) * Cin + ci] : 0.f;
-        m.wd[k] = __float2bfloat16_rn(v);
-      }
-    }
+    for (unsigned i = (unsigned)base + threadIdx.x; i < (unsigned)end; i += 256) pack_element<unsigned>(m, i, (unsigned)nf);
     return;
   }
-  for (size_t i = base + threadIdx.x; i < end; i += 256) {
-    if (i < nf) {
-      const int ci = i % m.CinP;
-      size_t t = i / m.CinP;
-      const int s = t % m.S; t /= m.S;
-      const int r = t % m.R;
-      const int co = t / m.R;
-      const float v = (ci < m.Cin && co < m.Cout) ? m.w[(((size_t)co * m.R + r) * m.S + s) * m.Cin + ci] : 0.f;
-      m.wf[i] = __float2bfloat16_rn(v);
-    } else {
-      const size_t k = i - nf;
-      const int co = k % m.CoutP;
-      size_t t = k / m.CoutP;
-      const int s = t % m.S; t /= m.S;
-      const int r = t % m.R;
-      const int ci = t / m.R;
-      const float v = (co < m.Cout && ci < m.Cin)
-                          ? m.w[(((size_t)co * m.R + (m.R - 1 - r)) * m.S + (m.S - 1 - s)) * m.Cin + ci] : 0.f;
-      m.wd[k] = __float2bfloat16_rn(v);
-    }
-  }
+  for (size_t i = base + threadIdx.x; i < end; i += 256) pack_element<size_t>(m, i, nf);
 }
 
 // Class filters of the stride-2 3x3 pad-1 data gradient (hb_conv2d_dgrad_s2_bf16). Output parity class (a, b) is a
@@ -275,10 +239,10 @@ extern "C" {
 int hb_pack_conv_weights(const float* w, void* wf, void* wd, int Cout, int Cin, int R, int S, int CinP, int CinD,
                          int CoutP, int CoutF, void* stream) {
   if (CoutF < Cout || CinP < Cin) return (int)cudaErrorInvalidValue;
-  const size_t n = (size_t)CoutF * R * S * CinP + (wd ? (size_t)CinD * R * S * CoutP : 0);
+  const PackMeta m{w, (__nv_bfloat16*)wf, (__nv_bfloat16*)wd, Cout, Cin, R, S, CinP, CinD, CoutP, CoutF};
+  const size_t n = m.total();
   if (n == 0) return 0;
-  pack_weights_kernel<<<stream_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(w, (__nv_bfloat16*)wf, (__nv_bfloat16*)wd,
-                                                                             Cout, Cin, R, S, CinP, CinD, CoutP, CoutF);
+  pack_weights_kernel<<<stream_grid(n, 256), 256, 0, (cudaStream_t)stream>>>(m);
   HB_LAUNCH_CHECK();
   return 0;
 }
@@ -319,51 +283,33 @@ int hb_nchw_to_nhwc_pad_bf16(const void* x, void* y, int N, int C, int H, int W,
   const size_t n = (size_t)N * H * W;
   if (n == 0) return 0;
   const int grid = stream_grid(n, 256);
-  cudaStream_t st = (cudaStream_t)stream;
-  switch (dtype) {
-    case HB_DTYPE_F32:
-      nchw_to_nhwc_pad_kernel<float><<<grid, 256, 0, st>>>((const float*)x, (__nv_bfloat16*)y, N, C, H * W, CP);
-      break;
-    case HB_DTYPE_BF16:
-      nchw_to_nhwc_pad_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)y, N, C,
-                                                                   H * W, CP);
-      break;
-    case HB_DTYPE_F16:
-      nchw_to_nhwc_pad_kernel<__half><<<grid, 256, 0, st>>>((const __half*)x, (__nv_bfloat16*)y, N, C, H * W, CP);
-      break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    nchw_to_nhwc_pad_kernel<T><<<grid, 256, 0, (cudaStream_t)stream>>>((const T*)x, (__nv_bfloat16*)y, N, C, H * W, CP);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 int hb_im2col_smallc_bf16(const void* x, void* col, int N, int C, int H, int W, int R, int S, int stride, int pad, int Kp,
                           int dtype, void* stream) {
   if (Kp % 8 != 0 || Kp < R * S * C) return (int)cudaErrorInvalidValue;
-  const int Ho = (H + 2 * pad - R) / stride + 1, Wo = (W + 2 * pad - S) / stride + 1;
+  int Ho, Wo;
+  if (!window_out(H, R, stride, pad, 1, Ho) || !window_out(W, S, stride, pad, 1, Wo)) return (int)cudaErrorInvalidValue;
   const size_t n = (size_t)N * Ho * Wo;
   if (n == 0) return 0;
   const int grid = stream_grid(n, 256, 16);
   cudaStream_t st = (cudaStream_t)stream;
   __nv_bfloat16* c = (__nv_bfloat16*)col;
-  if (C == 3 && R == 3 && S == 3 && Kp == 32 && n < 0xffffffffull) {
-    switch (dtype) {
-      case HB_DTYPE_F32: im2col_c3k3_kernel<float><<<grid, 256, 0, st>>>((const float*)x, c, N, H, W, Ho, Wo, stride, pad); break;
-      case HB_DTYPE_BF16: im2col_c3k3_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, c, N, H, W, Ho, Wo, stride, pad); break;
-      case HB_DTYPE_F16: im2col_c3k3_kernel<__half><<<grid, 256, 0, st>>>((const __half*)x, c, N, H, W, Ho, Wo, stride, pad); break;
-      default: return (int)cudaErrorInvalidValue;
-    }
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    if (C == 3 && R == 3 && S == 3 && Kp == 32 && n < 0xffffffffull)
+      im2col_c3k3_kernel<T><<<grid, 256, 0, st>>>((const T*)x, c, N, H, W, Ho, Wo, stride, pad);
+    else
+      im2col_smallc_kernel<T><<<grid, 256, 0, st>>>((const T*)x, c, N, C, H, W, Ho, Wo, R, S, stride, pad, Kp);
     HB_LAUNCH_CHECK();
     return 0;
-  }
-  switch (dtype) {
-    case HB_DTYPE_F32: im2col_smallc_kernel<float><<<grid, 256, 0, st>>>((const float*)x, c, N, C, H, W, Ho, Wo, R, S, stride, pad, Kp); break;
-    case HB_DTYPE_BF16: im2col_smallc_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, c, N, C, H, W, Ho, Wo, R, S, stride, pad, Kp); break;
-    case HB_DTYPE_F16: im2col_smallc_kernel<__half><<<grid, 256, 0, st>>>((const __half*)x, c, N, C, H, W, Ho, Wo, R, S, stride, pad, Kp); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  });
 }
 
 int hb_gap_bwd_bf16(const void* dy, void* dx, int N, int HW, int C, void* stream) {

@@ -494,9 +494,9 @@ int hb_conv2d_fused_bf16(const hb_conv_args* c, int* stat_slots, void* stream) {
   if (Cin % 8 != 0 || Cout % 16 != 0) return (int)cudaErrorInvalidValue;
   if (!hb::aligned16(c->x) || !hb::aligned16(c->w) || !hb::aligned16(c->y)) return (int)cudaErrorMisalignedAddress;
   if (c->w2 && (!hb::aligned16(c->w2) || !hb::aligned16(c->y2))) return (int)cudaErrorMisalignedAddress;
-  const int Ho = (H + 2 * pad - dil * (R - 1) - 1) / stride + 1;
-  const int Wo = (W + 2 * pad - dil * (S - 1) - 1) / stride + 1;
-  if (Ho <= 0 || Wo <= 0) return (int)cudaErrorInvalidValue;
+  int Ho, Wo;
+  if (!hb::window_out(H, R, stride, pad, dil, Ho) || !hb::window_out(W, S, stride, pad, dil, Wo))
+    return (int)cudaErrorInvalidValue;
   if ((long long)N * Ho * Wo > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
   if (c->w2 && pad != (R / 2) * dil) return (int)cudaErrorInvalidValue;   // centre tap == the 1x1 pad-0 conv's input
   if ((c->stats || c->stats2) && !stat_slots) return (int)cudaErrorInvalidValue;

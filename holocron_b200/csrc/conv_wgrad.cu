@@ -240,10 +240,11 @@ struct WgradPlan {
 int plan_wgrad(WgradPlan& plan, int N, int H, int W, int Cin, int Cout, int R, int S, int stride, int pad, int dil,
                int num_ctas) {
   WgradParams& p = plan.p;
-  const int Ho = (H + 2 * pad - dil * (R - 1) - 1) / stride + 1;
-  const int Wo = (W + 2 * pad - dil * (S - 1) - 1) / stride + 1;
+  int Ho, Wo;
+  if (!hb::window_out(H, R, stride, pad, dil, Ho) || !hb::window_out(W, S, stride, pad, dil, Wo))
+    return (int)cudaErrorInvalidValue;
   const long long m_ll = (long long)N * Ho * Wo;
-  if (Ho <= 0 || Wo <= 0 || m_ll > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
+  if (m_ll > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
   p.m_total = (int)m_ll; p.Ho = Ho; p.Wo = Wo; p.stride = stride; p.pad = pad; p.dil = dil;
   p.R = R; p.S = S; p.Cin = Cin; p.Cout = Cout;
   const int RS = R * S;

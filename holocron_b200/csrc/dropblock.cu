@@ -111,21 +111,13 @@ int hb_dropblock_apply(const void* x, void* out, const float* mask, const float*
   const float numel = (float)((long long)N * HW);
   const int grid = stream_grid((size_t)total, 256 * 4);
   cudaStream_t st = (cudaStream_t)stream;
-  if (channels_last) {
-    bool done = false;
-    if (dtype == HB_DTYPE_BF16) done = launch_nhwc_vec<__nv_bfloat16>(x, out, mask, kept, total, C, numel, st);
-    else if (dtype == HB_DTYPE_F16) done = launch_nhwc_vec<__half>(x, out, mask, kept, total, C, numel, st);
-    else if (dtype == HB_DTYPE_F32) done = launch_nhwc_vec<float>(x, out, mask, kept, total, C, numel, st);
-    if (done) { HB_LAUNCH_CHECK(); return 0; }
-  }
-  switch (dtype) {
-    case HB_DTYPE_F32: dropblock_apply_kernel<float><<<grid, 256, 0, st>>>((const float*)x, (float*)out, mask, kept, total, C, HW, channels_last, numel); break;
-    case HB_DTYPE_BF16: dropblock_apply_kernel<__nv_bfloat16><<<grid, 256, 0, st>>>((const __nv_bfloat16*)x, (__nv_bfloat16*)out, mask, kept, total, C, HW, channels_last, numel); break;
-    case HB_DTYPE_F16: dropblock_apply_kernel<__half><<<grid, 256, 0, st>>>((const __half*)x, (__half*)out, mask, kept, total, C, HW, channels_last, numel); break;
-    default: return (int)cudaErrorInvalidValue;
-  }
-  HB_LAUNCH_CHECK();
-  return 0;
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    if (!(channels_last && launch_nhwc_vec<T>(x, out, mask, kept, total, C, numel, st)))
+      dropblock_apply_kernel<T><<<grid, 256, 0, st>>>((const T*)x, (T*)out, mask, kept, total, C, HW, channels_last, numel);
+    HB_LAUNCH_CHECK();
+    return 0;
+  });
 }
 
 }  // extern "C"

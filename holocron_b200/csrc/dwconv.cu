@@ -541,14 +541,12 @@ void launch_dw3x3(dim3 grid, cudaStream_t st, const __nv_bfloat16* src, const fl
 }
 
 // 0 when the geometry is supported (fills p), otherwise cudaErrorInvalidValue, before any launch or device query:
-// N, H, W, C, K, stride >= 1, pad >= 0, C % 8 == 0 and a filter that fits the padded input (Ho, Wo >= 1). Integer
-// division truncates towards zero, so H + 2 * pad - K is checked for a negative value itself: (H + 2 * pad - K) / stride + 1
-// alone gives Ho = 1 for a filter up to stride - 1 pixels too large.
+// N, C >= 1, C % 8 == 0 and a K x K filter window_out accepts on both axes.
 int make_params(DwParams& p, int N, int H, int W, int C, int K, int stride, int pad) {
-  if (N < 1 || H < 1 || W < 1 || C < 1 || C % 8 != 0 || K < 1 || stride < 1 || pad < 0) return (int)cudaErrorInvalidValue;
-  const long long h = (long long)H + 2LL * pad - K, w = (long long)W + 2LL * pad - K;
-  if (h < 0 || w < 0 || h / stride >= 0x7fffffffLL || w / stride >= 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-  p = DwParams{N, H, W, C, (int)(h / stride + 1), (int)(w / stride + 1), K, stride, pad};
+  int Ho, Wo;
+  if (N < 1 || C < 1 || C % 8 != 0 || !window_out(H, K, stride, pad, 1, Ho) || !window_out(W, K, stride, pad, 1, Wo))
+    return (int)cudaErrorInvalidValue;
+  p = DwParams{N, H, W, C, Ho, Wo, K, stride, pad};
   return 0;
 }
 

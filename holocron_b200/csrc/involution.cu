@@ -305,13 +305,13 @@ int launch_bwd_kernel(const bf16* x, const bf16* dy, bf16* dker, const InvParams
 
 // 0 when the shape is supported (fills p), otherwise cudaErrorInvalidValue
 int make_params(InvParams& p, int N, int H, int W, int C, int Cp, int Kp, int K, int G, int stride, int pad, int dil) {
-  if (N <= 0 || H <= 0 || W <= 0 || C <= 0 || G <= 0 || C % G != 0 || Cp < C || Cp % 8 != 0 || Kp < G * K * K ||
-      stride < 1 || pad < 0 || dil < 1 || (K != 1 && K != 3 && K != 5 && K != 7))
+  if (N <= 0 || C <= 0 || G <= 0 || C % G != 0 || Cp < C || Cp % 8 != 0 || Kp < G * K * K ||
+      (K != 1 && K != 3 && K != 5 && K != 7))
     return (int)cudaErrorInvalidValue;
-  p = InvParams{N, H, W, C, Cp, 0, 0, Kp, G, stride, pad, dil};
-  p.Ho = (H + 2 * pad - dil * (K - 1) - 1) / stride + 1;
-  p.Wo = (W + 2 * pad - dil * (K - 1) - 1) / stride + 1;
-  if (p.Ho <= 0 || p.Wo <= 0 || N > 65535) return (int)cudaErrorInvalidValue;
+  int Ho, Wo;
+  if (!window_out(H, K, stride, pad, dil, Ho) || !window_out(W, K, stride, pad, dil, Wo) || N > 65535)
+    return (int)cudaErrorInvalidValue;
+  p = InvParams{N, H, W, C, Cp, Ho, Wo, Kp, G, stride, pad, dil};
   // 32-bit element indices in the grid-stride kernels
   if ((long long)N * H * W * Cp >= 0x7fffffffLL || (long long)N * p.Ho * p.Wo * (Cp > Kp ? Cp : Kp) >= 0x7fffffffLL)
     return (int)cudaErrorInvalidValue;

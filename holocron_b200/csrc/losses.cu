@@ -504,19 +504,6 @@ bool vec_eligible(const LossParams& p) {
 }
 
 // ---- host dispatch ---------------------------------------------------------------------------------
-template <typename T> struct Type { using type = T; };
-
-// f(Type<T>{}) for the dtype code; cudaErrorInvalidValue for an unknown code
-template <class F>
-int dispatch_dtype(int dtype, F f) {
-  switch (dtype) {
-    case HB_DTYPE_F32: return f(Type<float>{});
-    case HB_DTYPE_BF16: return f(Type<__nv_bfloat16>{});
-    case HB_DTYPE_F16: return f(Type<__half>{});
-    default: return (int)cudaErrorInvalidValue;
-  }
-}
-
 // f(std::integral_constant<int, KMAX>{}) for the smallest register-column instantiation that holds K (K <= 32)
 template <class F>
 void dispatch_kmax(int K, F f) {

@@ -59,19 +59,14 @@ __global__ void __launch_bounds__(256) patch_stats_kernel(const float2* __restri
 extern "C" int hb_patch_stats_bf16(const void* x, float* mean, float* rstd, float* scratch, int N, int H, int W, int C, int kh,
                                    int kw, int stride, int pad, int dil, int k_logical, float eps, void* stream) {
   if (C % 8 != 0 || !hb::aligned16(x) || !scratch) return (int)cudaErrorInvalidValue;
-  // geometry, before any host division: positive sizes, stride and dilation, non-negative padding, a dilated window that
-  // fits the padded input (tested before the division: (2 - 3) / 2 truncates to 0), int-sized pixel and patch counts,
-  // and a logical patch length (the unpadded Cin*kh*kw) no longer than the padded one
-  if (N <= 0 || H <= 0 || W <= 0 || C <= 0 || kh <= 0 || kw <= 0 || stride <= 0 || dil <= 0 || pad < 0)
+  // geometry, before any host division: positive sizes, a window window_out accepts on both axes, int-sized pixel and
+  // patch counts, and a logical patch length (the unpadded Cin*kh*kw) no longer than the padded one
+  int Ho, Wo;
+  if (N <= 0 || C <= 0 || !hb::window_out(H, kh, stride, pad, dil, Ho) || !hb::window_out(W, kw, stride, pad, dil, Wo))
     return (int)cudaErrorInvalidValue;
-  const long long span_h = (long long)H + 2LL * pad - (long long)dil * (kh - 1) - 1;
-  const long long span_w = (long long)W + 2LL * pad - (long long)dil * (kw - 1) - 1;
-  if (span_h < 0 || span_w < 0) return (int)cudaErrorInvalidValue;
-  const long long ho = span_h / stride + 1, wo = span_w / stride + 1;
-  if (ho > INT_MAX || wo > INT_MAX || ho * wo > INT_MAX || N * ho * wo > INT_MAX) return (int)cudaErrorInvalidValue;
+  if ((long long)Ho * Wo > INT_MAX || (long long)N * Ho * Wo > INT_MAX) return (int)cudaErrorInvalidValue;
   if ((long long)C * kh > INT_MAX || (long long)C * kh * kw > INT_MAX || k_logical <= 0 || k_logical > C * kh * kw)
     return (int)cudaErrorInvalidValue;
-  const int Ho = (int)ho, Wo = (int)wo;
   cudaStream_t st = (cudaStream_t)stream;
   const long long npix = (long long)N * H * W, nout = (long long)N * Ho * Wo;
   pixel_moments_kernel<<<(unsigned)((npix + 255) / 256), 256, 0, st>>>((const __nv_bfloat16*)x, (float2*)scratch, npix, C);

@@ -145,32 +145,36 @@ int launch_binary(const void* a, const void* b, void* y, size_t n, Op op, cudaSt
   return 0;
 }
 
-#define HB_DISPATCH_DTYPE(dtype, CALL)                        \
-  switch (dtype) {                                            \
-    case HB_DTYPE_F32: { using T = float; return CALL; }      \
-    case HB_DTYPE_BF16: { using T = __nv_bfloat16; return CALL; } \
-    case HB_DTYPE_F16: { using T = __half; return CALL; }     \
-    default: return (int)cudaErrorInvalidValue;               \
-  }
-
 }  // namespace
 
 extern "C" {
 
 int hb_hard_mish_fwd(const void* x, void* y, size_t n, int dtype, void* stream) {
-  HB_DISPATCH_DTYPE(dtype, (launch_unary<T>(x, y, n, HardMishFwd{}, (cudaStream_t)stream)));
+  return dispatch_dtype(dtype, [&](auto type) {
+    return launch_unary<typename decltype(type)::type>(x, y, n, HardMishFwd{}, (cudaStream_t)stream);
+  });
 }
 int hb_hard_mish_bwd(const void* x, const void* dy, void* dx, size_t n, int dtype, void* stream) {
-  HB_DISPATCH_DTYPE(dtype, (launch_binary<T>(x, dy, dx, n, HardMishBwd{}, (cudaStream_t)stream)));
+  return dispatch_dtype(dtype, [&](auto type) {
+    return launch_binary<typename decltype(type)::type>(x, dy, dx, n, HardMishBwd{}, (cudaStream_t)stream);
+  });
 }
 int hb_nl_relu_fwd(const void* x, void* y, size_t n, float beta, int dtype, void* stream) {
-  HB_DISPATCH_DTYPE(dtype, (launch_unary<T>(x, y, n, NLReluFwd<(sizeof(T) < 4)>{beta}, (cudaStream_t)stream)));
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    return launch_unary<T>(x, y, n, NLReluFwd<(sizeof(T) < 4)>{beta}, (cudaStream_t)stream);
+  });
 }
 int hb_nl_relu_bwd(const void* x, const void* dy, void* dx, size_t n, float beta, int dtype, void* stream) {
-  HB_DISPATCH_DTYPE(dtype, (launch_binary<T>(x, dy, dx, n, NLReluBwd<(sizeof(T) < 4)>{beta}, (cudaStream_t)stream)));
+  return dispatch_dtype(dtype, [&](auto type) {
+    using T = typename decltype(type)::type;
+    return launch_binary<T>(x, dy, dx, n, NLReluBwd<(sizeof(T) < 4)>{beta}, (cudaStream_t)stream);
+  });
 }
 int hb_nl_relu_bwd_from_out(const void* y, const void* dy, void* dx, size_t n, float beta, int dtype, void* stream) {
-  HB_DISPATCH_DTYPE(dtype, (launch_binary<T>(y, dy, dx, n, NLReluBwdFromOut{beta}, (cudaStream_t)stream)));
+  return dispatch_dtype(dtype, [&](auto type) {
+    return launch_binary<typename decltype(type)::type>(y, dy, dx, n, NLReluBwdFromOut{beta}, (cudaStream_t)stream);
+  });
 }
 
 }  // extern "C"

@@ -294,9 +294,8 @@ int make_blur(BlurParams& p, const float* taps, int N, int H, int W, int C, int 
   p.N = N; p.H = H; p.W = W; p.C = C; p.Cp = Cp; p.K = K; p.stride = stride;
   p.pad = ((stride - 1) + (K - 1)) / 2;
   if (p.pad >= H || p.pad >= W) return (int)cudaErrorInvalidValue;   // ReflectionPad2d's own limit
-  p.Ho = (H + 2 * p.pad - K) / stride + 1;
-  p.Wo = (W + 2 * p.pad - K) / stride + 1;
-  if (p.Ho <= 0 || p.Wo <= 0 || (long long)N * H >= 0x7fffffffLL || (long long)N * p.Ho >= 0x7fffffffLL)
+  if (!window_out(H, K, stride, p.pad, 1, p.Ho) || !window_out(W, K, stride, p.pad, 1, p.Wo) ||
+      (long long)N * H >= 0x7fffffffLL || (long long)N * p.Ho >= 0x7fffffffLL)
     return (int)cudaErrorInvalidValue;
   for (int t = 0; t < K * K; ++t) p.w[t] = taps[t];
   return 0;

@@ -214,29 +214,17 @@ __global__ void adder_dgrad_kernel(const float* __restrict__ x, const float* __r
   }
 }
 
-// The geometry every entry point accepts, checked before any host division or device call: positive sizes, stride and
-// dilation, non-negative padding, a dilated window that fits the padded input (tested before the division, since
-// (2 - 3) / 2 truncates to 0 and would give one output row), and int-sized pixel (N*Ho*Wo) and patch (Cin*KH*KW) counts.
-bool geometry_ok(int N, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil) {
-  if (N <= 0 || Cin <= 0 || H <= 0 || W <= 0 || Cout <= 0 || KH <= 0 || KW <= 0) return false;
-  if (stride <= 0 || dil <= 0 || pad < 0) return false;
-  const long long span_h = (long long)H + 2LL * pad - (long long)dil * (KH - 1) - 1;
-  const long long span_w = (long long)W + 2LL * pad - (long long)dil * (KW - 1) - 1;
-  if (span_h < 0 || span_w < 0) return false;
-  const long long ho = span_h / stride + 1, wo = span_w / stride + 1;
-  if (ho > INT_MAX || wo > INT_MAX || ho * wo > INT_MAX || N * ho * wo > INT_MAX) return false;
-  return (long long)Cin * KH <= INT_MAX && (long long)Cin * KH * KW <= INT_MAX;
-}
-
-XcParams make_params(int N, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil, int normalize,
-                     float eps) {
-  XcParams p{};
-  p.N = N; p.Cin = Cin; p.H = H; p.W = W; p.Cout = Cout; p.KH = KH; p.KW = KW;
-  p.stride = stride; p.pad = pad; p.dil = dil;
-  p.Ho = (H + 2 * pad - dil * (KH - 1) - 1) / stride + 1;
-  p.Wo = (W + 2 * pad - dil * (KW - 1) - 1) / stride + 1;
-  p.K = Cin * KH * KW; p.L = p.Ho * p.Wo; p.normalize = normalize; p.eps = eps;
-  return p;
+// Fills p when the geometry is accepted, checked before any host division or device call: positive sizes, a window
+// window_out accepts on both axes, and int-sized pixel (N*Ho*Wo) and patch (Cin*KH*KW) counts.
+bool make_params(XcParams& p, int N, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil,
+                 int normalize, float eps) {
+  if (N <= 0 || Cin <= 0 || Cout <= 0) return false;
+  int Ho, Wo;
+  if (!hb::window_out(H, KH, stride, pad, dil, Ho) || !hb::window_out(W, KW, stride, pad, dil, Wo)) return false;
+  if ((long long)Ho * Wo > INT_MAX || (long long)N * Ho * Wo > INT_MAX) return false;
+  if ((long long)Cin * KH > INT_MAX || (long long)Cin * KH * KW > INT_MAX) return false;
+  p = XcParams{N, Cin, H, W, Cout, KH, KW, Ho, Wo, stride, pad, dil, Cin * KH * KW, Ho * Wo, normalize, eps};
+  return true;
 }
 
 }  // namespace
@@ -249,9 +237,10 @@ int hb_xcorr2d_fwd(const float* x, const float* w, const float* bias, float* out
                    int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil, int mode, int normalize,
                    float eps, void* stream) {
   // grid: (L tiles, Cout tiles, N)
-  if (!geometry_ok(N, Cin, H, W, Cout, KH, KW, stride, pad, dil) || N > 65535 || (Cout + TC - 1) / TC > 65535)
+  XcParams p;
+  if (!make_params(p, N, Cin, H, W, Cout, KH, KW, stride, pad, dil, normalize, eps) || N > 65535 ||
+      (Cout + TC - 1) / TC > 65535)
     return (int)cudaErrorInvalidValue;
-  XcParams p = make_params(N, Cin, H, W, Cout, KH, KW, stride, pad, dil, normalize, eps);
   cudaStream_t st = (cudaStream_t)stream;
   if (normalize) {
     const long long warps = (long long)N * p.L;
@@ -270,9 +259,9 @@ int hb_xcorr2d_wgrad(const float* x, const float* w, const float* g, const float
                      int N, int Cin, int H, int W, int Cout, int KH, int KW, int stride, int pad, int dil, int mode,
                      int normalize, float eps, void* stream) {
   // grid: (K tiles, Cout tiles, splits over N*L)
-  if (!geometry_ok(N, Cin, H, W, Cout, KH, KW, stride, pad, dil) || (Cout + TC - 1) / TC > 65535)
+  XcParams p;
+  if (!make_params(p, N, Cin, H, W, Cout, KH, KW, stride, pad, dil, normalize, eps) || (Cout + TC - 1) / TC > 65535)
     return (int)cudaErrorInvalidValue;
-  XcParams p = make_params(N, Cin, H, W, Cout, KH, KW, stride, pad, dil, normalize, eps);
   cudaStream_t st = (cudaStream_t)stream;
   cudaError_t e = cudaMemsetAsync(dw, 0, sizeof(float) * (size_t)Cout * p.K, st);
   if (e != cudaSuccess) return (int)e;
@@ -295,8 +284,8 @@ int hb_xcorr2d_wgrad(const float* x, const float* w, const float* g, const float
 // backward reaches x: with normalisation its in-place patch update makes autograd raise).
 int hb_add2d_dgrad(const float* x, const float* w, const float* g, float* dx, int N, int Cin, int H, int W, int Cout,
                    int KH, int KW, int stride, int pad, int dil, void* stream) {
-  if (!geometry_ok(N, Cin, H, W, Cout, KH, KW, stride, pad, dil)) return (int)cudaErrorInvalidValue;
-  XcParams p = make_params(N, Cin, H, W, Cout, KH, KW, stride, pad, dil, 0, 0.f);
+  XcParams p;
+  if (!make_params(p, N, Cin, H, W, Cout, KH, KW, stride, pad, dil, 0, 0.f)) return (int)cudaErrorInvalidValue;
   const long long total = (long long)N * Cin * H * W;
   adder_dgrad_kernel<<<hb::stream_grid((size_t)total, 256), 256, 0, (cudaStream_t)stream>>>(x, w, g, dx, p);
   HB_LAUNCH_CHECK();

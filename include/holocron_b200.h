@@ -11,6 +11,10 @@
  *   - return value: 0 on success, otherwise a cudaError_t (launch-configuration errors included);
  *   - re-entrant, no global mutable state apart from one-time kernel attribute setup;
  *   - dtype codes: 0 = float32, 1 = bfloat16, 2 = float16;
+ *   - window geometry: every entry point that slides a K-tap window (dilation dil, 1 where it takes none) over H input
+ *     pixels computes Ho = (H + 2*pad - dil*(K-1) - 1) / stride + 1, and Wo likewise. It refuses the call with
+ *     cudaErrorInvalidValue (a size query returns 0) before any device call unless H, K, stride, dil >= 1, pad >= 0,
+ *     H + 2*pad >= dil*(K-1) + 1 (the dilated window fits the padded input) and Ho fits an int;
  *   - activation tensors of the convolution / BatchNorm entry points are NHWC bf16 ("channels_last"),
  *     filters are KRSC ([Cout][R][S][Cin]).
  */
