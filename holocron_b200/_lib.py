@@ -140,6 +140,7 @@ SIGNATURES = {
     "hb_erase_batch": "pp" + "i" * 4 + "p",
     "hb_autoaugment_batch": "pppp" + "i" * 5 + "p",
     "hb_color_jitter_batch": "pppp" + "i" * 6 + "p",
+    "hb_box_transform_batch": "ppp" + "iii" + "pppp",
     "hb_detect_scratch_bytes": "piii",
     "hb_detect": "piii" + "p" * 6,
 }

@@ -5,6 +5,9 @@
 // reference's operation order (no FMA contraction) so the exact-value vectors of the reference's own tests
 // (tests/test_ops.py:25-76) hold bit for bit.
 //
+// Also the box steps of the detection recipe's transforms (references/detection/transforms.py:58-127), every box of a
+// batch in one launch (box_transform_kernel below).
+//
 // NB (reference quirk, reproduced): ciou_loss adds its alpha*v term to a masked COPY (boxes.py:209), so it
 // returns exactly the DIoU loss.
 #include "common.cuh"
@@ -207,9 +210,111 @@ __global__ void pairwise_bwd_kernel(const float* __restrict__ b1, const float* _
   }
 }
 
+// ---- detection transforms ----------------------------------------------------------------------------
+// Reference: references/detection/transforms.py:58-127. The box steps of a transform chain are one op sequence shared
+// by every image; each op reads its operands from the image's fp32 parameter row, in order. Every step rounds as the
+// reference's separate torch ops round (one _rn intrinsic each, so no two steps contract into an FMA).
+enum BoxOp {
+  B_SCALE = 0,   // (sx, sy): x *= sx, y *= sy
+  B_CLAMP = 1,   // (x_lo, x_hi, y_lo, y_hi): clamp, NaN kept as torch's clamp keeps it
+  B_SUB = 2,     // (dx, dy): x -= dx, y -= dy
+  B_FILTER = 3,  // (): drop the box when x1 == x2 or y1 == y2
+  B_FLIP = 4,    // (flag, width): when flag != 0, (x1, x2) = (width - x2, width - x1)
+  B_DIV = 5,     // (dx, dy): x /= dx, y /= dy
+};
+
+struct BoxDesc {
+  long long boxes, labels, box_stride, label_stride, n, offset, unused0, unused1;
+};
+
+constexpr int kBoxWarps = 8;
+
+__device__ __forceinline__ float clampf(float v, float lo, float hi) { return v != v ? v : fminf(fmaxf(v, lo), hi); }
+
+// One warp per image walks its boxes 32 at a time; the survivors of each 32 are written after those of the previous
+// ones (ballot + popc), so the image's boxes keep their order at its output offset. No atomics.
+__global__ void __launch_bounds__(kBoxWarps * 32) box_transform_kernel(const BoxDesc* __restrict__ descs,
+                                                                      const float* __restrict__ params,
+                                                                      const int* __restrict__ ops, int n_ops,
+                                                                      int n_params, int N, float* __restrict__ out_boxes,
+                                                                      long long* __restrict__ out_labels,
+                                                                      int* __restrict__ counts) {
+  const int img = blockIdx.x * kBoxWarps + (int)(threadIdx.x >> 5);
+  const unsigned lane = threadIdx.x & 31;
+  if (img >= N) return;
+  const BoxDesc d = descs[img];
+  const float* src = reinterpret_cast<const float*>(d.boxes);
+  const long long* lab = reinterpret_cast<const long long*>(d.labels);
+  const float* p = params + (size_t)img * n_params;
+  long long kept = 0;
+  for (long long base = 0; base < d.n; base += 32) {
+    const long long i = base + lane;
+    bool keep = i < d.n;
+    float x1 = 0.f, y1 = 0.f, x2 = 0.f, y2 = 0.f;
+    long long label = 0;
+    if (keep) {
+      const float* b = src + i * d.box_stride;
+      x1 = b[0], y1 = b[1], x2 = b[2], y2 = b[3];
+      label = lab[i * d.label_stride];
+    }
+    for (int k = 0, q = 0; k < n_ops; ++k) {
+      switch (__ldg(ops + k)) {
+        case B_SCALE:
+          x1 = mul(x1, p[q]), x2 = mul(x2, p[q]), y1 = mul(y1, p[q + 1]), y2 = mul(y2, p[q + 1]);
+          q += 2;
+          break;
+        case B_CLAMP:
+          x1 = clampf(x1, p[q], p[q + 1]), x2 = clampf(x2, p[q], p[q + 1]);
+          y1 = clampf(y1, p[q + 2], p[q + 3]), y2 = clampf(y2, p[q + 2], p[q + 3]);
+          q += 4;
+          break;
+        case B_SUB:
+          x1 = sub(x1, p[q]), x2 = sub(x2, p[q]), y1 = sub(y1, p[q + 1]), y2 = sub(y2, p[q + 1]);
+          q += 2;
+          break;
+        case B_FILTER:
+          keep = keep && x1 != x2 && y1 != y2;
+          break;
+        case B_FLIP:
+          if (p[q] != 0.f) {
+            const float a = sub(p[q + 1], x2);
+            x2 = sub(p[q + 1], x1);
+            x1 = a;
+          }
+          q += 2;
+          break;
+        case B_DIV:
+          x1 = dvd(x1, p[q]), x2 = dvd(x2, p[q]), y1 = dvd(y1, p[q + 1]), y2 = dvd(y2, p[q + 1]);
+          q += 2;
+          break;
+      }
+    }
+    const unsigned ballot = __ballot_sync(0xffffffffu, keep);
+    if (keep) {
+      const long long o = d.offset + kept + __popc(ballot & ((1u << lane) - 1u));
+      float* ob = out_boxes + 4 * o;
+      ob[0] = x1, ob[1] = y1, ob[2] = x2, ob[3] = y2;
+      out_labels[o] = label;
+    }
+    kept += __popc(ballot);
+  }
+  if (lane == 0) counts[img] = (int)kept;
+}
+
 }  // namespace
 
 extern "C" {
+
+int hb_box_transform_batch(const void* descs, const float* params, const int* ops, int n_ops, int n_params, int N,
+                           float* out_boxes, long long* out_labels, int* counts, void* stream) {
+  if (N < 0 || n_ops < 0 || n_params < 0) return (int)cudaErrorInvalidValue;
+  if (N == 0) return 0;
+  const int blocks = (N + kBoxWarps - 1) / kBoxWarps;
+  box_transform_kernel<<<blocks, kBoxWarps * 32, 0, (cudaStream_t)stream>>>(
+      static_cast<const BoxDesc*>(descs), params, ops, n_ops, n_params, N, out_boxes, out_labels, counts);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
 
 // mode: 0 IoU, 1 GIoU, 2 DIoU penalty (rho^2/c^2), 3 DIoU loss (= the reference's ciou_loss too), 4 aspect-ratio
 // consistency. boxes: fp32 [M,4] / [N,4] xyxy contiguous; out: fp32 [M,N].

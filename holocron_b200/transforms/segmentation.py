@@ -40,17 +40,17 @@ draws, before any launch.
 >>> masks = [torch.randint(0, 21, (375, 500), dtype=torch.uint8, device="cuda") for _ in range(4)]
 >>> x, target = tf(images, masks)  # (4, 3, 256, 256) float32, (4, 256, 256) int64
 """
-from dataclasses import dataclass
 from typing import Any, List, Optional, Sequence, Tuple, Union
 
 import torch
 from PIL import Image
 from torch import Tensor
 from torchvision.transforms import transforms as T
-from torchvision.transforms.functional import InterpolationMode, _compute_resized_output_size
+from torchvision.transforms.functional import InterpolationMode
 
 from .._lib import HolocronB200Error, require_cuda
 from ._color import jitter
+from ._fold import _Fold, check_stackable, draw, group, resized
 from ._resample import resample
 from ._table import check_images
 from . import _color
@@ -146,33 +146,6 @@ _RESIZES = (Resize, RandomResize)
 _GEOMETRIC = (Resize, RandomResize, RandomCrop, RandomHorizontalFlip)
 
 
-@dataclass
-class _Fold:
-    """One image's run folded: its source resized to ``inner``, placed at (top, left) on a canvas of ``canvas``, the
-    canvas mirrored when ``mirror``."""
-
-    inner: Tuple[int, int]
-    canvas: Tuple[int, int]
-    top: int = 0
-    left: int = 0
-    mirror: bool = False
-
-    def flip(self) -> None:
-        self.mirror = not self.mirror
-
-    def pad(self, bottom: int, right: int) -> None:
-        """torchvision's pad of the bottom and right of the canvas: in a mirrored canvas the new columns are on the
-        right of what is read, so the box moves right."""
-        if self.mirror:
-            self.left += right
-        self.canvas = (self.canvas[0] + bottom, self.canvas[1] + right)
-
-    def crop(self, i: int, j: int, h: int, w: int) -> None:
-        self.top -= i
-        self.left -= (self.canvas[1] - w - j) if self.mirror else j
-        self.canvas = (h, w)
-
-
 def fold_run(steps: Sequence[Any], size: Tuple[int, int]) -> _Fold:
     """One image's run (``steps``, the first possibly a resize) from an image of ``size`` = (H, W), folded; its draws
     are the reference's, in its order, on the default CPU generator."""
@@ -180,10 +153,10 @@ def fold_run(steps: Sequence[Any], size: Tuple[int, int]) -> _Fold:
     for t in steps:
         if isinstance(t, Resize):
             out = t.output_size
-            f = _Fold(*(2 * [_resized(size, [out] if isinstance(out, int) else list(out))]))
+            f = _Fold(*(2 * [resized(size, [out] if isinstance(out, int) else list(out))]))
         elif isinstance(t, RandomResize):
             s = t.min_size if t.min_size == t.max_size else torch.randint(t.min_size, t.max_size, (1,)).item()
-            f = _Fold(*(2 * [_resized(size, [s])]))
+            f = _Fold(*(2 * [resized(size, [s])]))
         elif isinstance(t, RandomCrop):
             h, w = f.canvas
             if min(h, w) < t.size:
@@ -194,34 +167,23 @@ def fold_run(steps: Sequence[Any], size: Tuple[int, int]) -> _Fold:
     return f
 
 
-def _resized(size: Tuple[int, int], out: List[int]) -> Tuple[int, int]:
-    h, w = _compute_resized_output_size(size, out)
-    return int(h), int(w)
-
-
 def _fixes_size(run: Sequence[Any]) -> bool:
     """Whether a run gives every image one output size whatever its input: it crops, or resizes to a pair."""
     return any(isinstance(t, RandomCrop) or
                (isinstance(t, Resize) and not isinstance(t.output_size, int) and len(t.output_size) == 2) for t in run)
 
 
+def _kind(t: Any) -> Optional[str]:
+    return "run" if isinstance(t, _GEOMETRIC) else "step" if isinstance(t, (ImageTransform, ToTensor)) else None
+
+
+def _starts_run(t: Any, run: List[Any]) -> bool:
+    return isinstance(t, _RESIZES) or (isinstance(t, RandomCrop) and any(isinstance(s, RandomCrop) for s in run))
+
+
 def _segments(transforms: Sequence[Any]) -> List[Union[List[Any], Any]]:
     """The steps grouped: runs (lists of geometric steps) and the image-only steps between them."""
-    segments: List[Union[List[Any], Any]] = []
-    run: Optional[List[Any]] = None
-    for t in transforms:
-        if isinstance(t, _GEOMETRIC):
-            if (run is None or isinstance(t, _RESIZES)
-                    or (isinstance(t, RandomCrop) and any(isinstance(s, RandomCrop) for s in run))):
-                run = []
-                segments.append(run)
-            run.append(t)
-        elif isinstance(t, (ImageTransform, ToTensor)):
-            run = None
-            segments.append(t)
-        else:
-            raise TypeError(f"{type(t).__name__} is not a transform of holocron_b200.transforms.segmentation")
-    return segments
+    return group(transforms, _kind, _starts_run, "segmentation")
 
 
 def _inputs(image, target) -> Tuple[List[Tensor], List[Tensor], int]:
@@ -284,7 +246,7 @@ class Compose(T.Compose):
             check_images(images, _color.SUPPORTED)
         # the draws, image by image as the reference's Compose applied sample by sample makes them
         plans = [_draw(segments, jitters, (int(x.shape[-2]), int(x.shape[-1]))) for x in images]
-        _check_stackable(segments, plans, [tuple(x.shape[-2:]) for x in images])
+        check_stackable(segments, plans, [tuple(x.shape[-2:]) for x in images])
 
         stacked_images: Optional[Tensor] = None
         stacked_masks: Optional[Tensor] = None
@@ -318,18 +280,7 @@ class Compose(T.Compose):
 def _draw(segments: Sequence[Any], jitters: Sequence[Any], size: Tuple[int, int]) -> List[Any]:
     """One image's draws for every step: the fold of each run, the ``get_params`` of each ColorJitter, None for the
     other steps."""
-    plan: List[Any] = []
-    for s in segments:
-        if isinstance(s, list):
-            fold = fold_run(s, size)
-            size = fold.canvas
-            plan.append(fold)
-        elif s in jitters:
-            j = s.transform
-            plan.append(j.get_params(j.brightness, j.contrast, j.saturation, j.hue))
-        else:
-            plan.append(None)
-    return plan
+    return draw(segments, jitters, size, fold_run)
 
 
 def _check_order(segments: Sequence[Any], dtype: torch.dtype) -> None:
@@ -345,13 +296,3 @@ def _check_order(segments: Sequence[Any], dtype: torch.dtype) -> None:
             converted = True
         if isinstance(s, ImageTransform) and not isinstance(s.transform, T.ColorJitter):
             dtype = None
-
-
-def _check_stackable(segments: Sequence[Any], plans: Sequence[Sequence[Any]], sizes: List[Tuple[int, int]]) -> None:
-    """Refuses an ``ImageTransform`` or ``ToTensor`` reached by images of different sizes."""
-    for k, s in enumerate(segments):
-        if isinstance(s, list):
-            sizes = [p[k].canvas for p in plans]
-        elif len(set(sizes)) > 1:
-            raise ValueError(f"{s!r} takes images of one size, but the images reaching it have {len(set(sizes))} "
-                             "sizes: crop or resize them to one size first")

@@ -541,6 +541,21 @@ int hb_autoaugment_batch(const void* descs, const float* params, const long long
 int hb_color_jitter_batch(const void* descs, const float* params, const long long* stat_images, void* scratch, int N,
                           int n_stat, int H, int W, int slices, int dtype, void* stream);
 
+/* ---- detection transforms: the box steps of references/detection/transforms.py:58-127 (CenterCrop :58-69, Resize
+ *      :72-82, RandomResizedCrop :85-105, convert_to_relative :108-116, RandomHorizontalFlip :119-127), as the
+ *      reference's detection recipe chains them (references/detection/train.py:116-125) - every box of a batch in one
+ *      launch ------------------------------------------------------------------------------------------------------ */
+/* descs: device table of N rows of 8 int64 {boxes, labels, box_row_stride, label_stride, n, out_offset, 0, 0}: image
+ * k's n boxes are read in place from the fp32 [n][4] boxes (unit column stride, rows box_row_stride elements apart)
+ * and its int64 labels (label_stride elements apart). ops: int32 [n_ops], one op sequence for every image, each op
+ * reading its operands from the image's row of params (fp32 [N][n_params]) in order: 0 scale (sx, sy), 1 clamp (x_lo,
+ * x_hi, y_lo, y_hi), 2 subtract (dx, dy), 3 drop boxes with x1 == x2 or y1 == y2 (), 4 flip (flag, width): when flag
+ * != 0, (x1, x2) = (width - x2, width - x1), 5 divide (dx, dy). Each op rounds to fp32 as a separate torch op does.
+ * The survivors of image k are written in order to out_boxes fp32 [*][4] and out_labels int64 [*] (contiguous) from
+ * row out_offset on, and counts[k] (int32) = their number. Nothing else is written. No atomics. */
+int hb_box_transform_batch(const void* descs, const float* params, const int* ops, int n_ops, int n_params, int N,
+                           float* out_boxes, long long* out_labels, int* counts, void* stream);
+
 /* ---- YOLO inference post-processing (holocron/models/detection/yolo.py:159-233, yolov4.py:303-335) ------------------
  * One segment = one set of decoded candidates per image: boxes fp32 [B, M, 4] xyxy (16-byte aligned), objectness fp32
  * [B, M] and class scores fp32 [B, M, K], all contiguous, with its own thresholds (YOLOv1/v2: one segment; YOLOv4: one
