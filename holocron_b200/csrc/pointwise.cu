@@ -22,12 +22,13 @@ struct HardMishFwd {
   }
 };
 struct HardMishBwd {
-  // d/dx [0.5 x clamp(x+2,0,2)] = 0.5*clamp(x+2,0,2) + 0.5*x*[0 <= x+2 <= 2]
+  // d/dx [0.5 x clamp(x+2,0,2)] = 0.5*clamp(x+2,0,2) + 0.5*x*[0 <= x+2 <= 2]. As in autograd, the clamp's mask selects
+  // (x = +-inf gives dy or 0, not inf * 0) and a NaN input propagates.
   __device__ __forceinline__ float operator()(float x, float dy) const {
-    float t = x + 2.0f;
-    float c = fminf(fmaxf(t, 0.0f), 2.0f);
-    float mask = (t >= 0.0f && t <= 2.0f) ? 1.0f : 0.0f;
-    return dy * (0.5f * c + 0.5f * x * mask);
+    const float t = x + 2.0f;
+    const float c = hb::clamp_nan(t, 0.0f, 2.0f);
+    const float inner = (t >= 0.0f && t <= 2.0f) ? 0.5f * x : 0.0f;
+    return dy * (0.5f * c + inner);
   }
 };
 // kFast (16-bit storage types): MUFU log / reciprocal. The argument is >= 1, where __logf is within 2^-21.4 absolute
@@ -45,7 +46,7 @@ template <bool kFast>
 struct NLReluBwd {
   float beta;
   __device__ __forceinline__ float operator()(float x, float dy) const {
-    if (!(x > 0.0f)) return 0.0f;
+    if (x <= 0.0f) return 0.0f;  // relu'(0) = 0; a NaN input propagates, as through autograd's threshold_backward
     return kFast ? dy * __fdividef(beta, 1.0f + beta * x) : dy * (beta / (1.0f + beta * x));
   }
 };
@@ -53,7 +54,7 @@ struct NLReluBwdFromOut {
   // y = log(1 + beta*relu(x))  =>  for y > 0: dy/dx = beta * exp(-y); else 0
   float beta;
   __device__ __forceinline__ float operator()(float y, float dy) const {
-    return y > 0.0f ? dy * (beta * expf(-y)) : 0.0f;
+    return y <= 0.0f ? 0.0f : dy * (beta * expf(-y));  // NaN propagates as in the out-of-place gradient
   }
 };
 

@@ -22,7 +22,7 @@ class _DropBlockFn(torch.autograd.Function):
         n, c, h, w = x.shape
         L = lib()
         mask = torch.empty((n, h, w), device=x.device, dtype=torch.float32)
-        kept = torch.empty(1, device=x.device, dtype=torch.float32)
+        kept = torch.empty(1, device=x.device, dtype=torch.int64)  # the kernels' 64-bit count of kept cells
         check(L.hb_dropblock_mask(ptr(noise), ptr(mask), ptr(kept), n, h, w, block_size, ctypes.c_float(gamma),
                                   stream_ptr()), "hb_dropblock_mask")
         out = x if inplace else torch.empty_like(x)
@@ -51,6 +51,12 @@ def dropblock2d(x: Tensor, drop_prob: float, block_size: int, inplace: bool = Fa
     ``drop_prob / block_size**2`` on an (N, H, W) grid shared by all channels, dilated to ``block_size`` squares, and
     the survivors are rescaled by ``mask.numel() / mask.sum()``. ``drop_prob == 0`` or ``training=False`` returns the
     input object itself. No host synchronisation (the reference syncs on ``mask.sum() > 0``).
+
+    The kept cells are counted exactly, in an integer, and the scale is rounded as the reference rounds
+    ``mask.numel() / one_count`` (``one_count.reciprocal() * numel``), so fp32 inputs give the reference's output bit
+    for bit for the same noise. For bf16 / fp16 inputs the reference builds its mask in ``x.dtype``, so its count and
+    scale are rounded to that type (a count of 6000 becomes 6016 in bf16); here the count stays exact and the scale
+    fp32, and the output is ``x * numel / kept`` rounded once to ``x.dtype``.
 
     ``noise`` (not in the reference API) lets tests inject the uniform noise the reference would have drawn.
     """

@@ -101,7 +101,15 @@ class _NLReluFn(torch.autograd.Function):
 
 
 def nl_relu(x: Tensor, beta: float = 1.0, inplace: bool = False) -> Tensor:
-    """Natural-logarithm ReLU ``log(1 + beta * max(0, x))`` — mirrors holocron/nn/functional.py:44-56."""
+    """Natural-logarithm ReLU ``log(1 + beta * max(0, x))`` — mirrors holocron/nn/functional.py:44-56.
+
+    With ``inplace=True`` ``x`` is overwritten, so the backward pass computes the gradient from the output as
+    ``beta * exp(-y)``. Two differences from the out-of-place gradient ``beta / (1 + beta * x)`` follow:
+
+    - where ``0 < beta * x < 2**-24``, ``y`` rounds to 0 and the gradient is 0 instead of ``beta * dy``;
+    - for bf16 / fp16 tensors ``y`` is stored rounded, so the gradient carries that rounding: a relative error of up to
+      ``y * 2**-8`` (bf16) or ``y * 2**-11`` (fp16).
+    """
     return _NLReluFn.apply(x, float(beta), inplace)
 
 

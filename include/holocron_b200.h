@@ -362,12 +362,14 @@ int hb_add2d_dgrad(const float* x, const float* w, const float* g, float* dx, in
                    int KH, int KW, int stride, int pad, int dil, void* stream);
 
 /* ---- DropBlock: holocron/nn/functional.py:465-500, nn/modules/dropblock.py:14-41 ------------------------ */
-/* mask[N,H,W] = 1 - maxpool_bs(noise <= gamma); *kept (device float) = sum(mask). block_size must be odd. */
-int hb_dropblock_mask(const float* noise, float* mask, float* kept, int N, int H, int W, int block_size, float gamma,
-                      void* stream);
-/* out = x * mask * (N*H*W / *kept) (no rescale when *kept == 0); x: [N,C,H,W] logical, physical NHWC if channels_last */
-int hb_dropblock_apply(const void* x, void* out, const float* mask, const float* kept, int N, int C, int H, int W,
-                       int channels_last, int dtype, void* stream);
+/* mask[N,H,W] = 1 - maxpool_bs(noise <= gamma); *kept (device 64-bit integer) = sum(mask), exact. block_size must be
+   odd. */
+int hb_dropblock_mask(const float* noise, float* mask, unsigned long long* kept, int N, int H, int W, int block_size,
+                      float gamma, void* stream);
+/* out = x * mask * scale, scale = fl(fl(1 / (float)*kept) * (float)(N*H*W)) as the reference rounds numel / kept (1 when
+   *kept == 0); x: [N,C,H,W] logical, physical NHWC if channels_last */
+int hb_dropblock_apply(const void* x, void* out, const float* mask, const unsigned long long* kept, int N, int C, int H,
+                       int W, int channels_last, int dtype, void* stream);
 
 /* ---- losses: holocron/nn/functional.py:59-113 (focal_loss), :540-613 (poly_loss), :503-537 (dice_loss) --- */
 /* logits x are [N, K, S] (S = prod of spatial dims); kind 0 focal / 1 poly-1; loss_pos: float[N*S];
