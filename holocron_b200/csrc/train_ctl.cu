@@ -51,7 +51,8 @@ __global__ void __launch_bounds__(256) sumsq_partials_kernel(const float* __rest
 }
 
 // ... then every block folds the partials in the same fixed order, forms torch's clip coefficient
-// min(1, max_norm / (norm + 1e-6)) (torch.nn.utils.clip_grad_norm_) and scales its slice in place
+// min(1, max_norm / (norm + 1e-6)) (torch.nn.utils.clip_grad_norm_) and scales its slice in place. As torch.clamp does,
+// the minimum keeps a NaN coefficient: a NaN norm makes every gradient NaN (an inf norm makes them 0, or NaN where inf).
 __global__ void __launch_bounds__(256) clip_scale_kernel(float* __restrict__ g, long long n, const double* __restrict__ parts,
                                                          int nparts, float max_norm, Ctl* c) {
   __shared__ float coef_s;
@@ -60,7 +61,7 @@ __global__ void __launch_bounds__(256) clip_scale_kernel(float* __restrict__ g, 
     for (int i = 0; i < nparts; ++i) tot += parts[i];
     const float norm = (float)sqrt(tot);
     float coef = max_norm / (norm + 1e-6f);
-    coef_s = coef < 1.f ? coef : 1.f;
+    coef_s = coef > 1.f ? 1.f : coef;
     if (blockIdx.x == 0 && c) c->grad_norm = norm;
   }
   __syncthreads();

@@ -15,7 +15,8 @@ CUDA-graph replay and one process per GPU can be driven without the host in the 
 
 * gradients accumulate in the flat :class:`~holocron_b200.distributed.GradBucket` (the backward kernels add into it);
 * one NCCL all-reduce (mean) of the bucket per optimizer update when a process group is active;
-* ``clip_grad_norm_`` = two launches on the flat bucket (``hb_grad_clip_norm``: fixed-order norm, in-place scaling);
+* ``clip_grad_norm_`` = two launches on the flat bucket (``hb_grad_clip_norm``: fixed-order norm, in-place scaling; a
+  NaN norm makes every gradient NaN, as ``clip_grad_norm_`` does);
 * the schedule is a device table ``[total_iterations][lr, beta1]`` produced by running the reference's own torch scheduler
   classes on the host once; a device control block (``train_ctl.cu``) selects the row of the current iteration and the
   optimizer kernels read lr / beta1 from it;

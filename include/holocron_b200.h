@@ -472,8 +472,8 @@ int hb_train_ctl_step(void* ctl, const float* table, int n, int phase, void* str
 /* once per iteration (the reference's scheduler.step()): iter += 1 */
 int hb_train_ctl_tick(void* ctl, void* stream);
 /* torch.nn.utils.clip_grad_norm_(params, max_norm) on a flat fp32 gradient buffer (core.py:194,205): fixed-order global L2
- * norm + in-place scaling by min(1, max_norm / (norm + 1e-6)), two launches; scratch: double
- * [hb_grad_clip_partials_max()]; ctl (may be NULL) receives the norm. */
+ * norm + in-place scaling by min(1, max_norm / (norm + 1e-6)), two launches; a NaN norm makes every gradient NaN, as in
+ * torch. scratch: double [hb_grad_clip_partials_max()]; ctl (may be NULL) receives the norm. */
 int hb_grad_clip_partials_max(void);
 int hb_grad_clip_norm(float* grads, long long n, float max_norm, double* scratch, void* ctl, void* stream);
 
