@@ -5,7 +5,7 @@
 // and never build either.
 //
 // Every thread owns one pixel x 8 consecutive channels (one 128-bit vector). Channels c >= C (the zero padding up to Cp)
-// are written as zeros. "Uniform" vectors (C/G % 8 == 0, the RedNet case) have all 8 channels in one group, so a pixel's
+// are written as zeros; those of x and dy, and the columns G*K^2 .. Kp-1 of ker, are never read. "Uniform" vectors (C/G % 8 == 0, the RedNet case) have all 8 channels in one group, so a pixel's
 // K^2 weights of that group are loaded once into registers; "mixed" vectors (e.g. C = 12, G = 6) look the group up per
 // channel. Nothing here synchronises with the host; reductions run in a fixed order (no atomics).
 #include <type_traits>

@@ -10,7 +10,8 @@
 // Every reduction runs in a fixed order (no atomics) and nothing synchronises with the host.
 //
 // Layouts: q [B,HW,Cqp] (channel h*dk+k), k [B,HW,Ckp] (k*u+u), v [B,HW,Cvp] (v*u+u), y / dy [B,HW,Cop] (h*dv+v), all bf16
-// with zero padding channels; stats [B,dk*u,2] fp32 (row max, sum of exponentials); lc / dlc [B,dk,dv] fp32;
+// with padding channels up to the pitch. Outputs get zeros there. The padding of q, k and dy is never read; that of v
+// is (the halo kernels stage whole vectors and weight its lanes by zero) and must hold zeros; stats [B,dk*u,2] fp32 (row max, sum of exponentials); lc / dlc [B,dk,dv] fp32;
 // Rt [r*r,u,dk] fp32 (R transposed tap-major); lp [B,HW,dk,dv] fp32 (global); dlp [B,HW,dk,dvp] bf16, dvp = dv rounded
 // up to 8 (the transient per-position gradient of lp, sum_h q * dy); dvpos [B,HW,dv*u] fp32 (global share of dv).
 #include <math.h>
@@ -61,6 +62,9 @@ __global__ void __launch_bounds__(kThreads) lam_content_kernel(const bf16* __res
     float mx = -INFINITY, s = 0.f;
     for (int m = t; m < p.HW; m += kThreads) {
       const float x = bf(kb[(size_t)m * p.Ckp + ch]);
+      // a -inf key has weight 0, as in torch.softmax; while mx is still -inf it would add exp(-inf - -inf) = NaN. A
+      // row of -inf keys keeps (-inf, 0), so its sigma is NaN, as torch gives it.
+      if (x == -INFINITY) continue;
       if (x > mx) { s = s * expf(mx - x) + 1.f; mx = x; }
       else s += expf(x - mx);
     }
