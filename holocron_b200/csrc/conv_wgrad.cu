@@ -8,8 +8,11 @@
 // are loaded by TMA exactly as they sit in HBM - no transposes:
 //   A stage = 64 pixels x 128 co   (two 64-wide TMA boxes, 128B-swizzled rows = pixels; one per consumer warpgroup)
 //   B stage = 64 pixels x Cin-tile (im2col TMA: padding / stride / row wrap handled in hardware)
-// One CTA owns (co tile, ci tile, tap, pixel range) units; the accumulators (64 co x <= 128 ci per warpgroup) live in
-// registers. Results are reduced across pixel ranges with fp32 red.global.add, written as per-range partials for a
+// The planner splits the work into (co tile, ci tile, tap, pixel range) units. A CTA runs up to T = 3 units that differ
+// only in tap at once: per stage it loads the dY boxes once and one im2col box per tap, and issues one wgmma per tap on
+// the same A descriptor, so each dY byte moved into shared memory feeds T taps. Each tap's accumulators (64 co x <= 128
+// ci per warpgroup) live in registers and see the same k-steps in the same order as a one-tap unit, so dW does not
+// depend on T. Results are reduced across pixel ranges with fp32 red.global.add, written as per-range partials for a
 // fixed-order reduction, or stored directly when there is a single range.
 // This replaces cuDNN's wgrad behind autograd for nn.Conv2d in the reference
 // (holocron/models/utils.py:71, models/classification/repvgg.py:55-62).
@@ -24,12 +27,15 @@ using namespace conv;
 constexpr int kBKpix = 64;     // pixels (reduction) per stage
 constexpr int kChunkBytes = kBKpix * 128;  // one 64px x 64ch box = 8 KiB
 constexpr int kABytes = 2 * kChunkBytes;   // 128 co
+constexpr int kMaxTaps = 3;                // 3 x 64 accumulators per thread at CIW = 128 (232 registers after setmaxnreg)
+constexpr int kProducerRegs = 40;          // per thread after setmaxnreg: 128 x (40 + 2 x 232) = 64 512 <= 64 K registers
+constexpr int kConsumerRegs = 232;
 
 struct WgradParams {
   int m_total, Ho, Wo, stride, pad, dil, R, S, Cin, Cout;
   int ci_tile;         // Cin tile (<= 128)
   int ci_chunks;       // ceil(ci_tile / 64)
-  int taps_per_group;  // taps per unit (1: the accumulators of one tap fill the register budget)
+  int taps_per_group;  // taps a CTA runs together (1 as planned; the launcher regroups them, see group_taps)
   int num_tap_groups, num_co_tiles, num_ci_tiles, k_splits;
   int kblocks_total;   // ceil(m_total / 64)
   int stages, stage_bytes;
@@ -39,11 +45,13 @@ struct WgradParams {
   long long dw_elems;
 };
 
-// CIW: the Cin tile rounded up to 16 (16 ... 128) = the MMA widths of its 64-channel chunks: min(CIW, 64), then CIW - 64
-template <int CIW>
+// CIW: the Cin tile rounded up to 16 (16 ... 128) = the MMA widths of its 64-channel chunks: min(CIW, 64), then CIW - 64.
+// T: taps per work item (p.taps_per_group); the last tap group of a filter may hold fewer (RS % T).
+template <int CIW, int T>
 __global__ void __launch_bounds__(kThreads, 1)
 conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constant__ CUtensorMap tmX, const WgradParams p) {
   constexpr int kChunks = (CIW + 63) / 64, kNLast = CIW - 64 * (kChunks - 1);
+  constexpr int kBTapBytes = kChunks * kChunkBytes;   // one tap's im2col boxes in a stage
   extern __shared__ __align__(1024) uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + (size_t)p.stages * p.stage_bytes);
@@ -60,9 +68,9 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
 
   const int RS = p.R * p.S;
   const int num_units = p.num_co_tiles * p.num_ci_tiles * p.num_tap_groups * p.k_splits;
-  const int b_tap_bytes = p.ci_chunks * kChunkBytes;
 
-  // unit decode: k_split fastest so neighbouring CTAs share the same filter slab / write target
+  // work-item decode (an item is the units of one tap group): k_split fastest so neighbouring CTAs share the same filter
+  // slab / write target
   auto decode = [&](int unit, int& co_t, int& ci_t, int& tg, int& ks) {
     ks = unit % p.k_splits; unit /= p.k_splits;
     tg = unit % p.num_tap_groups; unit /= p.num_tap_groups;
@@ -75,15 +83,16 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
   };
 
   if (warp < 4) {
+    regs_release<kProducerRegs>();
     if (warp == 0 && lane == 0) {
       Ring ring;
       for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
         int co_t, ci_t, tg, ks, kb0, kb1;
         decode(unit, co_t, ci_t, tg, ks);
         kb_range(ks, kb0, kb1);
-        const int tap0 = tg * p.taps_per_group;
-        const int ntaps = min(p.taps_per_group, RS - tap0);
-        const uint32_t tx = kABytes + ntaps * b_tap_bytes;
+        const int tap0 = tg * T;
+        const int ntaps = min(T, RS - tap0);
+        const uint32_t tx = kABytes + ntaps * kBTapBytes;
         for (int kb = kb0; kb < kb1; ++kb) {
           const int m0 = kb * kBKpix;
           const int q0 = m0 % p.Wo, p0 = (m0 / p.Wo) % p.Ho, n0 = m0 / (p.Wo * p.Ho);
@@ -96,8 +105,8 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
           tma_load_2d(&tmDY, bar, sa + kChunkBytes, co_t * 128 + 64, m0);
           for (int t = 0; t < ntaps; ++t) {
             const int tap = tap0 + t, r = tap / p.S, s = tap % p.S;
-            uint8_t* sb = sa + kABytes + t * b_tap_bytes;
-            for (int c = 0; c < p.ci_chunks; ++c)
+            uint8_t* sb = sa + kABytes + t * kBTapBytes;
+            for (int c = 0; c < kChunks; ++c)
               tma_load_im2col_4d(&tmX, bar, sb + c * kChunkBytes, ci_t * p.ci_tile + c * 64, base_w, base_h, n0,
                                  (uint16_t)(s * p.dil), (uint16_t)(r * p.dil));
           }
@@ -109,17 +118,18 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
   }
 
   // ================= consumers: warpgroup wg owns output channels [64*wg, 64*wg + 64) of the co tile =================
+  regs_acquire<kConsumerRegs>();
   const int et = threadIdx.x - 128;
   const int wg = et >> 7;
   const int frow = frag_row(et & 127), fcol = frag_col(et & 127);
   const uint32_t dhi = desc_hi(1024);
-  float acc[CIW / 2];   // [chunk 0: 32 | chunk 1: kNLast / 2]
+  float acc[T][CIW / 2];   // per tap: [chunk 0: 32 | chunk 1: kNLast / 2]
   Ring ring;
-  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
-    int co_t, ci_t, tg, ks, kb0, kb1;
-    decode(unit, co_t, ci_t, tg, ks);
-    kb_range(ks, kb0, kb1);
-    const int tap = tg * p.taps_per_group;
+  // The pixel range [kb0, kb1) of NT taps: one commit group per stage, every tap's MMAs on the same A descriptor. NT is
+  // a template argument so that each fence -> commit region is straight-line (a tap group shorter than T is its own
+  // instantiation, picked by a branch outside the region).
+  auto mainloop = [&](auto nt, int kb0, int kb1) {
+    constexpr int NT = decltype(nt)::value;
     int prev = -1;
     for (int kb = kb0; kb < kb1; ++kb) {
       mbar_wait(&full_bar[ring.stage], ring.phase);
@@ -133,11 +143,15 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
       for (int k = 0; k < kBKpix / 16; ++k) {
         const uint64_t ad = make_desc(a_lo + k * (2048 >> 4), dhi);
         const uint32_t sc = acc0 | (uint32_t)k;
-        if constexpr (kChunks == 1) {
-          wgmma<kNLast, 1, 1>(acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
-        } else {
-          wgmma<64, 1, 1>(acc, ad, make_desc(b_lo + k * (2048 >> 4), dhi), sc);
-          wgmma<kNLast, 1, 1>(acc + 32, ad, make_desc(b_lo + (kChunkBytes >> 4) + k * (2048 >> 4), dhi), sc);
+#pragma unroll
+        for (int t = 0; t < NT; ++t) {
+          const uint32_t bt = b_lo + t * (kBTapBytes >> 4) + k * (2048 >> 4);
+          if constexpr (kChunks == 1) {
+            wgmma<kNLast, 1, 1>(acc[t], ad, make_desc(bt, dhi), sc);
+          } else {
+            wgmma<64, 1, 1>(acc[t], ad, make_desc(bt, dhi), sc);
+            wgmma<kNLast, 1, 1>(acc[t] + 32, ad, make_desc(bt + (kChunkBytes >> 4), dhi), sc);
+          }
         }
       }
       wgmma_commit();
@@ -147,8 +161,25 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
       ring.next(p.stages);
     }
     wgmma_wait<0>();
-    fence_regs(acc);
+#pragma unroll
+    for (int t = 0; t < NT; ++t) fence_regs(acc[t]);
     if (prev >= 0 && lane == 0) mbar_arrive(&empty_bar[prev]);
+  };
+
+  for (int unit = blockIdx.x; unit < num_units; unit += gridDim.x) {
+    int co_t, ci_t, tg, ks, kb0, kb1;
+    decode(unit, co_t, ci_t, tg, ks);
+    kb_range(ks, kb0, kb1);
+    const int tap0 = tg * T;
+    const int ntaps = min(T, RS - tap0);
+    if (ntaps == T) {
+      mainloop(std::integral_constant<int, T>{}, kb0, kb1);
+    } else if constexpr (T == 3) {
+      if (ntaps == 2) mainloop(std::integral_constant<int, 2>{}, kb0, kb1);
+      else mainloop(std::integral_constant<int, 1>{}, kb0, kb1);
+    } else if constexpr (T == 2) {
+      mainloop(std::integral_constant<int, 1>{}, kb0, kb1);
+    }
 
     const bool have = kb1 > kb0;   // empty pixel range: this unit's slice of the partial buffer must still read as zero
     if (!have && p.use_atomics != 2) continue;
@@ -157,19 +188,23 @@ conv_wgrad_kernel(const __grid_constant__ CUtensorMap tmDY, const __grid_constan
     for (int h = 0; h < 2; ++h) {
       const int co = co_t * 128 + 64 * wg + frow + 8 * h;
       if (co >= p.Cout) continue;
-      float* drow = base + ((size_t)co * RS + tap) * p.Cin;
 #pragma unroll
-      for (int j = 0; j < CIW / 8; ++j) {
-        // register block j: chunk j / 8, columns 8 * (j % 8) + fcol of that chunk
-        const int c = (j >> 3) * 64 + 8 * (j & 7) + fcol;
-        const int ci = ci_t * p.ci_tile + c;
-        if (c >= p.ci_tile || ci >= p.Cin) continue;
-        const float v0 = have ? acc[4 * j + 2 * h] : 0.f, v1 = have ? acc[4 * j + 2 * h + 1] : 0.f;
-        if (p.use_atomics == 1) {
-          atomicAdd(drow + ci, v0);
-          atomicAdd(drow + ci + 1, v1);
-        } else {
-          *reinterpret_cast<float2*>(drow + ci) = make_float2(v0, v1);   // Cin % 8 == 0 and ci even: 8-byte aligned
+      for (int t = 0; t < T; ++t) {
+        if (t >= ntaps) break;
+        float* drow = base + ((size_t)co * RS + tap0 + t) * p.Cin;
+#pragma unroll
+        for (int j = 0; j < CIW / 8; ++j) {
+          // register block j: chunk j / 8, columns 8 * (j % 8) + fcol of that chunk
+          const int c = (j >> 3) * 64 + 8 * (j & 7) + fcol;
+          const int ci = ci_t * p.ci_tile + c;
+          if (c >= p.ci_tile || ci >= p.Cin) continue;
+          const float v0 = have ? acc[t][4 * j + 2 * h] : 0.f, v1 = have ? acc[t][4 * j + 2 * h + 1] : 0.f;
+          if (p.use_atomics == 1) {
+            atomicAdd(drow + ci, v0);
+            atomicAdd(drow + ci + 1, v1);
+          } else {
+            *reinterpret_cast<float2*>(drow + ci) = make_float2(v0, v1);   // Cin % 8 == 0 and ci even: 8-byte aligned
+          }
         }
       }
     }
@@ -276,6 +311,23 @@ int plan_wgrad(WgradPlan& plan, int N, int H, int W, int Cin, int Cout, int R, i
   return 0;
 }
 
+// Regroups the planned one-tap units into work items of up to `taps` taps of the same (co tile, ci tile, pixel range)
+// and sizes the shared-memory ring for their stages. k_splits, the workspace and every unit's result stay as planned.
+void group_taps(WgradParams& p, int taps) {
+  p.taps_per_group = taps;
+  p.num_tap_groups = (p.R * p.S + taps - 1) / taps;
+  p.stage_bytes = kABytes + taps * p.ci_chunks * kChunkBytes;
+  p.stages = min(6, (200 * 1024) / p.stage_bytes);
+}
+
+// Most taps a work item may hold: kMaxTaps, or HB_WGRAD_TAPS_PER_UNIT (1 .. kMaxTaps; 1 runs one tap per unit) so that
+// executions can be compared within one build. dW is the same bits for every value.
+int max_taps_per_unit() {
+  const char* v = getenv("HB_WGRAD_TAPS_PER_UNIT");
+  const int n = v ? atoi(v) : kMaxTaps;
+  return n < 1 ? 1 : (n > kMaxTaps ? kMaxTaps : n);
+}
+
 }  // namespace
 
 extern "C" {
@@ -319,6 +371,8 @@ static int wgrad_impl(const void* x, const void* dy, float* dw, float* workspace
     return (int)cudaErrorNotSupported;
   const int RS = R * S;
   const int k_splits = p.k_splits;
+  static const int max_taps = max_taps_per_unit();
+  group_taps(p, RS < max_taps ? RS : max_taps);
   const int base_units = p.num_co_tiles * p.num_ci_tiles * p.num_tap_groups;
   const int ctas = num_ctas > 0 ? num_ctas : HB_NUM_SMS;
   p.dw = dw;
@@ -341,9 +395,11 @@ static int wgrad_impl(const void* x, const void* dy, float* dw, float* workspace
   const size_t smem_bytes = (size_t)p.stages * p.stage_bytes + 2 * p.stages * sizeof(uint64_t) + 1024;
   const int num_units = base_units * k_splits;
   int grid = ctas < num_units ? ctas : num_units;
-  // one instantiation per Cin tile width (rounded up to 16)
+  // one instantiation per Cin tile width (rounded up to 16) and taps per work item
   const cudaError_t e = dispatch_width<16, 128>((p.ci_tile + 15) & ~15, [&](auto ciw) {
-    return launch<conv_wgrad_kernel<decltype(ciw)::value>>(grid, smem_bytes, st, tmDY, tmX, p);
+    return dispatch_width<1, kMaxTaps>(p.taps_per_group, [&](auto taps) {
+      return launch<conv_wgrad_kernel<decltype(ciw)::value, decltype(taps)::value>>(grid, smem_bytes, st, tmDY, tmX, p);
+    });
   });
   if (e != cudaSuccess) return (int)e;
   if (p.use_atomics == 2) {
