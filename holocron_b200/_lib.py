@@ -141,6 +141,7 @@ SIGNATURES = {
     "hb_autoaugment_batch": "pppp" + "i" * 5 + "p",
     "hb_color_jitter_batch": "pppp" + "i" * 6 + "p",
     "hb_box_transform_batch": "ppp" + "iii" + "pppp",
+    "hb_assign_iou_batch": "pifpppp",
     "hb_detect_scratch_bytes": "piii",
     "hb_detect": "piii" + "p" * 6,
 }

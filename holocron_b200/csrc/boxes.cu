@@ -6,7 +6,8 @@
 // (tests/test_ops.py:25-76) hold bit for bit.
 //
 // Also the box steps of the detection recipe's transforms (references/detection/transforms.py:58-127), every box of a
-// batch in one launch (box_transform_kernel below).
+// batch in one launch (box_transform_kernel below), and the ground-truth matching of the detection trainer's evaluation
+// (holocron/trainer/detection.py:17-32), every image of a batch in one launch (match_kernel below).
 //
 // NB (reference quirk, reproduced): ciou_loss adds its alpha*v term to a masked COPY (boxes.py:209), so it
 // returns exactly the DIoU loss.
@@ -301,6 +302,149 @@ __global__ void __launch_bounds__(kBoxWarps * 32) box_transform_kernel(const Box
   if (lane == 0) counts[img] = (int)kept;
 }
 
+// ---- detection evaluation: ground truth matched to predictions ---------------------------------------
+// Reference: holocron/trainer/detection.py:17-32, as holocron_b200.trainer.assign_iou computes it on CUDA tensors: box_iou
+// (pair_value's IoU), max(dim=1), values >= threshold, and of the kept targets claiming one prediction the one with the
+// largest IoU (the lowest index on a tie) keeps it. One CTA per image.
+enum LabelType { L_I64 = 0, L_I32 = 1 };
+
+// codes: box dtypes (HB_DTYPE_*) and label types (LabelType), one byte each: gt boxes, pred boxes, gt labels, pred labels.
+// Strides in elements. labels are 0 when the caller counts nothing.
+struct MatchDesc {
+  long long gt, pred, gt_labels, pred_labels, n_gt, n_pred, gt_rs, gt_cs, pred_rs, pred_cs, gt_ls, pred_ls, codes,
+      offset, unused0, unused1;
+};
+
+constexpr int kMatchWarps = 8;
+constexpr int kMatchRows = 4;      // ground-truth rows a warp holds in registers per pass
+constexpr int kMatchTile = 1024;   // predictions staged in shared memory at a time (16 KB)
+
+// Box i of a strided [n, 4] tensor, converted to fp32 as Tensor.float() converts it.
+__device__ __forceinline__ Box load_box_any(long long base, long long i, long long rs, long long cs, int dtype) {
+  switch (dtype) {
+    case HB_DTYPE_BF16: {
+      const __nv_bfloat16* p = reinterpret_cast<const __nv_bfloat16*>(base) + i * rs;
+      return Box{__bfloat162float(p[0]), __bfloat162float(p[cs]), __bfloat162float(p[2 * cs]), __bfloat162float(p[3 * cs])};
+    }
+    case HB_DTYPE_F16: {
+      const __half* p = reinterpret_cast<const __half*>(base) + i * rs;
+      return Box{__half2float(p[0]), __half2float(p[cs]), __half2float(p[2 * cs]), __half2float(p[3 * cs])};
+    }
+    case HB_DTYPE_F64: {
+      const double* p = reinterpret_cast<const double*>(base) + i * rs;
+      return Box{__double2float_rn(p[0]), __double2float_rn(p[cs]), __double2float_rn(p[2 * cs]),
+                 __double2float_rn(p[3 * cs])};
+    }
+    default: {
+      const float* p = reinterpret_cast<const float*>(base) + i * rs;
+      return Box{p[0], p[cs], p[2 * cs], p[3 * cs]};
+    }
+  }
+}
+
+__device__ __forceinline__ long long load_label(long long base, long long i, long long stride, int type) {
+  return type == L_I32 ? (long long)reinterpret_cast<const int*>(base)[i * stride]
+                       : reinterpret_cast<const long long*>(base)[i * stride];
+}
+
+// (va, ia) comes before (vb, ib) in torch's CUDA max(dim): NaN first, then the larger value, then the lower index.
+// An index < 0 is "no candidate yet".
+__device__ __forceinline__ bool beats(float va, int ia, float vb, int ib) {
+  if (ib < 0) return ia >= 0;
+  if (ia < 0) return false;
+  if (va != va) return vb == vb || ia < ib;
+  if (vb != vb) return false;
+  return va > vb || (va == vb && ia < ib);
+}
+
+// scratch: (IoU bits, index) of every ground-truth row's maximum, 8 bytes per row at the image's offset. counts (or
+// NULL): int64 {assigned, correct}, added to.
+__global__ void __launch_bounds__(kMatchWarps * 32) match_kernel(const MatchDesc* __restrict__ descs, float thr,
+                                                                 int2* scratch, long long* __restrict__ match,
+                                                                 unsigned long long* __restrict__ counts) {
+  __shared__ Box tile[kMatchTile];
+  __shared__ unsigned long long red[2][kMatchWarps];
+  const MatchDesc d = descs[blockIdx.x];
+  const int warp = (int)(threadIdx.x >> 5), lane = (int)(threadIdx.x & 31);
+  const int gt_dt = (int)(d.codes & 0xff), pred_dt = (int)((d.codes >> 8) & 0xff);
+  int2* best = scratch + d.offset;
+  // 1. every row's first maximal IoU: each lane walks its predictions in index order, then the warp merges the lanes
+  for (long long g0 = 0; g0 < d.n_gt; g0 += kMatchWarps * kMatchRows) {
+    Box a[kMatchRows];
+    float bv[kMatchRows];
+    int bi[kMatchRows];
+#pragma unroll
+    for (int r = 0; r < kMatchRows; ++r) {
+      const long long g = g0 + warp + r * kMatchWarps;
+      a[r] = g < d.n_gt ? load_box_any(d.gt, g, d.gt_rs, d.gt_cs, gt_dt) : Box{0.f, 0.f, 0.f, 0.f};
+      bv[r] = 0.f;
+      bi[r] = -1;
+    }
+    for (long long p0 = 0; p0 < d.n_pred; p0 += kMatchTile) {
+      const int nt = (int)min((long long)kMatchTile, d.n_pred - p0);
+      __syncthreads();
+      for (int j = threadIdx.x; j < nt; j += kMatchWarps * 32) tile[j] = load_box_any(d.pred, p0 + j, d.pred_rs, d.pred_cs, pred_dt);
+      __syncthreads();
+      for (int j = lane; j < nt; j += 32) {
+        const Box b = tile[j];
+#pragma unroll
+        for (int r = 0; r < kMatchRows; ++r) {
+          float inter, uni;
+          inter_union(a[r], b, inter, uni);
+          const float v = dvd(inter, uni);
+          if (beats(v, (int)p0 + j, bv[r], bi[r])) bv[r] = v, bi[r] = (int)p0 + j;
+        }
+      }
+    }
+#pragma unroll
+    for (int r = 0; r < kMatchRows; ++r) {
+#pragma unroll
+      for (int s = 16; s > 0; s >>= 1) {
+        const float ov = __shfl_xor_sync(0xffffffffu, bv[r], s);
+        const int oi = __shfl_xor_sync(0xffffffffu, bi[r], s);
+        if (beats(ov, oi, bv[r], bi[r])) bv[r] = ov, bi[r] = oi;
+      }
+      const long long g = g0 + warp + r * kMatchWarps;
+      if (lane == 0 && g < d.n_gt) best[g] = make_int2(__float_as_int(bv[r]), bi[r]);
+    }
+  }
+  __syncthreads();
+  // 2. a kept row keeps its prediction unless another row claims it with a larger IoU, or an equal one at a lower index
+  unsigned long long assigned = 0, correct = 0;
+  const int gl_t = (int)((d.codes >> 16) & 0xff), pl_t = (int)((d.codes >> 24) & 0xff);
+  for (long long g = threadIdx.x; g < d.n_gt; g += kMatchWarps * 32) {
+    const int2 e = best[g];
+    const float v = __int_as_float(e.x);
+    bool keep = e.y >= 0 && v >= thr;
+    for (long long o = 0; keep && o < d.n_gt; ++o) {
+      const int2 f = best[o];
+      const float w = __int_as_float(f.x);
+      keep = !(f.y == e.y && (w > v || (w == v && o < g)));
+    }
+    match[d.offset + g] = keep ? e.y : -1;
+    if (keep) {
+      ++assigned;
+      if (d.gt_labels && d.pred_labels)
+        correct += load_label(d.gt_labels, g, d.gt_ls, gl_t) == load_label(d.pred_labels, e.y, d.pred_ls, pl_t);
+    }
+  }
+  if (!counts) return;
+#pragma unroll
+  for (int s = 16; s > 0; s >>= 1) {
+    assigned += __shfl_xor_sync(0xffffffffu, assigned, s);
+    correct += __shfl_xor_sync(0xffffffffu, correct, s);
+  }
+  if (lane == 0) red[0][warp] = assigned, red[1][warp] = correct;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    assigned = correct = 0;
+#pragma unroll
+    for (int w = 0; w < kMatchWarps; ++w) assigned += red[0][w], correct += red[1][w];
+    if (assigned) atomicAdd(counts, assigned);
+    if (correct) atomicAdd(counts + 1, correct);
+  }
+}
+
 }  // namespace
 
 extern "C" {
@@ -312,6 +456,17 @@ int hb_box_transform_batch(const void* descs, const float* params, const int* op
   const int blocks = (N + kBoxWarps - 1) / kBoxWarps;
   box_transform_kernel<<<blocks, kBoxWarps * 32, 0, (cudaStream_t)stream>>>(
       static_cast<const BoxDesc*>(descs), params, ops, n_ops, n_params, N, out_boxes, out_labels, counts);
+  HB_LAUNCH_CHECK();
+  return 0;
+}
+
+int hb_assign_iou_batch(const void* descs, int N, float iou_threshold, void* scratch, long long* match,
+                        long long* counts, void* stream) {
+  if (N < 0) return (int)cudaErrorInvalidValue;
+  if (N == 0) return 0;
+  match_kernel<<<N, kMatchWarps * 32, 0, (cudaStream_t)stream>>>(static_cast<const MatchDesc*>(descs), iou_threshold,
+                                                                static_cast<int2*>(scratch), match,
+                                                                reinterpret_cast<unsigned long long*>(counts));
   HB_LAUNCH_CHECK();
   return 0;
 }

@@ -26,15 +26,18 @@ import math
 from collections import defaultdict
 from typing import Any, Callable, Dict, List, Optional, Sequence, Tuple, Union
 
+import numpy as np
 import torch
 from torch import Tensor, nn
 from torch.optim.lr_scheduler import CosineAnnealingLR, MultiplicativeLR, OneCycleLR
 
+from .._lib import check, lib, ptr, require_cuda, stream_ptr
+from ..transforms._table import upload
 from .core import TrainStep, lr_schedule_table
 from .utils import freeze_bn, freeze_model, split_normalization_params
 
 __all__ = ["BinaryClassificationTrainer", "ClassificationTrainer", "DetectionTrainer", "SegmentationTrainer", "Trainer",
-           "assign_iou"]
+           "assign_iou", "assign_iou_batch"]
 
 ParamSeq = Sequence[torch.nn.Parameter]
 
@@ -528,6 +531,97 @@ def assign_iou(gt_boxes: Tensor, pred_boxes: Tensor, iou_threshold: float = 0.5)
     return gt_indices, pred_indices
 
 
+# the codes of hb_assign_iou_batch's descriptor rows (include/holocron_b200.h)
+_BOX_CODES = {torch.float32: 0, torch.bfloat16: 1, torch.float16: 2, torch.float64: 4}
+_LABEL_CODES = {torch.int64: 0, torch.int32: 1}
+_MATCH_WORDS = 16
+_INT32_MAX = 2 ** 31 - 1
+
+
+def _match_table(gt_boxes: Sequence[Tensor], pred_boxes: Sequence[Tensor], gt_labels: Optional[Sequence[Tensor]],
+                 pred_labels: Optional[Sequence[Tensor]]) -> Tuple[np.ndarray, List[int]]:
+    """The descriptor rows of ``hb_assign_iou_batch`` (one per image: the boxes and labels are read in place through
+    their strides) and each image's ground-truth count, refusing what the kernel does not read."""
+    if len(gt_boxes) != len(pred_boxes):
+        raise ValueError(f"{len(gt_boxes)} ground-truth sets but {len(pred_boxes)} prediction sets")
+    labels = gt_labels is not None
+    if labels and (pred_labels is None or len(gt_labels) != len(gt_boxes) or len(pred_labels) != len(gt_boxes)):
+        raise ValueError("expected one ground-truth and one predicted label tensor per image")
+    tensors = [*gt_boxes, *pred_boxes, *(gt_labels if labels else []), *(pred_labels if labels else [])]
+    if len({t.device for t in tensors}) > 1:
+        raise ValueError("all boxes and labels of a batch must be on one device")
+    table = np.zeros((len(gt_boxes), _MATCH_WORDS), dtype=np.int64)
+    ns, offset = [], 0
+    for k, (g, p) in enumerate(zip(gt_boxes, pred_boxes)):
+        for b in (g, p):
+            if b.ndim != 2 or b.shape[1] != 4 or b.shape[0] > _INT32_MAX:
+                raise ValueError(f"boxes are expected as (num_boxes, 4) tensors in xyxy format, got {tuple(b.shape)}")
+            if b.dtype not in _BOX_CODES:
+                raise TypeError(f"unsupported box dtype {b.dtype}: expected one of {', '.join(map(str, _BOX_CODES))}")
+        n = int(g.shape[0])
+        codes = _BOX_CODES[g.dtype] | _BOX_CODES[p.dtype] << 8
+        row = [g.data_ptr(), p.data_ptr(), 0, 0, n, p.shape[0], *g.stride(), *p.stride(), 0, 0, 0, offset]
+        if labels:
+            gl, pl = gt_labels[k], pred_labels[k]
+            for lab, m in ((gl, n), (pl, p.shape[0])):
+                if lab.ndim != 1 or lab.shape[0] != m:
+                    raise ValueError(f"{m} boxes but labels of shape {tuple(lab.shape)}")
+                if lab.dtype not in _LABEL_CODES:
+                    raise TypeError(f"unsupported label dtype {lab.dtype}: expected torch.int64 or torch.int32")
+            codes |= _LABEL_CODES[gl.dtype] << 16 | _LABEL_CODES[pl.dtype] << 24
+            row[2:4], row[10:12] = [gl.data_ptr(), pl.data_ptr()], [gl.stride(0), pl.stride(0)]
+        row[12] = codes
+        table[k, :14] = row
+        ns.append(n)
+        offset += n
+    return table, ns
+
+
+def _assign_batch(gt_boxes: Sequence[Tensor], pred_boxes: Sequence[Tensor], iou_threshold: float,
+                  gt_labels: Optional[Sequence[Tensor]] = None, pred_labels: Optional[Sequence[Tensor]] = None,
+                  counts: Optional[Tensor] = None) -> Tuple[Tensor, List[int]]:
+    """One ``hb_assign_iou_batch`` launch over a non-empty batch: the flat int64 match vector and each image's
+    ground-truth count. With labels, {assigned, correct} are added to ``counts`` (int64 [2] on the batch's device)."""
+    require_cuda(*gt_boxes, *pred_boxes, *(gt_labels or ()), *(pred_labels or ()))
+    table, ns = _match_table(gt_boxes, pred_boxes, gt_labels, pred_labels)
+    device = gt_boxes[0].device
+    with torch.cuda.device(device):
+        match = torch.empty(sum(ns), dtype=torch.int64, device=device)
+        scratch = torch.empty(2 * sum(ns), dtype=torch.int32, device=device)
+        _dev, (descs,) = upload(device, table)
+        check(lib().hb_assign_iou_batch(descs, len(ns), iou_threshold, ptr(scratch), ptr(match), ptr(counts),
+                                        stream_ptr()), "hb_assign_iou_batch")
+    return match, ns
+
+
+def assign_iou_batch(gt_boxes: Sequence[Tensor], pred_boxes: Sequence[Tensor], iou_threshold: float = 0.5
+                     ) -> List[Tensor]:
+    """:func:`assign_iou` for every image of a batch in one CUDA launch, with no host synchronisation.
+
+    ``gt_boxes[i]`` and ``pred_boxes[i]`` are image i's (n, 4) xyxy boxes (fp32, bf16, fp16 or fp64, any strides, all on
+    one CUDA device; box arithmetic in fp32). Returns one int64 vector per image, views of one flat tensor: entry g is
+    the prediction paired with ground-truth box g, or -1, so that {(g, m[g]) : m[g] >= 0} is the set of pairs
+    ``assign_iou(gt_boxes[i], pred_boxes[i], iou_threshold)`` returns on CUDA tensors. The threshold is rounded to fp32,
+    as torch rounds a scalar compared with an fp32 tensor."""
+    if not gt_boxes and not pred_boxes:
+        return []
+    match, ns = _assign_batch(gt_boxes, pred_boxes, iou_threshold)
+    return list(match.split(ns))
+
+
+def _matchable(target: List[Dict[str, Tensor]], detections: List[Dict[str, Tensor]],
+               counts: Optional[Tensor]) -> bool:
+    """Whether hb_assign_iou_batch reads the batch: every box and label tensor on one CUDA device (counts' own, once
+    it exists), in dtypes the kernel takes."""
+    if not target or len(target) != len(detections):
+        return False
+    tensors = [d[k] for d in (*target, *detections) for k in ("boxes", "labels")]
+    device = tensors[0].device if counts is None else counts.device
+    return (device.type == "cuda" and all(t.device == device for t in tensors)
+            and all(d["boxes"].dtype in _BOX_CODES and d["labels"].dtype in _LABEL_CODES
+                    for d in (*target, *detections)))
+
+
 class DetectionTrainer(Trainer):
     """Object detection: the model computes its own losses (reference trainer/detection.py:35-126)."""
 
@@ -551,14 +645,29 @@ class DetectionTrainer(Trainer):
 
     @torch.no_grad()
     def evaluate(self, iou_threshold: float = 0.5) -> Dict[str, Optional[float]]:
-        """Localisation / classification / end-to-end detection error rates (reference detection.py:77-126)."""
+        """Localisation / classification / end-to-end detection error rates (reference detection.py:77-126).
+
+        Batches whose boxes and labels are all on one CUDA device are matched by one ``hb_assign_iou_batch`` launch
+        each, their {assigned, correct} counts summed on the device and read back once per call; other batches take
+        the reference's per-image loop."""
         self.model.eval()
         loc_assigns = 0
         correct, clf_error, loc_fn, loc_fp, num_samples = 0, 0, 0, 0, 0
+        counts: Optional[Tensor] = None       # {assigned, correct} of the batches matched on the device
+        dev_gt, dev_pred = 0, 0               # their ground-truth and predicted boxes
         for x, target in self.val_loader:
             x, target = self.to_cuda(x, target)
             with self._autocast():
                 detections = self.model(x)
+            num_samples += sum(t["boxes"].shape[0] for t in target)
+            if _matchable(target, detections, counts):
+                if counts is None:
+                    counts = torch.zeros(2, dtype=torch.int64, device=target[0]["boxes"].device)
+                _assign_batch([t["boxes"] for t in target], [d["boxes"] for d in detections], iou_threshold,
+                              [t["labels"] for t in target], [d["labels"] for d in detections], counts)
+                dev_gt += sum(t["boxes"].shape[0] for t in target)
+                dev_pred += sum(d["boxes"].shape[0] for d in detections)
+                continue
             for dets, t in zip(detections, target):
                 if t["boxes"].shape[0] > 0 and dets["boxes"].shape[0] > 0:
                     gt_indices, pred_indices = assign_iou(t["boxes"], dets["boxes"], iou_threshold)
@@ -571,7 +680,13 @@ class DetectionTrainer(Trainer):
                 clf_error += len(gt_indices) - correct_
                 loc_fn += t["boxes"].shape[0] - len(gt_indices)
                 loc_fp += dets["boxes"].shape[0] - len(pred_indices)
-            num_samples += sum(t["boxes"].shape[0] for t in target)
+        if counts is not None:
+            assigned, correct_ = counts.tolist()
+            loc_assigns += assigned
+            correct += correct_
+            clf_error += assigned - correct_
+            loc_fn += dev_gt - assigned
+            loc_fp += dev_pred - assigned
         nb_preds = num_samples - loc_fn + loc_fp
         loc_err = 1 - 2 * loc_assigns / (nb_preds + num_samples) if nb_preds + num_samples > 0 else None
         clf_err = 1 - correct / loc_assigns if loc_assigns > 0 else None

@@ -558,6 +558,21 @@ int hb_color_jitter_batch(const void* descs, const float* params, const long lon
 int hb_box_transform_batch(const void* descs, const float* params, const int* ops, int n_ops, int n_params, int N,
                            float* out_boxes, long long* out_labels, int* counts, void* stream);
 
+/* ---- detection evaluation: holocron/trainer/detection.py:17-32 (assign_iou), every image of a batch in one launch --
+ * descs: device table of N rows of 16 int64 {gt, pred, gt_labels, pred_labels, n_gt, n_pred, gt_row_stride,
+ * gt_col_stride, pred_row_stride, pred_col_stride, gt_label_stride, pred_label_stride, codes, out_offset, 0, 0}: image
+ * k's [n_gt][4] ground-truth and [n_pred][4] predicted xyxy boxes are read in place through their strides (elements),
+ * converted to fp32 as Tensor.float() converts them. codes holds one byte each, from the lowest: the gt and pred box
+ * dtypes (0 fp32, 1 bf16, 2 fp16, 4 fp64), the gt and pred label types (0 int64, 1 int32). Labels (0 = not counted)
+ * are read only for counts. Per image: the IoU of hb_box_pairwise mode 0, the first maximal prediction of each
+ * ground-truth box (NaN wins, as in torch's max(dim=1)), kept when IoU >= iou_threshold; of the kept boxes claiming
+ * one prediction, the one with the largest IoU (the lowest index on a tie) keeps it. match int64 [sum of n_gt]: from
+ * out_offset on, the prediction paired with each ground-truth box, or -1. counts (int64 {assigned, correct}, or NULL)
+ * is added to: the paired boxes, and those whose labels equal their prediction's. scratch: 8 bytes per ground-truth
+ * box of the batch. One CTA per image; no host synchronisation. */
+int hb_assign_iou_batch(const void* descs, int N, float iou_threshold, void* scratch, long long* match,
+                        long long* counts, void* stream);
+
 /* ---- YOLO inference post-processing (holocron/models/detection/yolo.py:159-233, yolov4.py:303-335) ------------------
  * One segment = one set of decoded candidates per image: boxes fp32 [B, M, 4] xyxy (16-byte aligned), objectness fp32
  * [B, M] and class scores fp32 [B, M, K], all contiguous, with its own thresholds (YOLOv1/v2: one segment; YOLOv4: one
