@@ -138,6 +138,7 @@ SIGNATURES = {
     "hb_lookahead_sync": "ppi" + "f" + "p",
     "hb_resample_batch": "p" + "i" * 8 + "p",
     "hb_erase_batch": "pp" + "i" * 4 + "p",
+    "hb_image_tail_batch": "pp" + "i" * 6 + "p",
     "hb_autoaugment_batch": "pppp" + "i" * 5 + "p",
     "hb_color_jitter_batch": "pppp" + "i" * 6 + "p",
     "hb_box_transform_batch": "ppp" + "iii" + "pppp",

@@ -16,32 +16,15 @@
 // A thread owns one 16-byte vector of a destination row segment (the whole row in copy mode, the rectangle's columns
 // in place). Vectors are aligned to 16 bytes in memory: the first one of a row starts up to V - 1 elements early and
 // covers its valid elements only, so every full vector is one 128-bit store, and one 128-bit load where the source row
-// is contiguous and aligned too. Other elements go one at a time. No atomics, no shared memory.
-#include "common.cuh"
+// is contiguous and aligned too. Other elements go one at a time (the walk of row_walk.cuh). No atomics, no shared
+// memory.
+#include "row_walk.cuh"
 
 using namespace hb;
 
 namespace {
 
-constexpr int kThreads = 256;
-
-enum Fill { kNone = 0, kPerChannel = 1, kPerPixel = 2 };
-
-// One row of the descriptor table (16 x int64, include/holocron_b200.h). Pointers are addresses, strides count
-// elements of the image dtype.
-struct EraseDesc {
-  long long src, dst, sc, sh, sw;
-  long long C, H, W, top, left, h, w, fill, voff, reserved0, reserved1;
-};
-
-template <typename T> __device__ __forceinline__ T cast_fill(float v);
-template <> __device__ __forceinline__ float cast_fill<float>(float v) { return v; }
-template <> __device__ __forceinline__ double cast_fill<double>(float v) { return (double)v; }
-template <> __device__ __forceinline__ __half cast_fill<__half>(float v) { return __float2half_rn(v); }
-template <> __device__ __forceinline__ __nv_bfloat16 cast_fill<__nv_bfloat16>(float v) { return __float2bfloat16_rn(v); }
-template <> __device__ __forceinline__ uint8_t cast_fill<uint8_t>(float v) {
-  return static_cast<uint8_t>(static_cast<long long>(v));
-}
+constexpr int kThreads = kWalkThreads;
 
 // One CTA per (image, 256 vectors of its rows). rows: the most row segments an image has (C*H in copy mode, C*h in
 // place); vpr: vectors per row segment, one more than the longest segment needs, for the alignment head.
@@ -79,51 +62,27 @@ __global__ void __launch_bounds__(kThreads) erase_kernel(const EraseDesc* __rest
   T* dst_row = in_place ? reinterpret_cast<T*>(d.dst) + c * d.sc + y * d.sh
                         : reinterpret_cast<T*>(d.dst) + ((long long)c * H + y) * W;
   const bool dst_contig = !in_place || sw == 1;
-  const int head = dst_contig ? (int)((reinterpret_cast<uintptr_t>(dst_row + x0) & 15) / sizeof(T)) : 0;
-  const int e0 = k * V - head;  // element offset of this vector within the row segment
-  if (e0 >= len) return;
-  const int xa = x0 + e0;  // column of the vector's first element
-  const bool full = e0 >= 0 && e0 + V <= len;
+  const RowVec<V, T> rv(dst_row + x0, dst_contig, k, x0, len);
+  if (rv.outside()) return;
+  const int xa = rv.xa;
 
-  const bool row_in_rect = fill != kNone && y >= top && y < top + h;
-  // value of column xx of this row: values[vrow + xx] per pixel, values[vrow] per channel
-  const long long vrow = d.voff + (fill == kPerPixel ? ((long long)c * h + (y - top)) * w - left : c);
-
-  Vec16<T> out;
-  if (!in_place) {
-    const T* s = src_row + xa * sw;
-    if (full && sw == 1 && aligned16(s)) {
-      out = ld16(s);
-    } else {
-#pragma unroll
-      for (int j = 0; j < V; ++j)
-        if (e0 + j >= 0 && e0 + j < len) out.v[j] = s[j * sw];
-    }
-  }
-  if (row_in_rect) {
-#pragma unroll
-    for (int j = 0; j < V; ++j) {
-      const int xx = xa + j;
-      if (xx >= left && xx < left + w) out.v[j] = cast_fill<T>(values[fill == kPerPixel ? vrow + xx : vrow]);
-    }
-  }
-  T* o = dst_row + xa * (dst_contig ? 1 : sw);
-  if (full && dst_contig) {
-    st16(o, out);
-  } else {
+  VecN<T, V> out;
+  if (!in_place) out = load_vec<T, V>(src_row + xa * sw, sw, rv);
+  const RectRow rect(d, c, y);
+  if (rect.hit) {
 #pragma unroll
     for (int j = 0; j < V; ++j)
-      if (e0 + j >= 0 && e0 + j < len) o[j * (dst_contig ? 1 : sw)] = out.v[j];
+      if (rect.covers(xa + j)) out.v[j] = cast_fill<T>(rect.value(values, xa + j));
   }
+  store_vec<T, V>(dst_row + xa * (dst_contig ? 1 : sw), dst_contig, sw, rv, out);
 }
 
 template <typename T>
 int launch(const EraseDesc* descs, const float* values, int N, int rows, int row_len, cudaStream_t stream) {
   constexpr int V = 16 / sizeof(T);
-  const int vpr = (row_len + V - 1) / V + 1;
-  const long long per_image = ((long long)rows * vpr + kThreads - 1) / kThreads;
-  if (per_image > 0x7fffffffLL || (long long)N * per_image > 0x7fffffffLL) return (int)cudaErrorInvalidValue;
-  erase_kernel<T><<<(unsigned)(N * per_image), kThreads, 0, stream>>>(descs, values, rows, vpr, (int)per_image);
+  int vpr, per_image;
+  if (!walk_grid(N, rows, row_len, V, vpr, per_image)) return (int)cudaErrorInvalidValue;
+  erase_kernel<T><<<(unsigned)(N * per_image), kThreads, 0, stream>>>(descs, values, rows, vpr, per_image);
   HB_LAUNCH_CHECK();
   return 0;
 }

@@ -32,7 +32,8 @@ def erase_table(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inpl
                 out: Optional[Tensor]) -> Tuple[np.ndarray, List[Tensor], int, int]:
     """(table, values, rows, row_len): the int64 [N_total, 16] rows of hb_erase_batch, the fp32 value tensors in the
     order of their offsets, and the grid extent (the most row segments an image writes, the longest segment).
-    Destinations are the sources themselves in place, else consecutive images of the contiguous ``out``."""
+    Destinations are the sources themselves in place, else consecutive images of the contiguous ``out`` (whose dtype
+    may differ from the sources': hb_image_tail_batch writes fp32)."""
     check_batch(sources, one_shape=True)
     ref = sources[0]
     C, H, W = ref.shape[-3:]
@@ -62,7 +63,7 @@ def erase_table(sources: Sequence[Tensor], rects: Sequence[Optional[Rect]], inpl
         # leading dimensions of a source are erased alike
         for o in planes(x):
             src = x.data_ptr() + o * es
-            dst = src if inplace else out.data_ptr() + len(rows) * C * H * W * es
+            dst = src if inplace else out.data_ptr() + len(rows) * C * H * W * out.element_size()
             rows.append([src, dst, sc, sh, sw, C, H, W, i, j, h, w, fill, off, 0, 0])
     return np.array(rows, dtype=np.int64).reshape(-1, DESC_WORDS), values, most_rows, row_len
 

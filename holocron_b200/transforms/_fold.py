@@ -1,4 +1,5 @@
-"""Run folding shared by the paired transforms of the reference's recipes (``segmentation``, ``detection``).
+"""Run folding shared by the transform chains of the reference's recipes (``segmentation``, ``detection``,
+``classification``).
 
 A chain is cut into segments: runs of geometric steps, each folded per image into one ``hb_resample_batch`` row, and
 the image-only steps between them. Each image's draws are made for every step in the chain's order before anything is
@@ -42,6 +43,15 @@ class _Fold:
 
     def crop(self, i: int, j: int, h: int, w: int) -> None:
         self.place(-i, -j, h, w)
+
+    def center_crop(self, ch: int, cw: int) -> None:
+        """torchvision's ``center_crop`` to ch x cw: zero padding where the crop is larger than the canvas, then the
+        crop at ``round((H - ch) / 2)``, ``round((W - cw) / 2)`` of the padded canvas."""
+        H, W = self.canvas
+        pl, pt = max(cw - W, 0) // 2, max(ch - H, 0) // 2
+        Hp, Wp = H + pt + max(ch - H + 1, 0) // 2, W + pl + max(cw - W + 1, 0) // 2
+        top, left = (0, 0) if (Hp, Wp) == (ch, cw) else (int(round((Hp - ch) / 2.0)), int(round((Wp - cw) / 2.0)))
+        self.place(pt - top, pl - left, ch, cw)
 
 
 def resized(size: Tuple[int, int], out: List[int], max_size: Optional[int] = None) -> Tuple[int, int]:

@@ -29,7 +29,7 @@ operation (their docstrings state where they may differ). Deviations: PIL images
 ``TrivialAugmentWide``, other than uint8 and fp32 for ``ColorJitter``); a crop needing more than 255 filter taps per
 axis (antialiased downscales beyond about 1/127 bilinear, 1/63 bicubic) raises ``NotImplementedError``.
 """
-from typing import List, Optional, Tuple
+from typing import Dict, List, Optional, Tuple
 
 import torch
 from torch import Tensor
@@ -55,6 +55,40 @@ def _one_shape(images: Images, items: List[Tensor]) -> None:
 
 def _hw(items: List[Tensor]) -> Tuple[int, int]:
     return int(items[0].shape[-2]), int(items[0].shape[-1])
+
+
+def erase_draw(t: T.RandomErasing, x: Tensor) -> Tuple[bool, Optional[Rect]]:
+    """torchvision's ``RandomErasing.forward`` of ``t`` up to ``F.erase`` for one image (only x's shape is read):
+    whether it erases, and the rectangle and values, None when get_params found no rectangle in its 10 attempts
+    (torchvision then assigns the image to itself)."""
+    if not torch.rand(1) < t.p:
+        return False, None
+    if isinstance(t.value, (int, float)):
+        value = [float(t.value)]
+    elif isinstance(t.value, str):
+        value = None
+    elif isinstance(t.value, (list, tuple)):
+        value = [float(v) for v in t.value]
+    else:
+        value = t.value
+    if value is not None and len(value) not in (1, x.shape[-3]):
+        raise ValueError("If value is a sequence, it should have either a single value or "
+                         f"{x.shape[-3]} (number of input channels)")
+    i, j, h, w, v = t.get_params(x, scale=t.scale, ratio=t.ratio, value=value)
+    return True, (None if v is x else (i, j, h, w, v))
+
+
+def trivial_draw(op_meta: Dict[str, Tuple[Tensor, bool]]) -> Tuple[str, float]:
+    """torchvision's ``TrivialAugmentWide.forward`` draws for one image, given its ``_augmentation_space``: the op,
+    then its magnitude bin when it has several, then its sign when it is signed."""
+    names = list(op_meta.keys())
+    op_name = names[int(torch.randint(len(op_meta), (1,)).item())]
+    magnitudes, signed = op_meta[op_name]
+    magnitude = (float(magnitudes[torch.randint(len(magnitudes), (1,), dtype=torch.long)].item())
+                 if magnitudes.ndim > 0 else 0.0)
+    if signed and torch.randint(2, (1,)):
+        magnitude *= -1.0
+    return op_name, magnitude
 
 
 class RandomResizedCrop(T.RandomResizedCrop):
@@ -118,29 +152,10 @@ class RandomErasing(T.RandomErasing):
     >>> out = RandomErasing(p=1.0, scale=(0.02, 0.2), value="random")(batch.unbind(0))
     """
 
-    def _draw(self, x: Tensor) -> Tuple[bool, Optional[Rect]]:
-        """torchvision's forward up to ``F.erase`` for one image: whether it erases, and the rectangle and values, None
-        when get_params found no rectangle in its 10 attempts (torchvision then assigns the image to itself)."""
-        if not torch.rand(1) < self.p:
-            return False, None
-        if isinstance(self.value, (int, float)):
-            value = [float(self.value)]
-        elif isinstance(self.value, str):
-            value = None
-        elif isinstance(self.value, (list, tuple)):
-            value = [float(v) for v in self.value]
-        else:
-            value = self.value
-        if value is not None and len(value) not in (1, x.shape[-3]):
-            raise ValueError("If value is a sequence, it should have either a single value or "
-                             f"{x.shape[-3]} (number of input channels)")
-        i, j, h, w, v = self.get_params(x, scale=self.scale, ratio=self.ratio, value=value)
-        return True, (None if v is x else (i, j, h, w, v))
-
     def forward(self, img: Images) -> Images:
         items = _batch(img, three_d=False)
         _one_shape(img, items)
-        draws = [self._draw(x) for x in items]
+        draws = [erase_draw(self, x) for x in items]
         if isinstance(img, Tensor):
             chosen, rect = draws[0]
             # torchvision hands back the input unless it erases a copy
@@ -181,16 +196,7 @@ class TrivialAugmentWide(autoaugment.TrivialAugmentWide):
         _one_shape(img, items)
         check_options(self.interpolation, self.fill, check_images(items, _autoaugment.SUPPORTED))
         op_meta = self._augmentation_space(self.num_magnitude_bins)
-        names = list(op_meta.keys())
-        ops = []
-        for _ in items:  # torchvision's forward, draw for draw
-            op_name = names[int(torch.randint(len(op_meta), (1,)).item())]
-            magnitudes, signed = op_meta[op_name]
-            magnitude = (float(magnitudes[torch.randint(len(magnitudes), (1,), dtype=torch.long)].item())
-                         if magnitudes.ndim > 0 else 0.0)
-            if signed and torch.randint(2, (1,)):
-                magnitude *= -1.0
-            ops.append((op_name, magnitude))
+        ops = [trivial_draw(op_meta) for _ in items]
         if isinstance(img, Tensor) and ops[0][0] == "Identity":
             return img
         out = apply_ops(items, ops, self.interpolation, self.fill)

@@ -253,10 +253,7 @@ def fold_run(steps: Sequence[Any], size: Tuple[int, int], row: List[float]) -> _
             f = _Fold(*(2 * [(int(t.size[0]), int(t.size[1]))]), box=(i, j, h, w))
         elif isinstance(t, CenterCrop):
             ch, cw = t.size
-            pl, pt = max(cw - W, 0) // 2, max(ch - H, 0) // 2
-            Hp, Wp = H + pt + max(ch - H + 1, 0) // 2, W + pl + max(cw - W + 1, 0) // 2
-            top, left = (0, 0) if (Hp, Wp) == (ch, cw) else (int(round((Hp - ch) / 2.0)), int(round((Wp - cw) / 2.0)))
-            f.place(pt - top, pl - left, ch, cw)
+            f.center_crop(ch, cw)
             x, y = int(cw / 2 - ch / 2), int(ch / 2 - cw / 2)
             row += [x, x + ch, y, y + cw, x, y]
         elif isinstance(t, RandomHorizontalFlip):

@@ -509,6 +509,20 @@ int hb_resample_batch(const void* descs, int N, int canvas_h, int canvas_w, int 
  * hb_resample_batch. */
 int hb_erase_batch(const void* descs, const float* values, int N, int rows, int row_len, int dtype, void* stream);
 
+/* ---- classification tail: torchvision's PILToTensor, ConvertImageDtype(torch.float32), Normalize and RandomErasing
+ *      (rectangle and values drawn on the host), as the reference's classification recipe ends its chains
+ *      (references/classification/train.py:100-107, 162-168) - a batch of images of one shape in one launch ------- */
+/* descs: device table of N rows of 16 int64 {src, dst, stride_c, stride_h, stride_w, C, H, W, top, left, h, w, fill,
+ * voff, 0, 0}, hb_erase_batch's rows in copy mode: image n is read from the strided src [C][H][W] (uint8 or fp32,
+ * src_dtype 3 or 0) and written to the contiguous fp32 dst [C][H][W]. ops: the op program every element runs in order,
+ * one op code per byte from the lowest, 0 ending it (at most 3 ops): 1 convert (v * f32(1/255), torch's uint8 to fp32
+ * division by 255), 2 normalise ((v - values[noff + c]) / values[noff + C + c], rounded after each op as torch's sub_
+ * and div_ round), 3 erase with the fill cast to uint8 ((uint8_t)(int64_t)v: the image is still uint8), 4 erase with
+ * the fp32 fill. Erasing fills the row's rectangle as hb_erase_batch does (fill 0 none, 1 per channel at values[voff +
+ * c], 2 per pixel at values[voff + (c*h + y)*w + x]). rows: C*H; row_len: W. No host synchronisation. */
+int hb_image_tail_batch(const void* descs, const float* values, int N, int rows, int row_len, int src_dtype, int ops,
+                        int noff, void* stream);
+
 /* ---- TrivialAugmentWide: torchvision.transforms.TrivialAugmentWide.forward (op, magnitude and sign drawn on the
  *      host) and the torchvision.transforms.autoaugment._apply_op it calls on a uint8 tensor, as the reference's
  *      classification recipe applies it (references/classification/train.py:103) - a batch in at most two launches -- */
